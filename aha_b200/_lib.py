@@ -104,6 +104,7 @@ SYMBOLS = {
     "aha_b200_sinc_resample_bank": (C.c_int, [C.c_int64, C.c_int64, _F32P, C.c_size_t, C.POINTER(C.c_int32)]),
     "aha_b200_split_audio_into_chunks": (C.c_int, [C.c_size_t, C.c_uint32, C.c_float, C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_embed": (C.c_int, [_P, _U32P, C.c_size_t, _F32P]),
+    "aha_b200_embed_batch": (C.c_int, [_P, _U32P, C.POINTER(C.c_size_t), C.c_size_t, _F32P]),
     "aha_b200_rerank": (C.c_int, [_P, _U32P, C.c_size_t, _U32P, C.POINTER(C.c_size_t), C.c_size_t, _F32P]),
     "aha_b200_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "aha_b200_rope_index": (C.c_int, [_U32P, C.c_size_t, _U32P, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,

@@ -37,6 +37,8 @@ struct aha_model {
     int audio_token_id = -1;
     int* d_scatter_idx = nullptr;
     int max_scatter = 0;
+    int* d_pack_work = nullptr;   // packed embeddings: varlen attention work list ([max_prefill][3]) and the pooled rows ([max_prefill]),
+    int* d_pack_rows = nullptr;   // allocated by the first aha_b200_embed_batch
     double last_vision_secs = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // pinned staging for the host<->device scalars of a step / the tokens of a burst
@@ -1460,10 +1462,89 @@ void embed_one(aha_model* m, const uint32_t* ids, size_t S, float* out) {
     AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
     drop_cache(m);   // clear_kv_cache()
 }
+
+// Qwen3Embedding::embed_multi (qwen3_embedding/mod.rs:38-48): embed_one for every text, computed as packed prefills.  The texts, in input
+// order, are cut into packs of at most min(max_prefill, max_ctx) tokens.  A pack is one prefill in which every text attends only to itself
+// and its positions restart at 0 (TextModel::prefill with PrefillSegments), so one pass over the weights serves many texts.  The last row of
+// every text then goes through the final RMSNorm and l2_normalize kernels that embed_one uses.
+void embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n, float* out) {
+    AHA_REQUIRE(n >= 1, "embedding input cannot be empty");
+    require_no_session(m);
+    AHA_REQUIRE(m->kind == aha_model::QWEN3, "embeddings need a qwen3 handle (Qwen3-Embedding shares Qwen3Model)");
+    AHA_REQUIRE(ids && lens && out, "ids, lens and out are required");
+    TextModel& T = m->text;
+    AHA_REQUIRE(T.tp_world == 1, "embed_batch is single-GPU (tp_world must be 1)");
+    size_t total = 0;
+    for (size_t j = 0; j < n; ++j) {
+        const size_t S = lens[j];
+        AHA_REQUIRE(S >= 1, "empty input_ids");
+        AHA_REQUIRE(S <= (size_t)T.max_prefill, "prompt of " + std::to_string(S) + " tokens exceeds max_prefill " + std::to_string(T.max_prefill));
+        AHA_REQUIRE(S <= (size_t)T.max_ctx, "context of " + std::to_string(S) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+        for (size_t i = 0; i < S; ++i) AHA_REQUIRE(ids[total + i] < (uint32_t)T.cfg.V, "token id out of range");
+        total += S;
+    }
+    Ctx& c = m->ctx;
+    if (!m->d_pack_work) {
+        m->d_pack_work = c.alloc<int>((size_t)3 * T.max_prefill);
+        m->d_pack_rows = c.alloc<int>((size_t)T.max_prefill);
+    }
+    const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
+    const int H = T.cfg.H;
+    drop_cache(m);
+    size_t first = 0, off = 0;
+    while (first < n) {
+        // Texts start on multiples of kPackAlign tokens: a segment's start is the innermost TMA coordinate of the attention kernel's V^T tiles,
+        // which has to sit on a 16-byte boundary.  The gap after a text is filled with token 0 and joins that text's segment: its rows come after
+        // every real row, so the causal mask keeps them out of the text's own rows, and the text's KV tiles and query tiles stay the same (a
+        // 16-token round-up never crosses a 64-token boundary).  The last text of a pack is not padded.
+        constexpr size_t kPackAlign = 16;
+        size_t last = first, S = 0;
+        std::vector<size_t> start;
+        while (last < n) {
+            const size_t s0 = last == first ? 0 : (S + kPackAlign - 1) / kPackAlign * kPackAlign;
+            if (s0 + lens[last] > cap) break;   // every text fits a pack on its own (checked above)
+            start.push_back(s0);
+            S = s0 + lens[last++];
+        }
+        PrefillSegments sg;
+        std::vector<uint32_t> pack_ids(S, 0);
+        std::vector<int> pos3((size_t)3 * S), work, rows;
+        for (size_t j = first; j < last; ++j) {
+            const int s0 = (int)start[j - first], len = (int)lens[j];
+            const int seg = (j + 1 < last ? (int)start[j + 1 - first] : (int)S) - s0;   // the text and the filler behind it
+            std::memcpy(pack_ids.data() + s0, ids + off, (size_t)len * sizeof(uint32_t));
+            off += len;
+            for (int r = 0; r < 3; ++r) for (int i = 0; i < seg; ++i) pos3[(size_t)r * S + s0 + i] = i;
+            sg.segs.emplace_back(s0, seg);
+            for (int q = 0; q < seg; q += kFaBQ) { work.push_back(s0); work.push_back(seg); work.push_back(q); }
+            rows.push_back(s0 + len - 1);
+        }
+        sg.d_work = m->d_pack_work;
+        sg.n_work = (int)(work.size() / 3);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_ids, pack_ids.data(), S * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, work.data(), work.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        upload_pos(m, pos3);
+        T.prefill((int)S, 0, false, nullptr, 0, {}, sg);
+        const int np = (int)(last - first);
+        gather_rows_kernel<<<np, 256, 0, c.stream>>>(m->d_pack_rows, T.x, T.xn, H);
+        rmsnorm_kernel<<<np, 256, 0, c.stream>>>(T.xn, T.norm, T.cfg.eps, T.x, H);
+        l2_normalize_kernel<<<np, 256, 0, c.stream>>>(T.x, T.xn, H);
+        c.cnt.kernels += 3;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(out + first * H, T.xn, (size_t)np * H * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        first = last;
+    }
+    drop_cache(m);
+}
 }  // namespace
 
 int aha_b200_embed(aha_model* m, const uint32_t* ids, size_t seq_len, float* out) {
     return guarded(m, [&] { embed_one(m, ids, seq_len, out); });
+}
+
+int aha_b200_embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n, float* out) {
+    return guarded(m, [&] { embed_batch(m, ids, lens, n, out); });
 }
 
 int aha_b200_rerank(aha_model* m, const uint32_t* query_ids, size_t query_len, const uint32_t* doc_ids, const size_t* doc_lens, size_t n_docs,

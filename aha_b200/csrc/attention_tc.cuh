@@ -96,6 +96,7 @@ struct FlashTcArgs {
     __half *out_hi, *out_lo;   // when set: the output goes out as fp16 hi + lo halves (operand format of the next GEMM) instead of fp32
     int Sq, Skv, q0, groups;
     float scaling;
+    const int* work = nullptr;   // VARLEN: [gridDim.x][3] = (seg_start, seg_len, qt0), one 128-query tile of one packed segment per item
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {   // 2^x on the MUFU, flush-to-zero (inputs here are <= 0; -inf -> 0)
@@ -111,7 +112,12 @@ __device__ __forceinline__ void fa_mma_pv(float (&o)[HD / 2], const uint32_t (&a
     else wgmma_rs_n128(o, a, db);
 }
 
-template <int HD, bool CAUSAL>
+// VARLEN: independent segments packed back to back in one tensor (Sq = Skv = the pack's length T).  blockIdx.x picks a work item; inside it
+// Sq = Skv = seg_len and every tensor row / column and the output row is offset by seg_start, while the KV tile grid and the masks stay
+// relative to the segment.  So each query row goes through the same operations in the same order as when its segment runs alone: keys of the
+// next segment that enter the last tile are masked (kj >= seg_len or kj > qi) and their V rows are multiplied by P = 0.  seg_start must be a
+// multiple of 16 tokens (flash_attn_tc_varlen).
+template <int HD, bool CAUSAL, bool VARLEN = false>
 __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_qh, const __grid_constant__ CUtensorMap tm_ql,
                                                                      const __grid_constant__ CUtensorMap tm_kh, const __grid_constant__ CUtensorMap tm_kl,
                                                                      const __grid_constant__ CUtensorMap tm_vh, const __grid_constant__ CUtensorMap tm_vl, FlashTcArgs a) {
@@ -129,10 +135,14 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int head = blockIdx.y, kvh = head / a.groups;
-    const int qt0 = blockIdx.x * BQ;
-    const int causal_shift = a.Skv - a.Sq;
-    int kv_end = a.Skv;
-    if (CAUSAL) kv_end = min(a.Skv, qt0 + BQ + causal_shift);
+    int seg0 = 0, Sq = a.Sq, Skv = a.Skv, qt0 = blockIdx.x * BQ;
+    if constexpr (VARLEN) {
+        const int* w = a.work + 3 * blockIdx.x;
+        seg0 = __ldg(w); Sq = Skv = __ldg(w + 1); qt0 = __ldg(w + 2);
+    }
+    const int causal_shift = Skv - Sq;
+    int kv_end = Skv;
+    if (CAUSAL) kv_end = min(Skv, qt0 + BQ + causal_shift);
     const int ntiles = (kv_end + BKV - 1) / BKV;
 
     if (tid == 0) {
@@ -145,7 +155,7 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
     if (warp == 8) {
         // ======================= producer lane: Q once, then the K / V^T tiles through the two-stage ring
         if (lane == 0) {
-            const int qrow = head * a.Sq + qt0, krow = kvh * a.Skv, vrow = kvh * HD;
+            const int qrow = head * a.Sq + seg0 + qt0, krow = kvh * a.Skv + seg0, vrow = kvh * HD;
             mbar_expect_tx(bar_q, 2 * kQBytes);
 #pragma unroll
             for (int kb = 0; kb < KB; ++kb) {
@@ -162,8 +172,8 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
                     tma_load_2d(st + kb * kKBlk, &tm_kh, kb * 64, krow + t * BKV, &full[s]);
                     tma_load_2d(st + kKBytes + kb * kKBlk, &tm_kl, kb * 64, krow + t * BKV, &full[s]);
                 }
-                tma_load_2d(st + 2 * kKBytes, &tm_vh, t * BKV, vrow, &full[s]);
-                tma_load_2d(st + 2 * kKBytes + kVBytes, &tm_vl, t * BKV, vrow, &full[s]);
+                tma_load_2d(st + 2 * kKBytes, &tm_vh, seg0 + t * BKV, vrow, &full[s]);
+                tma_load_2d(st + 2 * kKBytes + kVBytes, &tm_vl, seg0 + t * BKV, vrow, &full[s]);
             }
         }
         return;
@@ -200,7 +210,7 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
         wgmma_fence_regs(sc);
         // masking only on the tiles that can need it (the last one / the causal diagonal); the max on raw scores (scale > 0 commutes
         // with max); scale and max subtraction in ONE fma feeding ex2.approx
-        const bool mask_tile = (kt0 + BKV > a.Skv) || (CAUSAL && kt0 + BKV - 1 > qt0 + wg * 64 + causal_shift);
+        const bool mask_tile = (kt0 + BKV > Skv) || (CAUSAL && kt0 + BKV - 1 > qt0 + wg * 64 + causal_shift);
         float alpha[2];
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
@@ -212,7 +222,7 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
                 for (int c = 0; c < 2; ++c) {
                     float& x = sc[4 * j + 2 * r + c];
                     const int kj = kt0 + 8 * j + c0 + c;
-                    if (mask_tile && (kj >= a.Skv || (CAUSAL && kj > qi + causal_shift))) x = -INFINITY;
+                    if (mask_tile && (kj >= Skv || (CAUSAL && kj > qi + causal_shift))) x = -INFINITY;
                     rmax = fmaxf(rmax, x);
                 }
             rmax = fmaxf(rmax, __shfl_xor_sync(0xffffffffu, rmax, 1));
@@ -257,14 +267,19 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage have retired
     }
+    if constexpr (VARLEN) {   // read again rather than held through the KV loop (keeps the register count of the plain kernel)
+        const int* w = a.work + 3 * blockIdx.x;
+        asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(seg0) : "l"(w));
+        asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(Sq) : "l"(w + 1));
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
         l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
         const int qi = qt0 + r0 + 8 * r;
-        if (qi >= a.Sq) continue;
+        if (qi >= Sq) continue;
         const float inv = 1.0f / l[r];
-        const size_t off = (size_t)(a.q0 + qi) * a.o_tok_stride + (size_t)head * a.o_head_stride + c0;
+        const size_t off = (size_t)(a.q0 + seg0 + qi) * a.o_tok_stride + (size_t)head * a.o_head_stride + c0;
 #pragma unroll
         for (int j = 0; j < HD / 8; ++j) {
             const float x = o[4 * j + 2 * r] * inv, y = o[4 * j + 2 * r + 1] * inv;
@@ -294,11 +309,15 @@ inline void flash_attn_tc_init() {
     AHA_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flash_tc_smem_bytes<64>()));
     AHA_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flash_tc_smem_bytes<128>()));
     AHA_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flash_tc_smem_bytes<128>()));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_tc_kernel<128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)flash_tc_smem_bytes<128>()));
 }
-// head_dim 64 (ViT, audio encoder: 96 KB of shared memory) and 128 (LLM prefill, causal, GQA, paged KV: 192 KB).  `ws`: at least flash_tc_ws_halfs<HD>() halfs.
+// The split pass over all of `a`, then the tensor maps and kernel arguments of the attention launch.
+struct FlashTcLaunch {
+    CUtensorMap tqh, tql, tkh, tkl, tvh, tvl;
+    FlashTcArgs m;
+};
 template <int HD>
-inline void flash_attn_tc(cudaStream_t st, const FlashArgs& a, int nheads, bool causal, __half* ws, int num_sms) {
-    if (a.Sq == 0) return;
+inline FlashTcLaunch flash_tc_prepare(cudaStream_t st, const FlashArgs& a, int nheads, __half* ws, int num_sms) {
     const int nkv = nheads / a.groups, pad = flash_tc_skv_pad(a.Skv);
     SplitTcArgs sp;
     sp.f = a; sp.nheads = nheads; sp.nkv = nkv; sp.skv_pad = pad;
@@ -306,16 +325,37 @@ inline void flash_attn_tc(cudaStream_t st, const FlashArgs& a, int nheads, bool 
     sp.q_hi = ws; sp.q_lo = ws + nq; sp.k_hi = ws + 2 * nq; sp.k_lo = sp.k_hi + nk; sp.vt_hi = sp.k_lo + nk; sp.vt_lo = sp.vt_hi + nv;
     const unsigned blocks = (unsigned)std::min<size_t>(std::max<size_t>(ceil_div((int)std::max((size_t)nheads * a.Sq, (size_t)nkv * a.Skv), 512 / HD), (size_t)nkv * (pad / 64)), (size_t)num_sms * 32);
     split_qkv_tc_kernel<HD><<<dim3(blocks, 3), 128, 0, st>>>(sp);
-    const CUtensorMap tqh = make_tmap_f16_box(sp.q_hi, (uint64_t)nheads * a.Sq, HD, kFaBQ), tql = make_tmap_f16_box(sp.q_lo, (uint64_t)nheads * a.Sq, HD, kFaBQ);
-    const CUtensorMap tkh = make_tmap_f16_box(sp.k_hi, (uint64_t)nkv * a.Skv, HD, kFaBKV), tkl = make_tmap_f16_box(sp.k_lo, (uint64_t)nkv * a.Skv, HD, kFaBKV);
-    const CUtensorMap tvh = make_tmap_f16_box(sp.vt_hi, (uint64_t)nkv * HD, (uint64_t)pad, HD), tvl = make_tmap_f16_box(sp.vt_lo, (uint64_t)nkv * HD, (uint64_t)pad, HD);
-    FlashTcArgs m;
+    FlashTcLaunch L;
+    L.tqh = make_tmap_f16_box(sp.q_hi, (uint64_t)nheads * a.Sq, HD, kFaBQ); L.tql = make_tmap_f16_box(sp.q_lo, (uint64_t)nheads * a.Sq, HD, kFaBQ);
+    L.tkh = make_tmap_f16_box(sp.k_hi, (uint64_t)nkv * a.Skv, HD, kFaBKV); L.tkl = make_tmap_f16_box(sp.k_lo, (uint64_t)nkv * a.Skv, HD, kFaBKV);
+    L.tvh = make_tmap_f16_box(sp.vt_hi, (uint64_t)nkv * HD, (uint64_t)pad, HD); L.tvl = make_tmap_f16_box(sp.vt_lo, (uint64_t)nkv * HD, (uint64_t)pad, HD);
+    FlashTcArgs& m = L.m;
     m.out = a.out; m.o_tok_stride = a.o_tok_stride; m.o_head_stride = a.o_head_stride; m.out_hi = a.out_hi; m.out_lo = a.out_lo;
     m.Sq = a.Sq; m.Skv = a.Skv; m.q0 = a.q0; m.groups = a.groups; m.scaling = a.scaling;
+    return L;
+}
+// head_dim 64 (ViT, audio encoder: 96 KB of shared memory) and 128 (LLM prefill, causal, GQA, paged KV: 192 KB).  `ws`: at least flash_tc_ws_halfs<HD>() halfs.
+template <int HD>
+inline void flash_attn_tc(cudaStream_t st, const FlashArgs& a, int nheads, bool causal, __half* ws, int num_sms) {
+    if (a.Sq == 0) return;
+    const FlashTcLaunch L = flash_tc_prepare<HD>(st, a, nheads, ws, num_sms);
     dim3 grid(ceil_div(a.Sq, kFaBQ), nheads);
     const size_t smem = flash_tc_smem_bytes<HD>();
-    if (causal) flash_attn_tc_kernel<HD, true><<<grid, kFaThreads, smem, st>>>(tqh, tql, tkh, tkl, tvh, tvl, m);
-    else flash_attn_tc_kernel<HD, false><<<grid, kFaThreads, smem, st>>>(tqh, tql, tkh, tkl, tvh, tvl, m);
+    if (causal) flash_attn_tc_kernel<HD, true><<<grid, kFaThreads, smem, st>>>(L.tqh, L.tql, L.tkh, L.tkl, L.tvh, L.tvl, L.m);
+    else flash_attn_tc_kernel<HD, false><<<grid, kFaThreads, smem, st>>>(L.tqh, L.tql, L.tkh, L.tkl, L.tvh, L.tvl, L.m);
+    AHA_CUDA_CHECK(cudaGetLastError());
+}
+// Causal attention over independent segments packed back to back (head_dim 128; packed embeddings).  `a` covers the whole pack
+// (Sq = Skv = T, q0 = kv0 = 0): the split pass runs once over it, then one launch of (n_work, nheads) CTAs.  work: device
+// [n_work][3] = (seg_start, seg_len, qt0), one item per 128-query tile of every segment.  `ws`: at least flash_tc_ws_halfs<128>(a) halfs.
+// seg_start is the innermost TMA coordinate of the V^T tiles, so it must keep them on a 16-byte boundary: callers pack segments on
+// multiples of 16 tokens.
+inline void flash_attn_tc_varlen(cudaStream_t st, const FlashArgs& a, int nheads, const int* work, int n_work, __half* ws, int num_sms) {
+    if (n_work == 0) return;
+    AHA_REQUIRE(a.Sq == a.Skv && a.q0 == 0 && a.kv0 == 0, "flash_attn_tc_varlen: the pack is its own key range");
+    FlashTcLaunch L = flash_tc_prepare<128>(st, a, nheads, ws, num_sms);
+    L.m.work = work;
+    flash_attn_tc_kernel<128, true, true><<<dim3(n_work, nheads), kFaThreads, flash_tc_smem_bytes<128>(), st>>>(L.tqh, L.tql, L.tkh, L.tkl, L.tvh, L.tvl, L.m);
     AHA_CUDA_CHECK(cudaGetLastError());
 }
 

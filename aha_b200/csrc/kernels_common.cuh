@@ -97,6 +97,14 @@ __global__ void scatter_rows_kernel(const int* __restrict__ idx, const float* __
     for (int i = threadIdx.x; i < H; i += blockDim.x) o[i] = add ? (o[i] + s[i]) : s[i];
 }
 
+// out[r] = src[idx[r]] (rows of H floats), one block per output row
+__global__ void gather_rows_kernel(const int* __restrict__ idx, const float* __restrict__ src, float* __restrict__ out, int H) {
+    const int r = blockIdx.x;
+    const float* s = src + (size_t)idx[r] * H;
+    float* o = out + (size_t)r * H;
+    for (int i = threadIdx.x; i < H; i += blockDim.x) o[i] = s[i];
+}
+
 // l2_normalize (src/models/common/modules.rs:1287-1294): x / sqrt(sum(x^2) + 1e-6), one row per block.
 __global__ void l2_normalize_kernel(const float* __restrict__ x, float* __restrict__ out, int H) {
     __shared__ float red[32];

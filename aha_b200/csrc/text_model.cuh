@@ -184,6 +184,30 @@ inline void flash_dispatch(Ctx& c, const FlashArgs& a, int nheads, bool causal) 
     c.cnt.kernels++;
 }
 
+// Independent texts packed into one prefill (aha_b200_embed_batch): each text attends only to itself, its RoPE positions restart at 0 and its
+// K/V take the packed cache slots [start, start + len).
+struct PrefillSegments {
+    std::vector<std::pair<int, int>> segs;   // (start, len) of every text, in pack order
+    const int* d_work = nullptr;             // device [n_work][3] = (seg_start, seg_len, qt0): the work list of flash_attn_tc_varlen
+    int n_work = 0;
+    bool empty() const { return segs.empty(); }
+};
+// Causal attention inside every segment of a pack (`a` covers the whole pack: Sq = Skv = T, q0 = kv0 = 0).  attn_impl 0: one launch of the
+// varlen wgmma kernel; the SIMT and mma.sync twins run one flash_dispatch per segment, as the ViT runs its segments.
+inline void flash_dispatch_segments(Ctx& c, const FlashArgs& a, int nheads, const PrefillSegments& sg) {
+    if (c.attn_impl == 0) {
+        for (const auto& s : sg.segs) AHA_REQUIRE(s.first % 16 == 0, "packed segments must start on multiples of 16 tokens");
+        flash_attn_tc_varlen(c.stream, a, nheads, sg.d_work, sg.n_work, c.split_buf((flash_tc_ws_halfs<128>(a, nheads) + 1) / 2), c.num_sms);
+        c.cnt.kernels += 2;
+        return;
+    }
+    for (const auto& s : sg.segs) {
+        FlashArgs f = a;
+        f.Sq = f.Skv = s.second; f.q0 = f.kv0 = s.first;
+        flash_dispatch<128>(c, f, nheads, true);
+    }
+}
+
 // y = x W^T with the fused epilogues of gemm_simt.cuh.  Dispatch: wgmma split-fp16 kernel (gemm_tc.cuh) when the
 // shape tiles (K % 64 == 0, N % 32 == 0) and there are enough rows to fill a tile, else the exact SIMT kernel.
 struct ActSplit {   // fp16 hi + lo halves of an activation tensor [rows, ld]
@@ -677,11 +701,14 @@ struct TextModel {
 
     // ---- prefill: ids already on device in d_ids (or embeddings already in x when embeds_ready), pos3 in d_pos3.
     // visual_idx/deepstack: Qwen3-VL deepstack injection (qwen3vl/model.rs:815-824).
-    void prefill(int S, int pos0, bool embeds_ready, const int* d_visual_idx, int n_visual, const std::vector<const float*>& deepstack) {
+    // segs (packed embeddings): the S tokens are independent texts; attention stays inside each one and no logits are computed (head() is skipped).
+    void prefill(int S, int pos0, bool embeds_ready, const int* d_visual_idx, int n_visual, const std::vector<const float*>& deepstack,
+                 const PrefillSegments& segs = PrefillSegments()) {
         Ctx& c = *ctx;
         cudaStream_t st = c.stream;
         const int H = cfg.H, hd = cfg.hd;
         AHA_REQUIRE(S <= max_prefill, "prompt of " + std::to_string(S) + " tokens exceeds max_prefill " + std::to_string(max_prefill));
+        AHA_REQUIRE(segs.empty() || pos0 == 0, "packed segments start from an empty cache");
         ensure_tokens(pos0 + S);
         if (!embeds_ready) { embed_gather_kernel<<<S, 256, 0, st>>>(d_ids, embed, x, S, H, cfg.V); c.cnt.kernels++; }
         RopeArgs rp{inv_freq, mrope_sel, d_pos3, S};
@@ -709,7 +736,8 @@ struct TextModel {
             if (ps) {
                 ActSplit ao = act_split(c, 1, (size_t)S * std::max(nh_l * hd, I_l));
                 fa.out_hi = ao.hi; fa.out_lo = ao.lo;
-                flash_dispatch<128>(c, fa, nh_l, true);
+                if (segs.empty()) flash_dispatch<128>(c, fa, nh_l, true);
+                else flash_dispatch_segments(c, fa, nh_l, segs);
                 if (tp_world > 1) { linear_gemm_split(c, EPI_STORE, ao.hi, ao.lo, T.o, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
                 else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.o, x, H, x, H, S);
                 ActSplit n2 = act_split(c, 0, (size_t)S * H);
@@ -718,7 +746,8 @@ struct TextModel {
                 if (tp_world > 1) { linear_gemm_split(c, EPI_STORE, ao.hi, ao.lo, T.down, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
                 else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.down, x, H, x, H, S);
             } else {
-                flash_dispatch<128>(c, fa, nh_l, true);
+                if (segs.empty()) flash_dispatch<128>(c, fa, nh_l, true);
+                else flash_dispatch_segments(c, fa, nh_l, segs);
                 if (tp_world > 1) { gemm(EPI_STORE, attn, nh_l * hd, T.o, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
                 else gemm(EPI_RESID, attn, nh_l * hd, T.o, x, H, x, H, S);
                 rmsnorm_kernel<<<S, 256, 0, st>>>(x, T.ln2, cfg.eps, xn, H); c.cnt.kernels++;
@@ -734,7 +763,7 @@ struct TextModel {
         trace_S = S;
         AHA_CUDA_CHECK(cudaGetLastError());
         // last-token logits: final RMSNorm fused into the lm_head GEMV (qwen3/model.rs:186-187,142)
-        head(x + (size_t)(S - 1) * H);
+        if (segs.empty()) head(x + (size_t)(S - 1) * H);
     }
 
     void head(const float* xrow) {

@@ -327,6 +327,17 @@ class B200Model:
                                              out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
 
+    def embed_batch(self, list_of_ids):
+        """Qwen3Embedding::embed_multi on token ids -> unit vectors (n, hidden_size) float32 in input order, the texts packed into
+        shared prefills (each text attends only to itself)."""
+        texts = [self._ids(t) for t in list_of_ids]
+        cat = np.ascontiguousarray(np.concatenate(texts)) if texts else np.zeros(0, np.uint32)
+        lens = (C.c_size_t * max(len(texts), 1))(*[t.size for t in texts])
+        out = np.empty((len(texts), self.hidden_size), np.float32)
+        self._check(self._lib.aha_b200_embed_batch(self._h, cat.ctypes.data_as(C.POINTER(C.c_uint32)), lens, len(texts),
+                                                   out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out
+
     def rerank(self, query_ids, documents_ids):
         """Qwen3Reranker::rerank on token ids -> cosine scores (n_docs,) float32."""
         q = self._ids(query_ids)

@@ -285,6 +285,10 @@ int aha_b200_split_audio_into_chunks(size_t total_len, uint32_t sample_rate, flo
                                      size_t* n_out);
 
 int aha_b200_embed(aha_model* m, const uint32_t* ids, size_t seq_len, float* out);
+/* Qwen3Embedding::embed_multi (src/models/qwen3_embedding/mod.rs:38-48): embed_one for every text, computed as packed prefills.
+ * ids: the n texts back to back; lens[n]: their lengths; out: [n][hidden_size] unit vectors, in input order.  "qwen3" handles,
+ * single GPU.  The cache is cleared before and after, like aha_b200_embed. */
+int aha_b200_embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n, float* out);
 /* Qwen3Reranker::rerank (src/models/qwen3_reranker/mod.rs:23-31): cosine score of the query embedding
  * against each document embedding (cosine_similarity_no_l2 on unit vectors).  doc_ids holds the documents back to back,
  * doc_lens[n_docs] their lengths; scores_out: n_docs floats. */
