@@ -37,8 +37,9 @@ struct aha_model {
     int audio_token_id = -1;
     int* d_scatter_idx = nullptr;
     int max_scatter = 0;
-    int* d_pack_work = nullptr;   // packed embeddings: varlen attention work list ([max_prefill][3]) and the pooled rows ([max_prefill]),
-    int* d_pack_rows = nullptr;   // allocated by the first aha_b200_embed_batch
+    int* d_pack_work = nullptr;   // packed prefills (embed_batch, batch_add_many): varlen attention work list ([max_prefill][3]), the rows
+    int* d_pack_rows = nullptr;   // taken from the pack ([max_prefill]) and the pack's page table ([num_pages]); allocated on first use
+    int* d_pack_table = nullptr;
     double last_vision_secs = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // pinned staging for the host<->device scalars of a step / the tokens of a burst
@@ -296,6 +297,14 @@ void drop_cache(aha_model* m) {
     m->rope_delta = 0;
     m->cached_ids.clear();
     m->cached_mm_fp = 0;
+}
+
+void alloc_pack_buffers(aha_model* m) {
+    if (m->d_pack_work) return;
+    const TextModel& T = m->text;
+    m->d_pack_work = m->ctx.alloc<int>((size_t)3 * T.max_prefill);
+    m->d_pack_rows = m->ctx.alloc<int>((size_t)T.max_prefill);
+    m->d_pack_table = m->ctx.alloc<int>((size_t)T.num_pages);
 }
 
 // The multi-token forward (prefill).  Mirrors Qwen3Model::forward / Qwen3VLModel::forward / Qwen3ASRThinker::forward.
@@ -803,6 +812,187 @@ void session_add(aha_model* m, const aha_batch_request& r, int* slot_out, uint32
     if (stop) session_release(m, slot);
     *slot_out = slot; *first_token = tok; *finished = stop ? 1 : 0;
 }
+// a request whose sampler failed (all-zero weights) raises the shared error flag
+void throw_on_sample_error(TextModel& T) {
+    if (!T.d_sample_err) return;
+    int e = 0;
+    AHA_CUDA_CHECK(cudaMemcpy(&e, T.d_sample_err, sizeof(int), cudaMemcpyDeviceToHost));
+    if (e) { cudaMemset(T.d_sample_err, 0, sizeof(int)); throw std::runtime_error("sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)"); }
+}
+// n requests admitted in one call (aha_b200_batch_add_many).  Text-only requests that fit max_prefill are cut, in input order, into packed
+// prefills (TextModel::prefill with PrefillSegments: each request attends only to itself and its positions restart at 0), so one pass over the
+// weights serves them all; their last rows then go through the step's batched lm_head and each request's own ArgMax / sampler.  A request
+// with multimodal tensors, or one longer than max_prefill, is prefilled alone by batch_prefill_slot, exactly as batch_add does it.
+//
+// Every request of a pack starts on a multiple of kPage tokens, so the pack's page table is the slots' own page lists laid end to end: pack
+// position p of the request starting at s0 is its page (p - s0) / kPage at the same offset, and the prefill writes every request's K/V straight
+// into that request's own pages.  The gap behind a request is filled with token 0 and joins its segment; those K/V land in the request's last
+// page at positions >= seq_len, which its decode steps overwrite before any step reads them.  A 32-token round-up never reaches a 64-token KV
+// tile or a 128-token query tile that the request's own rows do not already touch, so each request runs the attention tiles it runs alone.
+void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out, uint32_t* first_tokens, int32_t* finished,
+                      aha_usage* usage) {
+    TextModel& T = m->text;
+    BatchDecoder& B = m->batch;
+    Ctx& c = m->ctx;
+    // ---- every check before any device work: a refused call leaves the session untouched
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    AHA_REQUIRE(n >= 1, "batch_add_many: no requests");
+    std::vector<int> slot;   // request i takes the i-th lowest free slot
+    for (int i = 0; i < kGemvBatchMax; ++i) if (!m->session.used[i]) slot.push_back(i);
+    AHA_REQUIRE(n <= slot.size(), "batch_add_many: " + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) +
+                                      " of the 8 slots are free (step until requests finish)");
+    slot.resize(n);
+    std::vector<size_t> sample_len(n);
+    std::vector<bool> packed(n);
+    size_t pages = 0;
+    for (size_t i = 0; i < n; ++i) {
+        const aha_batch_request& r = reqs[i];
+        AHA_REQUIRE(r.ids && r.seq_len >= 1, "batch_add_many: request " + std::to_string(i) + " needs input_ids");
+        for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
+        AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "batch_add_many: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+        if (m->kind == aha_model::QWEN3VL) AHA_REQUIRE(r.mm && r.mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
+        if (m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(r.mm && r.mm->n == 1, "Qwen3 asr process data error, must have input_features");
+        sample_len[i] = std::max<size_t>(r.params.max_tokens, 1);
+        pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
+        bool has_mm = false;   // (a qwen3 handle ignores the tensors)
+        for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
+        packed[i] = !has_mm && r.seq_len <= (size_t)T.max_prefill;
+    }
+    AHA_REQUIRE(pages <= T.free_pages.size(), "batch_add_many: the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
+                                                  std::to_string(T.free_pages.size() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+    for (size_t i = 0; i < n; ++i) {   // (only reachable when max_ctx is not a multiple of the page)
+        const size_t ctx = reqs[i].seq_len + sample_len[i];
+        AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+    }
+    using clk = std::chrono::steady_clock;
+    const auto t0 = clk::now();
+    struct Guard {   // a failure leaves the session as it was: the model's own page table back in place, every slot this call took released
+        aha_model* m; const std::vector<int>& slots;
+        int swapped = -1;                                    // slot whose table is swapped into the TextModel
+        bool pack_in = false; std::vector<int> h; int mapped = 0; int* d = nullptr;   // a pack's table, or the model's own while the pack's is in
+        bool ok = false;
+        void swap_pack() { TextModel& T = m->text; std::swap(T.h_page_table, h); std::swap(T.pages_mapped, mapped); std::swap(T.d_page_table, d); pack_in = !pack_in; }
+        ~Guard() {
+            if (pack_in) swap_pack();
+            if (ok) return;
+            if (swapped >= 0) m->batch.swap_table(swapped);
+            for (int s : slots) session_release(m, s);
+            m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
+        }
+    } guard{m, slot};
+    for (int s : slot) m->session.used[s] = true;
+    std::vector<uint32_t> tok(n);
+    std::vector<double> secs(n), vision(n, 0.0);
+    // ---- packed requests: map every page each can touch (as batch_prefill_slot does after its prefill), then prefill them pack by pack
+    std::vector<size_t> pk;
+    for (size_t i = 0; i < n; ++i) {
+        if (!packed[i]) continue;
+        pk.push_back(i);
+        B.swap_table(slot[i]); guard.swapped = slot[i];
+        T.ensure_tokens((int)(reqs[i].seq_len + sample_len[i]));
+        B.swap_table(slot[i]); guard.swapped = -1;
+    }
+    if (!pk.empty()) {
+        alloc_pack_buffers(m);
+        const int H = T.cfg.H;
+        const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
+        size_t first = 0;
+        while (first < pk.size()) {
+            size_t last = first, S = 0;
+            std::vector<size_t> start;
+            while (last < pk.size()) {
+                const size_t s0 = last == first ? 0 : (S + kPage - 1) / kPage * kPage;
+                if (s0 + reqs[pk[last]].seq_len > cap) break;   // every packed request fits a pack on its own
+                start.push_back(s0);
+                S = s0 + reqs[pk[last++]].seq_len;
+            }
+            PrefillSegments sg;
+            std::vector<uint32_t> ids(S, 0);
+            std::vector<int> pos3((size_t)3 * S), work, rows, table;
+            for (size_t j = first; j < last; ++j) {
+                const aha_batch_request& r = reqs[pk[j]];
+                const int s0 = (int)start[j - first], len = (int)r.seq_len;
+                const int seg = (j + 1 < last ? (int)start[j + 1 - first] : (int)S) - s0;   // the request and the filler behind it
+                std::memcpy(ids.data() + s0, r.ids, (size_t)len * sizeof(uint32_t));
+                for (int k = 0; k < 3; ++k) for (int i = 0; i < seg; ++i) pos3[(size_t)k * S + s0 + i] = i;
+                sg.segs.emplace_back(s0, seg);
+                for (int q = 0; q < seg; q += kFaBQ) { work.push_back(s0); work.push_back(seg); work.push_back(q); }
+                rows.push_back(s0 + len - 1);
+                const BatchSlot& bs = B.slots[slot[pk[j]]];
+                for (int p = 0; p < ceil_div(seg, kPage); ++p) table.push_back(bs.h_table[p]);
+            }
+            sg.d_work = m->d_pack_work;
+            sg.n_work = (int)(work.size() / 3);
+            AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_ids, ids.data(), S * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, work.data(), work.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_table, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            upload_pos(m, pos3);   // (synchronises: the host vectors above are free after it)
+            // the pack's table stands in for the model's own while it prefills; every page is mapped, so ensure_tokens takes none
+            guard.mapped = (int)table.size();
+            table.resize(T.num_pages, 0);
+            guard.h.swap(table);
+            guard.d = m->d_pack_table;
+            guard.swap_pack();
+            T.prefill((int)S, 0, false, nullptr, 0, {}, sg);
+            guard.swap_pack();
+            gather_rows_kernel<<<(unsigned)(last - first), 256, 0, c.stream>>>(m->d_pack_rows, T.x, B.xb + first * H, H);
+            c.cnt.kernels++;
+            first = last;
+        }
+        // first tokens: batched lm_head over the gathered rows, then each request's ArgMax / sampler against an empty state (forward_any's draw)
+        std::vector<int> act;
+        for (size_t i : pk) {
+            const aha_gen_params& p = reqs[i].params;
+            T.set_sampler(sampling_mode(p), p.temperature, p.top_p, p.top_k, p.repeat_penalty, p.repeat_last_n, p.seed);
+            B.bind_sampler(slot[i]);
+            act.push_back(slot[i]);
+        }
+        const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};
+        for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
+        B.head_rows(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), true);
+        uint32_t h_tok[kGemvBatchMax];
+        DecodeState h_st[kGemvBatchMax];
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok, B.d_tok, sizeof(h_tok), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st, B.d_states, sizeof(h_st), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        throw_on_sample_error(T);
+        const double t_first = std::chrono::duration<double>(clk::now() - t0).count();
+        for (size_t i : pk) {
+            const aha_gen_params& p = reqs[i].params;
+            T.set_sampler(sampling_mode(p), p.temperature, p.top_p, p.top_k, p.repeat_penalty, p.repeat_last_n, p.seed);
+            B.adopt(slot[i], h_tok[slot[i]], (int)reqs[i].seq_len, 0, h_st[slot[i]].n_draws);
+            tok[i] = h_tok[slot[i]];
+            secs[i] = t_first;
+        }
+    }
+    // ---- the others: one prefill each, on the slot's own table
+    for (size_t i = 0; i < n; ++i) {
+        if (packed[i]) continue;
+        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], &guard.swapped);
+        secs[i] = std::chrono::duration<double>(clk::now() - t0).count();
+        vision[i] = m->last_vision_secs;
+    }
+    guard.ok = true;
+    T.clear_sampler();
+    B.table_for.clear();
+    B.clear_graphs();
+    for (size_t i = 0; i < n; ++i) {
+        const int s = slot[i];
+        m->session.budget[s] = sample_len[i];
+        m->session.produced[s] = 1;
+        bool stop = sample_len[i] == 1;
+        if ((reqs[i].params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[i]) stop = true;
+        if (usage) {
+            usage[i] = aha_usage{};
+            usage[i].prompt_tokens = (uint32_t)reqs[i].seq_len; usage[i].completion_tokens = 1;
+            usage[i].prompt_secs = secs[i];
+            usage[i].vision_secs = vision[i];
+        }
+        if (stop) session_release(m, s);
+        slots_out[i] = s; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
+    }
+}
 size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out) {
     AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
     std::vector<int> act;
@@ -823,14 +1013,7 @@ size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out) {
     }
     for (int slot : act) if (status_out[slot] == 2) session_release(m, slot);
     // sampler errors surface after the bookkeeping so that the slots stay consistent
-    {
-        TextModel& T = m->text;
-        if (T.d_sample_err) {
-            int e = 0;
-            AHA_CUDA_CHECK(cudaMemcpy(&e, T.d_sample_err, sizeof(int), cudaMemcpyDeviceToHost));
-            if (e) { cudaMemset(T.d_sample_err, 0, sizeof(int)); throw std::runtime_error("sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)"); }
-        }
-    }
+    throw_on_sample_error(m->text);
     return act.size();
 }
 
@@ -918,6 +1101,14 @@ int aha_b200_batch_add(aha_model* m, const aha_batch_request* req, int32_t* slot
         int slot = -1, fin = 0;
         session_add(m, *req, &slot, first_token_out, &fin, usage);
         *slot_out = slot; *finished_out = fin;
+    });
+}
+
+int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out, uint32_t* first_tokens_out,
+                            int32_t* finished_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(reqs && slots_out && first_tokens_out && finished_out, "reqs, slots_out, first_tokens_out and finished_out are required");
+        session_add_many(m, reqs, n, slots_out, first_tokens_out, finished_out, usage);
     });
 }
 
@@ -1484,10 +1675,7 @@ void embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n
         total += S;
     }
     Ctx& c = m->ctx;
-    if (!m->d_pack_work) {
-        m->d_pack_work = c.alloc<int>((size_t)3 * T.max_prefill);
-        m->d_pack_rows = c.alloc<int>((size_t)T.max_prefill);
-    }
+    alloc_pack_buffers(m);
     const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
     const int H = T.cfg.H;
     drop_cache(m);

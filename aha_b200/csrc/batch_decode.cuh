@@ -13,6 +13,7 @@
 // the GEMV accumulates every (row, sequence) in gemv_kernel's order and the attention / sampler kernels are the single-sequence
 // ones (tests/test_batch_gpu.py compares every sequence with its own fresh oracle run).
 // Finished sequences leave the step (the activation rows are rebuilt from the token embeddings every step, so compaction is free).
+// Packed admission (aha_b200_batch_add_many) borrows xb / logitsb between two steps for the first tokens of several requests at once (head_rows).
 #pragma once
 #include "gemv_batch.cuh"
 #include "text_model.cuh"
@@ -83,11 +84,15 @@ struct BatchDecoder {
     // after the prefill of slot i (the model's d_state / d_history / samp hold the request's state): move it into the slot
     void adopt(int i, uint32_t first_token, int seq_len, int rope_delta, uint32_t n_draws) {
         Ctx& c = *T->ctx;
-        BatchSlot& s = slots[i];
         DecodeState st{first_token, seq_len, rope_delta, 1, n_draws, {0, 0, 0}};
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_states + i, &st, sizeof(st), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_hist + (size_t)i * T->hist_cap, &first_token, sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
+        bind_sampler(i);
+    }
+    // the sampler set on the TextModel (set_sampler) becomes slot i's, with the slot's own state, history and token
+    void bind_sampler(int i) {
+        BatchSlot& s = slots[i];
         s.samp_active = T->samp_active;
         if (s.samp_active) {
             s.samp = T->samp;
@@ -197,6 +202,17 @@ struct BatchDecoder {
             proj(PRO_RMSNORM, GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb, simt);
             proj(PRO_NONE, GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb, simt);
         }
+        head_rows(act, simt, false);
+    }
+    // Final norm + lm_head over rows 0 .. nb-1 of xb, then for row j the two-stage ArgMax of slot act[j] and, when its request samples, its
+    // sampler.  A decode step (first = false) advances the slot's DecodeState and the sampled token replaces the ArgMax one the step pushed
+    // (the single-sequence loop does the same).  A request's first token (first = true, packed admission) is drawn the way forward_any draws
+    // it: no advance, no overwrite, against the slot's state as the caller set it (empty history, draw index 0); only n_draws moves.
+    void head_rows(const std::vector<int>& act, int simt, bool first) {
+        Ctx& c = *T->ctx;
+        cudaStream_t st = c.stream;
+        const TextCfg& cf = T->cfg;
+        const int nb = (int)act.size(), H = cf.H;
         LinearW head; head.w = T->lm_head; head.b = nullptr; head.N = cf.V; head.K = H;
         proj(PRO_RMSNORM, GEPI_STORE, head, xb, H, T->norm, nullptr, 0, logitsb, cf.V, nb, simt);
         for (int j = 0; j < nb; ++j) {
@@ -204,13 +220,13 @@ struct BatchDecoder {
             const float* lg = logitsb + (size_t)j * cf.V;
             argmax_partial_kernel<<<n_pcand, 256, 0, st>>>(lg, cf.V, pmaxb + (size_t)j * n_pcand, pidxb + (size_t)j * n_pcand);
             argmax_final_kernel<<<1, 32, 0, st>>>(pmaxb + (size_t)j * n_pcand, pidxb + (size_t)j * n_pcand, n_pcand, d_tok + slot, d_states + slot,
-                                                  d_hist + (size_t)slot * T->hist_cap, T->hist_cap, 1);
+                                                  d_hist + (size_t)slot * T->hist_cap, T->hist_cap, first ? 0 : 1);
             c.cnt.kernels += 2;
             BatchSlot& s = slots[slot];
-            if (s.samp_active) {   // the sampled token replaces the ArgMax one the step just pushed (the single-sequence loop does the same)
+            if (s.samp_active) {
                 SampleArgs a = s.samp;
                 a.logits = lg;
-                a.overwrite = 1;
+                a.overwrite = first ? 0 : 1;
                 sample_kernel<<<1, kSampleThreads, 0, st>>>(a);
                 c.cnt.kernels++;
             }

@@ -184,8 +184,9 @@ inline void flash_dispatch(Ctx& c, const FlashArgs& a, int nheads, bool causal) 
     c.cnt.kernels++;
 }
 
-// Independent texts packed into one prefill (aha_b200_embed_batch): each text attends only to itself, its RoPE positions restart at 0 and its
-// K/V take the packed cache slots [start, start + len).
+// Independent texts packed into one prefill (aha_b200_embed_batch, aha_b200_batch_add_many): each text attends only to itself, its RoPE
+// positions restart at 0 and its K/V take the packed cache slots [start, start + len) (which the page table in place maps to the text's own pages
+// when batch_add_many composes it from the requests' slots).
 struct PrefillSegments {
     std::vector<std::pair<int, int>> segs;   // (start, len) of every text, in pack order
     const int* d_work = nullptr;             // device [n_work][3] = (seg_start, seg_len, qt0): the work list of flash_attn_tc_varlen
@@ -701,7 +702,8 @@ struct TextModel {
 
     // ---- prefill: ids already on device in d_ids (or embeddings already in x when embeds_ready), pos3 in d_pos3.
     // visual_idx/deepstack: Qwen3-VL deepstack injection (qwen3vl/model.rs:815-824).
-    // segs (packed embeddings): the S tokens are independent texts; attention stays inside each one and no logits are computed (head() is skipped).
+    // segs (packed prefills): the S tokens are independent texts; attention stays inside each one and no logits are computed (head() is skipped;
+    // the caller takes the rows it needs from x).
     void prefill(int S, int pos0, bool embeds_ready, const int* d_visual_idx, int n_visual, const std::vector<const float*>& deepstack,
                  const PrefillSegments& segs = PrefillSegments()) {
         Ctx& c = *ctx;

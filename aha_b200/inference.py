@@ -214,9 +214,18 @@ class B200Model:
         top_k=..., repeat_penalty=..., repeat_last_n=..., seed=...), ...] (at most 8) decoded in lockstep on this handle.
         -> [(generated ids, usage dict), ...]: per request exactly what generate() returns for it alone."""
         n = len(requests)
-        arr = (L.BatchRequest * n)()
+        arr, _keep = self._batch_requests(requests)
+        cap = max([1] + [r.get("max_tokens", 1024) for r in requests])
+        out = (C.c_uint32 * (n * cap))()
+        n_out = (C.c_size_t * n)()
+        us = (L.Usage * n)()
+        self._check(self._lib.aha_b200_generate_batch(self._h, arr, n, out, cap, n_out, us))
+        return [([int(out[i * cap + j]) for j in range(n_out[i])], self._usage(us[i])) for i in range(n)]
+
+    def _batch_requests(self, requests):
+        """request dicts -> (aha_batch_request array, the buffers it points into)"""
+        arr = (L.BatchRequest * max(len(requests), 1))()
         keep = []
-        cap = 1
         for i, r in enumerate(requests):
             ids = self._ids(r["input_ids"])
             mm, k = self._mm(r.get("data"))
@@ -226,12 +235,7 @@ class B200Model:
             arr[i].mm = C.pointer(mm) if mm is not None else None
             arr[i].params = self._gen_params(r.get("max_tokens", 1024), r.get("temperature", 0.0), r.get("top_p"), r.get("top_k"),
                                              r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), r.get("flags", 0))
-            cap = max(cap, r.get("max_tokens", 1024))
-        out = (C.c_uint32 * (n * cap))()
-        n_out = (C.c_size_t * n)()
-        us = (L.Usage * n)()
-        self._check(self._lib.aha_b200_generate_batch(self._h, arr, n, out, cap, n_out, us))
-        return [([int(out[i * cap + j]) for j in range(n_out[i])], self._usage(us[i])) for i in range(n)]
+        return arr, keep
 
     # ---- continuous batching: requests join / leave a running batch between steps (aha_b200_batch_open / _add / _step / _close)
     def batch_open(self):
@@ -251,6 +255,17 @@ class B200Model:
         u = L.Usage()
         self._check(self._lib.aha_b200_batch_add(self._h, C.byref(req), C.byref(slot), C.byref(tok), C.byref(fin), C.byref(u)))
         return int(slot.value), int(tok.value), bool(fin.value)
+
+    def batch_add_many(self, requests, return_usage=False):
+        """Admit several requests (dicts as for generate_batch) in one call, the text-only ones packed into shared prefills; all or
+        nothing.  -> [(slot, first token, finished), ...] in input order, and with return_usage=True also the prompt-side usage dicts."""
+        n = len(requests)
+        arr, _keep = self._batch_requests(requests)
+        slots, toks, fins = (C.c_int32 * max(n, 1))(), (C.c_uint32 * max(n, 1))(), (C.c_int32 * max(n, 1))()
+        us = (L.Usage * max(n, 1))()
+        self._check(self._lib.aha_b200_batch_add_many(self._h, arr, n, slots, toks, fins, us))
+        res = [(int(slots[i]), int(toks[i]), bool(fins[i])) for i in range(n)]
+        return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
 
     def batch_step(self):
         """One decode step of every running request -> {slot: (token, finished)} (empty when nothing is running)."""

@@ -197,6 +197,15 @@ int aha_b200_generate_batch(aha_model* m, const aha_batch_request* reqs, size_t 
 int aha_b200_batch_open(aha_model* m);
 int aha_b200_batch_add(aha_model* m, const aha_batch_request* req, int32_t* slot_out, uint32_t* first_token_out,
                        int32_t* finished_out, aha_usage* usage /* prompt side only; may be NULL */);
+/* Continuous batching: admit n requests at once.  Text-only requests that fit are packed into shared prefills (each attends only to
+ * itself); a request with multimodal tensors, or one longer than max_prefill, is prefilled alone exactly as batch_add does it.
+ * All or nothing: if the requests do not all fit (free slots, free KV pages) or one is malformed, nothing is admitted and the session
+ * is unchanged.  Slots are assigned in input order, lowest free slot first (what n batch_add calls would assign, except that a request
+ * finished at admission keeps its slot until the call returns).
+ * Each request yields the ids its own generate_generic run yields; for prompts of 32 tokens or more (every prompt with gemm_impl 1)
+ * exactly the ids batch_add gives it.  slots_out / first_tokens_out / finished_out: [n]; usage: [n] or NULL (prompt side only). */
+int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out,
+                            uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage);
 int aha_b200_batch_step(aha_model* m, uint32_t* tokens_out /* [8] */, int32_t* status_out /* [8] */, size_t* n_stepped_out /* may be NULL */);
 int aha_b200_batch_close(aha_model* m);
 
