@@ -82,6 +82,8 @@ SYMBOLS = {
                                           C.POINTER(Usage)]),
     "aha_b200_batch_step": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.POINTER(C.c_size_t)]),
     "aha_b200_batch_close": (C.c_int, [_P]),
+    "aha_b200_batch_open_wide": (C.c_int, [_P, C.c_size_t]),
+    "aha_b200_batch_step_n": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_generate_stream": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), TOKEN_CALLBACK, C.c_void_p,
                                            C.POINTER(Usage)]),
     "aha_b200_asr_generate": (C.c_int, [_P, C.POINTER(AsrChunk), C.c_size_t, C.POINTER(GenParams), _U32P, C.c_size_t,

@@ -53,12 +53,16 @@ struct aha_model {
     uint64_t cached_mm_fp = 0;          // fingerprint of the multimodal tensors those tokens were embedded with (0 = none)
     size_t last_prefix_hit = 0;         // tokens the last generate call did not have to prefill
     BatchDecoder batch;                 // several sequences decoded in lockstep (aha_b200_generate_batch); buffers allocated on first use
+    BatchDecoder wide_batch;            // the tensor-core decoder of wide sessions (aha_b200_batch_open_wide); buffers allocated on first use
     // Continuous batching (aha_b200_batch_open / _add / _step / _close): requests join and leave a running batch between steps
     struct BatchSession {
         bool open = false;
-        bool used[kGemvBatchMax] = {};
-        size_t budget[kGemvBatchMax] = {}, produced[kGemvBatchMax] = {};
+        bool wide = false;              // opened by batch_open_wide: wide_batch runs it
+        int width = kGemvBatchMax;      // slots of the session
+        bool used[kWideSeqs] = {};
+        size_t budget[kWideSeqs] = {}, produced[kWideSeqs] = {};
     } session;
+    BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
 };
 
 namespace {
@@ -501,6 +505,7 @@ int aha_b200_create(const char* kind, const char* config_json, const aha_tensor_
         for (auto& e : m->ev_tok) AHA_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         gemv_init();
         gemm_tc_init();
+        gemv_wide_init();
         flash_attn_tc_init();
         const std::string k = kind;
         const std::string cfg_text = config_json;
@@ -585,9 +590,9 @@ int aha_b200_clear_cache(aha_model* m) {
     return guarded(m, [&] {
         AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         if (m->session.open) {   // clear_cache ends a batch session too: every sequence's K/V is gone
-            for (auto& sl : m->batch.slots) sl.mapped = 0;
-            m->batch.table_for.clear();
-            m->batch.clear_graphs();
+            for (auto& sl : m->sess().slots) sl.mapped = 0;
+            m->sess().table_for.clear();
+            m->sess().clear_graphs();
             m->session = aha_model::BatchSession{};
             m->text.clear_sampler();
         }
@@ -727,7 +732,7 @@ namespace {
 // and sampler move into the slot.  *swapped tells the caller's guard which table is swapped in if this throws.
 uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int* swapped) {
     TextModel& T = m->text;
-    BatchDecoder& B = m->batch;
+    BatchDecoder& B = m->sess();
     B.swap_table(slot); *swapped = slot;
     m->have_rope_delta = false; m->rope_delta = 0;
     T.set_sampler(sampling_mode(r.params), r.params.temperature, r.params.top_p, r.params.top_k, r.params.repeat_penalty, r.params.repeat_last_n, r.params.seed);
@@ -747,32 +752,43 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
 // (new design; the reference's server holds ONE request behind a write lock, server/api.rs:117.)  A finished request's pages go back to the
 // free list at once, so a waiting request can take its place while the others keep decoding.
 void session_release(aha_model* m, int slot) {
-    BatchSlot& sl = m->batch.slots[slot];
+    BatchSlot& sl = m->sess().slots[slot];
     for (int k = 0; k < sl.mapped; ++k) m->text.free_pages.push_back(sl.h_table[k]);
     sl.mapped = 0;
     sl.samp_active = false;
     m->session.used[slot] = false;
-    m->batch.table_for.clear();
-    m->batch.clear_graphs();       // the graphs of compositions holding this slot carry its sampler arguments by value
+    m->sess().composition_changed();   // (narrow: the graphs of compositions holding this slot carry its sampler arguments by value)
 }
 void session_close(aha_model* m) {
-    if (m->batch.cap) { for (auto& sl : m->batch.slots) sl.mapped = 0; m->batch.table_for.clear(); m->batch.clear_graphs(); }
+    for (BatchDecoder* B : {&m->batch, &m->wide_batch})
+        if (B->cap) { for (auto& sl : B->slots) sl.mapped = 0; B->table_for.clear(); B->clear_graphs(); }
     m->session = aha_model::BatchSession{};
     drop_cache(m);
     m->text.clear_sampler();
 }
-void session_open(aha_model* m) {
+// width 0: the narrow session (8 slots, batched CUDA-core GEMV); 1..64: a wide session (gemv_wide.cuh)
+void session_open(aha_model* m, int width) {
     TextModel& T = m->text;
     require_no_session(m);
     AHA_REQUIRE(T.tp_world == 1, "batch sessions are single-GPU");
-    AHA_REQUIRE(T.max_prefill >= kGemvBatchMax, "batch sessions need max_prefill >= 8");
+    if (width == 0) AHA_REQUIRE(T.max_prefill >= kGemvBatchMax, "batch sessions need max_prefill >= 8");
+    else {
+        AHA_REQUIRE(width >= 1 && width <= kWideSeqs, "batch_open_wide: max_seqs must be 1 to 64");
+        AHA_REQUIRE(BatchDecoder::wide_shapes_ok(T), "batch_open_wide: every projection's rows and columns must be multiples of 64 "
+                                                     "(hidden " + std::to_string(T.cfg.H) + ", intermediate " + std::to_string(T.I_l) +
+                                                     ", qkv rows " + std::to_string(T.qkv_dim) + ", vocabulary " + std::to_string(T.cfg.V) + ")");
+    }
     drop_cache(m);
-    m->batch.init(T, kGemvBatchMax);
-    for (auto& sl : m->batch.slots) sl.mapped = 0;
-    m->batch.table_for.clear();
-    m->batch.clear_graphs();
+    BatchDecoder& B = width == 0 ? m->batch : m->wide_batch;
+    if (width == 0) B.init(T, kGemvBatchMax);
+    else B.init_wide(T);
+    for (auto& sl : B.slots) sl.mapped = 0;
+    B.table_for.clear();
+    B.clear_graphs();
     m->session = aha_model::BatchSession{};
     m->session.open = true;
+    m->session.wide = width != 0;
+    m->session.width = width == 0 ? kGemvBatchMax : width;
 }
 void session_add(aha_model* m, const aha_batch_request& r, int* slot_out, uint32_t* first_token, int* finished, aha_usage* usage) {
     TextModel& T = m->text;
@@ -780,8 +796,8 @@ void session_add(aha_model* m, const aha_batch_request& r, int* slot_out, uint32
     AHA_REQUIRE(r.ids && r.seq_len >= 1, "batch_add: the request needs input_ids");
     AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "batch_add: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
     int slot = -1;
-    for (int i = 0; i < kGemvBatchMax; ++i) if (!m->session.used[i]) { slot = i; break; }
-    AHA_REQUIRE(slot >= 0, "batch_add: all 8 slots are decoding (step until one finishes)");
+    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) { slot = i; break; }
+    AHA_REQUIRE(slot >= 0, "batch_add: all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
     const size_t sample_len = std::max<size_t>(r.params.max_tokens, 1);
     const size_t need = (r.seq_len + sample_len + kPage - 1) / kPage;
     AHA_REQUIRE(need <= T.free_pages.size(), "batch_add: the request needs " + std::to_string(need * kPage) + " tokens of KV capacity, " +
@@ -791,14 +807,13 @@ void session_add(aha_model* m, const aha_batch_request& r, int* slot_out, uint32
     int swapped = -1;
     struct Guard {   // a failed prefill leaves the session as it was: own table back in place, the slot's pages back in the pool
         aha_model* m; int slot; int* swapped; bool ok = false;
-        ~Guard() { if (ok) return; if (*swapped >= 0) m->batch.swap_table(*swapped); session_release(m, slot); m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler(); }
+        ~Guard() { if (ok) return; if (*swapped >= 0) m->sess().swap_table(*swapped); session_release(m, slot); m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler(); }
     } guard{m, slot, &swapped};
     m->session.used[slot] = true;
     const uint32_t tok = batch_prefill_slot(m, slot, r, sample_len, &swapped);
     guard.ok = true;
     m->text.clear_sampler();
-    m->batch.table_for.clear();
-    m->batch.clear_graphs();
+    m->sess().composition_changed();
     m->session.budget[slot] = sample_len;
     m->session.produced[slot] = 1;
     bool stop = sample_len == 1;
@@ -832,15 +847,15 @@ void throw_on_sample_error(TextModel& T) {
 void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out, uint32_t* first_tokens, int32_t* finished,
                       aha_usage* usage) {
     TextModel& T = m->text;
-    BatchDecoder& B = m->batch;
+    BatchDecoder& B = m->sess();
     Ctx& c = m->ctx;
     // ---- every check before any device work: a refused call leaves the session untouched
     AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
     AHA_REQUIRE(n >= 1, "batch_add_many: no requests");
     std::vector<int> slot;   // request i takes the i-th lowest free slot
-    for (int i = 0; i < kGemvBatchMax; ++i) if (!m->session.used[i]) slot.push_back(i);
+    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) slot.push_back(i);
     AHA_REQUIRE(n <= slot.size(), "batch_add_many: " + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) +
-                                      " of the 8 slots are free (step until requests finish)");
+                                      " of the " + std::to_string(m->session.width) + " slots are free (step until requests finish)");
     slot.resize(n);
     std::vector<size_t> sample_len(n);
     std::vector<bool> packed(n);
@@ -875,7 +890,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         ~Guard() {
             if (pack_in) swap_pack();
             if (ok) return;
-            if (swapped >= 0) m->batch.swap_table(swapped);
+            if (swapped >= 0) m->sess().swap_table(swapped);
             for (int s : slots) session_release(m, s);
             m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
         }
@@ -951,10 +966,10 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};
         for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
         B.head_rows(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), true);
-        uint32_t h_tok[kGemvBatchMax];
-        DecodeState h_st[kGemvBatchMax];
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok, B.d_tok, sizeof(h_tok), cudaMemcpyDeviceToHost, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st, B.d_states, sizeof(h_st), cudaMemcpyDeviceToHost, c.stream));
+        std::vector<uint32_t> h_tok((size_t)B.cap);
+        std::vector<DecodeState> h_st((size_t)B.cap);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
         throw_on_sample_error(T);
         const double t_first = std::chrono::duration<double>(clk::now() - t0).count();
@@ -975,8 +990,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     }
     guard.ok = true;
     T.clear_sampler();
-    B.table_for.clear();
-    B.clear_graphs();
+    B.composition_changed();
     for (size_t i = 0; i < n; ++i) {
         const int s = slot[i];
         m->session.budget[s] = sample_len[i];
@@ -993,14 +1007,22 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         slots_out[i] = s; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
     }
 }
-size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out) {
+// tokens_out / status_out: [cap] entries, cap >= the session width (8 for batch_step)
+size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8) {
     AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    const int width = m->session.width;
+    if (step8)
+        AHA_REQUIRE(width <= kGemvBatchMax, "batch_step: tokens_out[8] cannot hold a session of " + std::to_string(width) + " slots: use aha_b200_batch_step_n");
+    AHA_REQUIRE(cap >= (size_t)width, "batch_step_n: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
     std::vector<int> act;
-    for (int i = 0; i < kGemvBatchMax; ++i) { status_out[i] = 0; tokens_out[i] = 0; if (m->session.used[i]) act.push_back(i); }
+    for (size_t i = 0; i < cap; ++i) { status_out[i] = 0; tokens_out[i] = 0; }
+    for (int i = 0; i < width; ++i) if (m->session.used[i]) act.push_back(i);
     if (act.empty()) return 0;
-    m->batch.step(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), env_flag("AHA_BATCH_GRAPH", true));
-    uint32_t h_tok[kGemvBatchMax];
-    AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok, m->batch.d_tok, sizeof(h_tok), cudaMemcpyDeviceToHost, m->ctx.stream));
+    BatchDecoder& B = m->sess();
+    // (AHA_BATCH_GEMV picks the narrow step's projections; the wide step always runs gemv_wide)
+    B.step(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), env_flag("AHA_BATCH_GRAPH", true));
+    std::vector<uint32_t> h_tok((size_t)B.cap);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
     AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
     // a request whose sampler failed (all-zero weights) poisons only the check below; the session is closed by the caller's error path
     for (int slot : act) {
@@ -1093,7 +1115,14 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
 }
 }  // namespace
 
-int aha_b200_batch_open(aha_model* m) { return guarded(m, [&] { session_open(m); }); }
+int aha_b200_batch_open(aha_model* m) { return guarded(m, [&] { session_open(m, 0); }); }
+
+int aha_b200_batch_open_wide(aha_model* m, size_t max_seqs) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(max_seqs >= 1 && max_seqs <= (size_t)kWideSeqs, "batch_open_wide: max_seqs must be 1 to 64");
+        session_open(m, (int)max_seqs);
+    });
+}
 
 int aha_b200_batch_add(aha_model* m, const aha_batch_request* req, int32_t* slot_out, uint32_t* first_token_out, int32_t* finished_out, aha_usage* usage) {
     return guarded(m, [&] {
@@ -1115,7 +1144,15 @@ int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t 
 int aha_b200_batch_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t* n_stepped_out) {
     return guarded(m, [&] {
         AHA_REQUIRE(tokens_out && status_out, "tokens_out[8] and status_out[8] are required");
-        const size_t n = session_step(m, tokens_out, status_out);
+        const size_t n = session_step(m, tokens_out, status_out, kGemvBatchMax, true);
+        if (n_stepped_out) *n_stepped_out = n;
+    });
+}
+
+int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, size_t* n_stepped_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(tokens_out && status_out, "tokens_out[cap] and status_out[cap] are required");
+        const size_t n = session_step(m, tokens_out, status_out, cap, false);
         if (n_stepped_out) *n_stepped_out = n;
     });
 }
@@ -1574,7 +1611,7 @@ int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, 
                         const float* resid, float* out, int iters, double* device_ms) {
     return guarded(m, [&] {
         AHA_REQUIRE(x && w && out && M > 0 && N > 0 && K > 0, "x, w, out and positive sizes are required");
-        AHA_REQUIRE((impl >= 1 && impl <= 3) || impl == 5 || impl == 6, "impl must be 1 (SIMT), 2 / 3 (wgmma 128 x 128 / 128 x 256) or 5 / 6 (batched GEMV)");
+        AHA_REQUIRE((impl >= 1 && impl <= 3) || (impl >= 5 && impl <= 7), "impl must be 1 (SIMT), 2 / 3 (wgmma 128 x 128 / 128 x 256), 5 / 6 (batched GEMV) or 7 (wide batched GEMV)");
         Ctx& c = m->ctx;
         float *dx = nullptr, *db = nullptr, *dr = nullptr, *dy = nullptr;
         __half* dw = nullptr;
@@ -1590,6 +1627,47 @@ int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, 
                 AHA_CUDA_CHECK(cudaMalloc(&dr, (size_t)M * N * 4)); AHA_CUDA_CHECK(cudaMemcpy(dr, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice));
             }
             LinearW W; W.w = dw; W.b = db; W.N = N; W.K = K;
+            if (impl == 7) {   // the wide decode projection (gemv_wide.cuh): M <= 64 rows split into fp16 hi / lo operand rows, then the kernel
+                AHA_REQUIRE(M <= kWideSeqs && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "wide batched GEMV: M <= 64, epilogue store / residual / SwiGLU");
+                AHA_REQUIRE(gemv_wide_supported(N, K), "wide batched GEMV: N and K must be multiples of 64");
+                const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
+                __half *hi = nullptr, *lo = nullptr;
+                float *ones = nullptr, *ws = nullptr;
+                int* cnt = nullptr;
+                auto free7 = [&] { cudaFree(hi); cudaFree(lo); cudaFree(ones); cudaFree(ws); cudaFree(cnt); };
+                try {
+                    const size_t xb = (size_t)kWideSeqs * K * sizeof(__half);
+                    AHA_CUDA_CHECK(cudaMalloc(&hi, xb)); AHA_CUDA_CHECK(cudaMalloc(&lo, xb));
+                    AHA_CUDA_CHECK(cudaMemset(hi, 0, xb)); AHA_CUDA_CHECK(cudaMemset(lo, 0, xb));   // rows M..63 stay zero
+                    const size_t wsf = wide_ws_floats(N, K, c.num_sms);
+                    const int tiles = wide_plan(N, K, c.num_sms).tiles;
+                    if (wsf) AHA_CUDA_CHECK(cudaMalloc(&ws, wsf * sizeof(float)));
+                    AHA_CUDA_CHECK(cudaMalloc(&cnt, (size_t)tiles * sizeof(int)));
+                    AHA_CUDA_CHECK(cudaMemset(cnt, 0, (size_t)tiles * sizeof(int)));
+                    if (gepi == GEPI_SWIGLU) {   // (behind a unit-gain RMSNorm prologue, as impl 5)
+                        std::vector<float> h1((size_t)K, 1.0f);
+                        AHA_CUDA_CHECK(cudaMalloc(&ones, (size_t)K * 4)); AHA_CUDA_CHECK(cudaMemcpy(ones, h1.data(), (size_t)K * 4, cudaMemcpyHostToDevice));
+                    }
+                    WideArgs a{};
+                    a.bias = db; a.resid = dr; a.ldr = N; a.out = dy; a.ldo = Nout; a.N = N; a.K = K; a.nb = M; a.ws = ws; a.counters = cnt;
+                    const CUtensorMap tm = make_tmap_f16(dw, (uint64_t)N, (uint64_t)K);
+                    auto run = [&] {
+                        if (ones) rmsnorm_split_kernel<<<M, 256, 0, c.stream>>>(dx, ones, 1e-6f, hi, lo, K);
+                        else split_f32_to_f16x2_kernel<<<(unsigned)(((size_t)M * K / 4 + 255) / 256), 256, 0, c.stream>>>(dx, K, hi, lo, M, K);
+                        gemv_wide(c.stream, gepi, tm, hi, lo, a, c.num_sms);
+                    };
+                    run();
+                    AHA_CUDA_CHECK(cudaEventRecord(m->ev0, c.stream));
+                    for (int i = 0; i < std::max(iters, 0); ++i) run();
+                    AHA_CUDA_CHECK(cudaEventRecord(m->ev1, c.stream));
+                    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+                } catch (...) { free7(); throw; }
+                free7();
+                if (device_ms) { float ms = 0.f; AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1)); *device_ms = ms; }
+                AHA_CUDA_CHECK(cudaMemcpy(out, dy, (size_t)M * Nout * 4, cudaMemcpyDeviceToHost));
+                cleanup();
+                return;
+            }
             if (impl == 5 || impl == 6) {   // the batched decode GEMV (gemv_batch.cuh; 6 = the cp.async ring version): M <= 8 activation rows against every weight row
                 AHA_REQUIRE(M <= kGemvBatchMax && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "batched GEMV: M <= 8, epilogue store / residual / SwiGLU");
                 GemvBatchArgs a{};
@@ -1804,6 +1882,7 @@ void aha_b200_destroy(aha_model* m) {
     if (m->ctx.stream) cudaStreamSynchronize(m->ctx.stream);
     m->text.destroy();
     m->batch.clear_graphs();
+    m->wide_batch.clear_graphs();
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
     if (m->ev0) cudaEventDestroy(m->ev0);
@@ -1904,6 +1983,9 @@ int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, s
         } else if (w == "logits") {   // logits of the last prefill / decode step (what the step's argmax was taken over)
             AHA_REQUIRE(T.tp_world == 1, "logits: the tensor-parallel ranks hold vocabulary shards");
             src = T.logits; cnt = (size_t)T.cfg.V;
+        } else if (w == "batch_graphs") {   // step graphs captured in the open batch session (wide: at most one per running count)
+            AHA_REQUIRE(cap >= 1, "out too small");
+            out[0] = (float)m->sess().graphs.size(); *n = 1; return;
         } else if (w == "rope_delta") {
             AHA_REQUIRE(cap >= 1, "out too small");
             out[0] = (float)m->rope_delta; *n = 1; return;

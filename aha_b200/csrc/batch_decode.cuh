@@ -14,8 +14,17 @@
 // ones (tests/test_batch_gpu.py compares every sequence with its own fresh oracle run).
 // Finished sequences leave the step (the activation rows are rebuilt from the token embeddings every step, so compaction is free).
 // Packed admission (aha_b200_batch_add_many) borrows xb / logitsb between two steps for the first tokens of several requests at once (head_rows).
+//
+// Wide mode (init_wide, aha_b200_batch_open_wide): up to 64 sequences, every projection and the lm_head on gemv_wide.cuh's tensor-core
+// kernel, each fed by a prep kernel that normalises and / or splits the nb fp32 rows into the fp16 hi / lo rows the kernel's TMA reads.
+// Everything that depends on WHICH slots run is read from device memory -- the active list d_act (row j -> slot), the attention table
+// d_attn, the per-slot sampler arguments d_samp -- and the embedding gather, ArgMax and sampler are row-indexed launches, so one CUDA graph
+// per running count serves every composition of that count.  A sequence's sums do not depend on its row or on the other rows (one MMA
+// width, split-K fixed by the shape), so its ids do not depend on its slot, its neighbours or the step it joined at; they are not those of
+// the single-sequence gemv_kernel, whose sums run in another order.
 #pragma once
 #include "gemv_batch.cuh"
+#include "gemv_wide.cuh"
 #include "text_model.cuh"
 
 namespace aha {
@@ -43,11 +52,63 @@ struct BatchDecoder {
     std::vector<int> table_for;          // active list the attention table was built for
     // One CUDA graph per composition of the batch (the active list changes only when a request finishes): ~170 launches per step become one.
     // The graphs hold the requests' sampler parameters by value, so they live for one generate_batch call.
-    struct StepGraph { std::vector<int> act; int simt; cudaGraphExec_t exec; uint64_t kernels; };
+    // A wide decoder keys its graphs by the running count alone (width = nb) and keeps them while requests come and go.
+    struct StepGraph { std::vector<int> act; int simt; cudaGraphExec_t exec; uint64_t kernels; int width = 0; };
     std::vector<StepGraph> graphs;
     void clear_graphs() {
         for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
         graphs.clear();
+    }
+    // the set of running requests or a slot's sampler changed: the attention table is rebuilt before the next step; a narrow decoder's
+    // graphs carry the old composition, a wide decoder's read it from device memory and stay
+    void composition_changed() {
+        table_for.clear();
+        if (!wide) clear_graphs();
+    }
+
+    // ---- wide mode
+    struct WideAct { __half* hi = nullptr; __half* lo = nullptr; int K = 0; };   // [64][K] operand rows of one K
+    bool wide = false;
+    WideAct act_h, act_q, act_i;         // K = H (qkv, gate_up, lm_head), K = heads x head_dim (o_proj), K = I (down)
+    int rows_live = 0;                   // operand rows that may be non-zero (rows >= the running count are zeroed when it falls)
+    float* wide_ws = nullptr; int* wide_cnt = nullptr;
+    float* workb = nullptr;              // [cap][V] sampler scratch, one row per slot (the rows sample concurrently)
+    int* d_act = nullptr;                // [cap] row -> slot
+    SampleArgs* d_samp = nullptr;        // [cap] per-slot sampler arguments
+    int* d_samp_on = nullptr;            // [cap]
+
+    // a wide decoder of kWideSeqs slots: the kernel's B tile is 64 sequences wide whatever the session width, so the buffers are too
+    void init_wide(TextModel& t) {
+        init(t, kWideSeqs);
+        if (wide) return;
+        Ctx& c = *t.ctx;
+        const TextCfg& cf = t.cfg;
+        auto mk = [&](int K) {
+            WideAct a; a.K = K;
+            a.hi = c.alloc<__half>((size_t)kWideSeqs * K); a.lo = c.alloc<__half>((size_t)kWideSeqs * K);
+            AHA_CUDA_CHECK(cudaMemset(a.hi, 0, (size_t)kWideSeqs * K * sizeof(__half)));
+            AHA_CUDA_CHECK(cudaMemset(a.lo, 0, (size_t)kWideSeqs * K * sizeof(__half)));
+            return a;
+        };
+        act_h = mk(cf.H); act_q = mk(t.nh_l * cf.hd); act_i = mk(t.I_l);
+        size_t ws = 0; int tiles = 0;
+        auto need = [&](int N, int K) { ws = std::max(ws, wide_ws_floats(N, K, c.num_sms)); tiles = std::max(tiles, wide_plan(N, K, c.num_sms).tiles); };
+        need(t.qkv_dim, cf.H); need(cf.H, t.nh_l * cf.hd); need(2 * t.I_l, cf.H); need(cf.H, t.I_l); need(cf.V, cf.H);
+        if (ws) wide_ws = c.alloc<float>(ws);
+        wide_cnt = c.alloc<int>(tiles);
+        AHA_CUDA_CHECK(cudaMemset(wide_cnt, 0, (size_t)tiles * sizeof(int)));
+        workb = c.alloc<float>((size_t)cap * cf.V);
+        d_act = c.alloc<int>(cap);
+        d_samp = c.alloc<SampleArgs>(cap);
+        d_samp_on = c.alloc<int>(cap);
+        rows_live = 0;
+        wide = true;
+    }
+    // every projection of the model tiles the wide kernel (N and K multiples of 64)
+    static bool wide_shapes_ok(const TextModel& t) {
+        const TextCfg& cf = t.cfg;
+        return gemv_wide_supported(t.qkv_dim, cf.H) && gemv_wide_supported(cf.H, t.nh_l * cf.hd) && gemv_wide_supported(2 * t.I_l, cf.H) &&
+               gemv_wide_supported(cf.H, t.I_l) && gemv_wide_supported(cf.V, cf.H);
     }
 
     void init(TextModel& t, int n) {
@@ -100,6 +161,7 @@ struct BatchDecoder {
             s.samp.st = d_states + i;
             s.samp.history = d_hist + (size_t)i * T->hist_cap;
             s.samp.token_out = d_tok + i;
+            if (wide) s.samp.work = workb + (size_t)i * T->cfg.V;
         }
     }
 
@@ -126,6 +188,15 @@ struct BatchDecoder {
         }
         Ctx& c = *T->ctx;
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_attn, h.data(), h.size() * sizeof(DecodeAttnArgs), cudaMemcpyHostToDevice, c.stream));
+        std::vector<SampleArgs> samp;
+        std::vector<int> on;
+        if (wide) {   // the rest of the composition the wide step reads from device memory
+            samp.resize((size_t)cap); on.assign((size_t)cap, 0);
+            for (int i = 0; i < cap; ++i) { on[i] = slots[i].samp_active ? 1 : 0; if (on[i]) samp[i] = slots[i].samp; }
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp, samp.data(), samp.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp_on, on.data(), on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        }
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
         table_for = act;
     }
@@ -161,16 +232,18 @@ struct BatchDecoder {
         Ctx& c = *T->ctx;
         AHA_REQUIRE(!act.empty() && (int)act.size() <= cap, "batch step: bad active list");
         if (act != table_for) build_attn_table(act);
-        if (!use_graph) { launches(act, simt); return; }
+        const int nb = (int)act.size();
+        if (wide) zero_rows_from(nb);
+        if (!use_graph) { if (wide) wide_launches(nb); else launches(act, simt); return; }
         StepGraph* g = nullptr;
-        for (auto& e : graphs) if (e.simt == simt && e.act == act) { g = &e; break; }
+        for (auto& e : graphs) if (wide ? e.width == nb : (e.width == 0 && e.simt == simt && e.act == act)) { g = &e; break; }
         if (!g) {
             const uint64_t k0 = c.cnt.kernels;
             cudaGraph_t cg = nullptr;
             AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-            try { launches(act, simt); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
+            try { if (wide) wide_launches(nb); else launches(act, simt); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
             AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &cg));
-            StepGraph e{act, simt, nullptr, c.cnt.kernels - k0};
+            StepGraph e{wide ? std::vector<int>{} : act, simt, nullptr, c.cnt.kernels - k0, wide ? nb : 0};
             c.cnt.kernels = k0;
             const cudaError_t err = cudaGraphInstantiate(&e.exec, cg, 0);
             cudaGraphDestroy(cg);
@@ -213,6 +286,12 @@ struct BatchDecoder {
         cudaStream_t st = c.stream;
         const TextCfg& cf = T->cfg;
         const int nb = (int)act.size(), H = cf.H;
+        if (wide) {   // packed admission's first tokens: the samplers were just bound, so the device copy of the composition is rebuilt
+            build_attn_table(act);
+            zero_rows_from(nb);
+            wide_head(nb, first);
+            return;
+        }
         LinearW head; head.w = T->lm_head; head.b = nullptr; head.N = cf.V; head.K = H;
         proj(PRO_RMSNORM, GEPI_STORE, head, xb, H, T->norm, nullptr, 0, logitsb, cf.V, nb, simt);
         for (int j = 0; j < nb; ++j) {
@@ -231,6 +310,83 @@ struct BatchDecoder {
                 c.cnt.kernels++;
             }
         }
+        AHA_CUDA_CHECK(cudaGetLastError());
+    }
+
+    // ---- the wide step (nb rows; row j is slot d_act[j])
+    // operand rows nb..63 left by a wider step are zeroed: their columns are never stored, but a zero B column keeps the stated invariant
+    void zero_rows_from(int nb) {
+        if (nb < rows_live) {
+            cudaStream_t st = T->ctx->stream;
+            for (const WideAct* a : {&act_h, &act_q, &act_i}) {
+                const size_t off = (size_t)nb * a->K, n = (size_t)(rows_live - nb) * a->K * sizeof(__half);
+                AHA_CUDA_CHECK(cudaMemsetAsync(a->hi + off, 0, n, st));
+                AHA_CUDA_CHECK(cudaMemsetAsync(a->lo + off, 0, n, st));
+            }
+        }
+        rows_live = nb;
+    }
+    // prep: rows 0..nb-1 of x (ldx floats apart) -> the hi / lo operand rows of `in`, RMSNorm-ed with norm_w when given
+    void wide_prep(const float* x, int ldx, const float* norm_w, const WideAct& in, int nb) {
+        Ctx& c = *T->ctx;
+        if (norm_w) {
+            AHA_REQUIRE(ldx == in.K, "wide prep: normalised rows must be packed");
+            rmsnorm_split_kernel<<<nb, 256, 0, c.stream>>>(x, norm_w, T->cfg.eps, in.hi, in.lo, in.K);
+        } else {
+            const size_t n4 = (size_t)nb * in.K / 4;
+            split_f32_to_f16x2_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, c.stream>>>(x, ldx, in.hi, in.lo, nb, in.K);
+        }
+        c.cnt.kernels++;
+    }
+    void wide_proj(int epi, const LinearW& W, const WideAct& in, const float* resid, int ldr, float* out, int ldo, int nb) {
+        Ctx& c = *T->ctx;
+        WideArgs a{};
+        a.bias = W.b; a.resid = resid; a.ldr = ldr; a.out = out; a.ldo = ldo; a.N = W.N; a.K = W.K; a.nb = nb;
+        a.ws = wide_ws; a.counters = wide_cnt;
+        AHA_REQUIRE(W.K == in.K, "wide projection: operand width mismatch");
+        const CUtensorMap tm = W.has_tmap ? W.tmap : make_tmap_f16(W.w, (uint64_t)W.N, (uint64_t)W.K);
+        gemv_wide(c.stream, epi, tm, in.hi, in.lo, a, c.num_sms);
+        c.cnt.kernels++;
+    }
+    void wide_launches(int nb) {
+        Ctx& c = *T->ctx;
+        cudaStream_t st = c.stream;
+        const TextCfg& cf = T->cfg;
+        const int H = cf.H;
+        embed_rows_kernel<<<nb, 256, 0, st>>>(d_act, d_states, T->embed, xb, H, cf.V);
+        c.cnt.kernels++;
+        for (int l = 0; l < cf.L; ++l) {
+            TextLayer& Ly = T->layers[l];
+            wide_prep(xb, H, Ly.ln1, act_h, nb);
+            wide_proj(GEPI_STORE, Ly.qkv, act_h, nullptr, 0, qkvb, T->qkv_dim, nb);
+            switch (T->nh_l / T->nkv_l) {
+                case 1: launch_attn<1>(l, nb); break;
+                case 2: launch_attn<2>(l, nb); break;
+                case 4: launch_attn<4>(l, nb); break;
+                default: launch_attn<6>(l, nb); break;
+            }
+            c.cnt.kernels++;
+            wide_prep(attnb, T->nh_l * cf.hd, nullptr, act_q, nb);
+            wide_proj(GEPI_RESID, Ly.o, act_q, xb, H, xb, H, nb);
+            wide_prep(xb, H, Ly.ln2, act_h, nb);
+            wide_proj(GEPI_SWIGLU, Ly.gu, act_h, nullptr, 0, hb, T->I_l, nb);
+            wide_prep(hb, T->I_l, nullptr, act_i, nb);
+            wide_proj(GEPI_RESID, Ly.down, act_i, xb, H, xb, H, nb);
+        }
+        wide_head(nb, false);
+    }
+    // final norm + lm_head over rows 0..nb-1 of xb, then per row the two-stage ArgMax and the sampler (head_rows' contract, row-indexed)
+    void wide_head(int nb, bool first) {
+        Ctx& c = *T->ctx;
+        cudaStream_t st = c.stream;
+        const TextCfg& cf = T->cfg;
+        LinearW head; head.w = T->lm_head; head.b = nullptr; head.N = cf.V; head.K = cf.H;
+        wide_prep(xb, cf.H, T->norm, act_h, nb);
+        wide_proj(GEPI_STORE, head, act_h, nullptr, 0, logitsb, cf.V, nb);
+        argmax_partial_rows_kernel<<<dim3(n_pcand, nb), 256, 0, st>>>(logitsb, cf.V, cf.V, pmaxb, pidxb);
+        argmax_final_rows_kernel<<<nb, 32, 0, st>>>(pmaxb, pidxb, n_pcand, d_act, d_tok, d_states, d_hist, T->hist_cap, first ? 0 : 1);
+        sample_rows_kernel<<<nb, kSampleThreads, 0, st>>>(d_samp, d_samp_on, d_act, logitsb, cf.V, first ? 0 : 1);
+        c.cnt.kernels += 3;
         AHA_CUDA_CHECK(cudaGetLastError());
     }
 };

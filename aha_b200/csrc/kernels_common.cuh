@@ -7,16 +7,18 @@
 namespace aha {
 
 // Embedding::forward (row gather), fp16 table -> fp32 rows.  src/models/qwen3/model.rs:191-193
-__global__ void embed_gather_kernel(const uint32_t* __restrict__ ids, const __half* __restrict__ table,
-                                    float* __restrict__ out, int S, int H, int V) {
-    const int s = blockIdx.x;
-    uint32_t id = ids[s];
+__device__ __forceinline__ void embed_row_dev(uint32_t id, const __half* __restrict__ table, float* __restrict__ out, int H, int V) {
     if (id >= (uint32_t)V) id = V - 1;  // host validates; keep the kernel memory-safe regardless
     const __half* row = table + (size_t)id * H;
     for (int i = threadIdx.x * 2; i < H; i += blockDim.x * 2) {
         float2 v = __half22float2(*reinterpret_cast<const __half2*>(row + i));
-        *reinterpret_cast<float2*>(out + (size_t)s * H + i) = v;
+        *reinterpret_cast<float2*>(out + i) = v;
     }
+}
+__global__ void embed_gather_kernel(const uint32_t* __restrict__ ids, const __half* __restrict__ table,
+                                    float* __restrict__ out, int S, int H, int V) {
+    const int s = blockIdx.x;
+    embed_row_dev(ids[s], table, out + (size_t)s * H, H, V);
 }
 
 // candle_nn RmsNorm over the last dim: x / sqrt(mean(x^2) + eps) * w.  One block per row.
@@ -123,10 +125,8 @@ __global__ void add_inplace_kernel(float* __restrict__ x, const float* __restric
 
 // Two-stage argmax, "first maximal index" like candle's Sampling::ArgMax.
 // Stage 1 is fused into the lm_head GEMV epilogue where possible; this standalone version covers logits[V].
-__global__ void argmax_partial_kernel(const float* __restrict__ logits, int V, float* __restrict__ pmax,
-                                      int* __restrict__ pidx) {
-    __shared__ float smax[32];
-    __shared__ int sidx[32];
+__device__ __forceinline__ void argmax_partial_dev(const float* __restrict__ logits, int V, float* __restrict__ pmax, int* __restrict__ pidx,
+                                                   float* smax, int* sidx) {
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < V; i += gridDim.x * blockDim.x) {
@@ -153,6 +153,19 @@ __global__ void argmax_partial_kernel(const float* __restrict__ logits, int V, f
         if (lane == 0) { pmax[blockIdx.x] = best; pidx[blockIdx.x] = bi; }
     }
 }
+__global__ void argmax_partial_kernel(const float* __restrict__ logits, int V, float* __restrict__ pmax,
+                                      int* __restrict__ pidx) {
+    __shared__ float smax[32];
+    __shared__ int sidx[32];
+    argmax_partial_dev(logits, V, pmax, pidx, smax, sidx);
+}
+// the same over nb logits rows (ld floats apart): blockIdx.y = row, gridDim.x candidates per row (pmax / pidx [nb][gridDim.x])
+__global__ void argmax_partial_rows_kernel(const float* __restrict__ logits, int ld, int V, float* __restrict__ pmax, int* __restrict__ pidx) {
+    __shared__ float smax[32];
+    __shared__ int sidx[32];
+    const size_t r = blockIdx.y;
+    argmax_partial_dev(logits + r * ld, V, pmax + r * gridDim.x, pidx + r * gridDim.x, smax, sidx);
+}
 
 // Stage 2: reduce the per-block candidates, publish the token, and advance the device-side decode state:
 // state[0] = next token, state[1] = position of the next token (ctx so far), history[state[2]++] = token.
@@ -164,9 +177,9 @@ struct DecodeState {
     uint32_t n_draws;    // random draws the request's sampler has consumed (index into its ChaCha12 stream)
     uint32_t pad_[3];
 };
-__global__ void argmax_final_kernel(const float* __restrict__ pmax, const int* __restrict__ pidx, int n,
-                                    uint32_t* __restrict__ argmax_out, DecodeState* __restrict__ st,
-                                    uint32_t* __restrict__ history, int hist_cap, int advance) {
+__device__ __forceinline__ void argmax_final_dev(const float* __restrict__ pmax, const int* __restrict__ pidx, int n,
+                                                 uint32_t* __restrict__ argmax_out, DecodeState* __restrict__ st,
+                                                 uint32_t* __restrict__ history, int hist_cap, int advance) {
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = threadIdx.x; i < n; i += 32) {
@@ -189,6 +202,25 @@ __global__ void argmax_final_kernel(const float* __restrict__ pmax, const int* _
             st->n_hist += 1;
         }
     }
+}
+__global__ void argmax_final_kernel(const float* __restrict__ pmax, const int* __restrict__ pidx, int n,
+                                    uint32_t* __restrict__ argmax_out, DecodeState* __restrict__ st,
+                                    uint32_t* __restrict__ history, int hist_cap, int advance) {
+    argmax_final_dev(pmax, pidx, n, argmax_out, st, history, hist_cap, advance);
+}
+
+// Row-indexed kernels of a wide batch step (batch_decode.cuh): row j belongs to slot act[j], read from device memory so that one launch
+// (and one captured graph) serves every composition of the same width.
+__global__ void embed_rows_kernel(const int* __restrict__ act, const DecodeState* __restrict__ st, const __half* __restrict__ table,
+                                  float* __restrict__ out, int H, int V) {
+    embed_row_dev(st[act[blockIdx.x]].token, table, out + (size_t)blockIdx.x * H, H, V);
+}
+// stage 2 of row j (one warp per row): the slot's token, decode state and history
+__global__ void argmax_final_rows_kernel(const float* __restrict__ pmax, const int* __restrict__ pidx, int n, const int* __restrict__ act,
+                                         uint32_t* __restrict__ tok, DecodeState* __restrict__ st, uint32_t* __restrict__ hist, int hist_cap,
+                                         int advance) {
+    const int j = blockIdx.x, slot = act[j];
+    argmax_final_dev(pmax + (size_t)j * n, pidx + (size_t)j * n, n, tok + slot, st + slot, hist + (size_t)slot * hist_cap, hist_cap, advance);
 }
 
 }  // namespace aha

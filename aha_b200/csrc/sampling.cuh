@@ -139,8 +139,9 @@ __device__ int blocked_pick_dev(SampleSmem& s, int V, F w, float draw01, int* er
     return r;
 }
 
-__global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
-    __shared__ SampleSmem s;
+// The sampler of one token, run by a CTA of kSampleThreads threads: sample_kernel (one request) and sample_rows_kernel (a wide batch step)
+// share it, so a request draws the same token whichever of the two runs it.
+__device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
     const int tid = threadIdx.x, V = a.V;
     float* p = a.work;
     const int n_hist = a.st->n_hist;
@@ -328,6 +329,25 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
             if (n_hist >= 1 && n_hist - 1 < a.hist_cap) a.history[n_hist - 1] = (uint32_t)token;
         }
     }
+}
+
+__global__ void __launch_bounds__(kSampleThreads) sample_kernel(SampleArgs a) {
+    __shared__ SampleSmem s;
+    sample_dev(a, s);
+}
+
+// Row-indexed sampler of a wide batch step: CTA j samples logits row j for the slot act[j] with that slot's SampleArgs (args[slot]); a
+// row whose request does not sample (on[slot] == 0) returns at once.  Which slots run is read from device memory, so one launch serves
+// every composition of the same width.
+__global__ void __launch_bounds__(kSampleThreads) sample_rows_kernel(const SampleArgs* __restrict__ args, const int* __restrict__ on,
+                                                                     const int* __restrict__ act, const float* logits, int ld, int overwrite) {
+    __shared__ SampleSmem s;
+    const int slot = act[blockIdx.x];
+    if (!on[slot]) return;
+    SampleArgs a = args[slot];
+    a.logits = logits + (size_t)blockIdx.x * ld;
+    a.overwrite = overwrite;
+    sample_dev(a, s);
 }
 
 }  // namespace aha

@@ -240,6 +240,12 @@ class B200Model:
     # ---- continuous batching: requests join / leave a running batch between steps (aha_b200_batch_open / _add / _step / _close)
     def batch_open(self):
         self._check(self._lib.aha_b200_batch_open(self._h))
+        self._batch_width = 8
+
+    def batch_open_wide(self, max_seqs):
+        """A session of max_seqs (1..64) slots stepped on the tensor cores; admission, stepping and closing as for batch_open."""
+        self._check(self._lib.aha_b200_batch_open_wide(self._h, int(max_seqs)))
+        self._batch_width = int(max_seqs)
 
     def batch_add(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64,
                   seed=299792458, flags=0):
@@ -269,6 +275,11 @@ class B200Model:
 
     def batch_step(self):
         """One decode step of every running request -> {slot: (token, finished)} (empty when nothing is running)."""
+        w = getattr(self, "_batch_width", 8)
+        if w > 8:
+            toks, status, n = (C.c_uint32 * w)(), (C.c_int32 * w)(), C.c_size_t(0)
+            self._check(self._lib.aha_b200_batch_step_n(self._h, toks, status, w, C.byref(n)))
+            return {i: (int(toks[i]), status[i] == 2) for i in range(w) if status[i] != 0}
         toks = (C.c_uint32 * 8)()
         status = (C.c_int32 * 8)()
         n = C.c_size_t(0)

@@ -208,6 +208,20 @@ int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t 
                             uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage);
 int aha_b200_batch_step(aha_model* m, uint32_t* tokens_out /* [8] */, int32_t* status_out /* [8] */, size_t* n_stepped_out /* may be NULL */);
 int aha_b200_batch_close(aha_model* m);
+/* Wide continuous batching: a session of max_seqs (1..64) slots whose decode step runs every projection and the lm_head on the tensor
+ * cores (wgmma, each weight streamed once per step for all running requests).  Requires no open session, a single GPU, and a model whose
+ * projections all have row and column counts that are multiples of 64 (every Qwen3 / Qwen3-VL / Qwen3-ASR text stack); anything else is
+ * refused with a message.  Requests are admitted with batch_add / batch_add_many (packing included) and the session ends with
+ * batch_close or clear_cache, as for batch_open.  aha_options.gemm_impl still selects the admission prefill's GEMM; AHA_BATCH_GEMV does not
+ * apply.  Buffers for 64 sequences are allocated on the first wide session of a handle and kept.
+ * Results: every request yields the ids of its own generate_generic run.  They are bit-identical whichever slot it holds, whatever runs
+ * beside it and at whatever step it joins, given the same admission entry (batch_add and batch_add_many differ below 32 prompt tokens).
+ * They need NOT equal aha_b200_generate's ids or a narrow session's in the last bits: the tensor-core sums run in another order than the
+ * CUDA-core GEMV's.  The narrow session (batch_open) keeps its own kernels and its bit-equality with single-request runs. */
+int aha_b200_batch_open_wide(aha_model* m, size_t max_seqs);
+/* batch_step over cap entries (cap >= the session width; works on narrow sessions too).  batch_step refuses a session wider than 8. */
+int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out /* [cap] */, int32_t* status_out /* [cap] */, size_t cap,
+                          size_t* n_stepped_out /* may be NULL */);
 
 /* WhisperFeatureExtractor::call (src/models/feature_extractor/
  * feature_extraction_whisper.rs:65-115): wave (n) f32 host -> log-mel (n_mels, n_frames) f32 host.
@@ -336,7 +350,8 @@ int aha_b200_get_stats(aha_model* m, aha_stats* out);
 int aha_b200_reset_stats(aha_model* m);
 /* Copy an internal activation to the host: what = "hidden" (text hidden states after layer `index`
  * of the last forward_initial, S*H floats; requires aha_b200_set_trace(m,1)), "vit" (ViT hidden after
- * block `index`), "image_embeds", "audio_embeds", "rope_delta" (1 float). */
+ * block `index`), "image_embeds", "audio_embeds", "rope_delta" (1 float), "batch_graphs" (1 float: step graphs
+ * captured in the open batch session; a wide session keeps at most one per running count). */
 int aha_b200_set_trace(aha_model* m, int on);
 int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, size_t cap, size_t* n);
 /* Run n decode steps back to back on the device (graph replays, token feedback on device) without any
@@ -353,7 +368,8 @@ int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_param
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);
 /* Run ONE Linear layer y = epilogue(x W^T + b) through the library's GEMM dispatch on host data (unit tests of the
  * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 5 = the batched decode GEMV (M <= 8; its SwiGLU
- * instantiation runs with a unit-gain RMSNorm prologue); epi 0 = store, 1 = residual
+ * instantiation runs with a unit-gain RMSNorm prologue), 6 = the same with the cp.async weight ring, 7 = the wide batched decode GEMV
+ * (wgmma, M <= 64, N and K multiples of 64; epilogues and SwiGLU prologue as impl 5); epi 0 = store, 1 = residual
  * add (resid [M,N]), 2 = activation (act: 1 silu, 2 gelu-erf, 3 gelu-tanh), 3 = SwiGLU on interleaved columns
  * (out [M,N/2]).  x [M,K] f32, w [N,K] f16 bits, bias [N] f32 or NULL.  device_ms: CUDA-event time of `iters` runs. */
 int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, int K, const float* x, const uint16_t* w,
