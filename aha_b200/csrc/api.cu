@@ -290,9 +290,10 @@ void require_no_session(aha_model* m) {
 }
 bool env_flag(const char* name, bool dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) != 0 : dflt; }
 int env_int(const char* name, int dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) : dflt; }
-// projections of the batched step: 0 = batched GEMV with the weights in registers, 1 = exact SIMT GEMM (validation twin), 2 = batched GEMV with the
-// cp.async weight ring
-constexpr int kBatchGemvDefault = 2;   // call 25: bit-identical to 0 on every tested shape and faster at every batch size (1.89 vs 2.19 ms per step at 1 request, 4.21 vs 4.31 at 8)
+// AHA_BATCH_GEMV's default (BatchDecoder::gemv).  The two batched GEMVs are bit-identical on every tested shape and neither wins everywhere: on
+// one H100 80GB HBM3 at 400 W (profiles/run_batch.py, ms per step at 1 / 8 requests) v2 takes 2.25 / 4.68-4.76 against v1's 2.22 / 4.17 on the
+// VL2 text stack, and 1.30 / 2.71 against 1.33 / 2.63-2.64 on the Qwen3-0.6B shape.
+constexpr int kBatchGemvDefault = 2;
 
 // model.clear_cache(): pages, rope_deltas, and what the prefix cache remembered
 void drop_cache(aha_model* m) {
@@ -301,6 +302,13 @@ void drop_cache(aha_model* m) {
     m->rope_delta = 0;
     m->cached_ids.clear();
     m->cached_mm_fp = 0;
+}
+// ends the batch session, if one is open, and leaves the handle as clear_cache() does
+void session_close(aha_model* m) {
+    for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->reset();
+    m->session = aha_model::BatchSession{};
+    drop_cache(m);
+    m->text.clear_sampler();
 }
 
 void alloc_pack_buffers(aha_model* m) {
@@ -589,14 +597,8 @@ uint64_t aha_b200_mm_fingerprint(const aha_mm* mm) { return mm_fingerprint(mm); 
 int aha_b200_clear_cache(aha_model* m) {
     return guarded(m, [&] {
         AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        if (m->session.open) {   // clear_cache ends a batch session too: every sequence's K/V is gone
-            for (auto& sl : m->sess().slots) sl.mapped = 0;
-            m->sess().table_for.clear();
-            m->sess().clear_graphs();
-            m->session = aha_model::BatchSession{};
-            m->text.clear_sampler();
-        }
-        drop_cache(m);
+        if (m->session.open) session_close(m);   // clear_cache ends a batch session too: every sequence's K/V is gone
+        else drop_cache(m);
     });
 }
 
@@ -757,14 +759,7 @@ void session_release(aha_model* m, int slot) {
     sl.mapped = 0;
     sl.samp_active = false;
     m->session.used[slot] = false;
-    m->sess().composition_changed();   // (narrow: the graphs of compositions holding this slot carry its sampler arguments by value)
-}
-void session_close(aha_model* m) {
-    for (BatchDecoder* B : {&m->batch, &m->wide_batch})
-        if (B->cap) { for (auto& sl : B->slots) sl.mapped = 0; B->table_for.clear(); B->clear_graphs(); }
-    m->session = aha_model::BatchSession{};
-    drop_cache(m);
-    m->text.clear_sampler();
+    m->sess().composition_changed();
 }
 // width 0: the narrow session (8 slots, batched CUDA-core GEMV); 1..64: a wide session (gemv_wide.cuh)
 void session_open(aha_model* m, int width) {
@@ -782,62 +777,19 @@ void session_open(aha_model* m, int width) {
     BatchDecoder& B = width == 0 ? m->batch : m->wide_batch;
     if (width == 0) B.init(T, kGemvBatchMax);
     else B.init_wide(T);
-    for (auto& sl : B.slots) sl.mapped = 0;
-    B.table_for.clear();
-    B.clear_graphs();
+    B.reset();
+    B.gemv = env_int("AHA_BATCH_GEMV", kBatchGemvDefault);   // (the wide step always runs gemv_wide)
+    B.use_graph = env_flag("AHA_BATCH_GRAPH", true);
     m->session = aha_model::BatchSession{};
     m->session.open = true;
     m->session.wide = width != 0;
     m->session.width = width == 0 ? kGemvBatchMax : width;
 }
-void session_add(aha_model* m, const aha_batch_request& r, int* slot_out, uint32_t* first_token, int* finished, aha_usage* usage) {
-    TextModel& T = m->text;
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
-    AHA_REQUIRE(r.ids && r.seq_len >= 1, "batch_add: the request needs input_ids");
-    AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "batch_add: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-    int slot = -1;
-    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) { slot = i; break; }
-    AHA_REQUIRE(slot >= 0, "batch_add: all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
-    const size_t sample_len = std::max<size_t>(r.params.max_tokens, 1);
-    const size_t need = (r.seq_len + sample_len + kPage - 1) / kPage;
-    AHA_REQUIRE(need <= T.free_pages.size(), "batch_add: the request needs " + std::to_string(need * kPage) + " tokens of KV capacity, " +
-                                                  std::to_string(T.free_pages.size() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
-    using clk = std::chrono::steady_clock;
-    const auto t0 = clk::now();
-    int swapped = -1;
-    struct Guard {   // a failed prefill leaves the session as it was: own table back in place, the slot's pages back in the pool
-        aha_model* m; int slot; int* swapped; bool ok = false;
-        ~Guard() { if (ok) return; if (*swapped >= 0) m->sess().swap_table(*swapped); session_release(m, slot); m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler(); }
-    } guard{m, slot, &swapped};
-    m->session.used[slot] = true;
-    const uint32_t tok = batch_prefill_slot(m, slot, r, sample_len, &swapped);
-    guard.ok = true;
-    m->text.clear_sampler();
-    m->sess().composition_changed();
-    m->session.budget[slot] = sample_len;
-    m->session.produced[slot] = 1;
-    bool stop = sample_len == 1;
-    if ((r.params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok) stop = true;
-    if (usage) {
-        *usage = aha_usage{};
-        usage->prompt_tokens = (uint32_t)r.seq_len; usage->completion_tokens = 1;
-        usage->prompt_secs = std::chrono::duration<double>(clk::now() - t0).count();
-        usage->vision_secs = m->last_vision_secs;
-    }
-    if (stop) session_release(m, slot);
-    *slot_out = slot; *first_token = tok; *finished = stop ? 1 : 0;
-}
-// a request whose sampler failed (all-zero weights) raises the shared error flag
-void throw_on_sample_error(TextModel& T) {
-    if (!T.d_sample_err) return;
-    int e = 0;
-    AHA_CUDA_CHECK(cudaMemcpy(&e, T.d_sample_err, sizeof(int), cudaMemcpyDeviceToHost));
-    if (e) { cudaMemset(T.d_sample_err, 0, sizeof(int)); throw std::runtime_error("sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)"); }
-}
 // n requests admitted in one call (aha_b200_batch_add_many).  Text-only requests that fit max_prefill are cut, in input order, into packed
 // prefills (TextModel::prefill with PrefillSegments: each request attends only to itself and its positions restart at 0), so one pass over the
 // weights serves them all; their last rows then go through the step's batched lm_head and each request's own ArgMax / sampler.  A request
-// with multimodal tensors, or one longer than max_prefill, is prefilled alone by batch_prefill_slot, exactly as batch_add does it.
+// with multimodal tensors, or one longer than max_prefill, is prefilled alone by batch_prefill_slot.  pack = false prefills every request
+// alone (aha_b200_batch_add, generate_batch).
 //
 // Every request of a pack starts on a multiple of kPage tokens, so the pack's page table is the slots' own page lists laid end to end: pack
 // position p of the request starting at s0 is its page (p - s0) / kPage at the same offset, and the prefill writes every request's K/V straight
@@ -845,35 +797,38 @@ void throw_on_sample_error(TextModel& T) {
 // page at positions >= seq_len, which its decode steps overwrite before any step reads them.  A 32-token round-up never reaches a 64-token KV
 // tile or a 128-token query tile that the request's own rows do not already touch, so each request runs the attention tiles it runs alone.
 void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out, uint32_t* first_tokens, int32_t* finished,
-                      aha_usage* usage) {
+                      aha_usage* usage, bool pack) {
     TextModel& T = m->text;
     BatchDecoder& B = m->sess();
     Ctx& c = m->ctx;
+    const std::string who = pack ? "batch_add_many: " : "batch_add: ";
     // ---- every check before any device work: a refused call leaves the session untouched
     AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
-    AHA_REQUIRE(n >= 1, "batch_add_many: no requests");
+    AHA_REQUIRE(n >= 1, who + "no requests");
     std::vector<int> slot;   // request i takes the i-th lowest free slot
     for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) slot.push_back(i);
-    AHA_REQUIRE(n <= slot.size(), "batch_add_many: " + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) +
-                                      " of the " + std::to_string(m->session.width) + " slots are free (step until requests finish)");
+    const std::string width = std::to_string(m->session.width);
+    AHA_REQUIRE(!slot.empty(), who + "all " + width + " slots are decoding (step until one finishes)");
+    AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) + " of the " + width +
+                                      " slots are free (step until requests finish)");
     slot.resize(n);
     std::vector<size_t> sample_len(n);
     std::vector<bool> packed(n);
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
         const aha_batch_request& r = reqs[i];
-        AHA_REQUIRE(r.ids && r.seq_len >= 1, "batch_add_many: request " + std::to_string(i) + " needs input_ids");
+        AHA_REQUIRE(r.ids && r.seq_len >= 1, who + "request " + std::to_string(i) + " needs input_ids");
         for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
-        AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "batch_add_many: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+        AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
         if (m->kind == aha_model::QWEN3VL) AHA_REQUIRE(r.mm && r.mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
         if (m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(r.mm && r.mm->n == 1, "Qwen3 asr process data error, must have input_features");
         sample_len[i] = std::max<size_t>(r.params.max_tokens, 1);
         pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
         bool has_mm = false;   // (a qwen3 handle ignores the tensors)
         for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
-        packed[i] = !has_mm && r.seq_len <= (size_t)T.max_prefill;
+        packed[i] = pack && !has_mm && r.seq_len <= (size_t)T.max_prefill;
     }
-    AHA_REQUIRE(pages <= T.free_pages.size(), "batch_add_many: the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
+    AHA_REQUIRE(pages <= T.free_pages.size(), who + "the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
                                                   std::to_string(T.free_pages.size() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
     for (size_t i = 0; i < n; ++i) {   // (only reachable when max_ctx is not a multiple of the page)
         const size_t ctx = reqs[i].seq_len + sample_len[i];
@@ -965,13 +920,13 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         }
         const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};
         for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
-        B.head_rows(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), true);
+        B.head_rows(act, true);
         std::vector<uint32_t> h_tok((size_t)B.cap);
         std::vector<DecodeState> h_st((size_t)B.cap);
         AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-        throw_on_sample_error(T);
+        T.check_sample_error();
         const double t_first = std::chrono::duration<double>(clk::now() - t0).count();
         for (size_t i : pk) {
             const aha_gen_params& p = reqs[i].params;
@@ -1019,8 +974,7 @@ size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, siz
     for (int i = 0; i < width; ++i) if (m->session.used[i]) act.push_back(i);
     if (act.empty()) return 0;
     BatchDecoder& B = m->sess();
-    // (AHA_BATCH_GEMV picks the narrow step's projections; the wide step always runs gemv_wide)
-    B.step(act, env_int("AHA_BATCH_GEMV", kBatchGemvDefault), env_flag("AHA_BATCH_GRAPH", true));
+    B.step(act);
     std::vector<uint32_t> h_tok((size_t)B.cap);
     AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
     AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
@@ -1035,81 +989,50 @@ size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, siz
     }
     for (int slot : act) if (status_out[slot] == 2) session_release(m, slot);
     // sampler errors surface after the bookkeeping so that the slots stay consistent
-    throw_on_sample_error(m->text);
+    m->text.check_sample_error();
     return act.size();
 }
 
-// Static batching: n independent requests, each prefilled on its own page table, then decoded in lockstep (batch_decode.cuh).  Every
-// request follows generate_generic's rules on its own (first token never EOS-checked, an EOS token is pushed and ends THAT request, its
-// own sampler / seed / repeat-penalty history) and so yields exactly the tokens aha_b200_generate would yield for it alone.
+// Static batching: a narrow session that admits the n requests one by one (each prefilled alone on its own page table) and steps until all
+// have finished.  Every request follows generate_generic's rules on its own (first token never EOS-checked, an EOS token is pushed and ends
+// THAT request, its own sampler / seed / repeat-penalty history) and so yields exactly the tokens aha_b200_generate would yield for it alone.
 void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, uint32_t* out_tokens, size_t cap, size_t* n_out, aha_usage* usage) {
     TextModel& T = m->text;
     require_no_session(m);
     AHA_REQUIRE(n >= 1 && n <= (size_t)kGemvBatchMax, "generate_batch: 1 to 8 requests");
-    AHA_REQUIRE(T.tp_world == 1, "generate_batch is single-GPU (run one batch per tensor-parallel group member instead)");
-    AHA_REQUIRE(T.max_prefill >= kGemvBatchMax, "generate_batch needs max_prefill >= 8");
-    using clk = std::chrono::steady_clock;
-    std::vector<size_t> sample_len(n);
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
         AHA_REQUIRE(reqs[i].ids && reqs[i].seq_len >= 1, "generate_batch: every request needs input_ids");
-        sample_len[i] = std::max<size_t>(reqs[i].params.max_tokens, 1);
-        AHA_REQUIRE(cap >= sample_len[i], "out_tokens capacity (per request) is smaller than max_tokens");
+        const size_t sample_len = std::max<size_t>(reqs[i].params.max_tokens, 1);
+        AHA_REQUIRE(cap >= sample_len, "out_tokens capacity (per request) is smaller than max_tokens");
         AHA_REQUIRE((reqs[i].params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "generate_batch: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-        pages += (reqs[i].seq_len + sample_len[i] + kPage - 1) / kPage;
+        pages += (reqs[i].seq_len + sample_len + kPage - 1) / kPage;
         n_out[i] = 0;
-        if (usage) usage[i] = aha_usage{};
     }
     AHA_REQUIRE(pages <= (size_t)T.num_pages, "the requests of the batch need " + std::to_string(pages * kPage) + " tokens of KV capacity, max_ctx is " + std::to_string(T.max_ctx));
-    const int simt = env_int("AHA_BATCH_GEMV", kBatchGemvDefault);
-    const bool use_graph = env_flag("AHA_BATCH_GRAPH", true);   // 0 = eager launches (A/B twin of the per-composition graphs)
-    BatchDecoder& B = m->batch;
-    drop_cache(m);
-    B.init(T, kGemvBatchMax);
-    for (auto& sl : B.slots) sl.mapped = 0;
-    B.table_for.clear();
-    B.clear_graphs();
-    int swapped = -1;
-    struct Reset {   // whatever happens, the handle is left as after clear_cache(), with its own page table in place
-        aha_model* m; BatchDecoder* B; int* swapped;
-        ~Reset() { if (*swapped >= 0) B->swap_table(*swapped); drop_cache(m); m->text.clear_sampler(); for (auto& sl : B->slots) sl.mapped = 0; B->clear_graphs(); }
-    } reset{m, &B, &swapped};
-    auto is_eos = [&](uint32_t t) { for (uint32_t e : m->stop_ids) if (e == t) return true; return false; };
-
-    // ---- prefill, one request after the other (each is the reference's forward_initial + sample_and_push)
-    std::vector<int> act;
-    std::vector<clk::time_point> t_first(n);
+    session_open(m, 0);
+    struct Close {   // whatever happens, the handle is left as after clear_cache()
+        aha_model* m;
+        ~Close() { session_close(m); }
+    } close{m};
+    std::vector<int> req_of(kGemvBatchMax, -1);   // slot -> request
     for (size_t i = 0; i < n; ++i) {
-        const aha_batch_request& r = reqs[i];
-        const auto t0 = clk::now();
-        const uint32_t tok = batch_prefill_slot(m, (int)i, r, sample_len[i], &swapped);
-        t_first[i] = clk::now();
-        out_tokens[i * cap] = tok; n_out[i] = 1;
-        if (usage) {
-            usage[i].prompt_tokens = (uint32_t)r.seq_len;
-            usage[i].prompt_secs = std::chrono::duration<double>(t_first[i] - t0).count();
-            usage[i].vision_secs = m->last_vision_secs;
-        }
-        const bool stop = (r.params.flags & AHA_GEN_EOS_ON_FIRST) != 0 && is_eos(tok);
-        if (sample_len[i] > 1 && !stop) act.push_back((int)i);
+        int32_t slot = 0, fin = 0;
+        session_add_many(m, reqs + i, 1, &slot, out_tokens + i * cap, &fin, usage ? usage + i : nullptr, false);
+        n_out[i] = 1;
+        if (!fin) req_of[slot] = (int)i;
     }
-    // ---- decode in lockstep; a request leaves the batch at its EOS token or at max_tokens
+    using clk = std::chrono::steady_clock;
     const auto t_dec = clk::now();
-    std::vector<uint32_t> h_tok(kGemvBatchMax);
-    while (!act.empty()) {
-        B.step(act, simt, use_graph);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, kGemvBatchMax * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        T.check_sample_error();
-        std::vector<int> next;
-        for (int slot : act) {
-            const uint32_t t = h_tok[slot];
-            out_tokens[(size_t)slot * cap + n_out[slot]] = t;
-            n_out[slot] += 1;
-            if (!(is_eos(t) || n_out[slot] >= sample_len[slot])) next.push_back(slot);
-            else if (usage) usage[slot].completion_secs = std::chrono::duration<double>(clk::now() - t_dec).count();
+    uint32_t tok[kGemvBatchMax];
+    int32_t status[kGemvBatchMax];
+    while (session_step(m, tok, status, kGemvBatchMax, true) > 0) {
+        for (int slot = 0; slot < kGemvBatchMax; ++slot) {
+            if (!status[slot]) continue;
+            const int i = req_of[slot];
+            out_tokens[(size_t)i * cap + n_out[i]++] = tok[slot];
+            if (status[slot] == 2 && usage) usage[i].completion_secs = std::chrono::duration<double>(clk::now() - t_dec).count();
         }
-        act.swap(next);
     }
     if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
 }
@@ -1127,9 +1050,7 @@ int aha_b200_batch_open_wide(aha_model* m, size_t max_seqs) {
 int aha_b200_batch_add(aha_model* m, const aha_batch_request* req, int32_t* slot_out, uint32_t* first_token_out, int32_t* finished_out, aha_usage* usage) {
     return guarded(m, [&] {
         AHA_REQUIRE(req && slot_out && first_token_out && finished_out, "req, slot_out, first_token_out and finished_out are required");
-        int slot = -1, fin = 0;
-        session_add(m, *req, &slot, first_token_out, &fin, usage);
-        *slot_out = slot; *finished_out = fin;
+        session_add_many(m, req, 1, slot_out, first_token_out, finished_out, usage, false);
     });
 }
 
@@ -1137,7 +1058,7 @@ int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t 
                             int32_t* finished_out, aha_usage* usage) {
     return guarded(m, [&] {
         AHA_REQUIRE(reqs && slots_out && first_tokens_out && finished_out, "reqs, slots_out, first_tokens_out and finished_out are required");
-        session_add_many(m, reqs, n, slots_out, first_tokens_out, finished_out, usage);
+        session_add_many(m, reqs, n, slots_out, first_tokens_out, finished_out, usage, true);
     });
 }
 

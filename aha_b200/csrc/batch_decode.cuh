@@ -1,27 +1,28 @@
 // batch_decode.cuh -- several sequences decoded in lockstep on one handle (SURVEY 8f rank 4, second half).
 //
 // The reference holds one request at a time behind a lock (src/server/api.rs:117) and every decode step
-// streams all weights for ONE token.  Here up to 8 sequences share a step: each has its own page table over the common
-// paged KV pool (text_model.cuh), its own DecodeState (token, position, rope_delta, sampler draw index), history and sampler
-// parameters; a step is per layer
-//     [rmsnorm + qkv]  gemv_batch_kernel        all sequences, every weight row read once
+// streams all weights for ONE token.  Here several sequences share a step: each has its own page table over the common paged KV pool
+// (text_model.cuh), its own DecodeState (token, position, rope_delta, sampler draw index), history and sampler parameters; a step is
+//     [embedding]      embed_rows_kernel        row j <- the last token of slot act[j]
+// then per layer
+//     [rmsnorm + qkv]  projection               all sequences, every weight row read once
 //     [attention]      decode_attn_batch_kernel grid.z = sequence: q/k norm, RoPE, KV append, split-KV attention, merge
-//     [o_proj + res]   gemv_batch_kernel
+//     [o_proj + res]   projection
 //     [rmsnorm + gate/up + SwiGLU], [down + res]
-// then final norm + lm_head for all rows and, per sequence, the two-stage ArgMax that advances its DecodeState plus (when the
-// request samples) sample_kernel on its logits row.  Each sequence therefore produces exactly the tokens it would produce alone:
-// the GEMV accumulates every (row, sequence) in gemv_kernel's order and the attention / sampler kernels are the single-sequence
-// ones (tests/test_batch_gpu.py compares every sequence with its own fresh oracle run).
+// then the head: final norm + lm_head for all rows, the two-stage ArgMax that advances every row's DecodeState, and the sampler of every row
+// whose request samples.  Everything that depends on WHICH slots run is read from device memory -- the active list d_act (row j -> slot), the
+// attention table d_attn, the per-slot sampler arguments d_samp -- so one CUDA graph per running count serves every composition of that count.
 // Finished sequences leave the step (the activation rows are rebuilt from the token embeddings every step, so compaction is free).
 // Packed admission (aha_b200_batch_add_many) borrows xb / logitsb between two steps for the first tokens of several requests at once (head_rows).
 //
-// Wide mode (init_wide, aha_b200_batch_open_wide): up to 64 sequences, every projection and the lm_head on gemv_wide.cuh's tensor-core
-// kernel, each fed by a prep kernel that normalises and / or splits the nb fp32 rows into the fp16 hi / lo rows the kernel's TMA reads.
-// Everything that depends on WHICH slots run is read from device memory -- the active list d_act (row j -> slot), the attention table
-// d_attn, the per-slot sampler arguments d_samp -- and the embedding gather, ArgMax and sampler are row-indexed launches, so one CUDA graph
-// per running count serves every composition of that count.  A sequence's sums do not depend on its row or on the other rows (one MMA
-// width, split-K fixed by the shape), so its ids do not depend on its slot, its neighbours or the step it joined at; they are not those of
-// the single-sequence gemv_kernel, whose sums run in another order.
+// The two widths differ only in how a projection is computed:
+//   * narrow (init, aha_b200_batch_open / generate_batch): up to 8 sequences on gemv_batch.cuh's CUDA-core GEMV.  It accumulates every
+//     (row, sequence) in gemv_kernel's order and the attention / ArgMax / sampler bodies are the single-sequence ones, so each sequence produces
+//     exactly the tokens it would produce alone (tests/test_batch_gpu.py compares every sequence with its own single-request run);
+//   * wide (init_wide, aha_b200_batch_open_wide): up to 64 sequences on gemv_wide.cuh's tensor-core kernel, each fed by a prep kernel that
+//     normalises and / or splits the nb fp32 rows into the fp16 hi / lo rows the kernel's TMA reads.  A sequence's sums do not depend on its
+//     row or on the other rows (one MMA width, split-K fixed by the shape), so its ids do not depend on its slot, its neighbours or the step it
+//     joined at; they are not those of the single-sequence gemv_kernel, whose sums run in another order.
 #pragma once
 #include "gemv_batch.cuh"
 #include "gemv_wide.cuh"
@@ -48,22 +49,30 @@ struct BatchDecoder {
     uint32_t* d_tok = nullptr;           // [cap] token of the last step per slot
     int* d_tables = nullptr;             // [cap][num_pages]
     DecodeAttnArgs* d_attn = nullptr;    // [L][cap] attention arguments of the current active list
+    int* d_act = nullptr;                // [cap] row -> slot
+    SampleArgs* d_samp = nullptr;        // [cap] per-slot sampler arguments
+    int* d_samp_on = nullptr;            // [cap]
+    float* workb = nullptr;              // [cap][V] sampler scratch, one row per slot (the rows sample concurrently)
     std::vector<BatchSlot> slots;
-    std::vector<int> table_for;          // active list the attention table was built for
-    // One CUDA graph per composition of the batch (the active list changes only when a request finishes): ~170 launches per step become one.
-    // The graphs hold the requests' sampler parameters by value, so they live for one generate_batch call.
-    // A wide decoder keys its graphs by the running count alone (width = nb) and keeps them while requests come and go.
-    struct StepGraph { std::vector<int> act; int simt; cudaGraphExec_t exec; uint64_t kernels; int width = 0; };
+    std::vector<int> table_for;          // active list the device copy of the composition was built for
+    // set when a session opens (AHA_BATCH_GEMV, AHA_BATCH_GRAPH): the narrow step's projections -- 0 = batched GEMV with the weights in
+    // registers, 1 = exact SIMT GEMM (validation twin), 2 = batched GEMV with the cp.async weight ring -- and eager launches instead of graphs
+    int gemv = 2;
+    bool use_graph = true;
+    // one CUDA graph per running count (~170 launches per step become one); they outlive composition changes
+    struct StepGraph { int width; cudaGraphExec_t exec; uint64_t kernels; };
     std::vector<StepGraph> graphs;
     void clear_graphs() {
         for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
         graphs.clear();
     }
-    // the set of running requests or a slot's sampler changed: the attention table is rebuilt before the next step; a narrow decoder's
-    // graphs carry the old composition, a wide decoder's read it from device memory and stay
-    void composition_changed() {
+    // the set of running requests or a slot's sampler changed: the device copy of the composition is rebuilt before the next step
+    void composition_changed() { table_for.clear(); }
+    // no sequence holds a slot any more (a session opens or closes)
+    void reset() {
+        for (auto& sl : slots) sl.mapped = 0;
         table_for.clear();
-        if (!wide) clear_graphs();
+        clear_graphs();
     }
 
     // ---- wide mode
@@ -72,10 +81,6 @@ struct BatchDecoder {
     WideAct act_h, act_q, act_i;         // K = H (qkv, gate_up, lm_head), K = heads x head_dim (o_proj), K = I (down)
     int rows_live = 0;                   // operand rows that may be non-zero (rows >= the running count are zeroed when it falls)
     float* wide_ws = nullptr; int* wide_cnt = nullptr;
-    float* workb = nullptr;              // [cap][V] sampler scratch, one row per slot (the rows sample concurrently)
-    int* d_act = nullptr;                // [cap] row -> slot
-    SampleArgs* d_samp = nullptr;        // [cap] per-slot sampler arguments
-    int* d_samp_on = nullptr;            // [cap]
 
     // a wide decoder of kWideSeqs slots: the kernel's B tile is 64 sequences wide whatever the session width, so the buffers are too
     void init_wide(TextModel& t) {
@@ -97,10 +102,6 @@ struct BatchDecoder {
         if (ws) wide_ws = c.alloc<float>(ws);
         wide_cnt = c.alloc<int>(tiles);
         AHA_CUDA_CHECK(cudaMemset(wide_cnt, 0, (size_t)tiles * sizeof(int)));
-        workb = c.alloc<float>((size_t)cap * cf.V);
-        d_act = c.alloc<int>(cap);
-        d_samp = c.alloc<SampleArgs>(cap);
-        d_samp_on = c.alloc<int>(cap);
         rows_live = 0;
         wide = true;
     }
@@ -130,6 +131,10 @@ struct BatchDecoder {
         d_tok = c.alloc<uint32_t>(n);
         d_tables = c.alloc<int>((size_t)n * t.num_pages);
         d_attn = c.alloc<DecodeAttnArgs>((size_t)cf.L * n);
+        d_act = c.alloc<int>(n);
+        d_samp = c.alloc<SampleArgs>(n);
+        d_samp_on = c.alloc<int>(n);
+        workb = c.alloc<float>((size_t)n * cf.V);
         slots.resize(n);
         for (int i = 0; i < n; ++i) { slots[i].h_table.assign(t.num_pages, 0); slots[i].d_table = d_tables + (size_t)i * t.num_pages; }
     }
@@ -151,20 +156,20 @@ struct BatchDecoder {
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
         bind_sampler(i);
     }
-    // the sampler set on the TextModel (set_sampler) becomes slot i's, with the slot's own state, history and token
+    // the sampler set on the TextModel (set_sampler) becomes slot i's, with the slot's own state, history, token and scratch row
     void bind_sampler(int i) {
         BatchSlot& s = slots[i];
         s.samp_active = T->samp_active;
         if (s.samp_active) {
             s.samp = T->samp;
-            s.samp.logits = logitsb;                 // row set per step (the slot's position in the active list)
             s.samp.st = d_states + i;
             s.samp.history = d_hist + (size_t)i * T->hist_cap;
             s.samp.token_out = d_tok + i;
-            if (wide) s.samp.work = workb + (size_t)i * T->cfg.V;
+            s.samp.work = workb + (size_t)i * T->cfg.V;
         }
     }
 
+    // the device copy of the composition `act`: attention table, active list and every slot's sampler arguments
     void build_attn_table(const std::vector<int>& act) {
         const TextCfg& cf = T->cfg;
         const int nb = (int)act.size();
@@ -186,17 +191,14 @@ struct BatchDecoder {
                 h[(size_t)l * cap + j] = d;
             }
         }
+        std::vector<SampleArgs> samp((size_t)cap);
+        std::vector<int> on((size_t)cap, 0);
+        for (int i = 0; i < cap; ++i) { on[i] = slots[i].samp_active ? 1 : 0; if (on[i]) samp[i] = slots[i].samp; }
         Ctx& c = *T->ctx;
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_attn, h.data(), h.size() * sizeof(DecodeAttnArgs), cudaMemcpyHostToDevice, c.stream));
-        std::vector<SampleArgs> samp;
-        std::vector<int> on;
-        if (wide) {   // the rest of the composition the wide step reads from device memory
-            samp.resize((size_t)cap); on.assign((size_t)cap, 0);
-            for (int i = 0; i < cap; ++i) { on[i] = slots[i].samp_active ? 1 : 0; if (on[i]) samp[i] = slots[i].samp; }
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp, samp.data(), samp.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp_on, on.data(), on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-        }
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp, samp.data(), samp.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp_on, on.data(), on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
         table_for = act;
     }
@@ -206,11 +208,18 @@ struct BatchDecoder {
         decode_attn_batch_kernel<128, G><<<dim3(kDecodeSplits, T->nkv_l, nb), 256, 0, T->ctx->stream>>>(d_attn + (size_t)l * cap);
     }
 
-    void proj(int pro, int epi, const LinearW& W, const float* x, int ldx, const float* norm_w, const float* resid, int ldr, float* out, int ldo, int nb, int simt) {   // simt: 0 = batched GEMV (registers), 1 = exact SIMT GEMM twin, 2 = batched GEMV with the cp.async weight ring
+    // rows 0..nb-1: out = epi(W . x), x RMSNorm-ed with norm_w first when given
+    void proj(int epi, const LinearW& W, const float* x, int ldx, const float* norm_w, const float* resid, int ldr, float* out, int ldo, int nb) {
         Ctx& c = *T->ctx;
-        if (simt == 1) {   // validation twin: the exact fp32 SIMT GEMM over the nb rows (normalised beforehand when a prologue is asked for)
+        if (wide) {
+            const WideAct& in = W.K == act_h.K ? act_h : (W.K == act_i.K ? act_i : act_q);   // (any [64][K] operand of the right K will do)
+            wide_prep(x, ldx, norm_w, in, nb);
+            wide_proj(epi, W, in, resid, ldr, out, ldo, nb);
+            return;
+        }
+        if (gemv == 1) {   // validation twin: the exact fp32 SIMT GEMM over the nb rows (normalised beforehand when a prologue is asked for)
             const float* a = x; int lda = ldx;
-            if (pro == PRO_RMSNORM) {
+            if (norm_w) {
                 rmsnorm_kernel<<<nb, 256, 0, c.stream>>>(x, norm_w, T->cfg.eps, T->xn, W.K); c.cnt.kernels++;   // xn: [max_prefill >= 8][H] scratch of the prefill
                 a = T->xn; lda = W.K;
             }
@@ -223,27 +232,27 @@ struct BatchDecoder {
         GemvBatchArgs a{};
         a.W = W.w; a.x = x; a.ldx = ldx; a.norm_w = norm_w; a.eps = T->cfg.eps; a.bias = W.b; a.resid = resid; a.ldr = ldr; a.out = out; a.ldo = ldo;
         a.N = W.N; a.K = W.K; a.nb = nb;
-        gemv_batch(c.stream, pro, epi, a, simt == 2);
+        gemv_batch(c.stream, norm_w ? PRO_RMSNORM : PRO_NONE, epi, a, gemv == 2);
         c.cnt.kernels++;
     }
 
     // one decode step of the sequences in `act` (slot indices, at most cap); leaves every slot's next token in d_tok[slot] and its DecodeState advanced
-    void step(const std::vector<int>& act, int simt, bool use_graph) {
+    void step(const std::vector<int>& act) {
         Ctx& c = *T->ctx;
         AHA_REQUIRE(!act.empty() && (int)act.size() <= cap, "batch step: bad active list");
         if (act != table_for) build_attn_table(act);
         const int nb = (int)act.size();
         if (wide) zero_rows_from(nb);
-        if (!use_graph) { if (wide) wide_launches(nb); else launches(act, simt); return; }
+        if (!use_graph) { launches(nb); return; }
         StepGraph* g = nullptr;
-        for (auto& e : graphs) if (wide ? e.width == nb : (e.width == 0 && e.simt == simt && e.act == act)) { g = &e; break; }
+        for (auto& e : graphs) if (e.width == nb) { g = &e; break; }
         if (!g) {
             const uint64_t k0 = c.cnt.kernels;
             cudaGraph_t cg = nullptr;
             AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-            try { if (wide) wide_launches(nb); else launches(act, simt); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
+            try { launches(nb); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
             AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &cg));
-            StepGraph e{wide ? std::vector<int>{} : act, simt, nullptr, c.cnt.kernels - k0, wide ? nb : 0};
+            StepGraph e{nb, nullptr, c.cnt.kernels - k0};
             c.cnt.kernels = k0;
             const cudaError_t err = cudaGraphInstantiate(&e.exec, cg, 0);
             cudaGraphDestroy(cg);
@@ -255,15 +264,15 @@ struct BatchDecoder {
         c.cnt.graphs++;
         c.cnt.kernels += g->kernels;
     }
-    void launches(const std::vector<int>& act, int simt) {
+    void launches(int nb) {
         Ctx& c = *T->ctx;
-        cudaStream_t st = c.stream;
         const TextCfg& cf = T->cfg;
-        const int nb = (int)act.size(), H = cf.H;
-        for (int j = 0; j < nb; ++j) { embed_gather_kernel<<<1, 256, 0, st>>>(&d_states[act[j]].token, T->embed, xb + (size_t)j * H, 1, H, cf.V); c.cnt.kernels++; }
+        const int H = cf.H;
+        embed_rows_kernel<<<nb, 256, 0, c.stream>>>(d_act, d_states, T->embed, xb, H, cf.V);
+        c.cnt.kernels++;
         for (int l = 0; l < cf.L; ++l) {
             TextLayer& Ly = T->layers[l];
-            proj(PRO_RMSNORM, GEPI_STORE, Ly.qkv, xb, H, Ly.ln1, nullptr, 0, qkvb, T->qkv_dim, nb, simt);
+            proj(GEPI_STORE, Ly.qkv, xb, H, Ly.ln1, nullptr, 0, qkvb, T->qkv_dim, nb);
             switch (T->nh_l / T->nkv_l) {
                 case 1: launch_attn<1>(l, nb); break;
                 case 2: launch_attn<2>(l, nb); break;
@@ -271,49 +280,37 @@ struct BatchDecoder {
                 default: launch_attn<6>(l, nb); break;
             }
             c.cnt.kernels++;
-            proj(PRO_NONE, GEPI_RESID, Ly.o, attnb, T->nh_l * cf.hd, nullptr, xb, H, xb, H, nb, simt);
-            proj(PRO_RMSNORM, GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb, simt);
-            proj(PRO_NONE, GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb, simt);
+            proj(GEPI_RESID, Ly.o, attnb, T->nh_l * cf.hd, nullptr, xb, H, xb, H, nb);
+            proj(GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb);
+            proj(GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb);
         }
-        head_rows(act, simt, false);
+        head(nb, false);
     }
-    // Final norm + lm_head over rows 0 .. nb-1 of xb, then for row j the two-stage ArgMax of slot act[j] and, when its request samples, its
+    // Final norm + lm_head over rows 0 .. nb-1 of xb, then for row j the two-stage ArgMax of slot d_act[j] and, when its request samples, its
     // sampler.  A decode step (first = false) advances the slot's DecodeState and the sampled token replaces the ArgMax one the step pushed
     // (the single-sequence loop does the same).  A request's first token (first = true, packed admission) is drawn the way forward_any draws
     // it: no advance, no overwrite, against the slot's state as the caller set it (empty history, draw index 0); only n_draws moves.
-    void head_rows(const std::vector<int>& act, int simt, bool first) {
+    void head(int nb, bool first) {
         Ctx& c = *T->ctx;
         cudaStream_t st = c.stream;
         const TextCfg& cf = T->cfg;
-        const int nb = (int)act.size(), H = cf.H;
-        if (wide) {   // packed admission's first tokens: the samplers were just bound, so the device copy of the composition is rebuilt
-            build_attn_table(act);
-            zero_rows_from(nb);
-            wide_head(nb, first);
-            return;
-        }
-        LinearW head; head.w = T->lm_head; head.b = nullptr; head.N = cf.V; head.K = H;
-        proj(PRO_RMSNORM, GEPI_STORE, head, xb, H, T->norm, nullptr, 0, logitsb, cf.V, nb, simt);
-        for (int j = 0; j < nb; ++j) {
-            const int slot = act[j];
-            const float* lg = logitsb + (size_t)j * cf.V;
-            argmax_partial_kernel<<<n_pcand, 256, 0, st>>>(lg, cf.V, pmaxb + (size_t)j * n_pcand, pidxb + (size_t)j * n_pcand);
-            argmax_final_kernel<<<1, 32, 0, st>>>(pmaxb + (size_t)j * n_pcand, pidxb + (size_t)j * n_pcand, n_pcand, d_tok + slot, d_states + slot,
-                                                  d_hist + (size_t)slot * T->hist_cap, T->hist_cap, first ? 0 : 1);
-            c.cnt.kernels += 2;
-            BatchSlot& s = slots[slot];
-            if (s.samp_active) {
-                SampleArgs a = s.samp;
-                a.logits = lg;
-                a.overwrite = first ? 0 : 1;
-                sample_kernel<<<1, kSampleThreads, 0, st>>>(a);
-                c.cnt.kernels++;
-            }
-        }
+        LinearW lm; lm.w = T->lm_head; lm.b = nullptr; lm.N = cf.V; lm.K = cf.H;
+        proj(GEPI_STORE, lm, xb, cf.H, T->norm, nullptr, 0, logitsb, cf.V, nb);
+        argmax_partial_rows_kernel<<<dim3(n_pcand, nb), 256, 0, st>>>(logitsb, cf.V, cf.V, pmaxb, pidxb);
+        argmax_final_rows_kernel<<<nb, 32, 0, st>>>(pmaxb, pidxb, n_pcand, d_act, d_tok, d_states, d_hist, T->hist_cap, first ? 0 : 1);
+        sample_rows_kernel<<<nb, kSampleThreads, 0, st>>>(d_samp, d_samp_on, d_act, logitsb, cf.V, first ? 0 : 1);
+        c.cnt.kernels += 3;
         AHA_CUDA_CHECK(cudaGetLastError());
     }
+    // the first tokens of the slots in `act`, whose last prompt rows packed admission gathered into xb and whose samplers were just bound
+    void head_rows(const std::vector<int>& act, bool first) {
+        build_attn_table(act);
+        const int nb = (int)act.size();
+        if (wide) zero_rows_from(nb);
+        head(nb, first);
+    }
 
-    // ---- the wide step (nb rows; row j is slot d_act[j])
+    // ---- the wide projection
     // operand rows nb..63 left by a wider step are zeroed: their columns are never stored, but a zero B column keeps the stated invariant
     void zero_rows_from(int nb) {
         if (nb < rows_live) {
@@ -347,47 +344,6 @@ struct BatchDecoder {
         const CUtensorMap tm = W.has_tmap ? W.tmap : make_tmap_f16(W.w, (uint64_t)W.N, (uint64_t)W.K);
         gemv_wide(c.stream, epi, tm, in.hi, in.lo, a, c.num_sms);
         c.cnt.kernels++;
-    }
-    void wide_launches(int nb) {
-        Ctx& c = *T->ctx;
-        cudaStream_t st = c.stream;
-        const TextCfg& cf = T->cfg;
-        const int H = cf.H;
-        embed_rows_kernel<<<nb, 256, 0, st>>>(d_act, d_states, T->embed, xb, H, cf.V);
-        c.cnt.kernels++;
-        for (int l = 0; l < cf.L; ++l) {
-            TextLayer& Ly = T->layers[l];
-            wide_prep(xb, H, Ly.ln1, act_h, nb);
-            wide_proj(GEPI_STORE, Ly.qkv, act_h, nullptr, 0, qkvb, T->qkv_dim, nb);
-            switch (T->nh_l / T->nkv_l) {
-                case 1: launch_attn<1>(l, nb); break;
-                case 2: launch_attn<2>(l, nb); break;
-                case 4: launch_attn<4>(l, nb); break;
-                default: launch_attn<6>(l, nb); break;
-            }
-            c.cnt.kernels++;
-            wide_prep(attnb, T->nh_l * cf.hd, nullptr, act_q, nb);
-            wide_proj(GEPI_RESID, Ly.o, act_q, xb, H, xb, H, nb);
-            wide_prep(xb, H, Ly.ln2, act_h, nb);
-            wide_proj(GEPI_SWIGLU, Ly.gu, act_h, nullptr, 0, hb, T->I_l, nb);
-            wide_prep(hb, T->I_l, nullptr, act_i, nb);
-            wide_proj(GEPI_RESID, Ly.down, act_i, xb, H, xb, H, nb);
-        }
-        wide_head(nb, false);
-    }
-    // final norm + lm_head over rows 0..nb-1 of xb, then per row the two-stage ArgMax and the sampler (head_rows' contract, row-indexed)
-    void wide_head(int nb, bool first) {
-        Ctx& c = *T->ctx;
-        cudaStream_t st = c.stream;
-        const TextCfg& cf = T->cfg;
-        LinearW head; head.w = T->lm_head; head.b = nullptr; head.N = cf.V; head.K = cf.H;
-        wide_prep(xb, cf.H, T->norm, act_h, nb);
-        wide_proj(GEPI_STORE, head, act_h, nullptr, 0, logitsb, cf.V, nb);
-        argmax_partial_rows_kernel<<<dim3(n_pcand, nb), 256, 0, st>>>(logitsb, cf.V, cf.V, pmaxb, pidxb);
-        argmax_final_rows_kernel<<<nb, 32, 0, st>>>(pmaxb, pidxb, n_pcand, d_act, d_tok, d_states, d_hist, T->hist_cap, first ? 0 : 1);
-        sample_rows_kernel<<<nb, kSampleThreads, 0, st>>>(d_samp, d_samp_on, d_act, logitsb, cf.V, first ? 0 : 1);
-        c.cnt.kernels += 3;
-        AHA_CUDA_CHECK(cudaGetLastError());
     }
 };
 

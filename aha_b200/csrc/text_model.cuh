@@ -950,8 +950,9 @@ struct TextModel {
         AHA_CUDA_CHECK(cudaGetLastError());
         ctx->cnt.kernels++;
     }
+    // raised by any sampler on the handle, including the batch samplers (which run with the model's own sampler cleared)
     void check_sample_error() {
-        if (!d_sample_err || !samp_active) return;
+        if (!d_sample_err) return;
         int e = 0;
         AHA_CUDA_CHECK(cudaMemcpy(&e, d_sample_err, sizeof(int), cudaMemcpyDeviceToHost));
         if (e) {

@@ -233,6 +233,35 @@ def test_continuous_batching_requests_join_and_leave(q3):
     assert toks == s.out["A"]
 
 
+def test_graph_per_running_count(q3):
+    """Many join / leave cycles at three running counts: at most one step graph per count, and every request's ids are those of its own
+    single-request generate."""
+    cfg, w, m, o = q3
+    V = cfg["vocab_size"]
+    m.clear_cache()
+    reqs, counts = {}, set()
+    s = _Session(m)
+    try:
+        k = 0
+        for cycle in range(15):
+            while len(s.running) < (3, 5, 8)[cycle % 3]:
+                kw = dict(max_tokens=2 + k % 5, **(dict(temperature=0.9, top_k=20, seed=k) if k % 3 == 0 else {}))
+                reqs[k] = (_ids(10 + 7 * k % 50, V, 5000 + k), kw)
+                s.add(k, reqs[k][0], **kw)
+                k += 1
+            counts.add(len(s.running))
+            s.step()
+        while s.running:
+            counts.add(len(s.running))
+            s.step()
+        graphs = int(m.debug_read("batch_graphs", 0, 1)[0])
+        assert k > 20 and 1 <= graphs <= len(counts), (k, graphs, counts)
+    finally:
+        m.batch_close()
+    for name, (ids, kw) in reqs.items():
+        assert s.out[name] == m.generate(ids, **kw)[0], name
+
+
 def test_batch_session_rules(q3):
     from aha_b200 import B200Error
     cfg, w, m, o = q3
