@@ -34,8 +34,46 @@ class GenParams(C.Structure):
                 ("flags", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX = 1, 2, 4
+GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX, GEN_LOGPROBS = 1, 2, 4, 8
+MAX_TOP_LOGPROBS = 20
 TOKEN_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32)
+
+
+def gen_top_logprobs(n):
+    """AHA_GEN_TOP_LOGPROBS(n): the count in bits 8 and up of flags, unmasked (an out-of-range count is refused, never wrapped)."""
+    return (int(n) << 8) & 0xFFFFFFFF
+
+
+def logprob_flags(logprobs=False, top_logprobs=0, vocab_size=None):
+    """flags bits of an OpenAI-style (logprobs, top_logprobs) pair, checked the way the library checks them."""
+    if isinstance(top_logprobs, bool) or not isinstance(top_logprobs, (int, np.integer)):
+        raise TypeError(f"top_logprobs must be an int, not {type(top_logprobs).__name__}")
+    n = int(top_logprobs)
+    if not logprobs:
+        if n:
+            raise ValueError("top_logprobs needs logprobs=True")
+        return 0
+    if n < 0 or n > MAX_TOP_LOGPROBS:
+        raise ValueError(f"top_logprobs must be 0 to {MAX_TOP_LOGPROBS}, got {n}")
+    if vocab_size is not None and n > vocab_size:
+        raise ValueError(f"top_logprobs {n} exceeds the vocabulary of {vocab_size}")
+    return GEN_LOGPROBS | gen_top_logprobs(n)
+
+
+class Logprobs(C.Structure):
+    _fields_ = [("token", C.c_uint32), ("index", C.c_uint32), ("logprob", C.c_float), ("n_top", C.c_uint32),
+                ("top_ids", C.c_uint32 * MAX_TOP_LOGPROBS), ("top_logprobs", C.c_float * MAX_TOP_LOGPROBS),
+                ("valid", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+def logprobs_record(r):
+    """aha_logprobs -> dict(token, index, logprob, top_ids, top_logprobs); the float32 values are kept exactly."""
+    n = int(r.n_top)
+    return dict(token=int(r.token), index=int(r.index), logprob=np.float32(r.logprob),
+                top_ids=[int(r.top_ids[i]) for i in range(n)], top_logprobs=[np.float32(r.top_logprobs[i]) for i in range(n)])
+
+
+LOGPROBS_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Logprobs))
 
 
 class AsrChunk(C.Structure):
@@ -75,6 +113,12 @@ SYMBOLS = {
     "aha_b200_stop_token_ids": (C.c_size_t, [_P, _U32P, C.c_size_t]),
     "aha_b200_generate": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), _U32P, C.c_size_t,
                                     C.POINTER(C.c_size_t), C.POINTER(Usage)]),
+    "aha_b200_generate_logprobs": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), _U32P, C.POINTER(Logprobs),
+                                             C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
+    "aha_b200_generate_stream_logprobs": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), LOGPROBS_CALLBACK, C.c_void_p,
+                                                    C.POINTER(Usage)]),
+    "aha_b200_batch_logprobs": (C.c_int, [_P, C.POINTER(Logprobs), C.c_size_t]),
+    "aha_b200_debug_logprobs": (C.c_int, [_P, _F32P, C.c_size_t, C.c_uint32, C.c_uint32, C.POINTER(Logprobs)]),
     "aha_b200_generate_batch": (C.c_int, [_P, C.POINTER(BatchRequest), C.c_size_t, _U32P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
     "aha_b200_batch_open": (C.c_int, [_P]),
     "aha_b200_batch_add": (C.c_int, [_P, C.POINTER(BatchRequest), C.POINTER(C.c_int32), _U32P, C.POINTER(C.c_int32), C.POINTER(Usage)]),

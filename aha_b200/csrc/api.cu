@@ -44,6 +44,7 @@ struct aha_model {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // pinned staging for the host<->device scalars of a step / the tokens of a burst
     uint32_t* h_pin = nullptr;
+    aha_logprobs* h_lp_pin = nullptr;        // [32] the records of a burst (generate_logprobs), allocated the first time a request asks
     static constexpr int kStreamBurst = 8;   // streaming: steps the device may run ahead of the token being delivered
     cudaEvent_t ev_tok[kStreamBurst] = {};
     // KV reuse across requests (SURVEY 8f rank 4; new design: the reference clears the cache after every request, common/generate.rs:147,
@@ -61,6 +62,7 @@ struct aha_model {
         int width = kGemvBatchMax;      // slots of the session
         bool used[kWideSeqs] = {};
         size_t budget[kWideSeqs] = {}, produced[kWideSeqs] = {};
+        bool lp_valid[kWideSeqs] = {};  // the slot's record row holds the record of the last token its request delivered
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
 };
@@ -290,6 +292,23 @@ void require_no_session(aha_model* m) {
 }
 bool env_flag(const char* name, bool dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) != 0 : dflt; }
 int env_int(const char* name, int dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) : dflt; }
+// AHA_GEN_LOGPROBS / AHA_GEN_TOP_LOGPROBS(n) of a request: -1 = no records, else the top count n (bits 8 and up of flags, unmasked)
+int logprob_request(const aha_gen_params& p, const TextModel& T, const std::string& who) {
+    const uint32_t n = p.flags >> 8;
+    if (!(p.flags & AHA_GEN_LOGPROBS)) {
+        AHA_REQUIRE(n == 0, who + "AHA_GEN_TOP_LOGPROBS(" + std::to_string(n) + ") needs AHA_GEN_LOGPROBS");
+        return -1;
+    }
+    AHA_REQUIRE(n <= AHA_MAX_TOP_LOGPROBS, who + "AHA_GEN_TOP_LOGPROBS(" + std::to_string(n) + "): at most " + std::to_string(AHA_MAX_TOP_LOGPROBS) + " alternatives");
+    AHA_REQUIRE(n <= (uint32_t)T.cfg.V, who + "AHA_GEN_TOP_LOGPROBS(" + std::to_string(n) + ") exceeds the vocabulary of " + std::to_string(T.cfg.V));
+    AHA_REQUIRE(T.tp_world == 1, who + "log-probabilities are single-GPU (under tensor parallelism the decode step holds only a vocabulary shard)");
+    AHA_REQUIRE(T.cfg.V <= kLpMaxParts * kLpSlice, who + "vocabulary too large for the log-probability kernels");
+    return (int)n;
+}
+// the entries that return no records refuse a request for them
+void refuse_logprobs(const aha_gen_params& p, const std::string& who, const std::string& instead) {
+    AHA_REQUIRE((p.flags & AHA_GEN_LOGPROBS) == 0 && (p.flags >> 8) == 0, who + " returns no log-probabilities: use " + instead);
+}
 // AHA_BATCH_GEMV's default (BatchDecoder::gemv).  The two batched GEMVs are bit-identical on every tested shape and neither wins everywhere: on
 // one H100 80GB HBM3 at 400 W (profiles/run_batch.py, ms per step at 1 / 8 requests) v2 takes 2.25 / 4.68-4.76 against v1's 2.22 / 4.17 on the
 // VL2 text stack, and 1.30 / 2.71 against 1.33 / 2.63-2.64 on the Qwen3-0.6B shape.
@@ -619,18 +638,24 @@ int sampling_mode(const aha_gen_params& p) {
     return has_p ? SAMPLE_TOPK_TOPP : SAMPLE_TOPK;
 }
 
-struct GenSink {   // receives every generated token in order; returns true to stop the request (client went away)
-    std::function<bool(uint32_t token, size_t index)> push;
+struct GenSink {   // receives every generated token in order (with its record when the request asked); returns true to stop the request (client went away)
+    std::function<bool(uint32_t token, size_t index, const aha_logprobs* lp)> push;
 };
 
 // generate_generic / generate_stream_generic (common/generate.rs:115-159, 231-368) with the loop on the device:
 // forward_initial + sample, then decode steps chained through DecodeState (token, position, history, RNG draw index all
 // live in HBM); the host only looks at the tokens, a burst behind the device.  `stream`: tokens are handed to the sink one
 // by one as their step completes (per-step event) while the device keeps running ahead inside the burst.
+// lp_n >= 0: every token's log-probability record (lp_n alternatives) is computed after its step and travels with it.
 void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params& params, const GenSink& sink, bool stream,
-                   aha_usage* usage, size_t* n_generated) {
+                   aha_usage* usage, size_t* n_generated, int lp_n = -1) {
     TextModel& T = m->text;
     require_no_session(m);
+    const bool lp = lp_n >= 0;
+    if (lp) {
+        T.set_logprobs(lp_n);
+        if (!m->h_lp_pin) AHA_CUDA_CHECK(cudaMallocHost(&m->h_lp_pin, 32 * sizeof(aha_logprobs)));
+    }
     const size_t sample_len = std::max<size_t>(params.max_tokens, 1);   // `for _ in 1..sample_len`: sample_len 0 and 1 both yield exactly one token
     AHA_REQUIRE(seq_len + sample_len <= (size_t)T.max_ctx,
                 "prompt + max_tokens exceeds max_ctx (the handle's KV capacity, aha_options.max_ctx; the reference's cache is unbounded)");
@@ -670,11 +695,16 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     if (hit > 0) forward_any(m, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
     else forward_any(m, ids, seq_len, 0, mm, true, nullptr, &tok);   // forward_initial + sample_and_push
     T.check_sample_error();
+    if (lp) {   // the first token's record, from the prefill logits
+        T.logprobs(true, T.d_lp, true);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_lp_pin, T.d_lp, sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+    }
     const auto t1 = clk::now();
     const double vision_secs = m->last_vision_secs;
     size_t done = 1;
     produced.push_back(tok);
-    bool stop = sink.push(tok, 0) || (eos_on_first && is_eos(tok));   // generate_generic never EOS-checks the first token; the ASR loop does
+    bool stop = sink.push(tok, 0, lp ? m->h_lp_pin : nullptr) || (eos_on_first && is_eos(tok));   // generate_generic never EOS-checks the first token; the ASR loop does
     if (sample_len > 1 && !stop) {
         T.ensure_tokens((int)(seq_len + sample_len));
         DecodeState cur;
@@ -685,14 +715,17 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
         while (done < sample_len && !stop) {
             const size_t n = std::min<size_t>(burst_max, sample_len - done);
             for (size_t i = 0; i < n; ++i) {
-                T.decode_step();
+                T.decode_step(lp);
+                if (lp) T.logprobs(false, T.d_lp, true);
                 if (stream) {
                     AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_pin + i, T.d_history + done + i, sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
+                    if (lp) AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_lp_pin + i, T.d_lp + done + i, sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
                     AHA_CUDA_CHECK(cudaEventRecord(m->ev_tok[i], m->ctx.stream));
                 }
             }
             if (!stream) {
                 AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_pin, T.d_history + done, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
+                if (lp) AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_lp_pin, T.d_lp + done, n * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
                 AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
             }
             for (size_t i = 0; i < n && !stop; ++i) {
@@ -700,7 +733,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
                 const uint32_t t = m->h_pin[i];
                 ++done;
                 produced.push_back(t);
-                stop = sink.push(t, done - 1) || is_eos(t);   // an EOS token is pushed before the break (generate.rs:139-141)
+                stop = sink.push(t, done - 1, lp ? m->h_lp_pin + i : nullptr) || is_eos(t);   // an EOS token is pushed before the break (generate.rs:139-141)
             }
             AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
             T.check_ll_abort();
@@ -732,7 +765,7 @@ namespace {
 // One request into slot `slot` of the batch decoder: the reference's forward_initial + sample_and_push on the slot's own page table (swapped into
 // the TextModel for the duration, so tower / M-RoPE / deepstack / sampler-on-prefill are the single-request code), then its decode state, history
 // and sampler move into the slot.  *swapped tells the caller's guard which table is swapped in if this throws.
-uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int* swapped) {
+uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int lp_n, int* swapped) {
     TextModel& T = m->text;
     BatchDecoder& B = m->sess();
     B.swap_table(slot); *swapped = slot;
@@ -742,6 +775,12 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
     uint32_t tok = 0;
     forward_any(m, r.ids, r.seq_len, 0, r.mm, true, nullptr, &tok, false, true);
     T.check_sample_error();
+    if (lp_n >= 0) {   // the first token's record goes straight into the slot's record row
+        T.set_logprobs(lp_n);
+        B.ensure_lp();
+        T.logprobs(true, B.d_lp_rec + slot, false);
+    }
+    B.slots[slot].lp = lp_n + 1;
     T.ensure_tokens((int)(r.seq_len + sample_len));       // every page the request can touch is mapped now (the step kernels only read the table)
     DecodeState cur;
     AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
@@ -758,6 +797,7 @@ void session_release(aha_model* m, int slot) {
     for (int k = 0; k < sl.mapped; ++k) m->text.free_pages.push_back(sl.h_table[k]);
     sl.mapped = 0;
     sl.samp_active = false;
+    sl.lp = 0;
     m->session.used[slot] = false;
     m->sess().composition_changed();
 }
@@ -814,10 +854,12 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     slot.resize(n);
     std::vector<size_t> sample_len(n);
     std::vector<bool> packed(n);
+    std::vector<int> lp_n(n);
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
         const aha_batch_request& r = reqs[i];
         AHA_REQUIRE(r.ids && r.seq_len >= 1, who + "request " + std::to_string(i) + " needs input_ids");
+        lp_n[i] = logprob_request(r.params, T, who + "request " + std::to_string(i) + ": ");
         for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
         AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
         if (m->kind == aha_model::QWEN3VL) AHA_REQUIRE(r.mm && r.mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
@@ -846,7 +888,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
             if (pack_in) swap_pack();
             if (ok) return;
             if (swapped >= 0) m->sess().swap_table(swapped);
-            for (int s : slots) session_release(m, s);
+            for (int s : slots) { session_release(m, s); m->session.lp_valid[s] = false; }
             m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
         }
     } guard{m, slot};
@@ -916,6 +958,8 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
             const aha_gen_params& p = reqs[i].params;
             T.set_sampler(sampling_mode(p), p.temperature, p.top_p, p.top_k, p.repeat_penalty, p.repeat_last_n, p.seed);
             B.bind_sampler(slot[i]);
+            B.slots[slot[i]].lp = lp_n[i] + 1;
+            if (lp_n[i] >= 0) B.ensure_lp();
             act.push_back(slot[i]);
         }
         const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};
@@ -939,7 +983,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     // ---- the others: one prefill each, on the slot's own table
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
-        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], &guard.swapped);
+        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i], &guard.swapped);
         secs[i] = std::chrono::duration<double>(clk::now() - t0).count();
         vision[i] = m->last_vision_secs;
     }
@@ -950,6 +994,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         const int s = slot[i];
         m->session.budget[s] = sample_len[i];
         m->session.produced[s] = 1;
+        m->session.lp_valid[s] = lp_n[i] >= 0;
         bool stop = sample_len[i] == 1;
         if ((reqs[i].params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[i]) stop = true;
         if (usage) {
@@ -983,6 +1028,7 @@ size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, siz
         const uint32_t t = h_tok[slot];
         tokens_out[slot] = t;
         m->session.produced[slot] += 1;
+        m->session.lp_valid[slot] = B.slots[slot].lp > 0;
         bool stop = m->session.produced[slot] >= m->session.budget[slot];
         for (uint32_t e : m->stop_ids) if (e == t) stop = true;     // an EOS token is delivered, then the request ends (generate.rs:139-141)
         status_out[slot] = stop ? 2 : 1;
@@ -1006,6 +1052,7 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
         const size_t sample_len = std::max<size_t>(reqs[i].params.max_tokens, 1);
         AHA_REQUIRE(cap >= sample_len, "out_tokens capacity (per request) is smaller than max_tokens");
         AHA_REQUIRE((reqs[i].params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "generate_batch: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+        refuse_logprobs(reqs[i].params, "generate_batch", "a batch session (aha_b200_batch_open, aha_b200_batch_logprobs)");
         pages += (reqs[i].seq_len + sample_len + kPage - 1) / kPage;
         n_out[i] = 0;
     }
@@ -1078,6 +1125,22 @@ int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out, int32_t* status_ou
     });
 }
 
+int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out, size_t cap) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        AHA_REQUIRE(out, "batch_logprobs: out[cap] is required");
+        const int width = m->session.width;
+        AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+        BatchDecoder& B = m->sess();
+        std::vector<aha_logprobs> h((size_t)width);
+        if (B.d_lp_rec) {
+            AHA_CUDA_CHECK(cudaMemcpyAsync(h.data(), B.d_lp_rec, h.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+        }
+        for (size_t i = 0; i < cap; ++i) out[i] = (i < (size_t)width && m->session.lp_valid[i]) ? h[i] : aha_logprobs{};
+    });
+}
+
 int aha_b200_batch_close(aha_model* m) {
     return guarded(m, [&] { AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream)); session_close(m); });
 }
@@ -1094,10 +1157,26 @@ int aha_b200_generate(aha_model* m, const uint32_t* ids, size_t seq_len, const a
     return guarded(m, [&] {
         AHA_REQUIRE(params && out_tokens && n_out, "params, out_tokens and n_out are required");
         AHA_REQUIRE(cap >= std::max<size_t>(params->max_tokens, 1), "out_tokens capacity is smaller than max_tokens");
+        refuse_logprobs(*params, "generate", "aha_b200_generate_logprobs");
         if (usage) *usage = aha_usage{};
         size_t n = 0;
-        GenSink sink{[&](uint32_t t, size_t i) { out_tokens[i] = t; n = i + 1; return false; }};
+        GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs*) { out_tokens[i] = t; n = i + 1; return false; }};
         generate_impl(m, ids, seq_len, mm, *params, sink, false, usage, nullptr);
+        *n_out = n;
+    });
+}
+
+int aha_b200_generate_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                               uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap, size_t* n_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(params && out_tokens && out_logprobs && n_out, "params, out_tokens, out_logprobs and n_out are required");
+        AHA_REQUIRE(cap >= std::max<size_t>(params->max_tokens, 1), "out_tokens capacity is smaller than max_tokens");
+        const int lp_n = logprob_request(*params, m->text, "generate_logprobs: ");
+        AHA_REQUIRE(lp_n >= 0, "generate_logprobs: params.flags must carry AHA_GEN_LOGPROBS");
+        if (usage) *usage = aha_usage{};
+        size_t n = 0;
+        GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs* lp) { out_tokens[i] = t; out_logprobs[i] = *lp; n = i + 1; return false; }};
+        generate_impl(m, ids, seq_len, mm, *params, sink, false, usage, nullptr, lp_n);
         *n_out = n;
     });
 }
@@ -1106,9 +1185,22 @@ int aha_b200_generate_stream(aha_model* m, const uint32_t* ids, size_t seq_len, 
                              aha_token_callback on_token, void* user, aha_usage* usage) {
     return guarded(m, [&] {
         AHA_REQUIRE(params && on_token, "params and on_token are required");
+        refuse_logprobs(*params, "generate_stream", "aha_b200_generate_stream_logprobs");
         if (usage) *usage = aha_usage{};
-        GenSink sink{[&](uint32_t t, size_t i) { return on_token(user, t, (uint32_t)i) != 0; }};
+        GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs*) { return on_token(user, t, (uint32_t)i) != 0; }};
         generate_impl(m, ids, seq_len, mm, *params, sink, true, usage, nullptr);
+    });
+}
+
+int aha_b200_generate_stream_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                                      aha_logprobs_callback on_token, void* user, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(params && on_token, "params and on_token are required");
+        const int lp_n = logprob_request(*params, m->text, "generate_stream_logprobs: ");
+        AHA_REQUIRE(lp_n >= 0, "generate_stream_logprobs: params.flags must carry AHA_GEN_LOGPROBS");
+        if (usage) *usage = aha_usage{};
+        GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs* lp) { return on_token(user, t, (uint32_t)i, lp) != 0; }};
+        generate_impl(m, ids, seq_len, mm, *params, sink, true, usage, nullptr, lp_n);
     });
 }
 
@@ -1117,6 +1209,7 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
     return guarded(m, [&] {
         AHA_REQUIRE(m->kind == aha_model::QWEN3_ASR, "asr_generate needs a qwen3_asr handle");
         AHA_REQUIRE(chunks && n_chunks >= 1 && params && out_tokens && n_out, "chunks, params, out_tokens and n_out are required");
+        refuse_logprobs(*params, "asr_generate", "aha_b200_generate_logprobs on each chunk's prompt");
         if (usage) *usage = aha_usage{};
         // Qwen3AsrGenerateModel::generate (qwen3_asr/generate.rs:130-186): ONE LogitsProcessor for the whole request (its RNG
         // stream runs on across the chunks), no repeat penalty, every token -- the first included -- is EOS-checked, the KV
@@ -1132,7 +1225,7 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
             aha_mm mm{&chunks[c].input_features, 1};
             const size_t base = total;
             bool abort = false;
-            GenSink sink{[&](uint32_t t, size_t i) {
+            GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs*) {
                 out_tokens[base + i] = t; total = base + i + 1;
                 if (on_token && on_token(user, t, (uint32_t)(base + i)) != 0) abort = true;
                 return abort;
@@ -1162,6 +1255,39 @@ int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_param
         T.check_sample_error();
         T.clear_sampler();
         *token_out = m->h_pin[0];
+    });
+}
+
+int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(logits && out, "logits and out are required");
+        AHA_REQUIRE(V >= 1 && V <= (size_t)kLpMaxParts * kLpSlice, "V must be 1 to " + std::to_string(kLpMaxParts * kLpSlice));
+        AHA_REQUIRE(n_top <= AHA_MAX_TOP_LOGPROBS && n_top <= V, "n_top must be at most 20 and at most V");
+        AHA_REQUIRE(token < V, "token out of range");
+        cudaStream_t st = m->ctx.stream;
+        const int P = lp_parts((int)V);
+        const int on = 1 + (int)n_top;
+        const DecodeState ds{token, 0, 0, 0, 0, {0, 0, 0}};
+        // scratch of this call only: [V] logits, the candidate lists, the on flag, the token, a state and the record
+        struct Scratch {
+            void* p = nullptr;
+            ~Scratch() { if (p) cudaFree(p); }
+        } mem;
+        const size_t o_part = V * sizeof(float), o_id = o_part + (size_t)P * kLpPartFloats * sizeof(float), o_on = o_id + (size_t)P * kLpMaxTop * sizeof(int);
+        const size_t o_tok = o_on + 16, o_st = o_tok + 16, o_rec = o_st + sizeof(DecodeState), bytes = o_rec + sizeof(aha_logprobs);
+        AHA_CUDA_CHECK(cudaMalloc(&mem.p, bytes));
+        char* b = static_cast<char*>(mem.p);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b, logits, V * sizeof(float), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b + o_on, &on, sizeof(int), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b + o_tok, &token, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b + o_st, &ds, sizeof(ds), cudaMemcpyHostToDevice, st));
+        logprobs_rows(st, reinterpret_cast<float*>(b), (int)V, (int)V, 1, nullptr, reinterpret_cast<int*>(b + o_on), reinterpret_cast<float*>(b + o_part),
+                      reinterpret_cast<int*>(b + o_id), reinterpret_cast<uint32_t*>(b + o_tok), reinterpret_cast<DecodeState*>(b + o_st), 1,
+                      reinterpret_cast<aha_logprobs*>(b + o_rec), 0, 1);
+        AHA_CUDA_CHECK(cudaGetLastError());
+        m->ctx.cnt.kernels += 2;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(out, b + o_rec, sizeof(aha_logprobs), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }
 
@@ -1806,6 +1932,7 @@ void aha_b200_destroy(aha_model* m) {
     m->wide_batch.clear_graphs();
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
+    if (m->h_lp_pin) cudaFreeHost(m->h_lp_pin);
     if (m->ev0) cudaEventDestroy(m->ev0);
     if (m->ev1) cudaEventDestroy(m->ev1);
     for (auto& e : m->ev_tok) if (e) cudaEventDestroy(e);

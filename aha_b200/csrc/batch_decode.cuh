@@ -10,8 +10,9 @@
 //     [o_proj + res]   projection
 //     [rmsnorm + gate/up + SwiGLU], [down + res]
 // then the head: final norm + lm_head for all rows, the two-stage ArgMax that advances every row's DecodeState, and the sampler of every row
-// whose request samples.  Everything that depends on WHICH slots run is read from device memory -- the active list d_act (row j -> slot), the
-// attention table d_attn, the per-slot sampler arguments d_samp -- so one CUDA graph per running count serves every composition of that count.
+// whose request samples, then, while a running request asks for them, the log-probability records (logprobs.cuh).  Everything that depends on
+// WHICH slots run is read from device memory -- the active list d_act (row j -> slot), the attention table d_attn, the per-slot sampler
+// arguments d_samp and log-probability flags d_lp_on -- so one CUDA graph per (running count, any request asks) serves every composition.
 // Finished sequences leave the step (the activation rows are rebuilt from the token embeddings every step, so compaction is free).
 // Packed admission (aha_b200_batch_add_many) borrows xb / logitsb between two steps for the first tokens of several requests at once (head_rows).
 //
@@ -36,6 +37,7 @@ struct BatchSlot {                       // one sequence of the batch
     int* d_table = nullptr;              // device copy: row of BatchDecoder::d_tables
     bool samp_active = false;
     SampleArgs samp{};                   // sampler of the request with the pointers of this slot
+    int lp = 0;                          // 0: the request asked for no log-probabilities, else 1 + its top count
 };
 
 struct BatchDecoder {
@@ -53,14 +55,21 @@ struct BatchDecoder {
     SampleArgs* d_samp = nullptr;        // [cap] per-slot sampler arguments
     int* d_samp_on = nullptr;            // [cap]
     float* workb = nullptr;              // [cap][V] sampler scratch, one row per slot (the rows sample concurrently)
+    // log-probabilities (logprobs.cuh), allocated when a request of the session first asks: per slot the on flag and the record of its
+    // latest token; the candidate lists of every row
+    int* d_lp_on = nullptr;              // [cap] BatchSlot::lp
+    aha_logprobs* d_lp_rec = nullptr;    // [cap]
+    float* lp_part = nullptr; int* lp_part_id = nullptr;
+    bool lp_any = false;                 // a request of the current composition asks: the head computes records
     std::vector<BatchSlot> slots;
     std::vector<int> table_for;          // active list the device copy of the composition was built for
     // set when a session opens (AHA_BATCH_GEMV, AHA_BATCH_GRAPH): the narrow step's projections -- 0 = batched GEMV with the weights in
     // registers, 1 = exact SIMT GEMM (validation twin), 2 = batched GEMV with the cp.async weight ring -- and eager launches instead of graphs
     int gemv = 2;
     bool use_graph = true;
-    // one CUDA graph per running count (~170 launches per step become one); they outlive composition changes
-    struct StepGraph { int width; cudaGraphExec_t exec; uint64_t kernels; };
+    // one CUDA graph per (running count, any request asks for log-probabilities) (~170 launches per step become one); they outlive
+    // composition changes
+    struct StepGraph { int width; bool lp; cudaGraphExec_t exec; uint64_t kernels; };
     std::vector<StepGraph> graphs;
     void clear_graphs() {
         for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
@@ -70,8 +79,9 @@ struct BatchDecoder {
     void composition_changed() { table_for.clear(); }
     // no sequence holds a slot any more (a session opens or closes)
     void reset() {
-        for (auto& sl : slots) sl.mapped = 0;
+        for (auto& sl : slots) { sl.mapped = 0; sl.lp = 0; }
         table_for.clear();
+        lp_any = false;
         clear_graphs();
     }
 
@@ -156,6 +166,16 @@ struct BatchDecoder {
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
         bind_sampler(i);
     }
+    void ensure_lp() {
+        if (d_lp_rec) return;
+        Ctx& c = *T->ctx;
+        const int P = lp_parts(T->cfg.V);
+        d_lp_on = c.alloc<int>(cap);
+        d_lp_rec = c.alloc<aha_logprobs>(cap);
+        lp_part = c.alloc<float>((size_t)cap * P * kLpPartFloats);
+        lp_part_id = c.alloc<int>((size_t)cap * P * kLpMaxTop);
+        AHA_CUDA_CHECK(cudaMemset(d_lp_on, 0, (size_t)cap * sizeof(int)));
+    }
     // the sampler set on the TextModel (set_sampler) becomes slot i's, with the slot's own state, history, token and scratch row
     void bind_sampler(int i) {
         BatchSlot& s = slots[i];
@@ -194,7 +214,12 @@ struct BatchDecoder {
         std::vector<SampleArgs> samp((size_t)cap);
         std::vector<int> on((size_t)cap, 0);
         for (int i = 0; i < cap; ++i) { on[i] = slots[i].samp_active ? 1 : 0; if (on[i]) samp[i] = slots[i].samp; }
+        std::vector<int> lp_on((size_t)cap, 0);
+        lp_any = false;
+        for (int i = 0; i < cap; ++i) lp_on[i] = slots[i].lp;
+        for (int s : act) lp_any = lp_any || slots[s].lp > 0;
         Ctx& c = *T->ctx;
+        if (d_lp_on) AHA_CUDA_CHECK(cudaMemcpyAsync(d_lp_on, lp_on.data(), lp_on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_attn, h.data(), h.size() * sizeof(DecodeAttnArgs), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_samp, samp.data(), samp.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
@@ -245,14 +270,14 @@ struct BatchDecoder {
         if (wide) zero_rows_from(nb);
         if (!use_graph) { launches(nb); return; }
         StepGraph* g = nullptr;
-        for (auto& e : graphs) if (e.width == nb) { g = &e; break; }
+        for (auto& e : graphs) if (e.width == nb && e.lp == lp_any) { g = &e; break; }
         if (!g) {
             const uint64_t k0 = c.cnt.kernels;
             cudaGraph_t cg = nullptr;
             AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
             try { launches(nb); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
             AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &cg));
-            StepGraph e{nb, nullptr, c.cnt.kernels - k0};
+            StepGraph e{nb, lp_any, nullptr, c.cnt.kernels - k0};
             c.cnt.kernels = k0;
             const cudaError_t err = cudaGraphInstantiate(&e.exec, cg, 0);
             cudaGraphDestroy(cg);
@@ -287,7 +312,8 @@ struct BatchDecoder {
         head(nb, false);
     }
     // Final norm + lm_head over rows 0 .. nb-1 of xb, then for row j the two-stage ArgMax of slot d_act[j] and, when its request samples, its
-    // sampler.  A decode step (first = false) advances the slot's DecodeState and the sampled token replaces the ArgMax one the step pushed
+    // sampler, then, when a request of the composition asks, the log-probability records of the rows whose request asks (into d_lp_rec[slot]).
+    // A decode step (first = false) advances the slot's DecodeState and the sampled token replaces the ArgMax one the step pushed
     // (the single-sequence loop does the same).  A request's first token (first = true, packed admission) is drawn the way forward_any draws
     // it: no advance, no overwrite, against the slot's state as the caller set it (empty history, draw index 0); only n_draws moves.
     void head(int nb, bool first) {
@@ -300,6 +326,10 @@ struct BatchDecoder {
         argmax_final_rows_kernel<<<nb, 32, 0, st>>>(pmaxb, pidxb, n_pcand, d_act, d_tok, d_states, d_hist, T->hist_cap, first ? 0 : 1);
         sample_rows_kernel<<<nb, kSampleThreads, 0, st>>>(d_samp, d_samp_on, d_act, logitsb, cf.V, first ? 0 : 1);
         c.cnt.kernels += 3;
+        if (lp_any) {
+            logprobs_rows(st, logitsb, cf.V, cf.V, nb, d_act, d_lp_on, lp_part, lp_part_id, d_tok, d_states, first ? 1 : 0, d_lp_rec, 0, cap);
+            c.cnt.kernels += 2;
+        }
         AHA_CUDA_CHECK(cudaGetLastError());
     }
     // the first tokens of the slots in `act`, whose last prompt rows packed admission gathered into xb and whose samplers were just bound

@@ -20,6 +20,7 @@
 #include "gemv.cuh"
 #include "json.hpp"
 #include "kernels_common.cuh"
+#include "logprobs.cuh"
 #include "nccl_shim.h"
 #include "sampling.cuh"
 
@@ -433,6 +434,12 @@ struct TextModel {
     SampleArgs samp{};
     float* sample_work = nullptr;
     int* d_sample_err = nullptr;
+
+    // log-probability records of the request (logprobs.cuh), allocated the first time a request asks: d_lp_on = 1 + its top count,
+    // d_lp[i] = the record of generated token i
+    int* d_lp_on = nullptr;
+    aha_logprobs* d_lp = nullptr;
+    float* lp_part = nullptr; int* lp_part_id = nullptr;
 
     // tracing (tests)
     bool trace = false;
@@ -959,6 +966,26 @@ struct TextModel {
             cudaMemset(d_sample_err, 0, sizeof(int));
             throw std::runtime_error("sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)");
         }
+    }
+    // ---- log-probabilities: the request asks for n_top alternatives per record
+    void set_logprobs(int n_top) {
+        AHA_REQUIRE(cfg.V <= kLpMaxParts * kLpSlice, "vocabulary too large for the log-probability kernels");
+        if (!d_lp) {
+            d_lp_on = ctx->alloc<int>(1);
+            d_lp = ctx->alloc<aha_logprobs>((size_t)hist_cap);
+            lp_part = ctx->alloc<float>((size_t)lp_parts(cfg.V) * kLpPartFloats);
+            lp_part_id = ctx->alloc<int>((size_t)lp_parts(cfg.V) * kLpMaxTop);
+        }
+        const int on = 1 + n_top;
+        AHA_CUDA_CHECK(cudaMemcpy(d_lp_on, &on, sizeof(int), cudaMemcpyHostToDevice));
+    }
+    // the record of the token in d_argmax, from the logits row: first = a first token (index 0), else a decode step's (n_hist - 1).
+    // by_index: out[index] (the request's record buffer), else out[0]
+    void logprobs(bool first, aha_logprobs* out, bool by_index) {
+        logprobs_rows(ctx->stream, logits, cfg.V, cfg.V, 1, nullptr, d_lp_on, lp_part, lp_part_id, d_argmax, d_state, first ? 1 : 0, out,
+                      by_index ? 1 : 0, hist_cap);
+        AHA_CUDA_CHECK(cudaGetLastError());
+        ctx->cnt.kernels += 2;
     }
     void set_state(uint32_t token, int pos, int rope_delta, int n_hist, uint32_t n_draws = 0) {
         DecodeState s{token, pos, rope_delta, n_hist, n_draws, {0, 0, 0}};

@@ -191,22 +191,28 @@ class B200Model:
                     completion_secs=u.completion_secs, vision_secs=u.vision_secs)
 
     def generate(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False):
+                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False, logprobs=False, top_logprobs=0):
         """-> (generated ids, usage dict).  temperature < 1e-7: ArgMax; else the device sampler (TopK / TopKThenTopP / TopP /
         All exactly as get_logit_processor picks them from temperature, top_p, top_k).  reuse_prefix: keep this request's K/V
-        and prefill only what follows the prefix shared with the cache (multi-turn chats; same tokens as without it)."""
+        and prefill only what follows the prefix shared with the cache (multi-turn chats; same tokens as without it).
+        logprobs=True (aha_b200_generate_logprobs): -> (ids, usage, records), one record dict per token (token, index, logprob,
+        top_ids, top_logprobs with top_logprobs alternatives; raw model log-probabilities, before penalty and temperature)."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         if reuse_prefix:
             flags |= L.GEN_REUSE_PREFIX
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
         p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
         cap = max(max_tokens, 1)
         out = (C.c_uint32 * cap)()
         n = C.c_size_t(0)
         u = L.Usage()
-        self._check(self._lib.aha_b200_generate(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint32)), ids.size,
-                                                C.byref(mm) if mm is not None else None, C.byref(p), out, cap,
-                                                C.byref(n), C.byref(u)))
+        ids_p, mm_p = ids.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(mm) if mm is not None else None
+        if logprobs:
+            recs = (L.Logprobs * cap)()
+            self._check(self._lib.aha_b200_generate_logprobs(self._h, ids_p, ids.size, mm_p, C.byref(p), out, recs, cap, C.byref(n), C.byref(u)))
+            return [int(out[i]) for i in range(n.value)], self._usage(u), [L.logprobs_record(recs[i]) for i in range(n.value)]
+        self._check(self._lib.aha_b200_generate(self._h, ids_p, ids.size, mm_p, C.byref(p), out, cap, C.byref(n), C.byref(u)))
         return [int(out[i]) for i in range(n.value)], self._usage(u)
 
     def generate_batch(self, requests):
@@ -233,8 +239,9 @@ class B200Model:
             arr[i].ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
             arr[i].seq_len = ids.size
             arr[i].mm = C.pointer(mm) if mm is not None else None
+            flags = r.get("flags", 0) | L.logprob_flags(r.get("logprobs", False), r.get("top_logprobs", 0), self.vocab_size)
             arr[i].params = self._gen_params(r.get("max_tokens", 1024), r.get("temperature", 0.0), r.get("top_p"), r.get("top_k"),
-                                             r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), r.get("flags", 0))
+                                             r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), flags)
         return arr, keep
 
     # ---- continuous batching: requests join / leave a running batch between steps (aha_b200_batch_open / _add / _step / _close)
@@ -248,8 +255,10 @@ class B200Model:
         self._batch_width = int(max_seqs)
 
     def batch_add(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64,
-                  seed=299792458, flags=0):
-        """Prefill one request into a free slot -> (slot, first token, finished)."""
+                  seed=299792458, flags=0, logprobs=False, top_logprobs=0):
+        """Prefill one request into a free slot -> (slot, first token, finished).  logprobs / top_logprobs: batch_logprobs() holds the
+        record of each token it delivers."""
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         req = L.BatchRequest()
@@ -286,29 +295,42 @@ class B200Model:
         self._check(self._lib.aha_b200_batch_step(self._h, toks, status, C.byref(n)))
         return {i: (int(toks[i]), status[i] == 2) for i in range(8) if status[i] != 0}
 
+    def batch_logprobs(self):
+        """-> {slot: record} for the slots whose request asked for log-probabilities: the record of the last token each delivered (by
+        batch_add, batch_add_many or the last batch_step, including the step that finished it)."""
+        w = getattr(self, "_batch_width", 8)
+        recs = (L.Logprobs * w)()
+        self._check(self._lib.aha_b200_batch_logprobs(self._h, recs, w))
+        return {i: L.logprobs_record(recs[i]) for i in range(w) if recs[i].valid}
+
     def batch_close(self):
         self._check(self._lib.aha_b200_batch_close(self._h))
 
     def generate_stream(self, input_ids, on_token, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None,
-                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False):
+                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0):
         """generate_stream_generic: on_token(token, index) is called per generated token as its step completes; a truthy
-        return value ends the request.  -> usage dict."""
+        return value ends the request.  logprobs=True: on_token(token, index, record).  -> usage dict."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed,
-                             L.GEN_REUSE_PREFIX if reuse_prefix else 0)
+        flags = (L.GEN_REUSE_PREFIX if reuse_prefix else 0) | L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
         err = []
 
-        def _cb(_user, token, index):
+        def _cb(_user, token, index, *lp):
             try:
-                return 1 if on_token(int(token), int(index)) else 0
+                args = (int(token), int(index)) + ((L.logprobs_record(lp[0].contents),) if lp else ())
+                return 1 if on_token(*args) else 0
             except Exception as e:  # never unwind through the C ABI
                 err.append(e)
                 return 1
-        cb = L.TOKEN_CALLBACK(_cb)
         u = L.Usage()
-        self._check(self._lib.aha_b200_generate_stream(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint32)), ids.size,
-                                                       C.byref(mm) if mm is not None else None, C.byref(p), cb, None, C.byref(u)))
+        ids_p, mm_p = ids.ctypes.data_as(C.POINTER(C.c_uint32)), C.byref(mm) if mm is not None else None
+        if logprobs:
+            cb = L.LOGPROBS_CALLBACK(_cb)
+            self._check(self._lib.aha_b200_generate_stream_logprobs(self._h, ids_p, ids.size, mm_p, C.byref(p), cb, None, C.byref(u)))
+        else:
+            cb = L.TOKEN_CALLBACK(_cb)
+            self._check(self._lib.aha_b200_generate_stream(self._h, ids_p, ids.size, mm_p, C.byref(p), cb, None, C.byref(u)))
         if err:
             raise err[0]
         return self._usage(u)
@@ -343,6 +365,14 @@ class B200Model:
         self._check(self._lib.aha_b200_debug_sample(self._h, lg.ctypes.data_as(C.POINTER(C.c_float)), C.byref(p),
                                                     ctx.ctypes.data_as(C.POINTER(C.c_uint32)), ctx.size, int(draw_index), C.byref(tok)))
         return int(tok.value)
+
+    def debug_logprobs(self, logits, token, n_top=0):
+        """The log-probability kernels on a given logits row of any length (tests) -> record dict."""
+        lg = np.ascontiguousarray(logits, np.float32).reshape(-1)
+        r = L.Logprobs()
+        self._check(self._lib.aha_b200_debug_logprobs(self._h, lg.ctypes.data_as(C.POINTER(C.c_float)), lg.size, int(token), int(n_top),
+                                                      C.byref(r)))
+        return L.logprobs_record(r)
 
     # ------------------------------------------------------------------ Qwen3-Embedding / Qwen3-Reranker
     def embed(self, input_ids):

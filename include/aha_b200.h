@@ -91,10 +91,39 @@ typedef struct aha_gen_params {      /* ChatCompletionParameters subset used by 
 #define AHA_GEN_REUSE_PREFIX 4u  /* KV reuse across requests (SURVEY 8f rank 4; the reference clears the cache after every request, generate.rs:147):
                                   * leave this request's K/V in the paged cache and, at its start, prefill only what follows the longest prefix
                                   * the prompt shares with the cache (same token ids and the same multimodal tensors).  Tokens are unchanged. */
+#define AHA_GEN_LOGPROBS 8u      /* one aha_logprobs record per generated token (OpenAI `logprobs`): aha_b200_generate_logprobs,
+                                  * aha_b200_generate_stream_logprobs and batch sessions (aha_b200_batch_logprobs); the other entries refuse it */
+#define AHA_GEN_TOP_LOGPROBS(n) ((uint32_t)(n) << 8)   /* OpenAI `top_logprobs`: n alternatives per record, in bits 8-15 of flags and up.
+                                  * Not masked: a count above AHA_MAX_TOP_LOGPROBS (or above the vocabulary) is refused, never wrapped.
+                                  * Needs AHA_GEN_LOGPROBS. */
+#define AHA_MAX_TOP_LOGPROBS 20
+
+/* The log-probability record of one generated token (new design; the reference's responses carry `logprobs: None`).
+ *   logprob = x[token] - (M + log sum_j exp(x[j] - M)), x = the fp32 logits row the step computed, M = its maximum: the model's own
+ *   distribution, taken BEFORE repeat penalty, temperature, top-k and top-p, so greedy and sampled requests report comparable numbers
+ *   (a sampled token that top-k would have excluded still has a finite value);
+ *   top_ids / top_logprobs[0 .. n_top): the n_top largest entries of x, by raw logit descending, ties by ascending id.  A greedy request
+ *   without repeat penalty has token == top_ids[0] and logprob == top_logprobs[0] bit for bit.  Entries from n_top on are zero;
+ *   index: the token's position in the request's output (0 = the first token, computed from the prefill logits);
+ *   valid: 1 for a record, 0 for an aha_b200_batch_logprobs slot that holds none.
+ * Computed on the device by one pair of kernels for every path, so a request's records are bit-identical whichever path computes them
+ * from the same logits.  Single GPU only (tp_world > 1 is refused). */
+typedef struct aha_logprobs {
+    uint32_t token;
+    uint32_t index;
+    float logprob;
+    uint32_t n_top;
+    uint32_t top_ids[AHA_MAX_TOP_LOGPROBS];
+    float top_logprobs[AHA_MAX_TOP_LOGPROBS];
+    uint32_t valid;
+    uint32_t reserved;
+} aha_logprobs;
 
 /* generate_stream: called once per generated token, in order, as soon as its step has completed (the device keeps running a few
  * steps ahead); a non-zero return ends the request (the reference's stream is dropped when the client goes away). */
 typedef int (*aha_token_callback)(void* user, uint32_t token, uint32_t index);
+/* generate_stream_logprobs: the same, with the token's record (valid for the duration of the call) */
+typedef int (*aha_logprobs_callback)(void* user, uint32_t token, uint32_t index, const aha_logprobs* lp);
 
 typedef struct aha_asr_chunk {       /* one AudioData of Qwen3AsrProcessor::process_info (qwen3_asr/processor.rs:181-184) */
     const uint32_t* ids;             /* prompt with the <|audio_pad|> run already expanded */
@@ -222,6 +251,12 @@ int aha_b200_batch_open_wide(aha_model* m, size_t max_seqs);
 /* batch_step over cap entries (cap >= the session width; works on narrow sessions too).  batch_step refuses a session wider than 8. */
 int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out /* [cap] */, int32_t* status_out /* [cap] */, size_t cap,
                           size_t* n_stepped_out /* may be NULL */);
+/* Log-probabilities in a batch session (narrow or wide): a request asks with AHA_GEN_LOGPROBS [| AHA_GEN_TOP_LOGPROBS(n)] in its
+ * params.flags.  out[slot] (cap >= the session width) receives the record of the last token the slot's request delivered -- by
+ * batch_add, batch_add_many or the last step, including the step that finished it -- until another request takes the slot.  Slots whose
+ * request did not ask, or that never held one, get valid = 0.  A step computes records only while a running request asks, so a session
+ * without such requests launches exactly the kernels it launched before. */
+int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out /* [cap] */, size_t cap);
 
 /* WhisperFeatureExtractor::call (src/models/feature_extractor/
  * feature_extraction_whisper.rs:65-115): wave (n) f32 host -> log-mel (n_mels, n_frames) f32 host.
@@ -229,6 +264,15 @@ int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out /* [cap] */, int32_
 /* generate_stream_generic (common/generate.rs:231-368) minus tokenizer / SSE framing: tokens are delivered through on_token. */
 int aha_b200_generate_stream(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm,
                              const aha_gen_params* params, aha_token_callback on_token, void* user, aha_usage* usage);
+/* aha_b200_generate / _generate_stream with one aha_logprobs record per generated token (params.flags must carry AHA_GEN_LOGPROBS;
+ * AHA_GEN_TOP_LOGPROBS(n) adds n alternatives).  out_logprobs: [cap] records, out_logprobs[i] belongs to out_tokens[i].  Tokens are
+ * exactly those of aha_b200_generate.  The records travel with the tokens, a burst at a time (the streaming variant: each behind its
+ * own step).  A handle allocates the record buffer the first time a request asks.  generate, generate_stream, generate_batch and
+ * asr_generate refuse the flag. */
+int aha_b200_generate_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                               uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap, size_t* n_out, aha_usage* usage);
+int aha_b200_generate_stream_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                                      aha_logprobs_callback on_token, void* user, aha_usage* usage);
 
 /* Qwen3AsrGenerateModel::generate / generate_stream (qwen3_asr/generate.rs:130-268): per-chunk loop, stop on either EOS id
  * (the handle's stop ids), KV cache cleared per chunk, one sampler for the whole request.  on_token may be NULL. */
@@ -351,7 +395,7 @@ int aha_b200_reset_stats(aha_model* m);
 /* Copy an internal activation to the host: what = "hidden" (text hidden states after layer `index`
  * of the last forward_initial, S*H floats; requires aha_b200_set_trace(m,1)), "vit" (ViT hidden after
  * block `index`), "image_embeds", "audio_embeds", "rope_delta" (1 float), "batch_graphs" (1 float: step graphs
- * captured in the open batch session; a wide session keeps at most one per running count). */
+ * captured in the open batch session: at most one per running count, two where requests asking for log-probabilities ran). */
 int aha_b200_set_trace(aha_model* m, int on);
 int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, size_t cap, size_t* n);
 /* Run n decode steps back to back on the device (graph replays, token feedback on device) without any
@@ -365,6 +409,8 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
 /* the device sampler on a given logits row (tests): context = tokens generated so far, draw_index = draws already consumed */
 int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_params* params, const uint32_t* context,
                           size_t n_context, uint32_t draw_index, uint32_t* token_out);
+/* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
+int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);
 /* Run ONE Linear layer y = epilogue(x W^T + b) through the library's GEMM dispatch on host data (unit tests of the
  * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 5 = the batched decode GEMV (M <= 8; its SwiGLU
