@@ -316,7 +316,8 @@ constexpr int kBatchGemvDefault = 2;
 
 // model.clear_cache(): pages, rope_deltas, and what the prefix cache remembered
 void drop_cache(aha_model* m) {
-    m->text.reset_pages();
+    m->text.pages.reset();
+    m->text.table.mapped = 0;
     m->have_rope_delta = false;  // qwen3vl/model.rs:1279-1282
     m->rope_delta = 0;
     m->cached_ids.clear();
@@ -338,8 +339,58 @@ void alloc_pack_buffers(aha_model* m) {
     m->d_pack_table = m->ctx.alloc<int>((size_t)T.num_pages);
 }
 
-// The multi-token forward (prefill).  Mirrors Qwen3Model::forward / Qwen3VLModel::forward / Qwen3ASRThinker::forward.
-void forward_prefill(aha_model* m, const uint32_t* ids, size_t S, size_t offset, const aha_mm* mm, bool initial) {
+// One packed prefill (embed_batch, batch_add_many): inputs [first, last) laid out in input order, input j starting at token start[j - first].
+// The first input starts at 0, every later one on the next multiple of the caller's alignment.  The gap behind an input is filled with token 0
+// and joins that input's segment: its rows come after every real row, so the causal mask keeps them out of the input's own rows.  The last
+// input of a pack is not padded.
+struct Pack {
+    size_t first = 0, last = 0;
+    size_t S = 0;                    // tokens in the pack
+    std::vector<size_t> start;
+    std::vector<uint32_t> ids;       // [S]
+    std::vector<int> pos3;           // [3][S]: positions restart at 0 in every segment
+    PrefillSegments sg;              // (start, length) of every segment; the work list's device copy is set by upload_pack
+    std::vector<int> work;           // [n_work][3] work list of flash_attn_tc_varlen
+    std::vector<int> rows;           // the last row of every input
+};
+// the pack that begins at input `first`: as many inputs as fit `cap` tokens, each starting on a multiple of `align`
+Pack plan_pack(const std::vector<const uint32_t*>& ids, const std::vector<size_t>& lens, size_t first, size_t align, size_t cap) {
+    Pack p;
+    p.first = p.last = first;
+    while (p.last < lens.size()) {
+        const size_t s0 = p.last == first ? 0 : (p.S + align - 1) / align * align;
+        if (s0 + lens[p.last] > cap) break;
+        p.start.push_back(s0);
+        p.S = s0 + lens[p.last++];
+    }
+    AHA_REQUIRE(p.last > first, "packed prefill: an input of " + std::to_string(lens[first]) + " tokens exceeds the pack capacity of " + std::to_string(cap));
+    const size_t S = p.S;
+    p.ids.assign(S, 0);
+    p.pos3.resize((size_t)3 * S);
+    for (size_t j = p.first; j < p.last; ++j) {
+        const int s0 = (int)p.start[j - first], len = (int)lens[j];
+        const int seg = (j + 1 < p.last ? (int)p.start[j + 1 - first] : (int)S) - s0;   // the input and the filler behind it
+        std::memcpy(p.ids.data() + s0, ids[j], (size_t)len * sizeof(uint32_t));
+        for (int k = 0; k < 3; ++k) for (int i = 0; i < seg; ++i) p.pos3[(size_t)k * S + s0 + i] = i;
+        p.sg.segs.emplace_back(s0, seg);
+        for (int q = 0; q < seg; q += kFaBQ) { p.work.push_back(s0); p.work.push_back(seg); p.work.push_back(q); }
+        p.rows.push_back(s0 + len - 1);
+    }
+    return p;
+}
+// the pack's ids, positions, work list and last rows to the device (synchronises: the host vectors are free after it)
+void upload_pack(aha_model* m, Pack& p) {
+    cudaStream_t st = m->ctx.stream;
+    p.sg.d_work = m->d_pack_work;
+    p.sg.n_work = (int)(p.work.size() / 3);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(m->text.d_ids, p.ids.data(), p.S * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, p.work.data(), p.work.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, p.rows.data(), p.rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    upload_pos(m, p.pos3);
+}
+
+// The multi-token forward (prefill) of the sequence of table `pt`.  Mirrors Qwen3Model::forward / Qwen3VLModel::forward / Qwen3ASRThinker::forward.
+void forward_prefill(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, size_t offset, const aha_mm* mm, bool initial) {
     TextModel& T = m->text;
     Ctx& c = m->ctx;
     upload_ids(m, ids, S);
@@ -442,30 +493,32 @@ void forward_prefill(aha_model* m, const uint32_t* ids, size_t S, size_t offset,
         for (int r = 0; r < 3; ++r) for (size_t i = 0; i < S; ++i) pos3[(size_t)r * S + i] = (int)(i + offset);
     }
     upload_pos(m, pos3);
-    T.prefill((int)S, (int)offset, embeds_ready, m->d_scatter_idx, n_visual, deepstack);
+    T.prefill(pt, (int)S, (int)offset, embeds_ready, m->d_scatter_idx, n_visual, deepstack);
 }
 
 // `extend`: prefill continuation (new design) -- S >= 1 further tokens against a cache that already holds `offset` tokens; the causal mask is
 // the (S, offset + S) one the reference never builds (its (S, S) mask makes a multi-token call with a non-empty cache fail, qwen3/model.rs:164-175).
-void forward_any(aha_model* m, const uint32_t* ids, size_t S, size_t offset, const aha_mm* mm, bool initial, float* logits_out, uint32_t* argmax_out,
-                 bool extend = false, bool force_prefill = false) {
+// `pt`: the sequence's page table.  The decode step runs on the model's own table only, so a single token on any other table (a batch slot's
+// first prefill) is prefilled.
+void forward_any(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, size_t offset, const aha_mm* mm, bool initial, float* logits_out,
+                 uint32_t* argmax_out, bool extend = false) {
     TextModel& T = m->text;
     AHA_REQUIRE(ids != nullptr && S >= 1, "input_ids must hold at least one token");
     AHA_REQUIRE(offset + S <= (size_t)T.max_ctx, "context exceeds max_ctx");
     const bool has_mm = initial && mm && ((m->kind == aha_model::QWEN3VL && (mm_entry(mm, 0) || mm_entry(mm, 2))) || (m->kind == aha_model::QWEN3_ASR && mm_entry(mm, 0)));
     if (initial && m->kind == aha_model::QWEN3VL) AHA_REQUIRE(mm && mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
     if (initial && m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(mm && mm->n == 1, "Qwen3 asr process data error, must have input_features");
-    if (S == 1 && !has_mm && !extend && !force_prefill && (m->kind != aha_model::QWEN3VL || m->have_rope_delta)) {
+    if (S == 1 && !has_mm && !extend && &pt == &T.table && (m->kind != aha_model::QWEN3VL || m->have_rope_delta)) {
         // decode step: single token against the cache
         AHA_REQUIRE(ids[0] < (uint32_t)T.cfg.V, "token id out of range");
-        T.ensure_tokens((int)offset + 1);
+        T.pages.map(T.table, (int)offset + 1);
         T.set_state(ids[0], (int)offset, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 0);
         T.decode_step(logits_out != nullptr);
     } else {
         // The reference builds an (S,S) causal mask with offset 0 for every multi-token call
         // (qwen3/model.rs:164-175); with a non-empty cache its broadcast_add against (S, off+S) scores fails.
         if (!extend) AHA_REQUIRE(offset == 0, "seq_len > 1 with seqlen_offset > 0 is not supported (the reference's mask shape rejects it too)");
-        else AHA_REQUIRE(offset <= (size_t)T.pages_mapped * kPage, "forward_extend: seqlen_offset is beyond the tokens in the cache");
+        else AHA_REQUIRE(offset <= (size_t)pt.mapped * kPage, "forward_extend: seqlen_offset is beyond the tokens in the cache");
         // A prompt longer than the activation workspace (max_prefill) runs as consecutive chunks against the growing cache: the first chunk is
         // the reference's call (multimodal rows are scattered there), the others are continuations.  Same K/V, same logits for the last token.
         const size_t chunk = (size_t)T.max_prefill;
@@ -479,8 +532,8 @@ void forward_any(aha_model* m, const uint32_t* ids, size_t S, size_t offset, con
                     for (size_t i = n; i < S; ++i) for (uint32_t t : mmt) AHA_REQUIRE(ids[i] != t, "prompt exceeds max_prefill before its last multimodal placeholder");
                 }
                 // (Qwen3-VL: get_rope_index over the first chunk yields the whole prompt's rope_delta, because only text follows the last placeholder)
-                forward_prefill(m, ids, n, offset, mm, initial);
-            } else forward_prefill(m, ids + done, n, offset + done, nullptr, false);
+                forward_prefill(m, pt, ids, n, offset, mm, initial);
+            } else forward_prefill(m, pt, ids + done, n, offset + done, nullptr, false);
             done += n;
         }
         T.finish_argmax(0);
@@ -592,15 +645,15 @@ int aha_b200_create(const char* kind, const char* config_json, const aha_tensor_
 
 int aha_b200_forward_initial(aha_model* m, const uint32_t* ids, size_t seq_len, size_t seqlen_offset, const aha_mm* mm, float* logits_out,
                              uint32_t* argmax_out) {
-    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, ids, seq_len, seqlen_offset, mm, true, logits_out, argmax_out); });
+    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, m->text.table, ids, seq_len, seqlen_offset, mm, true, logits_out, argmax_out); });
 }
 
 int aha_b200_forward_step(aha_model* m, const uint32_t* ids, size_t seq_len, size_t seqlen_offset, float* logits_out, uint32_t* argmax_out) {
-    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, ids, seq_len, seqlen_offset, nullptr, false, logits_out, argmax_out); });
+    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, m->text.table, ids, seq_len, seqlen_offset, nullptr, false, logits_out, argmax_out); });
 }
 
 int aha_b200_forward_extend(aha_model* m, const uint32_t* ids, size_t seq_len, size_t seqlen_offset, float* logits_out, uint32_t* argmax_out) {
-    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, ids, seq_len, seqlen_offset, nullptr, false, logits_out, argmax_out, true); });
+    return guarded(m, [&] { require_no_session(m); m->cached_ids.clear(); forward_any(m, m->text.table, ids, seq_len, seqlen_offset, nullptr, false, logits_out, argmax_out, true); });
 }
 
 size_t aha_b200_last_prefix_hit(aha_model* m) { return m ? m->last_prefix_hit : 0; }
@@ -692,8 +745,8 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     T.set_state(0, 0, 0, 0, draws0);    // empty history: the first token sees no repeat-penalty context
     auto is_eos = [&](uint32_t t) { for (uint32_t e : m->stop_ids) if (e == t) return true; return false; };
     uint32_t tok = 0;
-    if (hit > 0) forward_any(m, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
-    else forward_any(m, ids, seq_len, 0, mm, true, nullptr, &tok);   // forward_initial + sample_and_push
+    if (hit > 0) forward_any(m, T.table, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
+    else forward_any(m, T.table, ids, seq_len, 0, mm, true, nullptr, &tok);   // forward_initial + sample_and_push
     T.check_sample_error();
     if (lp) {   // the first token's record, from the prefill logits
         T.logprobs(true, T.d_lp, true);
@@ -706,7 +759,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     produced.push_back(tok);
     bool stop = sink.push(tok, 0, lp ? m->h_lp_pin : nullptr) || (eos_on_first && is_eos(tok));   // generate_generic never EOS-checks the first token; the ASR loop does
     if (sample_len > 1 && !stop) {
-        T.ensure_tokens((int)(seq_len + sample_len));
+        T.pages.map(T.table, (int)(seq_len + sample_len));
         DecodeState cur;
         AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
         T.set_state(tok, (int)seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 1, cur.n_draws);
@@ -762,18 +815,18 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
 }  // namespace
 
 namespace {
-// One request into slot `slot` of the batch decoder: the reference's forward_initial + sample_and_push on the slot's own page table (swapped into
-// the TextModel for the duration, so tower / M-RoPE / deepstack / sampler-on-prefill are the single-request code), then its decode state, history
-// and sampler move into the slot.  *swapped tells the caller's guard which table is swapped in if this throws.
-uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int lp_n, int* swapped) {
+// One request into slot `slot` of the batch decoder: the reference's forward_initial + sample_and_push on the slot's own page table (the
+// single-request code, so tower / M-RoPE / deepstack / sampler-on-prefill are shared), then its decode state, history and sampler move into the
+// slot.  If this throws, the slot's table holds whatever pages it took and the caller releases them with the slot.
+uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int lp_n) {
     TextModel& T = m->text;
     BatchDecoder& B = m->sess();
-    B.swap_table(slot); *swapped = slot;
+    PageTable& pt = B.slots[slot].table;
     m->have_rope_delta = false; m->rope_delta = 0;
     T.set_sampler(sampling_mode(r.params), r.params.temperature, r.params.top_p, r.params.top_k, r.params.repeat_penalty, r.params.repeat_last_n, r.params.seed);
     T.set_state(0, 0, 0, 0, 0);
     uint32_t tok = 0;
-    forward_any(m, r.ids, r.seq_len, 0, r.mm, true, nullptr, &tok, false, true);
+    forward_any(m, pt, r.ids, r.seq_len, 0, r.mm, true, nullptr, &tok);
     T.check_sample_error();
     if (lp_n >= 0) {   // the first token's record goes straight into the slot's record row
         T.set_logprobs(lp_n);
@@ -781,11 +834,10 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
         T.logprobs(true, B.d_lp_rec + slot, false);
     }
     B.slots[slot].lp = lp_n + 1;
-    T.ensure_tokens((int)(r.seq_len + sample_len));       // every page the request can touch is mapped now (the step kernels only read the table)
+    T.pages.map(pt, (int)(r.seq_len + sample_len));       // every page the request can touch is mapped now (the step kernels only read the table)
     DecodeState cur;
     AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
     B.adopt(slot, tok, (int)r.seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, cur.n_draws);
-    B.swap_table(slot); *swapped = -1;
     return tok;
 }
 
@@ -794,8 +846,7 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
 // free list at once, so a waiting request can take its place while the others keep decoding.
 void session_release(aha_model* m, int slot) {
     BatchSlot& sl = m->sess().slots[slot];
-    for (int k = 0; k < sl.mapped; ++k) m->text.free_pages.push_back(sl.h_table[k]);
-    sl.mapped = 0;
+    m->text.pages.release(sl.table);
     sl.samp_active = false;
     sl.lp = 0;
     m->session.used[slot] = false;
@@ -870,24 +921,19 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
         packed[i] = pack && !has_mm && r.seq_len <= (size_t)T.max_prefill;
     }
-    AHA_REQUIRE(pages <= T.free_pages.size(), who + "the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
-                                                  std::to_string(T.free_pages.size() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+    AHA_REQUIRE(pages <= T.pages.free_count(), who + "the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
+                                                   std::to_string(T.pages.free_count() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
     for (size_t i = 0; i < n; ++i) {   // (only reachable when max_ctx is not a multiple of the page)
         const size_t ctx = reqs[i].seq_len + sample_len[i];
         AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     }
     using clk = std::chrono::steady_clock;
     const auto t0 = clk::now();
-    struct Guard {   // a failure leaves the session as it was: the model's own page table back in place, every slot this call took released
+    struct Guard {   // a failure leaves the session as it was: every slot this call took is released with its pages
         aha_model* m; const std::vector<int>& slots;
-        int swapped = -1;                                    // slot whose table is swapped into the TextModel
-        bool pack_in = false; std::vector<int> h; int mapped = 0; int* d = nullptr;   // a pack's table, or the model's own while the pack's is in
         bool ok = false;
-        void swap_pack() { TextModel& T = m->text; std::swap(T.h_page_table, h); std::swap(T.pages_mapped, mapped); std::swap(T.d_page_table, d); pack_in = !pack_in; }
         ~Guard() {
-            if (pack_in) swap_pack();
             if (ok) return;
-            if (swapped >= 0) m->sess().swap_table(swapped);
             for (int s : slots) { session_release(m, s); m->session.lp_valid[s] = false; }
             m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
         }
@@ -897,60 +943,35 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     std::vector<double> secs(n), vision(n, 0.0);
     // ---- packed requests: map every page each can touch (as batch_prefill_slot does after its prefill), then prefill them pack by pack
     std::vector<size_t> pk;
+    std::vector<const uint32_t*> pk_ids;
+    std::vector<size_t> pk_lens;
     for (size_t i = 0; i < n; ++i) {
         if (!packed[i]) continue;
-        pk.push_back(i);
-        B.swap_table(slot[i]); guard.swapped = slot[i];
-        T.ensure_tokens((int)(reqs[i].seq_len + sample_len[i]));
-        B.swap_table(slot[i]); guard.swapped = -1;
+        pk.push_back(i); pk_ids.push_back(reqs[i].ids); pk_lens.push_back(reqs[i].seq_len);
+        T.pages.map(B.slots[slot[i]].table, (int)(reqs[i].seq_len + sample_len[i]));
     }
     if (!pk.empty()) {
         alloc_pack_buffers(m);
         const int H = T.cfg.H;
         const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
-        size_t first = 0;
-        while (first < pk.size()) {
-            size_t last = first, S = 0;
-            std::vector<size_t> start;
-            while (last < pk.size()) {
-                const size_t s0 = last == first ? 0 : (S + kPage - 1) / kPage * kPage;
-                if (s0 + reqs[pk[last]].seq_len > cap) break;   // every packed request fits a pack on its own
-                start.push_back(s0);
-                S = s0 + reqs[pk[last++]].seq_len;
+        for (size_t first = 0; first < pk.size();) {
+            Pack p = plan_pack(pk_ids, pk_lens, first, kPage, cap);
+            // the pack's table: the requests' own pages laid end to end, all mapped above, so the prefill takes no page from the pool
+            PageTable pt;
+            for (size_t j = p.first; j < p.last; ++j) {
+                const std::vector<int>& own = B.slots[slot[pk[j]]].table.h;
+                pt.h.insert(pt.h.end(), own.begin(), own.begin() + ceil_div(p.sg.segs[j - p.first].second, kPage));
             }
-            PrefillSegments sg;
-            std::vector<uint32_t> ids(S, 0);
-            std::vector<int> pos3((size_t)3 * S), work, rows, table;
-            for (size_t j = first; j < last; ++j) {
-                const aha_batch_request& r = reqs[pk[j]];
-                const int s0 = (int)start[j - first], len = (int)r.seq_len;
-                const int seg = (j + 1 < last ? (int)start[j + 1 - first] : (int)S) - s0;   // the request and the filler behind it
-                std::memcpy(ids.data() + s0, r.ids, (size_t)len * sizeof(uint32_t));
-                for (int k = 0; k < 3; ++k) for (int i = 0; i < seg; ++i) pos3[(size_t)k * S + s0 + i] = i;
-                sg.segs.emplace_back(s0, seg);
-                for (int q = 0; q < seg; q += kFaBQ) { work.push_back(s0); work.push_back(seg); work.push_back(q); }
-                rows.push_back(s0 + len - 1);
-                const BatchSlot& bs = B.slots[slot[pk[j]]];
-                for (int p = 0; p < ceil_div(seg, kPage); ++p) table.push_back(bs.h_table[p]);
-            }
-            sg.d_work = m->d_pack_work;
-            sg.n_work = (int)(work.size() / 3);
-            AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_ids, ids.data(), S * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, work.data(), work.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_table, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-            upload_pos(m, pos3);   // (synchronises: the host vectors above are free after it)
-            // the pack's table stands in for the model's own while it prefills; every page is mapped, so ensure_tokens takes none
-            guard.mapped = (int)table.size();
-            table.resize(T.num_pages, 0);
-            guard.h.swap(table);
-            guard.d = m->d_pack_table;
-            guard.swap_pack();
-            T.prefill((int)S, 0, false, nullptr, 0, {}, sg);
-            guard.swap_pack();
-            gather_rows_kernel<<<(unsigned)(last - first), 256, 0, c.stream>>>(m->d_pack_rows, T.x, B.xb + first * H, H);
+            pt.mapped = (int)pt.h.size();
+            AHA_REQUIRE(ceil_div((int)p.S, kPage) <= pt.mapped, "batch_add_many: the pack's page table does not cover the pack");
+            pt.h.resize(T.num_pages, 0);
+            pt.d = m->d_pack_table;
+            AHA_CUDA_CHECK(cudaMemcpyAsync(pt.d, pt.h.data(), (size_t)pt.mapped * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            upload_pack(m, p);
+            T.prefill(pt, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
+            gather_rows_kernel<<<(unsigned)(p.last - p.first), 256, 0, c.stream>>>(m->d_pack_rows, T.x, B.xb + p.first * H, H);
             c.cnt.kernels++;
-            first = last;
+            first = p.last;
         }
         // first tokens: batched lm_head over the gathered rows, then each request's ArgMax / sampler against an empty state (forward_any's draw)
         std::vector<int> act;
@@ -983,7 +1004,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     // ---- the others: one prefill each, on the slot's own table
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
-        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i], &guard.swapped);
+        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i]);
         secs[i] = std::chrono::duration<double>(clk::now() - t0).count();
         vision[i] = m->last_vision_secs;
     }
@@ -1298,7 +1319,7 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
         AHA_REQUIRE(seqlen_offset + n_steps <= (size_t)T.max_ctx, "context exceeds max_ctx");
         require_no_session(m);
         m->cached_ids.clear();
-        T.ensure_tokens((int)(seqlen_offset + n_steps));
+        T.pages.map(T.table, (int)(seqlen_offset + n_steps));
         T.set_state(first_token, (int)seqlen_offset, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 0);
         if (n_steps > 0 && !T.step_graph && T.use_graph) {  // build the graph outside the timed region (pos is restored below)
             T.decode_step();
@@ -1769,7 +1790,7 @@ void embed_one(aha_model* m, const uint32_t* ids, size_t S, float* out) {
     std::vector<int> pos3((size_t)3 * S);
     for (int r = 0; r < 3; ++r) for (size_t i = 0; i < S; ++i) pos3[(size_t)r * S + i] = (int)i;
     upload_pos(m, pos3);
-    T.prefill((int)S, 0, false, nullptr, 0, {});
+    T.prefill(T.table, (int)S, 0, false, nullptr, 0, {});
     const int H = T.cfg.H;
     rmsnorm_kernel<<<1, 256, 0, m->ctx.stream>>>(T.x + (size_t)(S - 1) * H, T.norm, T.cfg.eps, T.xn, H);
     l2_normalize_kernel<<<1, 256, 0, m->ctx.stream>>>(T.xn, T.xn + H, H);
@@ -1790,9 +1811,11 @@ void embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n
     AHA_REQUIRE(ids && lens && out, "ids, lens and out are required");
     TextModel& T = m->text;
     AHA_REQUIRE(T.tp_world == 1, "embed_batch is single-GPU (tp_world must be 1)");
+    std::vector<const uint32_t*> text_ids(n);
     size_t total = 0;
     for (size_t j = 0; j < n; ++j) {
         const size_t S = lens[j];
+        text_ids[j] = ids + total;
         AHA_REQUIRE(S >= 1, "empty input_ids");
         AHA_REQUIRE(S <= (size_t)T.max_prefill, "prompt of " + std::to_string(S) + " tokens exceeds max_prefill " + std::to_string(T.max_prefill));
         AHA_REQUIRE(S <= (size_t)T.max_ctx, "context of " + std::to_string(S) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
@@ -1804,49 +1827,22 @@ void embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n
     const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
     const int H = T.cfg.H;
     drop_cache(m);
-    size_t first = 0, off = 0;
-    while (first < n) {
-        // Texts start on multiples of kPackAlign tokens: a segment's start is the innermost TMA coordinate of the attention kernel's V^T tiles,
-        // which has to sit on a 16-byte boundary.  The gap after a text is filled with token 0 and joins that text's segment: its rows come after
-        // every real row, so the causal mask keeps them out of the text's own rows, and the text's KV tiles and query tiles stay the same (a
-        // 16-token round-up never crosses a 64-token boundary).  The last text of a pack is not padded.
-        constexpr size_t kPackAlign = 16;
-        size_t last = first, S = 0;
-        std::vector<size_t> start;
-        while (last < n) {
-            const size_t s0 = last == first ? 0 : (S + kPackAlign - 1) / kPackAlign * kPackAlign;
-            if (s0 + lens[last] > cap) break;   // every text fits a pack on its own (checked above)
-            start.push_back(s0);
-            S = s0 + lens[last++];
-        }
-        PrefillSegments sg;
-        std::vector<uint32_t> pack_ids(S, 0);
-        std::vector<int> pos3((size_t)3 * S), work, rows;
-        for (size_t j = first; j < last; ++j) {
-            const int s0 = (int)start[j - first], len = (int)lens[j];
-            const int seg = (j + 1 < last ? (int)start[j + 1 - first] : (int)S) - s0;   // the text and the filler behind it
-            std::memcpy(pack_ids.data() + s0, ids + off, (size_t)len * sizeof(uint32_t));
-            off += len;
-            for (int r = 0; r < 3; ++r) for (int i = 0; i < seg; ++i) pos3[(size_t)r * S + s0 + i] = i;
-            sg.segs.emplace_back(s0, seg);
-            for (int q = 0; q < seg; q += kFaBQ) { work.push_back(s0); work.push_back(seg); work.push_back(q); }
-            rows.push_back(s0 + len - 1);
-        }
-        sg.d_work = m->d_pack_work;
-        sg.n_work = (int)(work.size() / 3);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_ids, pack_ids.data(), S * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, work.data(), work.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, rows.data(), rows.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-        upload_pos(m, pos3);
-        T.prefill((int)S, 0, false, nullptr, 0, {}, sg);
-        const int np = (int)(last - first);
+    const std::vector<size_t> text_lens(lens, lens + n);
+    for (size_t first = 0; first < n;) {
+        // Texts start on multiples of 16 tokens: a segment's start is the innermost TMA coordinate of the attention kernel's V^T tiles, which
+        // has to sit on a 16-byte boundary.  A text's KV tiles and query tiles stay the ones it runs alone (a 16-token round-up never crosses a
+        // 64-token boundary).
+        Pack p = plan_pack(text_ids, text_lens, first, 16, cap);
+        upload_pack(m, p);
+        T.prefill(T.table, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
+        const int np = (int)(p.last - first);
         gather_rows_kernel<<<np, 256, 0, c.stream>>>(m->d_pack_rows, T.x, T.xn, H);
         rmsnorm_kernel<<<np, 256, 0, c.stream>>>(T.xn, T.norm, T.cfg.eps, T.x, H);
         l2_normalize_kernel<<<np, 256, 0, c.stream>>>(T.x, T.xn, H);
         c.cnt.kernels += 3;
         AHA_CUDA_CHECK(cudaMemcpyAsync(out + first * H, T.xn, (size_t)np * H * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-        first = last;
+        first = p.last;
     }
     drop_cache(m);
 }

@@ -1,8 +1,9 @@
 // batch_decode.cuh -- several sequences decoded in lockstep on one handle (SURVEY 8f rank 4, second half).
 //
 // The reference holds one request at a time behind a lock (src/server/api.rs:117) and every decode step
-// streams all weights for ONE token.  Here several sequences share a step: each has its own page table over the common paged KV pool
-// (text_model.cuh), its own DecodeState (token, position, rope_delta, sampler draw index), history and sampler parameters; a step is
+// streams all weights for ONE token.  Here several sequences share a step: each slot owns a PageTable over the common paged KV pool
+// (text_model.cuh; the TextModel's PagePool maps its pages when it is admitted, its prefill writes through that table, and the pool takes the
+// pages back when it is released), its own DecodeState (token, position, rope_delta, sampler draw index), history and sampler parameters; a step is
 //     [embedding]      embed_rows_kernel        row j <- the last token of slot act[j]
 // then per layer
 //     [rmsnorm + qkv]  projection               all sequences, every weight row read once
@@ -32,9 +33,7 @@
 namespace aha {
 
 struct BatchSlot {                       // one sequence of the batch
-    std::vector<int> h_table;            // its page table (host copy), swapped into the TextModel while the sequence prefills
-    int mapped = 0;
-    int* d_table = nullptr;              // device copy: row of BatchDecoder::d_tables
+    PageTable table;                     // its pages, which it holds from its prefill until it is released; device copy: row of BatchDecoder::d_tables
     bool samp_active = false;
     SampleArgs samp{};                   // sampler of the request with the pointers of this slot
     int lp = 0;                          // 0: the request asked for no log-probabilities, else 1 + its top count
@@ -79,7 +78,7 @@ struct BatchDecoder {
     void composition_changed() { table_for.clear(); }
     // no sequence holds a slot any more (a session opens or closes)
     void reset() {
-        for (auto& sl : slots) { sl.mapped = 0; sl.lp = 0; }
+        for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; }
         table_for.clear();
         lp_any = false;
         clear_graphs();
@@ -146,15 +145,7 @@ struct BatchDecoder {
         d_samp_on = c.alloc<int>(n);
         workb = c.alloc<float>((size_t)n * cf.V);
         slots.resize(n);
-        for (int i = 0; i < n; ++i) { slots[i].h_table.assign(t.num_pages, 0); slots[i].d_table = d_tables + (size_t)i * t.num_pages; }
-    }
-
-    // While slot i prefills, the TextModel's own page-table members are this slot's (prefill / ensure_tokens / kv_src work on them unchanged)
-    void swap_table(int i) {
-        BatchSlot& s = slots[i];
-        std::swap(T->h_page_table, s.h_table);
-        std::swap(T->pages_mapped, s.mapped);
-        std::swap(T->d_page_table, s.d_table);
+        for (int i = 0; i < n; ++i) { slots[i].table.h.assign(t.num_pages, 0); slots[i].table.d = d_tables + (size_t)i * t.num_pages; }
     }
 
     // after the prefill of slot i (the model's d_state / d_history / samp hold the request's state): move it into the slot
@@ -197,13 +188,13 @@ struct BatchDecoder {
         const float scaling = (float)(1.0 / std::sqrt((double)cf.hd));
         for (int l = 0; l < cf.L; ++l) {
             TextLayer& Ly = T->layers[l];
-            KVSrc kv = T->kv_src(l);
             for (int j = 0; j < nb; ++j) {
                 DecodeAttnArgs d{};
                 const int slot = act[j];
+                const KVSrc kv = T->kv_src(l, slots[slot].table);
                 d.qkv = qkvb + (size_t)j * T->qkv_dim; d.qw = Ly.qn; d.kw = Ly.kn; d.eps = cf.eps; d.inv_freq = T->inv_freq; d.st = d_states + slot;
                 d.kbase = const_cast<float*>(kv.k); d.vbase = const_cast<float*>(kv.v);
-                d.kv = kv; d.kv.page_table = d_tables + (size_t)slot * T->num_pages;
+                d.kv = kv;
                 d.partial = partialb + (size_t)j * T->nh_l * kDecodeSplits * (cf.hd + 2);
                 d.counters = countersb + (size_t)j * T->nkv_l;
                 d.out = attnb + (size_t)j * T->nh_l * cf.hd;

@@ -186,7 +186,7 @@ inline void flash_dispatch(Ctx& c, const FlashArgs& a, int nheads, bool causal) 
 }
 
 // Independent texts packed into one prefill (aha_b200_embed_batch, aha_b200_batch_add_many): each text attends only to itself, its RoPE
-// positions restart at 0 and its K/V take the packed cache slots [start, start + len) (which the page table in place maps to the text's own pages
+// positions restart at 0 and its K/V take the packed cache slots [start, start + len) (which the pack's page table maps to the text's own pages
 // when batch_add_many composes it from the requests' slots).
 struct PrefillSegments {
     std::vector<std::pair<int, int>> segs;   // (start, len) of every text, in pack order
@@ -367,6 +367,46 @@ struct TextLayer {
 
 constexpr int kDecodeSplits = 16;        // split-KV factor of the decode attention
 
+// One sequence's logical -> physical map over the paged KV pool: entry p of `h` is the pool page of the sequence's tokens
+// [p * kPage, (p + 1) * kPage); entries 0 .. mapped-1 hold pages, and `d` is the device copy the kernels read.
+struct PageTable {
+    std::vector<int> h;
+    int mapped = 0;
+    int* d = nullptr;
+};
+
+// The free pages of the KV pool.  Only the pool takes pages from the free list or gives them back.  Pages are handed out from the END of
+// the pool, so the logical -> physical mapping is never the identity (the indirection is always exercised).
+struct PagePool {
+    int num_pages = 0, max_ctx = 0;
+    cudaStream_t stream = nullptr;
+    std::vector<int> free;
+    size_t free_count() const { return free.size(); }
+    // every page free again; the tables that held pages must drop them (mapped = 0) themselves
+    void reset() {
+        free.clear();
+        for (int p = 0; p < num_pages; ++p) free.push_back(p);
+    }
+    // map pages to `t` until it covers n_tokens, and upload the new entries
+    void map(PageTable& t, int n_tokens) {
+        AHA_REQUIRE(n_tokens <= max_ctx, "context of " + std::to_string(n_tokens) + " tokens exceeds max_ctx " + std::to_string(max_ctx));
+        const int need = ceil_div(n_tokens, kPage);
+        if (need <= t.mapped) return;
+        AHA_REQUIRE((size_t)(need - t.mapped) <= free.size(), "KV pool exhausted: " + std::to_string(need - t.mapped) + " more pages needed, " +
+                                                                   std::to_string(free.size()) + " are free");
+        const int first = t.mapped;
+        while (t.mapped < need) {
+            t.h[t.mapped++] = free.back();
+            free.pop_back();
+        }
+        AHA_CUDA_CHECK(cudaMemcpyAsync(t.d + first, t.h.data() + first, (size_t)(t.mapped - first) * sizeof(int), cudaMemcpyHostToDevice, stream));
+    }
+    void release(PageTable& t) {
+        for (int k = 0; k < t.mapped; ++k) free.push_back(t.h[k]);
+        t.mapped = 0;
+    }
+};
+
 struct TextModel {
     TextCfg cfg;
     Ctx* ctx = nullptr;
@@ -386,9 +426,8 @@ struct TextModel {
     int max_ctx = 0, num_pages = 0;
     float* kv_pool = nullptr;
     size_t layer_stride = 0, page_stride = 0;
-    int* d_page_table = nullptr;
-    std::vector<int> h_page_table, free_pages;
-    int pages_mapped = 0;
+    PagePool pages;
+    PageTable table;                  // the single-request path's sequence: its prefills and its decode step
 
     // prefill workspaces
     int max_prefill = 0;
@@ -565,9 +604,10 @@ struct TextModel {
         layer_stride = page_stride * num_pages;
         kv_pool = c.alloc<float>(layer_stride * cfg.L);
         AHA_CUDA_CHECK(cudaMemset(kv_pool, 0, layer_stride * cfg.L * sizeof(float)));   // never feed uninitialised bits to the FMA pipes
-        d_page_table = c.alloc<int>(num_pages);
-        h_page_table.assign(num_pages, 0);
-        reset_pages();
+        pages.num_pages = num_pages; pages.max_ctx = max_ctx; pages.stream = c.stream;
+        pages.reset();
+        table.h.assign(num_pages, 0);
+        table.d = c.alloc<int>(num_pages);
         const size_t S = max_prefill;
         x = c.alloc<float>(S * cfg.H); xn = c.alloc<float>(S * cfg.H);
         qkv = c.alloc<float>(S * qkv_dim); attn = c.alloc<float>(S * nh_l * cfg.hd); hbuf = c.alloc<float>(S * I_l);
@@ -630,30 +670,12 @@ struct TextModel {
         trace = on;
     }
 
-    // ---- paged KV management (host side).  Physical pages are handed out from the END of the pool so the
-    // logical->physical mapping is never the identity (the indirection is always exercised).
-    void reset_pages() {
-        free_pages.clear();
-        for (int p = 0; p < num_pages; ++p) free_pages.push_back(p);
-        pages_mapped = 0;
-    }
-    void ensure_tokens(int n_tokens) {
-        AHA_REQUIRE(n_tokens <= max_ctx, "context of " + std::to_string(n_tokens) + " tokens exceeds max_ctx " + std::to_string(max_ctx));
-        const int need = ceil_div(n_tokens, kPage);
-        if (need <= pages_mapped) return;
-        const int first = pages_mapped;
-        while (pages_mapped < need) {
-            h_page_table[pages_mapped++] = free_pages.back();
-            free_pages.pop_back();
-        }
-        AHA_CUDA_CHECK(cudaMemcpyAsync(d_page_table + first, h_page_table.data() + first, (size_t)(pages_mapped - first) * sizeof(int),
-                                       cudaMemcpyHostToDevice, ctx->stream));
-    }
-    KVSrc kv_src(int layer) const {
+    // layer `layer` of the paged KV cache as the sequence of table `t` sees it
+    KVSrc kv_src(int layer, const PageTable& t) const {
         KVSrc s;
         s.k = kv_pool + (size_t)layer * layer_stride;
         s.v = s.k + (size_t)nkv_l * kPage * cfg.hd;
-        s.page_table = d_page_table; s.page_shift = kPageShift; s.page_stride = page_stride;
+        s.page_table = t.d; s.page_shift = kPageShift; s.page_stride = page_stride;
         s.tok_stride = cfg.hd; s.head_stride = (size_t)kPage * cfg.hd;
         return s;
     }
@@ -707,18 +729,19 @@ struct TextModel {
         ctx->cnt.kernels++;
     }
 
-    // ---- prefill: ids already on device in d_ids (or embeddings already in x when embeds_ready), pos3 in d_pos3.
+    // ---- prefill of tokens pos0 .. pos0+S-1 of the sequence of table `pt` (pages are mapped as needed): ids already on device in d_ids (or
+    // embeddings already in x when embeds_ready), pos3 in d_pos3.
     // visual_idx/deepstack: Qwen3-VL deepstack injection (qwen3vl/model.rs:815-824).
     // segs (packed prefills): the S tokens are independent texts; attention stays inside each one and no logits are computed (head() is skipped;
     // the caller takes the rows it needs from x).
-    void prefill(int S, int pos0, bool embeds_ready, const int* d_visual_idx, int n_visual, const std::vector<const float*>& deepstack,
+    void prefill(PageTable& pt, int S, int pos0, bool embeds_ready, const int* d_visual_idx, int n_visual, const std::vector<const float*>& deepstack,
                  const PrefillSegments& segs = PrefillSegments()) {
         Ctx& c = *ctx;
         cudaStream_t st = c.stream;
         const int H = cfg.H, hd = cfg.hd;
         AHA_REQUIRE(S <= max_prefill, "prompt of " + std::to_string(S) + " tokens exceeds max_prefill " + std::to_string(max_prefill));
         AHA_REQUIRE(segs.empty() || pos0 == 0, "packed segments start from an empty cache");
-        ensure_tokens(pos0 + S);
+        pages.map(pt, pos0 + S);
         if (!embeds_ready) { embed_gather_kernel<<<S, 256, 0, st>>>(d_ids, embed, x, S, H, cfg.V); c.cnt.kernels++; }
         RopeArgs rp{inv_freq, mrope_sel, d_pos3, S};
         const float scaling = (float)(1.0 / std::sqrt((double)hd));
@@ -735,7 +758,7 @@ struct TextModel {
                 rmsnorm_kernel<<<S, 256, 0, st>>>(x, T.ln1, cfg.eps, xn, H); c.cnt.kernels++;
                 gemm(EPI_STORE, xn, H, T.qkv, nullptr, 0, qkv, qkv_dim, S);
             }
-            KVSrc kv = kv_src(l);
+            KVSrc kv = kv_src(l, pt);
             qk_norm_rope_kv_kernel<128><<<dim3(S, nh_l + 2 * nkv_l), 128, 0, st>>>(qkv, T.qn, T.kn, cfg.eps, rp, const_cast<float*>(kv.k), const_cast<float*>(kv.v), kv, nh_l, nkv_l, pos0);
             c.cnt.kernels++;
             FlashArgs fa;
@@ -802,7 +825,7 @@ struct TextModel {
             GemvArgs a{};
             a.W = T.qkv.w; a.bias = T.qkv.b; a.x = x1; a.norm_w = T.ln1; a.eps = cfg.eps; a.out = qkv1; a.N = T.qkv.N; a.K = T.qkv.K;
             gemv(st, PRO_RMSNORM, GEPI_STORE, a); c.cnt.kernels++;
-            KVSrc kv = kv_src(l);
+            KVSrc kv = kv_src(l, table);
             DecodeAttnArgs d{};
             d.qkv = qkv1; d.qw = T.qn; d.kw = T.kn; d.eps = cfg.eps; d.inv_freq = inv_freq; d.st = d_state;
             d.kbase = const_cast<float*>(kv.k); d.vbase = const_cast<float*>(kv.v); d.kv = kv;
@@ -844,7 +867,7 @@ struct TextModel {
         fa.x = x1; fa.qkv1 = qkv1; fa.h1 = h1; fa.logits = logits; fa.partial = partial;
         fa.sync = d_sync; fa.pmax = pmax; fa.pidx = pidx; fa.argmax_out = d_argmax;
         fa.history = d_history; fa.hist_cap = hist_cap; fa.kv_pool = kv_pool; fa.layer_stride = layer_stride; fa.page_stride = page_stride;
-        fa.page_table = d_page_table; fa.nsplit = fused_nsplit;
+        fa.page_table = table.d; fa.nsplit = fused_nsplit;
         { const char* e = getenv("AHA_FUSED_DBG"); fa.dbg = e ? atoi(e) : 0; }
         fa.trace = d_ftrace;
         { const char* e = getenv("AHA_FUSED_STAGES"); fa.stages = e ? std::max(2, std::min(kFusedStages, atoi(e))) : fused_stages; }
