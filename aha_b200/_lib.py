@@ -76,6 +76,40 @@ def logprobs_record(r):
 LOGPROBS_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Logprobs))
 
 
+SPEC_PROMPT_LOOKUP = 1
+SPEC_MAX_DRAFT = 15
+SPEC_MAX_NGRAM = 8
+
+
+class SpecParams(C.Structure):
+    _fields_ = [("prediction", C.POINTER(C.c_uint32)), ("n_prediction", C.c_size_t), ("max_draft", C.c_uint32), ("ngram", C.c_uint32),
+                ("flags", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+
+
+class SpecStats(C.Structure):
+    _fields_ = [("passes", C.c_uint32), ("drafted", C.c_uint32), ("accepted", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+def spec_params(prediction=None, prompt_lookup=False, max_draft=7, ngram=3, vocab_size=None):
+    """(SpecParams, prediction array to keep alive) of a speculative request, checked the way the library checks them."""
+    for name, v, lo, hi in (("max_draft", max_draft, 1, SPEC_MAX_DRAFT), ("ngram", ngram, 0, SPEC_MAX_NGRAM)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise TypeError(f"{name} must be an int, not {type(v).__name__}")
+        if not lo <= int(v) <= hi:
+            raise ValueError(f"{name} must be {lo} to {hi}, got {int(v)}")
+    pred = np.zeros(0, np.uint32)
+    if prediction is not None:
+        p = np.asarray(prediction).reshape(-1)
+        if p.size and not np.issubdtype(p.dtype, np.integer):
+            raise TypeError("prediction must hold token ids (integers)")
+        if p.size and (p.min() < 0 or (vocab_size is not None and p.max() >= vocab_size)):
+            raise ValueError("prediction token id out of range")
+        pred = np.ascontiguousarray(p.astype(np.uint32))
+    sp = SpecParams(prediction=pred.ctypes.data_as(C.POINTER(C.c_uint32)) if pred.size else None, n_prediction=pred.size,
+                    max_draft=int(max_draft), ngram=int(ngram), flags=SPEC_PROMPT_LOOKUP if prompt_lookup else 0)
+    return sp, pred
+
+
 class AsrChunk(C.Structure):
     _fields_ = [("ids", C.POINTER(C.c_uint32)), ("seq_len", C.c_size_t), ("input_features", TensorDesc)]
 
@@ -118,6 +152,9 @@ SYMBOLS = {
     "aha_b200_generate_stream_logprobs": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), LOGPROBS_CALLBACK, C.c_void_p,
                                                     C.POINTER(Usage)]),
     "aha_b200_batch_logprobs": (C.c_int, [_P, C.POINTER(Logprobs), C.c_size_t]),
+    "aha_b200_generate_speculative": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), C.POINTER(SpecParams), _U32P,
+                                                C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage), C.POINTER(SpecStats)]),
+    "aha_b200_debug_verify_attn": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _F32P, _F32P, _F32P]),
     "aha_b200_debug_logprobs": (C.c_int, [_P, _F32P, C.c_size_t, C.c_uint32, C.c_uint32, C.POINTER(Logprobs)]),
     "aha_b200_generate_batch": (C.c_int, [_P, C.POINTER(BatchRequest), C.c_size_t, _U32P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
     "aha_b200_batch_open": (C.c_int, [_P]),

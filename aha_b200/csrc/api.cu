@@ -13,6 +13,7 @@
 #include "preprocess.cuh"
 #include "text_model.cuh"
 #include "batch_decode.cuh"
+#include "speculative.cuh"
 #include "vision_model.cuh"
 
 using namespace aha;
@@ -65,6 +66,7 @@ struct aha_model {
         bool lp_valid[kWideSeqs] = {};  // the slot's record row holds the record of the last token its request delivered
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
+    SpecDecoder spec;                   // speculative single requests (aha_b200_generate_speculative) on wide_batch's buffers
 };
 
 namespace {
@@ -812,6 +814,94 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     }
 }
 
+// generate_impl's request in verify passes (speculative.cuh): the same prefill, first token, Reset guard and Usage split; then passes of
+// R = max_draft + 1 rows in bursts, the emitted tokens (and records) read from the request's history after each burst.
+void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params& params,
+                               const aha_spec_params& sp, uint32_t* out_tokens, aha_logprobs* out_lp, size_t cap, size_t* n_out, aha_usage* usage,
+                               aha_spec_stats* stats) {
+    TextModel& T = m->text;
+    const std::string who = "generate_speculative: ";
+    AHA_REQUIRE(T.tp_world == 1, who + "speculative decoding is single-GPU");
+    require_no_session(m);
+    AHA_REQUIRE(m->kind != aha_model::QWEN3_ASR, who + "Qwen3-ASR handles decode through asr_generate");
+    AHA_REQUIRE(BatchDecoder::wide_shapes_ok(T) && T.cfg.hd == 128,
+                who + "every projection's rows and columns must be multiples of 64 and head_dim 128 (hidden " + std::to_string(T.cfg.H) +
+                    ", intermediate " + std::to_string(T.I_l) + ", qkv rows " + std::to_string(T.qkv_dim) + ", vocabulary " + std::to_string(T.cfg.V) + ")");
+    AHA_REQUIRE(sp.max_draft >= 1 && sp.max_draft <= (uint32_t)(kSpecMaxRows - 1), who + "max_draft must be 1 to " + std::to_string(kSpecMaxRows - 1));
+    const int ngram = sp.ngram == 0 ? kSpecDefaultNgram : (int)sp.ngram;
+    AHA_REQUIRE(ngram >= 1 && ngram <= kSpecMaxNgram, who + "ngram must be 0 (default " + std::to_string(kSpecDefaultNgram) + ") to " + std::to_string(kSpecMaxNgram));
+    AHA_REQUIRE((sp.flags & ~AHA_SPEC_PROMPT_LOOKUP) == 0, who + "unknown spec flags");
+    AHA_REQUIRE(sp.prediction || sp.n_prediction == 0, who + "prediction is NULL but n_prediction is not 0");
+    for (size_t i = 0; i < sp.n_prediction; ++i) AHA_REQUIRE(sp.prediction[i] < (uint32_t)T.cfg.V, who + "prediction token id out of range");
+    AHA_REQUIRE((params.flags & (AHA_GEN_REUSE_PREFIX | AHA_GEN_CONTINUE_RNG | AHA_GEN_EOS_ON_FIRST)) == 0,
+                who + "REUSE_PREFIX, CONTINUE_RNG and EOS_ON_FIRST are not supported with speculative decoding");
+    const int lp_n = logprob_request(params, T, who);
+    AHA_REQUIRE(lp_n < 0 || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
+    const size_t sample_len = std::max<size_t>(params.max_tokens, 1);
+    AHA_REQUIRE(cap >= sample_len, who + "out_tokens capacity is smaller than max_tokens");
+    const size_t need = seq_len + sample_len + sp.max_draft;
+    AHA_REQUIRE(need <= (size_t)T.max_ctx, who + "prompt + max_tokens + max_draft = " + std::to_string(need) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+    const int R = (int)sp.max_draft + 1;
+    SpecDecoder& S = m->spec;
+    S.init(T, m->wide_batch);
+    if (lp_n >= 0) {
+        T.set_logprobs(lp_n);
+        if (!m->h_lp_pin) AHA_CUDA_CHECK(cudaMallocHost(&m->h_lp_pin, 32 * sizeof(aha_logprobs)));
+    }
+    using clk = std::chrono::steady_clock;
+    const auto t0 = clk::now();
+    drop_cache(m);
+    m->last_prefix_hit = 0;
+    struct Reset {
+        aha_model* m;
+        ~Reset() { drop_cache(m); m->text.clear_sampler(); }
+    } reset{m};
+    T.set_sampler(sampling_mode(params), params.temperature, params.top_p, params.top_k, params.repeat_penalty, params.repeat_last_n, params.seed);
+    T.set_state(0, 0, 0, 0, 0);
+    uint32_t tok = 0;
+    forward_any(m, T.table, ids, seq_len, 0, mm, true, nullptr, &tok);
+    T.check_sample_error();
+    if (lp_n >= 0) T.logprobs(true, T.d_lp, true);   // record 0, from the prefill logits
+    const auto t1 = clk::now();
+    const double vision_secs = m->last_vision_secs;
+    SpecCtl ctl{};
+    size_t E = 1;
+    if (sample_len > 1) {
+        T.pages.map(T.table, (int)need);
+        DecodeState cur;
+        AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
+        T.set_state(tok, (int)seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 1, cur.n_draws);
+        AHA_CUDA_CHECK(cudaMemcpy(T.d_history, &tok, sizeof(uint32_t), cudaMemcpyHostToDevice));
+        const std::vector<uint32_t> pred(sp.prediction, sp.prediction + sp.n_prediction);
+        const bool lookup = (sp.flags & AHA_SPEC_PROMPT_LOOKUP) != 0;
+        S.prepare(R, pred, ids, lookup ? seq_len : 0, m->stop_ids, (int)sample_len, ngram, lp_n >= 0 ? lp_n + 1 : 0);
+        while (true) {
+            // a pass emits 1 .. R tokens: never launch more passes than the remaining budget could need at R tokens each
+            const size_t burst = std::min<size_t>(8, std::max<size_t>(1, (sample_len - E + R - 1) / R));
+            for (size_t i = 0; i < burst; ++i) S.pass(R);
+            AHA_CUDA_CHECK(cudaMemcpyAsync(&ctl, S.d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost, m->ctx.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost, m->ctx.stream));
+            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+            T.check_sample_error();
+            E = (size_t)cur.n_hist;
+            if (ctl.done) break;
+        }
+    }
+    AHA_CUDA_CHECK(cudaMemcpy(out_tokens, T.d_history, E * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    out_tokens[0] = tok;
+    if (lp_n >= 0) AHA_CUDA_CHECK(cudaMemcpy(out_lp, T.d_lp, E * sizeof(aha_logprobs), cudaMemcpyDeviceToHost));
+    const auto t2 = clk::now();
+    *n_out = E;
+    if (stats) { *stats = aha_spec_stats{}; stats->passes = ctl.passes; stats->drafted = ctl.drafted; stats->accepted = ctl.accepted; }
+    if (usage) {
+        usage->prompt_tokens += (uint32_t)seq_len;
+        usage->completion_tokens += (uint32_t)E;
+        usage->prompt_secs += std::chrono::duration<double>(t1 - t0).count();
+        usage->completion_secs += std::chrono::duration<double>(t2 - t1).count();
+        usage->vision_secs += vision_secs;
+    }
+}
+
 }  // namespace
 
 namespace {
@@ -1184,6 +1274,76 @@ int aha_b200_generate(aha_model* m, const uint32_t* ids, size_t seq_len, const a
         GenSink sink{[&](uint32_t t, size_t i, const aha_logprobs*) { out_tokens[i] = t; n = i + 1; return false; }};
         generate_impl(m, ids, seq_len, mm, *params, sink, false, usage, nullptr);
         *n_out = n;
+    });
+}
+
+int aha_b200_generate_speculative(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                                  const aha_spec_params* spec, uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap, size_t* n_out,
+                                  aha_usage* usage, aha_spec_stats* stats) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(params && spec && out_tokens && n_out, "params, spec, out_tokens and n_out are required");
+        AHA_REQUIRE(ids && seq_len >= 1, "input_ids must hold at least one token");
+        if (usage) *usage = aha_usage{};
+        *n_out = 0;
+        generate_speculative_impl(m, ids, seq_len, mm, *params, *spec, out_tokens, out_logprobs, cap, n_out, usage, stats);
+    });
+}
+
+int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
+                               const float* v, float* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(q && k && v && out, "q, k, v and out are required");
+        AHA_REQUIRE(rows >= 1 && rows <= (size_t)kSpecMaxRows, "debug_verify_attn: rows must be 1 to " + std::to_string(kSpecMaxRows));
+        AHA_REQUIRE(n_kv_heads >= 1 && n_heads >= n_kv_heads && n_heads % n_kv_heads == 0 && n_heads <= 64, "debug_verify_attn: bad head counts");
+        constexpr int HD = 128;
+        Ctx& c = m->ctx;
+        const int R = (int)rows, nh = (int)n_heads, nkv = (int)n_kv_heads;
+        const int ctx = (int)pos0 + R;
+        // a paged pool with the pages in reverse order, laid out like the model's ([page][K|V][kv_head][kPage][hd])
+        const int np = ceil_div(ctx, kPage);
+        const size_t page_stride = (size_t)2 * nkv * kPage * HD;
+        std::vector<float> pool((size_t)np * page_stride);
+        std::vector<int> table(np);
+        for (int p = 0; p < np; ++p) table[p] = np - 1 - p;
+        for (int t = 0; t < ctx; ++t)
+            for (int h = 0; h < nkv; ++h) {
+                const size_t base = (size_t)table[t / kPage] * page_stride + (size_t)h * kPage * HD + (size_t)(t % kPage) * HD;
+                std::memcpy(&pool[base], k + ((size_t)t * nkv + h) * HD, HD * sizeof(float));
+                std::memcpy(&pool[base + (size_t)nkv * kPage * HD], v + ((size_t)t * nkv + h) * HD, HD * sizeof(float));
+            }
+        std::vector<DecodeState> st(R);
+        for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, {0, 0, 0}};
+        const int max_chunks = ceil_div(ctx, kSpecChunk);
+        float *d_pool = nullptr, *d_q = nullptr, *d_out = nullptr, *d_part = nullptr;
+        int* d_table = nullptr;
+        DecodeState* d_st = nullptr;
+        auto cleanup = [&] { cudaFree(d_pool); cudaFree(d_q); cudaFree(d_out); cudaFree(d_part); cudaFree(d_table); cudaFree(d_st); };
+        try {
+            AHA_CUDA_CHECK(cudaMalloc(&d_pool, pool.size() * sizeof(float)));
+            AHA_CUDA_CHECK(cudaMalloc(&d_q, (size_t)R * nh * HD * sizeof(float)));
+            AHA_CUDA_CHECK(cudaMalloc(&d_out, (size_t)R * nh * HD * sizeof(float)));
+            AHA_CUDA_CHECK(cudaMalloc(&d_part, (size_t)R * nh * max_chunks * spec_part_stride(HD) * sizeof(float)));
+            AHA_CUDA_CHECK(cudaMalloc(&d_table, np * sizeof(int)));
+            AHA_CUDA_CHECK(cudaMalloc(&d_st, R * sizeof(DecodeState)));
+            AHA_CUDA_CHECK(cudaMemcpy(d_pool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice));
+            AHA_CUDA_CHECK(cudaMemcpy(d_q, q, (size_t)R * nh * HD * sizeof(float), cudaMemcpyHostToDevice));
+            AHA_CUDA_CHECK(cudaMemcpy(d_table, table.data(), np * sizeof(int), cudaMemcpyHostToDevice));
+            AHA_CUDA_CHECK(cudaMemcpy(d_st, st.data(), R * sizeof(DecodeState), cudaMemcpyHostToDevice));
+            SpecAttnArgs a{};
+            a.q = d_q; a.ldq = nh * HD;
+            a.kv.k = d_pool; a.kv.v = d_pool + (size_t)nkv * kPage * HD; a.kv.page_table = d_table; a.kv.page_shift = kPageShift;
+            a.kv.page_stride = page_stride; a.kv.tok_stride = HD; a.kv.head_stride = (size_t)kPage * HD;
+            a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
+            a.R = R; a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
+            AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
+            // few CTAs, so that a CTA walks several chunks
+            spec_verify_attn_kernel<HD><<<dim3(std::min(3, max_chunks), nkv), kSpecAttnThreads, spec_attn_smem_bytes<HD>(), c.stream>>>(a);
+            spec_verify_merge_kernel<HD><<<dim3(nh, R), HD, 0, c.stream>>>(a);
+            AHA_CUDA_CHECK(cudaGetLastError());
+            AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+            AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)R * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
+        } catch (...) { cleanup(); throw; }
+        cleanup();
     });
 }
 
@@ -1926,6 +2086,7 @@ void aha_b200_destroy(aha_model* m) {
     m->text.destroy();
     m->batch.clear_graphs();
     m->wide_batch.clear_graphs();
+    m->spec.destroy();
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
     if (m->h_lp_pin) cudaFreeHost(m->h_lp_pin);
@@ -2030,6 +2191,9 @@ int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, s
         } else if (w == "batch_graphs") {   // step graphs captured in the open batch session (wide: at most one per running count)
             AHA_REQUIRE(cap >= 1, "out too small");
             out[0] = (float)m->sess().graphs.size(); *n = 1; return;
+        } else if (w == "spec_graphs") {    // pass graphs of speculative requests (one per row count R)
+            AHA_REQUIRE(cap >= 1, "out too small");
+            out[0] = (float)m->spec.graphs.size(); *n = 1; return;
         } else if (w == "rope_delta") {
             AHA_REQUIRE(cap >= 1, "out too small");
             out[0] = (float)m->rope_delta; *n = 1; return;

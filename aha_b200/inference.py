@@ -215,6 +215,48 @@ class B200Model:
         self._check(self._lib.aha_b200_generate(self._h, ids_p, ids.size, mm_p, C.byref(p), out, cap, C.byref(n), C.byref(u)))
         return [int(out[i]) for i in range(n.value)], self._usage(u)
 
+    def generate_speculative(self, input_ids, data=None, prediction=None, prompt_lookup=False, max_draft=7, ngram=3, max_tokens=1024,
+                             temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64, seed=299792458, flags=0,
+                             logprobs=False, top_logprobs=0):
+        """Speculative decoding of one request (aha_b200_generate_speculative): verify passes of max_draft + 1 rows, drafted from
+        `prediction` (token ids the answer will largely repeat) and, with prompt_lookup, from the prompt and the output so far.
+        -> (ids, usage, stats) with stats = dict(passes, drafted, accepted); (ids, usage, stats, records) with logprobs=True.
+        The ids and records do not depend on the drafts; they follow the model as wide batch sessions do."""
+        ids = self._ids(input_ids)
+        mm, _keep = self._mm(data)
+        sp, _pred = L.spec_params(prediction, prompt_lookup, max_draft, ngram, self.vocab_size)
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        cap = max(max_tokens, 1)
+        out = (C.c_uint32 * cap)()
+        recs = (L.Logprobs * cap)() if logprobs else None
+        n = C.c_size_t(0)
+        u = L.Usage()
+        st = L.SpecStats()
+        self._check(self._lib.aha_b200_generate_speculative(
+            self._h, ids.ctypes.data_as(C.POINTER(C.c_uint32)), ids.size, C.byref(mm) if mm is not None else None, C.byref(p), C.byref(sp),
+            out, recs, cap, C.byref(n), C.byref(u), C.byref(st)))
+        toks = [int(out[i]) for i in range(n.value)]
+        stats = dict(passes=int(st.passes), drafted=int(st.drafted), accepted=int(st.accepted))
+        if logprobs:
+            return toks, self._usage(u), stats, [L.logprobs_record(recs[i]) for i in range(n.value)]
+        return toks, self._usage(u), stats
+
+    def debug_verify_attn(self, q, k, v, pos0):
+        """The verify attention of speculative decoding on host data: q [R][nh][128] at positions pos0 .. pos0 + R - 1,
+        k / v [pos0 + R][nkv][128] -> [R][nh][128]."""
+        q = np.ascontiguousarray(q, np.float32)
+        k = np.ascontiguousarray(k, np.float32)
+        v = np.ascontiguousarray(v, np.float32)
+        R, nh, hd = q.shape
+        nkv = k.shape[1]
+        if hd != 128 or k.shape != (pos0 + R, nkv, 128) or v.shape != k.shape:
+            raise ValueError("q [R][nh][128], k and v [pos0 + R][nkv][128]")
+        out = np.empty_like(q)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        self._check(self._lib.aha_b200_debug_verify_attn(self._h, R, nh, nkv, int(pos0), f(q), f(k), f(v), f(out)))
+        return out
+
     def generate_batch(self, requests):
         """Static batching (aha_b200_generate_batch): requests = [dict(input_ids=..., data=None, max_tokens=..., temperature=..., top_p=...,
         top_k=..., repeat_penalty=..., repeat_last_n=..., seed=...), ...] (at most 8) decoded in lockstep on this handle.

@@ -274,6 +274,42 @@ int aha_b200_generate_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len
 int aha_b200_generate_stream_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
                                       aha_logprobs_callback on_token, void* user, aha_usage* usage);
 
+/* Speculative decoding of one request (new design; the reference decodes one token per forward_step and ignores
+ * ChatCompletionParameters.prediction, src/params/chat.rs:102-105).  After the normal prefill and first token the request runs in verify
+ * passes of R = max_draft + 1 rows through one weight stream: row 0 is the last emitted token, rows 1..R-1 are drafted tokens at the
+ * following positions.  A pass emits the longest run of drafts that the request's own sampler reproduces, plus the sampler's next token.
+ *   Drafts: for n = min(ngram, emitted) down to 1, the last n emitted tokens are looked up first in `prediction` (OpenAI "Predicted
+ *   Outputs": text the answer will largely repeat), then, with AHA_SPEC_PROMPT_LOOKUP, in the prompt followed by the tokens emitted so
+ *   far.  The most recent occurrence that is followed by at least one token wins, and the up to max_draft tokens after it are the drafts.
+ *   Exact: row r is sampled with draw index n_draws + r and the repeat-penalty context "history followed by drafts 1..r", which is what a
+ *   sequential decode does with the same logits, so ids and records do not depend on the drafts, max_draft or use_graph.  A wrong draft
+ *   costs time, never the answer.
+ *   Numerics: the first token equals aha_b200_generate's.  The tokens after it follow the model as wide batch sessions do (tensor-core
+ *   projections): they need NOT equal aha_b200_generate's in the last bits.
+ *   Cost: every pass costs R rows, so a request whose drafts are rarely accepted runs SLOWER than aha_b200_generate.
+ *   EOS inside an accepted run ends the request after the EOS token; max_tokens cuts a run.  KV pages for seq_len + max_tokens + max_draft
+ *   tokens are mapped up front; a request that does not fit max_ctx is refused.  Single GPU, no open batch session, models whose
+ *   projections tile by 64 with head_dim 128; Qwen3-ASR handles and AHA_GEN_REUSE_PREFIX / _CONTINUE_RNG / _EOS_ON_FIRST are refused.
+ * out_logprobs: [cap] records when params.flags carries AHA_GEN_LOGPROBS, else may be NULL.  stats may be NULL. */
+#define AHA_SPEC_PROMPT_LOOKUP 1u    /* also draft from the prompt and the tokens generated so far */
+typedef struct aha_spec_params {
+    const uint32_t* prediction;      /* the caller's predicted output (token ids), or NULL */
+    size_t n_prediction;
+    uint32_t max_draft;              /* 1..15 drafted tokens per pass (R = max_draft + 1 rows) */
+    uint32_t ngram;                  /* longest suffix looked up, 1..8; 0 = default (3) */
+    uint32_t flags;                  /* AHA_SPEC_PROMPT_LOOKUP */
+    uint32_t reserved[3];
+} aha_spec_params;
+typedef struct aha_spec_stats {
+    uint32_t passes;                 /* verify passes run */
+    uint32_t drafted;                /* drafted tokens over all passes */
+    uint32_t accepted;               /* drafted tokens that were emitted */
+    uint32_t reserved;
+} aha_spec_stats;
+int aha_b200_generate_speculative(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params,
+                                  const aha_spec_params* spec, uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap,
+                                  size_t* n_out, aha_usage* usage, aha_spec_stats* stats);
+
 /* Qwen3AsrGenerateModel::generate / generate_stream (qwen3_asr/generate.rs:130-268): per-chunk loop, stop on either EOS id
  * (the handle's stop ids), KV cache cleared per chunk, one sampler for the whole request.  on_token may be NULL. */
 int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_chunks, const aha_gen_params* params,
@@ -395,7 +431,8 @@ int aha_b200_reset_stats(aha_model* m);
 /* Copy an internal activation to the host: what = "hidden" (text hidden states after layer `index`
  * of the last forward_initial, S*H floats; requires aha_b200_set_trace(m,1)), "vit" (ViT hidden after
  * block `index`), "image_embeds", "audio_embeds", "rope_delta" (1 float), "batch_graphs" (1 float: step graphs
- * captured in the open batch session: at most one per running count, two where requests asking for log-probabilities ran). */
+ * captured in the open batch session: at most one per running count, two where requests asking for log-probabilities ran),
+ * "spec_graphs" (1 float: pass graphs of speculative requests, at most one per row count). */
 int aha_b200_set_trace(aha_model* m, int on);
 int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, size_t cap, size_t* n);
 /* Run n decode steps back to back on the device (graph replays, token feedback on device) without any
@@ -412,6 +449,11 @@ int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_param
 /* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
 int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);
+/* the verify attention of speculative decoding on host data (tests): `rows` query rows at positions pos0 .. pos0 + rows - 1 over K / V of
+ * pos0 + rows positions (laid out on a paged pool with the pages in reverse order), head_dim 128.  q, out: [rows][n_heads][128] (q
+ * normalised and rotated); k, v: [pos0 + rows][n_kv_heads][128].  Row r attends to positions 0 .. pos0 + r. */
+int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
+                               const float* v, float* out);
 /* Run ONE Linear layer y = epilogue(x W^T + b) through the library's GEMM dispatch on host data (unit tests of the
  * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 5 = the batched decode GEMV (M <= 8; its SwiGLU
  * instantiation runs with a unit-gain RMSNorm prologue), 6 = the same with the cp.async weight ring, 7 = the wide batched decode GEMV

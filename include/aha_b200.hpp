@@ -247,6 +247,25 @@ public:
         }
         return res;
     }
+    // Speculative decoding of one greedy request (aha_b200_generate_speculative): verify passes of max_draft + 1 rows drafted from
+    // `prediction` and, with prompt_lookup, from the prompt and the output so far.  The ids do not depend on the drafts.
+    std::vector<uint32_t> generate_speculative(const std::vector<uint32_t>& ids, const MultiModalData* data, const GenerationContext& ctx,
+                                               const std::vector<uint32_t>& prediction, bool prompt_lookup = false, uint32_t max_draft = 7,
+                                               uint32_t ngram = 0, Usage* usage = nullptr, aha_spec_stats* stats = nullptr) {
+        aha_gen_params p{};
+        p.temperature = 0.f; p.repeat_penalty = ctx.repeat_penalty; p.repeat_last_n = (int32_t)ctx.repeat_last_n; p.max_tokens = (uint32_t)ctx.sample_len;
+        aha_spec_params s{};
+        s.prediction = prediction.empty() ? nullptr : prediction.data(); s.n_prediction = prediction.size();
+        s.max_draft = max_draft; s.ngram = ngram; s.flags = prompt_lookup ? AHA_SPEC_PROMPT_LOOKUP : 0u;
+        std::vector<uint32_t> out(std::max<size_t>(ctx.sample_len, 1));
+        size_t n = 0;
+        aha_usage u{};
+        const aha_mm mm = data ? data->view() : aha_mm{nullptr, 0};
+        check(aha_b200_generate_speculative(h_, ids.data(), ids.size(), data ? &mm : nullptr, &p, &s, out.data(), nullptr, out.size(), &n, &u, stats));
+        out.resize(n);
+        if (usage) *usage = Usage{u.prompt_tokens, u.completion_tokens, u.prompt_secs, u.completion_secs, u.vision_secs};
+        return out;
+    }
     size_t last_prefix_hit() const { return aha_b200_last_prefix_hit(h_); }
     // Prefill continuation (aha_b200_forward_extend): further prompt tokens against the `off` tokens already in the cache.
     std::vector<float> forward_extend(const std::vector<uint32_t>& ids, size_t off) {
