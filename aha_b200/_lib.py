@@ -73,6 +73,21 @@ def logprobs_record(r):
                 top_ids=[int(r.top_ids[i]) for i in range(n)], top_logprobs=[np.float32(r.top_logprobs[i]) for i in range(n)])
 
 
+# aha_logprobs as a numpy record: the scoring entries fill arrays of them in one call (no Python object per record)
+LOGPROBS_DTYPE = np.dtype([("token", "<u4"), ("index", "<u4"), ("logprob", "<f4"), ("n_top", "<u4"), ("top_ids", "<u4", (MAX_TOP_LOGPROBS,)),
+                           ("top_logprobs", "<f4", (MAX_TOP_LOGPROBS,)), ("valid", "<u4"), ("reserved", "<u4")])
+assert LOGPROBS_DTYPE.itemsize == C.sizeof(Logprobs)
+
+
+def score_arrays(recs, top):
+    """records of a scoring call -> dict(tokens, logprobs[, top_ids [n, top], top_logprobs [n, top]]) of numpy arrays"""
+    d = dict(tokens=recs["token"].copy(), logprobs=recs["logprob"].copy())
+    if top:
+        d["top_ids"] = recs["top_ids"][:, :top].copy()
+        d["top_logprobs"] = recs["top_logprobs"][:, :top].copy()
+    return d
+
+
 LOGPROBS_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(Logprobs))
 
 
@@ -190,6 +205,10 @@ SYMBOLS = {
     "aha_b200_split_audio_into_chunks": (C.c_int, [C.c_size_t, C.c_uint32, C.c_float, C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_embed": (C.c_int, [_P, _U32P, C.c_size_t, _F32P]),
     "aha_b200_embed_batch": (C.c_int, [_P, _U32P, C.POINTER(C.c_size_t), C.c_size_t, _F32P]),
+    "aha_b200_score": (C.c_int, [_P, _U32P, C.c_size_t, C.c_size_t, C.c_uint32, C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "aha_b200_score_batch": (C.c_int, [_P, _U32P, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.c_size_t, C.c_uint32, C.POINTER(Logprobs),
+                                       C.c_size_t, C.POINTER(C.c_size_t)]),
+    "aha_b200_debug_score_head": (C.c_int, [_P, C.c_int, _F32P, C.c_size_t, _U32P, C.c_uint32, C.POINTER(Logprobs)]),
     "aha_b200_rerank": (C.c_int, [_P, _U32P, C.c_size_t, _U32P, C.POINTER(C.c_size_t), C.c_size_t, _F32P]),
     "aha_b200_nccl_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),
     "aha_b200_rope_index": (C.c_int, [_U32P, C.c_size_t, _U32P, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,

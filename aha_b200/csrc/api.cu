@@ -4,13 +4,16 @@
 // Qwen3ASRModel (qwen3_asr/model.rs:308-425) and generate_generic (common/generate.rs:115-159).
 #include <array>
 #include <chrono>
+#include <cstdio>
 #include <functional>
 #include <mutex>
 #include <system_error>
 #include <thread>
+#include <type_traits>
 
 #include "audio_model.cuh"
 #include "preprocess.cuh"
+#include "score_head.cuh"
 #include "text_model.cuh"
 #include "batch_decode.cuh"
 #include "speculative.cuh"
@@ -67,6 +70,20 @@ struct aha_model {
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
     SpecDecoder spec;                   // speculative single requests (aha_b200_generate_speculative) on wide_batch's buffers
+    // scoring (aha_b200_score / _score_batch): the buffers of one head launch over up to max_prefill rows and the lm_head's tensor map,
+    // set up by the first scoring call
+    struct ScoreBufs {
+        int* rows = nullptr;            // [M] rows of TextModel::x to score
+        uint32_t* tgt = nullptr;        // [M] the token each row is scored at
+        uint32_t* index = nullptr;      // [M] the records' index fields
+        float* tlogit = nullptr;        // [M] the targets' raw logits (score_head_kernel)
+        float* part = nullptr;          // [M][P][kLpPartFloats] slice results
+        int* part_id = nullptr;         // [M][P][kLpMaxTop]
+        int* on = nullptr;              // [1] 1 + the top count (the twin's logprob_partial_rows_kernel)
+        aha_logprobs* rec = nullptr;    // [M]
+    } score;
+    CUtensorMap score_tm_w{};
+    bool score_ready = false;
 };
 
 namespace {
@@ -498,6 +515,29 @@ void forward_prefill(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S,
     T.prefill(pt, (int)S, (int)offset, embeds_ready, m->d_scatter_idx, n_visual, deepstack);
 }
 
+// A prompt longer than the activation workspace (max_prefill) runs as consecutive chunks against the growing cache: the first chunk is
+// the reference's call (multimodal rows are scattered there), the others are continuations.  Same K/V, same logits for the last token.
+// after_chunk(done, n) runs after the chunk of tokens [done, done + n), while its rows are still in TextModel::x.
+void prefill_chunked(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, size_t offset, const aha_mm* mm, bool initial, bool has_mm, bool extend,
+                     const std::function<void(size_t, size_t)>& after_chunk = nullptr) {
+    const size_t chunk = (size_t)m->text.max_prefill;
+    size_t done = 0;
+    while (done < S) {
+        const size_t n = std::min(chunk, S - done);
+        const bool first = done == 0;
+        if (first && !extend) {
+            if (n < S && has_mm) {   // every placeholder row must be embedded by the call that carries the tensors
+                const auto mmt = mm_token_ids(m);
+                for (size_t i = n; i < S; ++i) for (uint32_t t : mmt) AHA_REQUIRE(ids[i] != t, "prompt exceeds max_prefill before its last multimodal placeholder");
+            }
+            // (Qwen3-VL: get_rope_index over the first chunk yields the whole prompt's rope_delta, because only text follows the last placeholder)
+            forward_prefill(m, pt, ids, n, offset, mm, initial);
+        } else forward_prefill(m, pt, ids + done, n, offset + done, nullptr, false);
+        if (after_chunk) after_chunk(done, n);
+        done += n;
+    }
+}
+
 // `extend`: prefill continuation (new design) -- S >= 1 further tokens against a cache that already holds `offset` tokens; the causal mask is
 // the (S, offset + S) one the reference never builds (its (S, S) mask makes a multi-token call with a non-empty cache fail, qwen3/model.rs:164-175).
 // `pt`: the sequence's page table.  The decode step runs on the model's own table only, so a single token on any other table (a batch slot's
@@ -521,23 +561,7 @@ void forward_any(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, siz
         // (qwen3/model.rs:164-175); with a non-empty cache its broadcast_add against (S, off+S) scores fails.
         if (!extend) AHA_REQUIRE(offset == 0, "seq_len > 1 with seqlen_offset > 0 is not supported (the reference's mask shape rejects it too)");
         else AHA_REQUIRE(offset <= (size_t)pt.mapped * kPage, "forward_extend: seqlen_offset is beyond the tokens in the cache");
-        // A prompt longer than the activation workspace (max_prefill) runs as consecutive chunks against the growing cache: the first chunk is
-        // the reference's call (multimodal rows are scattered there), the others are continuations.  Same K/V, same logits for the last token.
-        const size_t chunk = (size_t)T.max_prefill;
-        size_t done = 0;
-        while (done < S) {
-            const size_t n = std::min(chunk, S - done);
-            const bool first = done == 0;
-            if (first && !extend) {
-                if (n < S && has_mm) {   // every placeholder row must be embedded by the call that carries the tensors
-                    const auto mmt = mm_token_ids(m);
-                    for (size_t i = n; i < S; ++i) for (uint32_t t : mmt) AHA_REQUIRE(ids[i] != t, "prompt exceeds max_prefill before its last multimodal placeholder");
-                }
-                // (Qwen3-VL: get_rope_index over the first chunk yields the whole prompt's rope_delta, because only text follows the last placeholder)
-                forward_prefill(m, pt, ids, n, offset, mm, initial);
-            } else forward_prefill(m, pt, ids + done, n, offset + done, nullptr, false);
-            done += n;
-        }
+        prefill_chunked(m, pt, ids, S, offset, mm, initial, has_mm, extend);
         T.finish_argmax(0);
         T.sample(0);   // device sampler of generate(): penalty / temperature / top-k / top-p on the prefill logits (no-op for plain ArgMax)
     }
@@ -587,6 +611,7 @@ int aha_b200_create(const char* kind, const char* config_json, const aha_tensor_
         for (auto& e : m->ev_tok) AHA_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         gemv_init();
         gemm_tc_init();
+        score_head_init();
         gemv_wide_init();
         flash_attn_tc_init();
         const std::string k = kind;
@@ -1495,6 +1520,10 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
     });
 }
 
+namespace {
+void bench_score(aha_model* m, const std::string& w, int iters, double* avg_ms, uint64_t* bytes);   // the score_head timings, defined with scoring
+}  // namespace
+
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch) {
     return guarded(m, [&] {
         AHA_REQUIRE(which && iters > 0 && avg_ms && bytes_per_launch, "which, iters, avg_ms, bytes_per_launch are required");
@@ -1502,6 +1531,7 @@ int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* av
         const std::string w = which;
         cudaStream_t st = m->ctx.stream;
         const int L = T.cfg.L;
+        if (w.rfind("score_", 0) == 0) { bench_score(m, w, iters, avg_ms, bytes_per_launch); return; }
         uint64_t bytes = 0;
         auto launch = [&](int i) {
             TextLayer& Y = T.layers[i % L];
@@ -2006,7 +2036,252 @@ void embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, size_t n
     }
     drop_cache(m);
 }
+
+// ---- scoring: log p(ids[i] | ids[0 .. i)) for given text (aha_b200_score, aha_b200_score_batch) --------------------------------------------
+// Record i of a text is the distribution at row i - 1 evaluated at ids[i].  The rows to score are gathered from TextModel::x right after the
+// prefill that computed them and go through the final RMSNorm (rmsnorm_split_kernel with a row list), score_head_kernel and
+// score_final_rows_kernel.  Scoring uses the prefill scratch and leaves the cache empty, like embed.
+using ScoreBufs = aha_model::ScoreBufs;
+
+// the buffers of M rows in one allocation at `base` (nullptr: only the size); returns the bytes they take
+size_t score_bufs_carve(char* base, size_t M, int V, ScoreBufs& b) {
+    const size_t P = (size_t)lp_parts(V);
+    size_t off = 0;
+    auto take = [&](auto*& ptr, size_t n) {
+        using E = std::remove_reference_t<decltype(*ptr)>;
+        off = (off + 255) & ~(size_t)255;
+        if (base) ptr = reinterpret_cast<E*>(base + off);
+        off += n * sizeof(E);
+    };
+    take(b.rows, M); take(b.tgt, M); take(b.index, M); take(b.tlogit, M);
+    take(b.part, M * P * kLpPartFloats); take(b.part_id, M * P * kLpMaxTop); take(b.on, 1); take(b.rec, M);
+    return off;
+}
+
+// what every scoring entry refuses
+void score_require(aha_model* m, uint32_t n_top) {
+    require_no_session(m);
+    AHA_REQUIRE(m->kind != aha_model::QWEN3_ASR, "scoring needs a qwen3 or qwen3vl handle (Qwen3-ASR prompts carry audio)");
+    const TextModel& T = m->text;
+    AHA_REQUIRE(T.tp_world == 1, "scoring is single-GPU (tp_world must be 1)");
+    AHA_REQUIRE(n_top <= AHA_MAX_TOP_LOGPROBS, "n_top " + std::to_string(n_top) + ": at most " + std::to_string(AHA_MAX_TOP_LOGPROBS) + " alternatives");
+    AHA_REQUIRE(n_top <= (uint32_t)T.cfg.V, "n_top " + std::to_string(n_top) + " exceeds the vocabulary of " + std::to_string(T.cfg.V));
+    AHA_REQUIRE(T.cfg.V <= kLpMaxParts * kLpSlice, "vocabulary too large for the log-probability kernels");
+    AHA_REQUIRE(score_head_supported(T.cfg.H), "scoring needs hidden_size to be a multiple of 64");
+}
+// one text: 1 <= start < len <= max_ctx, ids inside the vocabulary and no multimodal placeholder (scoring takes text-only prompts)
+void score_check_text(aha_model* m, const uint32_t* ids, size_t S, size_t start) {
+    const TextModel& T = m->text;
+    AHA_REQUIRE(start >= 1, "start must be at least 1 (token 0 has no prefix to be scored against)");
+    AHA_REQUIRE(start < S, "start " + std::to_string(start) + " leaves nothing to score in a text of " + std::to_string(S) + " tokens");
+    AHA_REQUIRE(S <= (size_t)T.max_ctx, "context of " + std::to_string(S) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+    const auto mmt = mm_token_ids(m);
+    for (size_t i = 0; i < S; ++i) {
+        AHA_REQUIRE(ids[i] < (uint32_t)T.cfg.V, "token id out of range");
+        for (uint32_t t : mmt) AHA_REQUIRE(ids[i] != t, "scoring takes text-only prompts: token " + std::to_string(i) + " is a multimodal placeholder");
+    }
+}
+void alloc_score_buffers(aha_model* m) {
+    if (m->score_ready) return;
+    const TextModel& T = m->text;
+    char* base = m->ctx.alloc<char>(score_bufs_carve(nullptr, (size_t)T.max_prefill, T.cfg.V, m->score));
+    score_bufs_carve(base, (size_t)T.max_prefill, T.cfg.V, m->score);
+    m->score_tm_w = make_tmap_f16_rows(T.lm_head, (uint64_t)T.cfg.V, (uint64_t)T.cfg.H, kShBN);
+    m->score_ready = true;
+}
+
+// The head over M rows of x [., H] (d_rows: the gather list, nullptr = rows 0 .. M-1) with b.tgt / b.index set: final RMSNorm + split, then
+// impl 0: score_head_kernel; impl 1 (tests, timing): gemm_tc EPI_STORE into `logits` [M][V] + logprob_partial_rows_kernel.  Then stage 2
+// into b.rec.
+void score_head_rows(aha_model* m, int impl, const float* x, const int* d_rows, int M, int n, const ScoreBufs& b, float* logits = nullptr) {
+    TextModel& T = m->text;
+    Ctx& c = m->ctx;
+    const int H = T.cfg.H, V = T.cfg.V, P = lp_parts(V);
+    const ActSplit a = act_split(c, 0, (size_t)M * H);
+    rmsnorm_split_kernel<<<M, 256, 0, c.stream>>>(x, T.norm, T.cfg.eps, a.hi, a.lo, H, d_rows);
+    if (impl == 0) {
+        const ScoreHeadArgs s{M, V, H, n, b.tgt, b.part, b.part_id, b.tlogit};
+        score_head_launch(c.stream, a.hi, a.lo, m->score_tm_w, s);
+    } else {
+        GemmTcArgs g{};
+        g.C = logits; g.ldc = V; g.M = M; g.N = V; g.K = H; g.act = ACT_NONE;
+        gemm_tc_launch<kShBN>(c.stream, EPI_STORE, a.hi, a.lo, m->score_tm_w, g);
+        const int on = 1 + n;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b.on, &on, sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        logprob_partial_rows_kernel<<<dim3(P, M), kLpThreads, 0, c.stream>>>(logits, V, V, nullptr, b.on, b.part, b.part_id);
+        c.cnt.kernels++;
+    }
+    score_final_rows_kernel<<<M, kLpMaxParts, 0, c.stream>>>(b.part, b.part_id, P, n, b.tgt, impl == 0 ? b.tlogit : nullptr, logits, V, b.index, b.rec);
+    c.cnt.kernels += 3;
+    AHA_CUDA_CHECK(cudaGetLastError());
+}
+
+// the head over the listed rows of TextModel::x, scored at tgt with record indices idx; the records go to out[0 .. rows.size())
+void score_gathered(aha_model* m, const std::vector<int>& rows, const std::vector<uint32_t>& tgt, const std::vector<uint32_t>& idx, int n, aha_logprobs* out) {
+    const int M = (int)rows.size();
+    if (M == 0) return;
+    const ScoreBufs& b = m->score;
+    cudaStream_t st = m->ctx.stream;
+    AHA_CUDA_CHECK(cudaMemcpyAsync(b.rows, rows.data(), (size_t)M * sizeof(int), cudaMemcpyHostToDevice, st));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(b.tgt, tgt.data(), (size_t)M * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(b.index, idx.data(), (size_t)M * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    score_head_rows(m, 0, m->text.x, b.rows, M, n, b);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(out, b.rec, (size_t)M * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, st));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// one checked text through the chunked prefill (forward_any's chunks: any length up to max_ctx); each chunk's scored rows go through the
+// head right after its prefill.  Records from out[0] = the record of ids[start].
+void score_text(aha_model* m, const uint32_t* ids, size_t S, size_t start, int n, aha_logprobs* out) {
+    drop_cache(m);
+    prefill_chunked(m, m->text.table, ids, S, 0, nullptr, false, false, false, [&](size_t done, size_t len) {
+        const size_t j0 = std::max(start - 1, done), j1 = std::min(S - 1, done + len);   // rows j0 .. j1 - 1 of the text
+        if (j0 >= j1) return;
+        std::vector<int> rows;
+        std::vector<uint32_t> tgt, idx;
+        for (size_t j = j0; j < j1; ++j) { rows.push_back((int)(j - done)); tgt.push_back(ids[j + 1]); idx.push_back((uint32_t)(j + 1)); }
+        score_gathered(m, rows, tgt, idx, n, out + (j0 + 1 - start));
+    });
+}
+
+void score_one(aha_model* m, const uint32_t* ids, size_t S, size_t start, uint32_t n_top, aha_logprobs* out, size_t cap, size_t* n_out) {
+    AHA_REQUIRE(ids && n_out, "ids and n_out are required");
+    score_require(m, n_top);
+    score_check_text(m, ids, S, start);
+    AHA_REQUIRE(out && S - start <= cap, "out holds " + std::to_string(cap) + " records, the text needs " + std::to_string(S - start));
+    *n_out = 0;
+    alloc_score_buffers(m);
+    score_text(m, ids, S, start, (int)n_top, out);
+    drop_cache(m);
+    *n_out = S - start;
+}
+
+// The texts, in input order, are cut into packs of at most min(max_prefill, max_ctx) tokens, as embed_batch cuts them.  A pack is one prefill
+// (each text attends only to itself, its positions restart at 0), then one head launch over the scored rows of all its texts.  A text longer
+// than a pack goes through score_text in its place.
+void score_batch(aha_model* m, const uint32_t* ids, const size_t* lens, const size_t* starts, size_t n, uint32_t n_top, aha_logprobs* out, size_t cap,
+                 size_t* n_out) {
+    AHA_REQUIRE(ids && lens && n >= 1 && n_out, "ids, lens, n >= 1 and n_out are required");
+    score_require(m, n_top);
+    TextModel& T = m->text;
+    std::vector<const uint32_t*> text_ids(n);
+    const std::vector<size_t> text_lens(lens, lens + n);
+    std::vector<size_t> st(n), first_rec(n);
+    size_t total = 0, recs = 0;
+    for (size_t j = 0; j < n; ++j) {
+        text_ids[j] = ids + total;
+        st[j] = starts ? starts[j] : 1;
+        AHA_REQUIRE(lens[j] >= 1, "text " + std::to_string(j) + " is empty");
+        score_check_text(m, text_ids[j], lens[j], st[j]);
+        first_rec[j] = recs;
+        recs += lens[j] - st[j];
+        total += lens[j];
+    }
+    AHA_REQUIRE(out && recs <= cap, "out holds " + std::to_string(cap) + " records, the texts need " + std::to_string(recs));
+    *n_out = 0;
+    alloc_score_buffers(m);
+    alloc_pack_buffers(m);
+    const size_t pcap = (size_t)std::min(T.max_prefill, T.max_ctx);
+    drop_cache(m);
+    for (size_t first = 0; first < n;) {
+        if (text_lens[first] > pcap) {
+            score_text(m, text_ids[first], text_lens[first], st[first], (int)n_top, out + first_rec[first]);
+            ++first;
+            continue;
+        }
+        // 16-token starts, as in embed_batch: a text's attention tiles stay the ones it runs alone
+        Pack p = plan_pack(text_ids, text_lens, first, 16, pcap);
+        upload_pack(m, p);
+        T.prefill(T.table, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
+        std::vector<int> rows;
+        std::vector<uint32_t> tgt, idx;
+        for (size_t j = p.first; j < p.last; ++j) {
+            const size_t s0 = p.start[j - first];
+            for (size_t i = st[j]; i < text_lens[j]; ++i) { rows.push_back((int)(s0 + i - 1)); tgt.push_back(text_ids[j][i]); idx.push_back((uint32_t)i); }
+        }
+        score_gathered(m, rows, tgt, idx, (int)n_top, out + first_rec[first]);
+        first = p.last;
+    }
+    drop_cache(m);
+    *n_out = recs;
+}
+
+// kernel timing (aha_b200_bench_kernel "score_head:M:n" / "score_twin:M:n"): the head over rows 0 .. M-1 of TextModel::x as the last
+// prefill left them, every row scored at token 0
+void bench_score(aha_model* m, const std::string& w, int iters, double* avg_ms, uint64_t* bytes) {
+    TextModel& T = m->text;
+    char kind[16] = {0};
+    int M = 0, n = 0;
+    AHA_REQUIRE(std::sscanf(w.c_str(), "score_%4[a-z]:%d:%d", kind, &M, &n) == 3 && (std::string(kind) == "head" || std::string(kind) == "twin"),
+                "score kernels are named score_head:M:n or score_twin:M:n");
+    const int impl = std::string(kind) == "head" ? 0 : 1;
+    score_require(m, (uint32_t)std::max(n, 0));
+    AHA_REQUIRE(M >= 1 && M <= T.max_prefill && n >= 0, "score bench: 1 <= M <= max_prefill");
+    AHA_REQUIRE(impl == 0 || T.cfg.V % 2 == 0, "the gemm_tc twin needs an even vocabulary");
+    alloc_score_buffers(m);
+    const ScoreBufs& b = m->score;
+    cudaStream_t st = m->ctx.stream;
+    AHA_CUDA_CHECK(cudaMemsetAsync(b.tgt, 0, (size_t)M * sizeof(uint32_t), st));
+    AHA_CUDA_CHECK(cudaMemsetAsync(b.index, 0, (size_t)M * sizeof(uint32_t), st));
+    float* logits = nullptr;
+    if (impl == 1) AHA_CUDA_CHECK(cudaMalloc(&logits, (size_t)M * T.cfg.V * sizeof(float)));
+    try {
+        score_head_rows(m, impl, T.x, nullptr, M, n, b, logits);
+        AHA_CUDA_CHECK(cudaEventRecord(m->ev0, st));
+        for (int i = 0; i < iters; ++i) score_head_rows(m, impl, T.x, nullptr, M, n, b, logits);
+        AHA_CUDA_CHECK(cudaEventRecord(m->ev1, st));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
+    } catch (...) { cudaFree(logits); throw; }
+    cudaFree(logits);
+    float ms = 0.f;
+    AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1));
+    *avg_ms = ms / iters;
+    *bytes = 2ull * T.cfg.V * T.cfg.H;
+}
 }  // namespace
+
+int aha_b200_score(aha_model* m, const uint32_t* ids, size_t seq_len, size_t start, uint32_t n_top, aha_logprobs* out, size_t cap, size_t* n_out) {
+    return guarded(m, [&] { score_one(m, ids, seq_len, start, n_top, out, cap, n_out); });
+}
+
+int aha_b200_score_batch(aha_model* m, const uint32_t* ids, const size_t* lens, const size_t* starts, size_t n, uint32_t n_top, aha_logprobs* out,
+                         size_t cap, size_t* n_out) {
+    return guarded(m, [&] { score_batch(m, ids, lens, starts, n, n_top, out, cap, n_out); });
+}
+
+int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_t M, const uint32_t* targets, uint32_t n_top, aha_logprobs* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(hidden && targets && out && M >= 1 && M <= 65535, "hidden, targets, out and 1 <= M <= 65535 are required");
+        AHA_REQUIRE(impl == 0 || impl == 1, "impl must be 0 (score_head_kernel) or 1 (gemm_tc + logprob_partial_rows_kernel)");
+        score_require(m, n_top);
+        const TextModel& T = m->text;
+        const int H = T.cfg.H, V = T.cfg.V;
+        for (size_t r = 0; r < M; ++r) AHA_REQUIRE(targets[r] < (uint32_t)V, "target id out of range");
+        AHA_REQUIRE(impl == 0 || V % 2 == 0, "the gemm_tc twin needs an even vocabulary");
+        alloc_score_buffers(m);
+        cudaStream_t st = m->ctx.stream;
+        // scratch of this call only: the hidden rows, the buffers of M rows and (twin) the logits block
+        struct Scratch {
+            void* p = nullptr;
+            ~Scratch() { if (p) cudaFree(p); }
+        } mem;
+        ScoreBufs b;
+        const size_t o_x = (score_bufs_carve(nullptr, M, V, b) + 255) & ~(size_t)255;
+        const size_t o_lg = (o_x + M * H * sizeof(float) + 255) & ~(size_t)255;
+        AHA_CUDA_CHECK(cudaMalloc(&mem.p, o_lg + (impl == 1 ? M * (size_t)V * sizeof(float) : 0)));
+        char* base = static_cast<char*>(mem.p);
+        score_bufs_carve(base, M, V, b);
+        float* x = reinterpret_cast<float*>(base + o_x);
+        std::vector<uint32_t> idx(M);
+        for (size_t r = 0; r < M; ++r) idx[r] = (uint32_t)r;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(x, hidden, M * H * sizeof(float), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b.tgt, targets, M * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(b.index, idx.data(), M * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        score_head_rows(m, impl, x, nullptr, (int)M, (int)n_top, b, impl == 1 ? reinterpret_cast<float*>(base + o_lg) : nullptr);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(out, b.rec, M * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
+    });
+}
 
 int aha_b200_embed(aha_model* m, const uint32_t* ids, size_t seq_len, float* out) {
     return guarded(m, [&] { embed_one(m, ids, seq_len, out); });

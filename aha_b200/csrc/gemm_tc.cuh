@@ -136,6 +136,52 @@ __device__ __forceinline__ void tc_mma(float (&acc)[BN / 2], uint64_t da, uint64
     else wgmma_ss_n256(acc, da, db);
 }
 
+// ------------------------------------------------------------------------------------------------ the shared mainloop
+// The ring is walked by a position `it` that counts k-blocks over the CTA's whole life: slot it % S, phase it / S.  gemm_tc_kernel walks
+// one tile (it = kb); score_head_kernel (score_head.cuh) walks several W tiles of the same A rows back to back through the same ring.
+//
+// TMA producer: k-block kb of A rows [m0, m0 + 128) and W rows [n0, n0 + BN) into the slot of ring position `it`
+template <int BN>
+__device__ __forceinline__ void tc_produce(uint8_t* tiles, uint64_t* full, uint64_t* empty, const CUtensorMap* tm_hi, const CUtensorMap* tm_lo,
+                                           const CUtensorMap* tm_w, int it, int kb, int m0, int n0) {
+    constexpr int S = tc_stages<BN>(), SB = tc_stage_bytes<BN>();
+    const int s = it % S;
+    mbar_wait(&empty[s], ((it / S) & 1) ^ 1);
+    uint8_t* st = tiles + (size_t)s * SB;
+    mbar_expect_tx(&full[s], SB);
+    tma_load_2d(st, tm_hi, kb * kTcBK, m0, &full[s]);
+    tma_load_2d(st + kTcTileBytes, tm_lo, kb * kTcBK, m0, &full[s]);
+    tma_load_2d(st + 2 * kTcTileBytes, tm_w, kb * kTcBK, n0, &full[s]);
+}
+// consumer warpgroup wg (rows [64 wg, 64 wg + 64) of the tile): acc = the tile's products over nkb k-blocks taken from ring positions
+// it0 .. it0 + nkb - 1, every k-block as 4 k-steps x {hi, lo}.  Every slot but the last one is released on its `empty` barrier; the caller
+// releases that one (or ends) once the accumulator has been read.
+template <int BN>
+__device__ __forceinline__ void tc_mainloop(float (&acc)[BN / 2], uint8_t* tiles, uint64_t* full, uint64_t* empty, int it0, int nkb, int wg, int lane) {
+    constexpr int S = tc_stages<BN>(), SB = tc_stage_bytes<BN>();
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int it = it0 + kb, s = it % S;
+        mbar_wait(&full[s], (it / S) & 1);
+        const uint32_t st = smem_u32(tiles + (size_t)s * SB);
+        const uint64_t d_hi = wgmma_desc_sw128(st + wg * 64 * 128), d_lo = wgmma_desc_sw128(st + kTcTileBytes + wg * 64 * 128);
+        const uint64_t d_w = wgmma_desc_sw128(st + 2 * kTcTileBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kTcBK / 16; ++ks) {
+            const uint64_t adv = (uint64_t)((ks * 16 * 2) >> 4);   // 32 bytes per K = 16 step inside the 128-byte swizzle atom
+            tc_mma<BN>(acc, d_hi + adv, d_w + adv);
+            tc_mma<BN>(acc, d_lo + adv, d_w + adv);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                      // the group of k-block kb - 1 has retired: its slot is free
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % S]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+}
+
 // ------------------------------------------------------------------------------------------------ the GEMM kernel
 template <int EPI, int BN>
 __global__ void __launch_bounds__(kTcThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
@@ -159,43 +205,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) gemm_tc_kernel(const __grid_con
 
     if (warp == 8) {
         // ======================= TMA producer
-        if (lane == 0) {
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % S;
-                mbar_wait(&empty[s], ((kb / S) & 1) ^ 1);
-                uint8_t* st = tiles + (size_t)s * SB;
-                mbar_expect_tx(&full[s], SB);
-                tma_load_2d(st, &tm_hi, kb * kTcBK, m0, &full[s]);
-                tma_load_2d(st + kTcTileBytes, &tm_lo, kb * kTcBK, m0, &full[s]);
-                tma_load_2d(st + 2 * kTcTileBytes, &tm_w, kb * kTcBK, n0, &full[s]);
-            }
-        }
+        if (lane == 0)
+            for (int kb = 0; kb < nkb; ++kb) tc_produce<BN>(tiles, full, empty, &tm_hi, &tm_lo, &tm_w, kb, kb, m0, n0);
         return;
     }
     // ======================= consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the tile
     const int wg = warp >> 2;
     float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % S;
-        mbar_wait(&full[s], (kb / S) & 1);
-        const uint32_t st = smem_u32(tiles + (size_t)s * SB);
-        const uint64_t d_hi = wgmma_desc_sw128(st + wg * 64 * 128), d_lo = wgmma_desc_sw128(st + kTcTileBytes + wg * 64 * 128);
-        const uint64_t d_w = wgmma_desc_sw128(st + 2 * kTcTileBytes);
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < kTcBK / 16; ++ks) {
-            const uint64_t adv = (uint64_t)((ks * 16 * 2) >> 4);   // 32 bytes per K = 16 step inside the 128-byte swizzle atom
-            tc_mma<BN>(acc, d_hi + adv, d_w + adv);
-            tc_mma<BN>(acc, d_lo + adv, d_w + adv);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                                      // the group of k-block kb - 1 has retired: its slot is free
-        if (kb > 0 && lane == 0) mbar_arrive(&empty[(kb - 1) % S]);
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
+    tc_mainloop<BN>(acc, tiles, full, empty, 0, nkb, wg, lane);
     const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), col = n0 + 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {

@@ -39,11 +39,11 @@ __device__ __forceinline__ void split_half(float x, __half& h, __half& l) {
     h = __float2half_rn(x);
     l = __float2half_rn(x - __half2float(h));
 }
-// rmsnorm_kernel with the split output: out_hi / out_lo [rows, H] fp16
+// rmsnorm_kernel with the split output: out_hi / out_lo [rows, H] fp16.  rows != nullptr gathers: output row r is input row rows[r].
 __global__ void rmsnorm_split_kernel(const float* __restrict__ x, const float* __restrict__ w, float eps, __half* __restrict__ out_hi,
-                                     __half* __restrict__ out_lo, int H) {
+                                     __half* __restrict__ out_lo, int H, const int* __restrict__ rows = nullptr) {
     __shared__ float red[32];
-    const float* xr = x + (size_t)blockIdx.x * H;
+    const float* xr = x + (size_t)(rows ? rows[blockIdx.x] : (int)blockIdx.x) * H;
     float ss = 0.f;
     for (int i = threadIdx.x; i < H; i += blockDim.x) { float v = xr[i]; ss = fmaf(v, v, ss); }
     ss = block_sum(ss, red);

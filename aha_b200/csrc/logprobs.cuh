@@ -112,23 +112,14 @@ __global__ void __launch_bounds__(kLpThreads) logprob_partial_rows_kernel(const 
     }
 }
 
-__global__ void __launch_bounds__(kLpMaxParts) logprob_final_rows_kernel(const float* __restrict__ logits, int ld, int V, int P, const int* __restrict__ act,
-                                                                         const int* __restrict__ on, const float* __restrict__ part,
-                                                                         const int* __restrict__ part_id, const uint32_t* __restrict__ tok,
-                                                                         const DecodeState* __restrict__ st, int first, aha_logprobs* __restrict__ out,
-                                                                         int by_index, int out_cap) {
+// stage 2 of one row, run by a CTA of kLpMaxParts threads: the row's P slice results pr / pi (n candidates each) -> record `rec` for token t
+// at `index`; xt: the row's logit of t (nullptr: t is outside the vocabulary, logprob -inf)
+__device__ __forceinline__ void lp_final_record(const float* __restrict__ pr, const int* __restrict__ pi, int P, int n, uint32_t t, const float* xt,
+                                                int index, aha_logprobs* __restrict__ rec) {
     __shared__ float rv[kLpMaxParts / 32];
     __shared__ int ri[kLpMaxParts / 32];
     __shared__ float s_lse;
-    const int row = blockIdx.x, tid = threadIdx.x;
-    const int slot = act ? act[row] : 0;
-    const int n = on[slot] - 1;
-    if (n < 0) return;
-    const float* pr = part + (size_t)row * P * kLpPartFloats;
-    const int* pi = part_id + (size_t)row * P * kLpMaxTop;
-    const int index = first ? 0 : st[slot].n_hist - 1;
-    aha_logprobs* rec = out + (by_index ? index : slot);
-    if (by_index && (index < 0 || index >= out_cap)) return;
+    const int tid = threadIdx.x;
     if (tid == 0) {
         float M = -INFINITY;
         for (int p = 0; p < P; ++p) M = fmaxf(M, pr[(size_t)p * kLpPartFloats]);
@@ -139,10 +130,9 @@ __global__ void __launch_bounds__(kLpMaxParts) logprob_final_rows_kernel(const f
         }
         const float lse = M + logf(S);
         s_lse = lse;
-        const uint32_t t = tok[slot];
         rec->token = t;
         rec->index = (uint32_t)index;
-        rec->logprob = t < (uint32_t)V ? logits[(size_t)row * ld + t] - lse : -INFINITY;
+        rec->logprob = xt ? *xt - lse : -INFINITY;
         rec->n_top = (uint32_t)n;
         rec->valid = 1u;
         rec->reserved = 0u;
@@ -160,6 +150,34 @@ __global__ void __launch_bounds__(kLpMaxParts) logprob_final_rows_kernel(const f
         if (tid == 0) { rec->top_ids[r] = bi == kLpNone ? 0u : (uint32_t)bi; rec->top_logprobs[r] = bv - lse; }
     }
     for (int r = n + tid; r < kLpMaxTop; r += kLpMaxParts) { rec->top_ids[r] = 0u; rec->top_logprobs[r] = 0.f; }
+}
+
+__global__ void __launch_bounds__(kLpMaxParts) logprob_final_rows_kernel(const float* __restrict__ logits, int ld, int V, int P, const int* __restrict__ act,
+                                                                         const int* __restrict__ on, const float* __restrict__ part,
+                                                                         const int* __restrict__ part_id, const uint32_t* __restrict__ tok,
+                                                                         const DecodeState* __restrict__ st, int first, aha_logprobs* __restrict__ out,
+                                                                         int by_index, int out_cap) {
+    const int row = blockIdx.x;
+    const int slot = act ? act[row] : 0;
+    const int n = on[slot] - 1;
+    if (n < 0) return;
+    const int index = first ? 0 : st[slot].n_hist - 1;
+    if (by_index && (index < 0 || index >= out_cap)) return;
+    const uint32_t t = tok[slot];
+    lp_final_record(part + (size_t)row * P * kLpPartFloats, part_id + (size_t)row * P * kLpMaxTop, P, n, t,
+                    t < (uint32_t)V ? logits + (size_t)row * ld + t : nullptr, index, out + (by_index ? index : slot));
+}
+
+// stage 2 of scored rows (score_head.cuh): row r's record for token tgt[r] at index[r] goes to out[r].  Its logit is tlogit[r] (written by
+// score_head_kernel) or, when tlogit is nullptr, logits[r * ld + tgt[r]] (a logits block from gemm_tc).  tgt[r] < V.
+__global__ void __launch_bounds__(kLpMaxParts) score_final_rows_kernel(const float* __restrict__ part, const int* __restrict__ part_id, int P, int n,
+                                                                       const uint32_t* __restrict__ tgt, const float* __restrict__ tlogit,
+                                                                       const float* __restrict__ logits, int ld, const uint32_t* __restrict__ index,
+                                                                       aha_logprobs* __restrict__ out) {
+    const int row = blockIdx.x;
+    const uint32_t t = tgt[row];
+    lp_final_record(part + (size_t)row * P * kLpPartFloats, part_id + (size_t)row * P * kLpMaxTop, P, n, t,
+                    tlogit ? tlogit + row : logits + (size_t)row * ld + t, (int)index[row], out + row);
 }
 
 // the two stages over `rows` logits rows (ld floats apart); part / part_id: [rows][lp_parts(V)] candidate lists

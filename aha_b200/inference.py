@@ -436,6 +436,50 @@ class B200Model:
                                                    out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
 
+    # ------------------------------------------------------------------ scoring given text
+    def score(self, input_ids, start=1, top=0):
+        """Log-probability of every token of input_ids from position `start` on (aha_b200_score): entry k is token input_ids[start + k]
+        under the model given the tokens before it.  -> dict of numpy arrays: tokens (n,) uint32, logprobs (n,) float32 and, with top > 0,
+        top_ids (n, top) uint32 and top_logprobs (n, top) float32 (the top alternatives at each position, by logit desc, id asc)."""
+        ids = self._ids(input_ids)
+        n = max(ids.size - int(start), 0)
+        recs = np.zeros(max(n, 1), L.LOGPROBS_DTYPE)
+        got = C.c_size_t()
+        self._check(self._lib.aha_b200_score(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint32)), ids.size, int(start), int(top),
+                                             recs.ctypes.data_as(C.POINTER(L.Logprobs)), n, C.byref(got)))
+        return L.score_arrays(recs[:got.value], top)
+
+    def score_batch(self, list_of_ids, starts=None, top=0):
+        """score() for many texts packed into shared prefills (aha_b200_score_batch) -> one dict of arrays per text, in input order.
+        starts: one start per text (None: 1 for every text)."""
+        texts = [self._ids(t) for t in list_of_ids]
+        if starts is not None and len(starts) != len(texts):
+            raise ValueError(f"{len(starts)} starts for {len(texts)} texts")
+        st = [1] * len(texts) if starts is None else [int(s) for s in starts]
+        counts = [max(t.size - s, 0) for t, s in zip(texts, st)]
+        cat = np.ascontiguousarray(np.concatenate(texts)) if texts else np.zeros(0, np.uint32)
+        lens = (C.c_size_t * max(len(texts), 1))(*[t.size for t in texts])
+        c_starts = (C.c_size_t * max(len(texts), 1))(*st)
+        recs = np.zeros(max(sum(counts), 1), L.LOGPROBS_DTYPE)
+        got = C.c_size_t()
+        self._check(self._lib.aha_b200_score_batch(self._h, cat.ctypes.data_as(C.POINTER(C.c_uint32)), lens, c_starts, len(texts), int(top),
+                                                   recs.ctypes.data_as(C.POINTER(L.Logprobs)), sum(counts), C.byref(got)))
+        bounds = np.cumsum([0] + counts)
+        return [L.score_arrays(recs[bounds[j]:bounds[j + 1]], top) for j in range(len(texts))]
+
+    def debug_score_head(self, hidden, targets, top=0, impl=0):
+        """The scoring head alone on pre-norm hidden rows [M, H] (tests): impl 0 = score_head_kernel, 1 = the gemm_tc + row-kernel twin.
+        -> dict of arrays as score(), row r scored at targets[r]."""
+        x = np.ascontiguousarray(hidden, np.float32).reshape(-1, self.hidden_size)
+        tg = np.ascontiguousarray(targets, np.uint32).reshape(-1)
+        if tg.size != x.shape[0]:
+            raise ValueError("one target per row")
+        recs = np.zeros(x.shape[0], L.LOGPROBS_DTYPE)
+        self._check(self._lib.aha_b200_debug_score_head(self._h, int(impl), x.ctypes.data_as(C.POINTER(C.c_float)), x.shape[0],
+                                                        tg.ctypes.data_as(C.POINTER(C.c_uint32)), int(top),
+                                                        recs.ctypes.data_as(C.POINTER(L.Logprobs))))
+        return L.score_arrays(recs, top)
+
     def rerank(self, query_ids, documents_ids):
         """Qwen3Reranker::rerank on token ids -> cosine scores (n_docs,) float32."""
         q = self._ids(query_ids)

@@ -398,6 +398,22 @@ int aha_b200_embed_batch(aha_model* m, const uint32_t* ids, const size_t* lens, 
 int aha_b200_rerank(aha_model* m, const uint32_t* query_ids, size_t query_len, const uint32_t* doc_ids, const size_t* doc_lens,
                     size_t n_docs, float* scores_out);
 
+/* Scoring given text (new design; the reference has no prompt log-probabilities): OpenAI `echo` + `logprobs`, evaluation harnesses
+ * (lm-eval loglikelihood and is_greedy), perplexity, label likelihoods.
+ * Log-probability of every given token from position `start` on: record i - start holds token ids[i], index i,
+ * logprob = log p(ids[i] | ids[0..i)) and the n_top alternatives at that position (aha_logprobs semantics: raw model distribution,
+ * (logit desc, id asc)).  1 <= start < seq_len <= max_ctx; prompts longer than max_prefill run as continuation chunks.  "qwen3" and
+ * "qwen3vl" handles with text-only ids (Qwen3-VL positions of a text-only prompt), single GPU, no open batch session, n_top <= 20 and
+ * <= V, cap >= seq_len - start.  Everything is refused before any device work.  The cache is cleared before and after, like
+ * aha_b200_embed. */
+int aha_b200_score(aha_model* m, const uint32_t* ids, size_t seq_len, size_t start, uint32_t n_top, aha_logprobs* out, size_t cap,
+                   size_t* n_out);
+/* The same for n texts packed into shared prefills (each text attends only to itself); starts == NULL means 1 for every text.  Records
+ * text by text in input order, `index` relative to the text; *n_out = sum of (lens[j] - starts[j]).  A text longer than
+ * min(max_prefill, max_ctx) is scored alone inside the same call. */
+int aha_b200_score_batch(aha_model* m, const uint32_t* ids, const size_t* lens, const size_t* starts, size_t n, uint32_t n_top,
+                         aha_logprobs* out, size_t cap, size_t* n_out);
+
 /* Tensor parallelism (new design; the reference has none): rank 0 creates a 128-byte ncclUniqueId, the host side
  * distributes it (bench.py broadcasts it between the per-GPU processes) and every rank passes it in aha_options.tp_comm together
  * with tp_rank / tp_world.  Heads and MLP rows are sharded; the only exchange steps are all-reduce(sum) after
@@ -442,13 +458,19 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
                           double* device_ms /* CUDA-event time of the n_steps on the launching stream, may be NULL */);
 /* Time one kernel of the decode step in isolation (CUDA events on the launching stream), cycling over the
  * layers' weights so that consecutive launches never hit L2.  which = "gemv_gate_up" | "gemv_qkv" |
- * "gemv_down" | "gemv_o" | "gemv_lm_head" | "decode_attn".  bytes_per_launch = algorithmic bytes. */
+ * "gemv_down" | "gemv_o" | "gemv_lm_head" | "decode_attn", or the scoring head over rows 0 .. M-1 of the last prefill with n
+ * alternatives: "score_head:M:n" (score_head_kernel) | "score_twin:M:n" (gemm_tc + logprob_partial_rows_kernel), each with its final
+ * RMSNorm and stage 2.  bytes_per_launch = algorithmic bytes (the score entries: the lm_head's). */
 /* the device sampler on a given logits row (tests): context = tokens generated so far, draw_index = draws already consumed */
 int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_params* params, const uint32_t* context,
                           size_t n_context, uint32_t draw_index, uint32_t* token_out);
 /* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
 int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);
+/* tests: the scoring head alone on given pre-norm hidden rows [M][H] (final RMSNorm, head, records; row r scored at targets[r], index r);
+ * impl 0 = score_head_kernel, 1 = the gemm_tc + row-kernel twin (a [M][V] logits block, then the generation path's stage-1 kernel) */
+int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_t M, const uint32_t* targets, uint32_t n_top,
+                              aha_logprobs* out);
 /* the verify attention of speculative decoding on host data (tests): `rows` query rows at positions pos0 .. pos0 + rows - 1 over K / V of
  * pos0 + rows positions (laid out on a paged pool with the pages in reverse order), head_dim 128.  q, out: [rows][n_heads][128] (q
  * normalised and rotated); k, v: [pos0 + rows][n_kv_heads][128].  Row r attends to positions 0 .. pos0 + r. */
