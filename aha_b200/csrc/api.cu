@@ -24,6 +24,16 @@ using namespace aha;
 namespace {
 std::mutex g_err_mu;
 std::string g_create_error;
+// the error of a call without a handle, read by aha_b200_last_error(NULL)
+void set_create_error(const char* what) {
+    std::lock_guard<std::mutex> lk(g_err_mu);
+    g_create_error = what;
+}
+template <typename F>
+int guarded_host(F&& f) {   // host-only entries (no handle)
+    try { f(); return 0; }
+    catch (const std::exception& e) { set_create_error(e.what()); return 1; }
+}
 }  // namespace
 
 struct aha_model {
@@ -99,7 +109,7 @@ int guarded(aha_model* m, F&& f) {
         return 0;
     } catch (const std::exception& e) {
         if (m) m->last_error = e.what();
-        else { std::lock_guard<std::mutex> lk(g_err_mu); g_create_error = e.what(); }
+        else set_create_error(e.what());
         // leave the stream usable: drop a dangling capture, clear sticky launch errors
         if (m && m->ctx.stream) {
             cudaStreamCaptureStatus cs;
@@ -309,6 +319,52 @@ std::vector<uint32_t> mm_token_ids(const aha_model* m) {
 void require_no_session(aha_model* m) {
     AHA_REQUIRE(!m->session.open, "a batch session is open on this handle: call aha_b200_batch_close first");
 }
+// the tensors a multimodal request must carry, present or empty (a qwen3 handle ignores them)
+void require_mm_arity(const aha_model* m, const aha_mm* mm) {
+    if (m->kind == aha_model::QWEN3VL) AHA_REQUIRE(mm && mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
+    if (m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(mm && mm->n == 1, "Qwen3 asr process data error, must have input_features");
+}
+// `for _ in 1..sample_len` (generate.rs): max_tokens 0 and 1 both yield exactly one token
+size_t token_budget(const aha_gen_params& p) { return std::max<size_t>(p.max_tokens, 1); }
+// the M-RoPE offset of the decode positions (rope_deltas; 0 for the models without one)
+int decode_rope_delta(const aha_model* m) { return m->kind == aha_model::QWEN3VL ? m->rope_delta : 0; }
+// device memory of one call, freed when the call returns or throws
+struct Scratch {
+    std::vector<void*> ptrs;
+    Scratch() = default;
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { for (void* p : ptrs) cudaFree(p); }
+    template <typename T>
+    T* alloc(size_t n) {
+        void* p = nullptr;
+        AHA_CUDA_CHECK(cudaMalloc(&p, n * sizeof(T)));
+        ptrs.push_back(p);
+        return static_cast<T*>(p);
+    }
+};
+// device time (ms) of launch(0) .. launch(n - 1) between ev0 and ev1 on the model's stream; warm-ups are the caller's
+template <typename F>
+float timed_ms(aha_model* m, size_t n, F&& launch) {
+    cudaStream_t st = m->ctx.stream;
+    AHA_CUDA_CHECK(cudaEventRecord(m->ev0, st));
+    for (size_t i = 0; i < n; ++i) launch(i);
+    AHA_CUDA_CHECK(cudaEventRecord(m->ev1, st));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1));
+    return ms;
+}
+using clk = std::chrono::steady_clock;
+double seconds(clk::duration d) { return std::chrono::duration<double>(d).count(); }
+void add_usage(aha_usage* u, size_t prompt_tokens, size_t completion_tokens, double prompt_secs, double completion_secs, double vision_secs) {
+    if (!u) return;
+    u->prompt_tokens += (uint32_t)prompt_tokens;
+    u->completion_tokens += (uint32_t)completion_tokens;
+    u->prompt_secs += prompt_secs;
+    u->completion_secs += completion_secs;
+    u->vision_secs += vision_secs;
+}
 bool env_flag(const char* name, bool dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) != 0 : dflt; }
 int env_int(const char* name, int dflt) { const char* v = std::getenv(name); return v ? std::atoi(v) : dflt; }
 // AHA_GEN_LOGPROBS / AHA_GEN_TOP_LOGPROBS(n) of a request: -1 = no records, else the top count n (bits 8 and up of flags, unmasked)
@@ -342,6 +398,13 @@ void drop_cache(aha_model* m) {
     m->cached_ids.clear();
     m->cached_mm_fp = 0;
 }
+// model.clear_cache() (generate.rs:147) when a single request ends -- also on the error path, so that a failed request never leaves
+// rope_delta / pages behind -- unless the request keeps its K/V for the next one (REUSE_PREFIX)
+struct RequestReset {
+    aha_model* m;
+    bool keep = false;
+    ~RequestReset() { if (!keep) drop_cache(m); m->text.clear_sampler(); }
+};
 // ends the batch session, if one is open, and leaves the handle as clear_cache() does
 void session_close(aha_model* m) {
     for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->reset();
@@ -419,7 +482,6 @@ void forward_prefill(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S,
     bool embeds_ready = false;
     m->last_vision_secs = 0;
     if (m->kind == aha_model::QWEN3VL) {
-        if (initial) AHA_REQUIRE(mm && mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
         const aha_tensor_desc* pv = initial ? mm_entry(mm, 0) : nullptr;
         const aha_tensor_desc* thw = initial ? mm_entry(mm, 1) : nullptr;
         const aha_tensor_desc* pvv = initial ? mm_entry(mm, 2) : nullptr;
@@ -486,7 +548,6 @@ void forward_prefill(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S,
             for (int r = 0; r < 3; ++r) for (size_t i = 0; i < S; ++i) pos3[(size_t)r * S + i] = (int)(i + offset) + m->rope_delta;
         }
     } else if (m->kind == aha_model::QWEN3_ASR) {
-        if (initial) AHA_REQUIRE(mm && mm->n == 1, "Qwen3 asr process data error, must have input_features");
         const aha_tensor_desc* feat = initial ? mm_entry(mm, 0) : nullptr;
         if (feat) {
             AHA_REQUIRE(feat->rank == 2 && feat->shape[0] == m->audio.cfg.mel, "input_features must be (num_mel_bins, frames)");
@@ -548,13 +609,12 @@ void forward_any(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, siz
     AHA_REQUIRE(ids != nullptr && S >= 1, "input_ids must hold at least one token");
     AHA_REQUIRE(offset + S <= (size_t)T.max_ctx, "context exceeds max_ctx");
     const bool has_mm = initial && mm && ((m->kind == aha_model::QWEN3VL && (mm_entry(mm, 0) || mm_entry(mm, 2))) || (m->kind == aha_model::QWEN3_ASR && mm_entry(mm, 0)));
-    if (initial && m->kind == aha_model::QWEN3VL) AHA_REQUIRE(mm && mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
-    if (initial && m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(mm && mm->n == 1, "Qwen3 asr process data error, must have input_features");
+    if (initial) require_mm_arity(m, mm);
     if (S == 1 && !has_mm && !extend && &pt == &T.table && (m->kind != aha_model::QWEN3VL || m->have_rope_delta)) {
         // decode step: single token against the cache
         AHA_REQUIRE(ids[0] < (uint32_t)T.cfg.V, "token id out of range");
         T.pages.map(T.table, (int)offset + 1);
-        T.set_state(ids[0], (int)offset, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 0);
+        T.set_state(ids[0], (int)offset, decode_rope_delta(m), 0);
         T.decode_step(logits_out != nullptr);
     } else {
         // The reference builds an (S,S) causal mask with offset 0 for every multi-token call
@@ -570,6 +630,44 @@ void forward_any(aha_model* m, PageTable& pt, const uint32_t* ids, size_t S, siz
         float ms = 0.f;
         if (cudaEventElapsedTime(&ms, m->ev0, m->ev1) == cudaSuccess) m->last_vision_secs = ms * 1e-3;
     }
+}
+
+// A request's first token (forward_initial + sample_and_push): its sampler is set on the model against an empty history at draw index
+// draws0, the prompt is prefilled on `pt` -- from `hit` on, as a continuation, when the cache already holds ids[0, hit) -- and the token is
+// drawn from the last row's logits.
+uint32_t first_token(aha_model* m, PageTable& pt, const uint32_t* ids, size_t seq_len, size_t hit, const aha_mm* mm, const Sampler& samp,
+                     uint32_t draws0) {
+    TextModel& T = m->text;
+    T.set_sampler(samp);
+    T.set_state(0, 0, 0, 0, draws0);    // empty history: the first token sees no repeat-penalty context
+    uint32_t tok = 0;
+    if (hit > 0) forward_any(m, pt, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
+    else forward_any(m, pt, ids, seq_len, 0, mm, true, nullptr, &tok);
+    T.check_sample_error();
+    return tok;
+}
+
+// The handoff to decode after first_token: every page positions [0, ctx) can touch is mapped on `pt` (the step kernels only read the
+// table), and the decode state starts from `tok` at position seq_len, with history[0] = tok and the draw index the first token left.  The
+// state is the model's own, or batch slot `slot`'s.
+void handoff(aha_model* m, PageTable& pt, size_t ctx, uint32_t tok, size_t seq_len, int slot = -1) {
+    TextModel& T = m->text;
+    T.pages.map(pt, (int)ctx);
+    DecodeState cur;
+    AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
+    if (slot >= 0) {
+        m->sess().adopt(slot, tok, (int)seq_len, decode_rope_delta(m), cur.n_draws);
+        return;
+    }
+    T.set_state(tok, (int)seq_len, decode_rope_delta(m), 1, cur.n_draws);
+    AHA_CUDA_CHECK(cudaMemcpy(T.d_history, &tok, sizeof(uint32_t), cudaMemcpyHostToDevice));
+}
+
+// a request that asks for records (lp_n >= 0 alternatives each); a burst's records are staged in pinned memory
+void request_logprobs(aha_model* m, int lp_n) {
+    if (lp_n < 0) return;
+    m->text.set_logprobs(lp_n);
+    if (!m->h_lp_pin) AHA_CUDA_CHECK(cudaMallocHost(&m->h_lp_pin, 32 * sizeof(aha_logprobs)));
 }
 
 }  // namespace
@@ -660,10 +758,7 @@ int aha_b200_create(const char* kind, const char* config_json, const aha_tensor_
         *out = m;
         return 0;
     } catch (const std::exception& e) {
-        {
-            std::lock_guard<std::mutex> lk(g_err_mu);
-            g_create_error = e.what();
-        }
+        set_create_error(e.what());
         cudaGetLastError();
         if (m) aha_b200_destroy(m);
         return 1;
@@ -709,15 +804,6 @@ size_t aha_b200_stop_token_ids(aha_model* m, uint32_t* out, size_t cap) {
 
 namespace {
 
-// get_logit_processor (sample.rs:7-38): which Sampling the request's parameters select
-int sampling_mode(const aha_gen_params& p) {
-    const bool has_t = !(p.temperature < 1e-7f);
-    const bool has_k = p.top_k > 0, has_p = p.top_p > 0.f;
-    if (!has_t) return SAMPLE_ARGMAX;
-    if (!has_k) return has_p ? SAMPLE_TOPP : SAMPLE_ALL;
-    return has_p ? SAMPLE_TOPK_TOPP : SAMPLE_TOPK;
-}
-
 struct GenSink {   // receives every generated token in order (with its record when the request asked); returns true to stop the request (client went away)
     std::function<bool(uint32_t token, size_t index, const aha_logprobs* lp)> push;
 };
@@ -732,14 +818,10 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     TextModel& T = m->text;
     require_no_session(m);
     const bool lp = lp_n >= 0;
-    if (lp) {
-        T.set_logprobs(lp_n);
-        if (!m->h_lp_pin) AHA_CUDA_CHECK(cudaMallocHost(&m->h_lp_pin, 32 * sizeof(aha_logprobs)));
-    }
-    const size_t sample_len = std::max<size_t>(params.max_tokens, 1);   // `for _ in 1..sample_len`: sample_len 0 and 1 both yield exactly one token
+    request_logprobs(m, lp_n);
+    const size_t sample_len = token_budget(params);
     AHA_REQUIRE(seq_len + sample_len <= (size_t)T.max_ctx,
                 "prompt + max_tokens exceeds max_ctx (the handle's KV capacity, aha_options.max_ctx; the reference's cache is unbounded)");
-    using clk = std::chrono::steady_clock;
     const auto t0 = clk::now();   // prompt_secs covers everything up to the first token, the prefix lookup (fingerprint of the tensors) included
     const bool eos_on_first = (params.flags & AHA_GEN_EOS_ON_FIRST) != 0;
     // KV reuse (AHA_GEN_REUSE_PREFIX): how much of this prompt the cache already holds.  Every path that is not a hit starts from
@@ -756,25 +838,15 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     m->cached_ids.clear();   // the cache is being written: nothing is reusable until this request has completed
     m->last_prefix_hit = hit;
     std::vector<uint32_t> produced;   // what the request generated (the K/V of all but the last token end up in the cache)
-    struct Reset {   // model.clear_cache() (generate.rs:147) -- also on the error path, so that a failed request never leaves rope_delta / pages behind
-        aha_model* m;
-        bool keep = false;
-        ~Reset() { if (!keep) drop_cache(m); m->text.clear_sampler(); }
-    } reset{m};
-    const int mode = sampling_mode(params);
+    RequestReset reset{m};
     uint32_t draws0 = 0;
     if ((params.flags & AHA_GEN_CONTINUE_RNG) != 0) {   // one LogitsProcessor across the chunks of a request: keep its stream position
         DecodeState cur;
         AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
         draws0 = cur.n_draws;
     }
-    T.set_sampler(mode, params.temperature, params.top_p, params.top_k, params.repeat_penalty, params.repeat_last_n, params.seed);
-    T.set_state(0, 0, 0, 0, draws0);    // empty history: the first token sees no repeat-penalty context
     auto is_eos = [&](uint32_t t) { for (uint32_t e : m->stop_ids) if (e == t) return true; return false; };
-    uint32_t tok = 0;
-    if (hit > 0) forward_any(m, T.table, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
-    else forward_any(m, T.table, ids, seq_len, 0, mm, true, nullptr, &tok);   // forward_initial + sample_and_push
-    T.check_sample_error();
+    const uint32_t tok = first_token(m, T.table, ids, seq_len, hit, mm, make_sampler(params, T.cfg.V), draws0);
     if (lp) {   // the first token's record, from the prefill logits
         T.logprobs(true, T.d_lp, true);
         AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_lp_pin, T.d_lp, sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
@@ -786,11 +858,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
     produced.push_back(tok);
     bool stop = sink.push(tok, 0, lp ? m->h_lp_pin : nullptr) || (eos_on_first && is_eos(tok));   // generate_generic never EOS-checks the first token; the ASR loop does
     if (sample_len > 1 && !stop) {
-        T.pages.map(T.table, (int)(seq_len + sample_len));
-        DecodeState cur;
-        AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
-        T.set_state(tok, (int)seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 1, cur.n_draws);
-        AHA_CUDA_CHECK(cudaMemcpy(T.d_history, &tok, sizeof(uint32_t), cudaMemcpyHostToDevice));   // history[0] = first token (penalty context)
+        handoff(m, T.table, seq_len + sample_len, tok, seq_len);
         const size_t burst_max = stream ? (size_t)aha_model::kStreamBurst : 32;
         while (done < sample_len && !stop) {
             const size_t n = std::min<size_t>(burst_max, sample_len - done);
@@ -830,13 +898,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
         reset.keep = true;
     }
     if (n_generated) *n_generated = done;
-    if (usage) {
-        usage->prompt_tokens += (uint32_t)seq_len;
-        usage->completion_tokens += (uint32_t)done;
-        usage->prompt_secs += std::chrono::duration<double>(t1 - t0).count();
-        usage->completion_secs += std::chrono::duration<double>(t2 - t1).count();
-        usage->vision_secs += vision_secs;
-    }
+    add_usage(usage, seq_len, done, seconds(t1 - t0), seconds(t2 - t1), vision_secs);
 }
 
 // generate_impl's request in verify passes (speculative.cuh): the same prefill, first token, Reset guard and Usage split; then passes of
@@ -862,44 +924,31 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
                 who + "REUSE_PREFIX, CONTINUE_RNG and EOS_ON_FIRST are not supported with speculative decoding");
     const int lp_n = logprob_request(params, T, who);
     AHA_REQUIRE(lp_n < 0 || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
-    const size_t sample_len = std::max<size_t>(params.max_tokens, 1);
+    const size_t sample_len = token_budget(params);
     AHA_REQUIRE(cap >= sample_len, who + "out_tokens capacity is smaller than max_tokens");
     const size_t need = seq_len + sample_len + sp.max_draft;
     AHA_REQUIRE(need <= (size_t)T.max_ctx, who + "prompt + max_tokens + max_draft = " + std::to_string(need) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     const int R = (int)sp.max_draft + 1;
     SpecDecoder& S = m->spec;
     S.init(T, m->wide_batch);
-    if (lp_n >= 0) {
-        T.set_logprobs(lp_n);
-        if (!m->h_lp_pin) AHA_CUDA_CHECK(cudaMallocHost(&m->h_lp_pin, 32 * sizeof(aha_logprobs)));
-    }
-    using clk = std::chrono::steady_clock;
+    request_logprobs(m, lp_n);
     const auto t0 = clk::now();
     drop_cache(m);
     m->last_prefix_hit = 0;
-    struct Reset {
-        aha_model* m;
-        ~Reset() { drop_cache(m); m->text.clear_sampler(); }
-    } reset{m};
-    T.set_sampler(sampling_mode(params), params.temperature, params.top_p, params.top_k, params.repeat_penalty, params.repeat_last_n, params.seed);
-    T.set_state(0, 0, 0, 0, 0);
-    uint32_t tok = 0;
-    forward_any(m, T.table, ids, seq_len, 0, mm, true, nullptr, &tok);
-    T.check_sample_error();
+    RequestReset reset{m};
+    const Sampler samp = make_sampler(params, T.cfg.V);
+    const uint32_t tok = first_token(m, T.table, ids, seq_len, 0, mm, samp, 0);
     if (lp_n >= 0) T.logprobs(true, T.d_lp, true);   // record 0, from the prefill logits
     const auto t1 = clk::now();
     const double vision_secs = m->last_vision_secs;
     SpecCtl ctl{};
     size_t E = 1;
     if (sample_len > 1) {
-        T.pages.map(T.table, (int)need);
-        DecodeState cur;
-        AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
-        T.set_state(tok, (int)seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 1, cur.n_draws);
-        AHA_CUDA_CHECK(cudaMemcpy(T.d_history, &tok, sizeof(uint32_t), cudaMemcpyHostToDevice));
+        handoff(m, T.table, need, tok, seq_len);
         const std::vector<uint32_t> pred(sp.prediction, sp.prediction + sp.n_prediction);
         const bool lookup = (sp.flags & AHA_SPEC_PROMPT_LOOKUP) != 0;
-        S.prepare(R, pred, ids, lookup ? seq_len : 0, m->stop_ids, (int)sample_len, ngram, lp_n >= 0 ? lp_n + 1 : 0);
+        S.prepare(R, samp, pred, ids, lookup ? seq_len : 0, m->stop_ids, (int)sample_len, ngram, lp_n >= 0 ? lp_n + 1 : 0);
+        DecodeState cur;
         while (true) {
             // a pass emits 1 .. R tokens: never launch more passes than the remaining budget could need at R tokens each
             const size_t burst = std::min<size_t>(8, std::max<size_t>(1, (sample_len - E + R - 1) / R));
@@ -918,13 +967,7 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
     const auto t2 = clk::now();
     *n_out = E;
     if (stats) { *stats = aha_spec_stats{}; stats->passes = ctl.passes; stats->drafted = ctl.drafted; stats->accepted = ctl.accepted; }
-    if (usage) {
-        usage->prompt_tokens += (uint32_t)seq_len;
-        usage->completion_tokens += (uint32_t)E;
-        usage->prompt_secs += std::chrono::duration<double>(t1 - t0).count();
-        usage->completion_secs += std::chrono::duration<double>(t2 - t1).count();
-        usage->vision_secs += vision_secs;
-    }
+    add_usage(usage, seq_len, E, seconds(t1 - t0), seconds(t2 - t1), vision_secs);
 }
 
 }  // namespace
@@ -938,21 +981,16 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
     BatchDecoder& B = m->sess();
     PageTable& pt = B.slots[slot].table;
     m->have_rope_delta = false; m->rope_delta = 0;
-    T.set_sampler(sampling_mode(r.params), r.params.temperature, r.params.top_p, r.params.top_k, r.params.repeat_penalty, r.params.repeat_last_n, r.params.seed);
-    T.set_state(0, 0, 0, 0, 0);
-    uint32_t tok = 0;
-    forward_any(m, pt, r.ids, r.seq_len, 0, r.mm, true, nullptr, &tok);
-    T.check_sample_error();
+    const Sampler samp = make_sampler(r.params, T.cfg.V);
+    const uint32_t tok = first_token(m, pt, r.ids, r.seq_len, 0, r.mm, samp, 0);
     if (lp_n >= 0) {   // the first token's record goes straight into the slot's record row
         T.set_logprobs(lp_n);
         B.ensure_lp();
         T.logprobs(true, B.d_lp_rec + slot, false);
     }
     B.slots[slot].lp = lp_n + 1;
-    T.pages.map(pt, (int)(r.seq_len + sample_len));       // every page the request can touch is mapped now (the step kernels only read the table)
-    DecodeState cur;
-    AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
-    B.adopt(slot, tok, (int)r.seq_len, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, cur.n_draws);
+    B.bind_sampler(slot, samp);
+    handoff(m, pt, r.seq_len + sample_len, tok, r.seq_len, slot);
     return tok;
 }
 
@@ -1028,9 +1066,8 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         lp_n[i] = logprob_request(r.params, T, who + "request " + std::to_string(i) + ": ");
         for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
         AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-        if (m->kind == aha_model::QWEN3VL) AHA_REQUIRE(r.mm && r.mm->n == 5, "Qwen3VL process data error, must have pixel_values, image_grid_thw, pixel_values_video, video_grid_thw, cache_position");
-        if (m->kind == aha_model::QWEN3_ASR) AHA_REQUIRE(r.mm && r.mm->n == 1, "Qwen3 asr process data error, must have input_features");
-        sample_len[i] = std::max<size_t>(r.params.max_tokens, 1);
+        require_mm_arity(m, r.mm);
+        sample_len[i] = token_budget(r.params);
         pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
         bool has_mm = false;   // (a qwen3 handle ignores the tensors)
         for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
@@ -1042,7 +1079,6 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         const size_t ctx = reqs[i].seq_len + sample_len[i];
         AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     }
-    using clk = std::chrono::steady_clock;
     const auto t0 = clk::now();
     struct Guard {   // a failure leaves the session as it was: every slot this call took is released with its pages
         aha_model* m; const std::vector<int>& slots;
@@ -1091,9 +1127,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         // first tokens: batched lm_head over the gathered rows, then each request's ArgMax / sampler against an empty state (forward_any's draw)
         std::vector<int> act;
         for (size_t i : pk) {
-            const aha_gen_params& p = reqs[i].params;
-            T.set_sampler(sampling_mode(p), p.temperature, p.top_p, p.top_k, p.repeat_penalty, p.repeat_last_n, p.seed);
-            B.bind_sampler(slot[i]);
+            B.bind_sampler(slot[i], make_sampler(reqs[i].params, T.cfg.V));
             B.slots[slot[i]].lp = lp_n[i] + 1;
             if (lp_n[i] >= 0) B.ensure_lp();
             act.push_back(slot[i]);
@@ -1107,10 +1141,8 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
         T.check_sample_error();
-        const double t_first = std::chrono::duration<double>(clk::now() - t0).count();
-        for (size_t i : pk) {
-            const aha_gen_params& p = reqs[i].params;
-            T.set_sampler(sampling_mode(p), p.temperature, p.top_p, p.top_k, p.repeat_penalty, p.repeat_last_n, p.seed);
+        const double t_first = seconds(clk::now() - t0);
+        for (size_t i : pk) {   // (their pages were mapped before the prefill)
             B.adopt(slot[i], h_tok[slot[i]], (int)reqs[i].seq_len, 0, h_st[slot[i]].n_draws);
             tok[i] = h_tok[slot[i]];
             secs[i] = t_first;
@@ -1120,7 +1152,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
         tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i]);
-        secs[i] = std::chrono::duration<double>(clk::now() - t0).count();
+        secs[i] = seconds(clk::now() - t0);
         vision[i] = m->last_vision_secs;
     }
     guard.ok = true;
@@ -1135,9 +1167,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         if ((reqs[i].params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[i]) stop = true;
         if (usage) {
             usage[i] = aha_usage{};
-            usage[i].prompt_tokens = (uint32_t)reqs[i].seq_len; usage[i].completion_tokens = 1;
-            usage[i].prompt_secs = secs[i];
-            usage[i].vision_secs = vision[i];
+            add_usage(&usage[i], reqs[i].seq_len, 1, secs[i], 0.0, vision[i]);
         }
         if (stop) session_release(m, s);
         slots_out[i] = s; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
@@ -1185,7 +1215,7 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
         AHA_REQUIRE(reqs[i].ids && reqs[i].seq_len >= 1, "generate_batch: every request needs input_ids");
-        const size_t sample_len = std::max<size_t>(reqs[i].params.max_tokens, 1);
+        const size_t sample_len = token_budget(reqs[i].params);
         AHA_REQUIRE(cap >= sample_len, "out_tokens capacity (per request) is smaller than max_tokens");
         AHA_REQUIRE((reqs[i].params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, "generate_batch: CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
         refuse_logprobs(reqs[i].params, "generate_batch", "a batch session (aha_b200_batch_open, aha_b200_batch_logprobs)");
@@ -1205,7 +1235,6 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
         n_out[i] = 1;
         if (!fin) req_of[slot] = (int)i;
     }
-    using clk = std::chrono::steady_clock;
     const auto t_dec = clk::now();
     uint32_t tok[kGemvBatchMax];
     int32_t status[kGemvBatchMax];
@@ -1214,7 +1243,7 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
             if (!status[slot]) continue;
             const int i = req_of[slot];
             out_tokens[(size_t)i * cap + n_out[i]++] = tok[slot];
-            if (status[slot] == 2 && usage) usage[i].completion_secs = std::chrono::duration<double>(clk::now() - t_dec).count();
+            if (status[slot] == 2 && usage) usage[i].completion_secs = seconds(clk::now() - t_dec);
         }
     }
     if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
@@ -1292,7 +1321,7 @@ int aha_b200_generate(aha_model* m, const uint32_t* ids, size_t seq_len, const a
                       size_t cap, size_t* n_out, aha_usage* usage) {
     return guarded(m, [&] {
         AHA_REQUIRE(params && out_tokens && n_out, "params, out_tokens and n_out are required");
-        AHA_REQUIRE(cap >= std::max<size_t>(params->max_tokens, 1), "out_tokens capacity is smaller than max_tokens");
+        AHA_REQUIRE(cap >= token_budget(*params), "out_tokens capacity is smaller than max_tokens");
         refuse_logprobs(*params, "generate", "aha_b200_generate_logprobs");
         if (usage) *usage = aha_usage{};
         size_t n = 0;
@@ -1339,36 +1368,30 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
         std::vector<DecodeState> st(R);
         for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, {0, 0, 0}};
         const int max_chunks = ceil_div(ctx, kSpecChunk);
-        float *d_pool = nullptr, *d_q = nullptr, *d_out = nullptr, *d_part = nullptr;
-        int* d_table = nullptr;
-        DecodeState* d_st = nullptr;
-        auto cleanup = [&] { cudaFree(d_pool); cudaFree(d_q); cudaFree(d_out); cudaFree(d_part); cudaFree(d_table); cudaFree(d_st); };
-        try {
-            AHA_CUDA_CHECK(cudaMalloc(&d_pool, pool.size() * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_q, (size_t)R * nh * HD * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_out, (size_t)R * nh * HD * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_part, (size_t)R * nh * max_chunks * spec_part_stride(HD) * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_table, np * sizeof(int)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_st, R * sizeof(DecodeState)));
-            AHA_CUDA_CHECK(cudaMemcpy(d_pool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice));
-            AHA_CUDA_CHECK(cudaMemcpy(d_q, q, (size_t)R * nh * HD * sizeof(float), cudaMemcpyHostToDevice));
-            AHA_CUDA_CHECK(cudaMemcpy(d_table, table.data(), np * sizeof(int), cudaMemcpyHostToDevice));
-            AHA_CUDA_CHECK(cudaMemcpy(d_st, st.data(), R * sizeof(DecodeState), cudaMemcpyHostToDevice));
-            SpecAttnArgs a{};
-            a.q = d_q; a.ldq = nh * HD;
-            a.kv.k = d_pool; a.kv.v = d_pool + (size_t)nkv * kPage * HD; a.kv.page_table = d_table; a.kv.page_shift = kPageShift;
-            a.kv.page_stride = page_stride; a.kv.tok_stride = HD; a.kv.head_stride = (size_t)kPage * HD;
-            a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
-            a.R = R; a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
-            AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
-            // few CTAs, so that a CTA walks several chunks
-            spec_verify_attn_kernel<HD><<<dim3(std::min(3, max_chunks), nkv), kSpecAttnThreads, spec_attn_smem_bytes<HD>(), c.stream>>>(a);
-            spec_verify_merge_kernel<HD><<<dim3(nh, R), HD, 0, c.stream>>>(a);
-            AHA_CUDA_CHECK(cudaGetLastError());
-            AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-            AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)R * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
-        } catch (...) { cleanup(); throw; }
-        cleanup();
+        Scratch mem;
+        float* d_pool = mem.alloc<float>(pool.size());
+        float* d_q = mem.alloc<float>((size_t)R * nh * HD);
+        float* d_out = mem.alloc<float>((size_t)R * nh * HD);
+        float* d_part = mem.alloc<float>((size_t)R * nh * max_chunks * spec_part_stride(HD));
+        int* d_table = mem.alloc<int>(np);
+        DecodeState* d_st = mem.alloc<DecodeState>(R);
+        AHA_CUDA_CHECK(cudaMemcpy(d_pool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice));
+        AHA_CUDA_CHECK(cudaMemcpy(d_q, q, (size_t)R * nh * HD * sizeof(float), cudaMemcpyHostToDevice));
+        AHA_CUDA_CHECK(cudaMemcpy(d_table, table.data(), np * sizeof(int), cudaMemcpyHostToDevice));
+        AHA_CUDA_CHECK(cudaMemcpy(d_st, st.data(), R * sizeof(DecodeState), cudaMemcpyHostToDevice));
+        SpecAttnArgs a{};
+        a.q = d_q; a.ldq = nh * HD;
+        a.kv.k = d_pool; a.kv.v = d_pool + (size_t)nkv * kPage * HD; a.kv.page_table = d_table; a.kv.page_shift = kPageShift;
+        a.kv.page_stride = page_stride; a.kv.tok_stride = HD; a.kv.head_stride = (size_t)kPage * HD;
+        a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
+        a.R = R; a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
+        AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
+        // few CTAs, so that a CTA walks several chunks
+        spec_verify_attn_kernel<HD><<<dim3(std::min(3, max_chunks), nkv), kSpecAttnThreads, spec_attn_smem_bytes<HD>(), c.stream>>>(a);
+        spec_verify_merge_kernel<HD><<<dim3(nh, R), HD, 0, c.stream>>>(a);
+        AHA_CUDA_CHECK(cudaGetLastError());
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)R * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
     });
 }
 
@@ -1376,7 +1399,7 @@ int aha_b200_generate_logprobs(aha_model* m, const uint32_t* ids, size_t seq_len
                                uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap, size_t* n_out, aha_usage* usage) {
     return guarded(m, [&] {
         AHA_REQUIRE(params && out_tokens && out_logprobs && n_out, "params, out_tokens, out_logprobs and n_out are required");
-        AHA_REQUIRE(cap >= std::max<size_t>(params->max_tokens, 1), "out_tokens capacity is smaller than max_tokens");
+        AHA_REQUIRE(cap >= token_budget(*params), "out_tokens capacity is smaller than max_tokens");
         const int lp_n = logprob_request(*params, m->text, "generate_logprobs: ");
         AHA_REQUIRE(lp_n >= 0, "generate_logprobs: params.flags must carry AHA_GEN_LOGPROBS");
         if (usage) *usage = aha_usage{};
@@ -1427,7 +1450,7 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
             p.top_k = 0;                                  // get_logit_processor(Some(temperature), top_p, None, seed)
             p.flags |= AHA_GEN_EOS_ON_FIRST;
             if (c > 0) p.flags |= AHA_GEN_CONTINUE_RNG;
-            AHA_REQUIRE(total + std::max<size_t>(p.max_tokens, 1) <= cap, "out_tokens capacity is smaller than n_chunks * max_tokens");
+            AHA_REQUIRE(total + token_budget(p) <= cap, "out_tokens capacity is smaller than n_chunks * max_tokens");
             aha_mm mm{&chunks[c].input_features, 1};
             const size_t base = total;
             bool abort = false;
@@ -1449,8 +1472,7 @@ int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_param
         AHA_REQUIRE(logits && params && token_out && (context || n_context == 0), "logits, params and token_out are required");
         TextModel& T = m->text;
         AHA_REQUIRE(n_context <= (size_t)T.hist_cap, "context longer than the history buffer");
-        const int mode = sampling_mode(*params);
-        T.set_sampler(mode, params->temperature, params->top_p, params->top_k, params->repeat_penalty, params->repeat_last_n, params->seed);
+        T.set_sampler(make_sampler(*params, T.cfg.V));
         AHA_REQUIRE(T.samp_active, "plain ArgMax needs no sampler (temperature < 1e-7 and no repeat penalty)");
         AHA_CUDA_CHECK(cudaMemcpyAsync(T.logits, logits, (size_t)T.cfg.V * sizeof(float), cudaMemcpyHostToDevice, m->ctx.stream));
         if (n_context) AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_history, context, n_context * sizeof(uint32_t), cudaMemcpyHostToDevice, m->ctx.stream));
@@ -1475,14 +1497,10 @@ int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_
         const int on = 1 + (int)n_top;
         const DecodeState ds{token, 0, 0, 0, 0, {0, 0, 0}};
         // scratch of this call only: [V] logits, the candidate lists, the on flag, the token, a state and the record
-        struct Scratch {
-            void* p = nullptr;
-            ~Scratch() { if (p) cudaFree(p); }
-        } mem;
         const size_t o_part = V * sizeof(float), o_id = o_part + (size_t)P * kLpPartFloats * sizeof(float), o_on = o_id + (size_t)P * kLpMaxTop * sizeof(int);
         const size_t o_tok = o_on + 16, o_st = o_tok + 16, o_rec = o_st + sizeof(DecodeState), bytes = o_rec + sizeof(aha_logprobs);
-        AHA_CUDA_CHECK(cudaMalloc(&mem.p, bytes));
-        char* b = static_cast<char*>(mem.p);
+        Scratch mem;
+        char* b = mem.alloc<char>(bytes);
         AHA_CUDA_CHECK(cudaMemcpyAsync(b, logits, V * sizeof(float), cudaMemcpyHostToDevice, st));
         AHA_CUDA_CHECK(cudaMemcpyAsync(b + o_on, &on, sizeof(int), cudaMemcpyHostToDevice, st));
         AHA_CUDA_CHECK(cudaMemcpyAsync(b + o_tok, &token, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
@@ -1505,18 +1523,15 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
         require_no_session(m);
         m->cached_ids.clear();
         T.pages.map(T.table, (int)(seqlen_offset + n_steps));
-        T.set_state(first_token, (int)seqlen_offset, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 0);
-        if (n_steps > 0 && !T.step_graph && T.use_graph) {  // build the graph outside the timed region (pos is restored below)
+        T.set_state(first_token, (int)seqlen_offset, decode_rope_delta(m), 0);
+        if (n_steps > 0 && T.step_graph.size() == 0 && T.use_graph) {  // build the graph outside the timed region (pos is restored below)
             T.decode_step();
-            T.set_state(first_token, (int)seqlen_offset, m->kind == aha_model::QWEN3VL ? m->rope_delta : 0, 0);
+            T.set_state(first_token, (int)seqlen_offset, decode_rope_delta(m), 0);
         }
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev0, m->ctx.stream));
-        for (size_t i = 0; i < n_steps; ++i) T.decode_step();
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev1, m->ctx.stream));
-        if (out_tokens) AHA_CUDA_CHECK(cudaMemcpyAsync(out_tokens, T.d_history, n_steps * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+        const float ms = timed_ms(m, n_steps, [&](size_t) { T.decode_step(); });
+        if (out_tokens) AHA_CUDA_CHECK(cudaMemcpy(out_tokens, T.d_history, n_steps * sizeof(uint32_t), cudaMemcpyDeviceToHost));
         T.check_ll_abort();
-        if (device_ms) { float ms = 0.f; AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1)); *device_ms = ms; }
+        if (device_ms) *device_ms = ms;
     });
 }
 
@@ -1545,13 +1560,7 @@ int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* av
             m->ctx.cnt.kernels++;
         };
         for (int i = 0; i < 3; ++i) launch(i);
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev0, st));
-        for (int i = 0; i < iters; ++i) launch(i + 3);
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev1, st));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
-        float ms = 0.f;
-        AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1));
-        *avg_ms = ms / iters;
+        *avg_ms = timed_ms(m, (size_t)iters, [&](size_t i) { launch((int)i + 3); }) / iters;
         *bytes_per_launch = bytes;
     });
 }
@@ -1618,17 +1627,14 @@ int aha_b200_video_preprocess(aha_model* m, const uint8_t* frames_thwc, size_t n
         const size_t N = (size_t)gt * gh * gw;
         AHA_REQUIRE(N <= (size_t)V.max_patches, "video needs " + std::to_string(N) + " patches, max_patches is " + std::to_string(V.max_patches));
         AHA_REQUIRE(N * V.patch_dim <= cap, "pixel_values_out too small");
-        uint8_t* d_in = nullptr;
         const size_t bytes = n_frames * h * w * 3;
-        AHA_CUDA_CHECK(cudaMalloc(&d_in, bytes));
-        try {
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, frames_thwc, bytes, cudaMemcpyHostToDevice, m->ctx.stream));
-            video_patchify_kernel<<<(unsigned)N, 256, 0, m->ctx.stream>>>(d_in, (int)n_frames, (int)h, (int)w, ps, mg, tp, V.pix);
-            m->ctx.cnt.kernels++;
-            AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        } catch (...) { cudaFree(d_in); throw; }
-        cudaFree(d_in);
+        Scratch mem;
+        uint8_t* d_in = mem.alloc<uint8_t>(bytes);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, frames_thwc, bytes, cudaMemcpyHostToDevice, m->ctx.stream));
+        video_patchify_kernel<<<(unsigned)N, 256, 0, m->ctx.stream>>>(d_in, (int)n_frames, (int)h, (int)w, ps, mg, tp, V.pix);
+        m->ctx.cnt.kernels++;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         grid_thw_out[0] = (uint32_t)gt; grid_thw_out[1] = (uint32_t)gh; grid_thw_out[2] = (uint32_t)gw;
     });
 }
@@ -1642,27 +1648,19 @@ int aha_b200_image_patchify(aha_model* m, const uint8_t* img_hwc, size_t h, size
         const int gh = (int)h / ps, gw = (int)w / ps, N = gh * gw;
         AHA_REQUIRE(N <= V.max_patches, "image exceeds max_patches");
         AHA_REQUIRE((size_t)N * V.patch_dim <= cap, "pixel_values_out too small");
-        uint8_t* d_img = nullptr;
-        AHA_CUDA_CHECK(cudaMalloc(&d_img, h * w * 3));
-        try {
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_img, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
-            patchify_kernel<<<N, 256, 0, m->ctx.stream>>>(d_img, (int)h, (int)w, ps, mg, V.cfg.tpatch, V.pix);
-            m->ctx.cnt.kernels++;
-            AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, (size_t)N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        } catch (...) { cudaFree(d_img); throw; }
-        cudaFree(d_img);
+        Scratch mem;
+        uint8_t* d_img = mem.alloc<uint8_t>(h * w * 3);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_img, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
+        patchify_kernel<<<N, 256, 0, m->ctx.stream>>>(d_img, (int)h, (int)w, ps, mg, V.cfg.tpatch, V.pix);
+        m->ctx.cnt.kernels++;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, (size_t)N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         grid_thw_out[0] = 1; grid_thw_out[1] = (uint32_t)gh; grid_thw_out[2] = (uint32_t)gw;
     });
 }
 
 extern "C++" {
 namespace {
-template <typename F>
-int guarded_host(F&& f) {   // host-only entries (no handle): errors land in the create-error slot read by aha_b200_last_error(NULL)
-    try { f(); return 0; }
-    catch (const std::exception& e) { std::lock_guard<std::mutex> lk(g_err_mu); g_create_error = e.what(); return 1; }
-}
 // resize (h, w, 3) u8 on the device -> (nh, nw, 3) u8 on the device; both buffers owned by the caller
 void resize_on_device(aha_model* m, const uint8_t* d_in, int h, int w, uint8_t* d_out, int nh, int nw, float* d_tmp) {
     if (nh == h && nw == w) {   // imageops::resize copies when the dimensions already match
@@ -1689,17 +1687,14 @@ int aha_b200_img_smart_resize(uint32_t img_h, uint32_t img_w, uint32_t factor, u
 int aha_b200_image_resize(aha_model* m, const uint8_t* img_hwc, size_t h, size_t w, size_t new_h, size_t new_w, uint8_t* out_hwc) {
     return guarded(m, [&] {
         AHA_REQUIRE(img_hwc && out_hwc && h > 0 && w > 0 && new_h > 0 && new_w > 0, "images and positive sizes are required");
-        uint8_t *d_in = nullptr, *d_out = nullptr;
-        float* d_tmp = nullptr;
-        auto cleanup = [&] { cudaFree(d_in); cudaFree(d_out); cudaFree(d_tmp); };
-        try {
-            AHA_CUDA_CHECK(cudaMalloc(&d_in, h * w * 3)); AHA_CUDA_CHECK(cudaMalloc(&d_out, new_h * new_w * 3)); AHA_CUDA_CHECK(cudaMalloc(&d_tmp, new_h * w * 3 * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
-            resize_on_device(m, d_in, (int)h, (int)w, d_out, (int)new_h, (int)new_w, d_tmp);
-            AHA_CUDA_CHECK(cudaMemcpyAsync(out_hwc, d_out, new_h * new_w * 3, cudaMemcpyDeviceToHost, m->ctx.stream));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        } catch (...) { cleanup(); throw; }
-        cleanup();
+        Scratch mem;
+        uint8_t* d_in = mem.alloc<uint8_t>(h * w * 3);
+        uint8_t* d_out = mem.alloc<uint8_t>(new_h * new_w * 3);
+        float* d_tmp = mem.alloc<float>(new_h * w * 3);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
+        resize_on_device(m, d_in, (int)h, (int)w, d_out, (int)new_h, (int)new_w, d_tmp);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(out_hwc, d_out, new_h * new_w * 3, cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
     });
 }
 
@@ -1715,19 +1710,16 @@ int aha_b200_image_preprocess(aha_model* m, const uint8_t* img_hwc, size_t h, si
         const int gh = (int)rh / ps, gw = (int)rw / ps, N = gh * gw;
         AHA_REQUIRE(N <= V.max_patches, "image needs " + std::to_string(N) + " patches after img_smart_resize, max_patches is " + std::to_string(V.max_patches));
         AHA_REQUIRE((size_t)N * V.patch_dim <= cap, "pixel_values_out too small");
-        uint8_t *d_in = nullptr, *d_rs = nullptr;
-        float* d_tmp = nullptr;
-        auto cleanup = [&] { cudaFree(d_in); cudaFree(d_rs); cudaFree(d_tmp); };
-        try {
-            AHA_CUDA_CHECK(cudaMalloc(&d_in, h * w * 3)); AHA_CUDA_CHECK(cudaMalloc(&d_rs, (size_t)rh * rw * 3)); AHA_CUDA_CHECK(cudaMalloc(&d_tmp, (size_t)rh * w * 3 * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
-            resize_on_device(m, d_in, (int)h, (int)w, d_rs, (int)rh, (int)rw, d_tmp);
-            patchify_kernel<<<N, 256, 0, m->ctx.stream>>>(d_rs, (int)rh, (int)rw, ps, mg, V.cfg.tpatch, V.pix);   // img_transform + frame duplication + 9-D permute
-            m->ctx.cnt.kernels++;
-            AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, (size_t)N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        } catch (...) { cleanup(); throw; }
-        cleanup();
+        Scratch mem;
+        uint8_t* d_in = mem.alloc<uint8_t>(h * w * 3);
+        uint8_t* d_rs = mem.alloc<uint8_t>((size_t)rh * rw * 3);
+        float* d_tmp = mem.alloc<float>((size_t)rh * w * 3);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_in, img_hwc, h * w * 3, cudaMemcpyHostToDevice, m->ctx.stream));
+        resize_on_device(m, d_in, (int)h, (int)w, d_rs, (int)rh, (int)rw, d_tmp);
+        patchify_kernel<<<N, 256, 0, m->ctx.stream>>>(d_rs, (int)rh, (int)rw, ps, mg, V.cfg.tpatch, V.pix);   // img_transform + frame duplication + 9-D permute
+        m->ctx.cnt.kernels++;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(pixel_values_out, V.pix, (size_t)N * V.patch_dim * sizeof(float), cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         grid_thw_out[0] = 1; grid_thw_out[1] = (uint32_t)gh; grid_thw_out[2] = (uint32_t)gw;
     });
 }
@@ -1816,32 +1808,29 @@ int aha_b200_resample(aha_model* m, const float* wave, size_t n, int64_t orig_fr
         if (!out) return;
         AHA_REQUIRE(cap >= len_out, "output buffer too small");
         if (len_out == 0) return;
-        float *d_w = nullptr, *d_t = nullptr, *d_o = nullptr;
-        auto cleanup = [&] { cudaFree(d_w); cudaFree(d_t); cudaFree(d_o); };
-        try {
-            cudaStream_t st = m->ctx.stream;
-            AHA_CUDA_CHECK(cudaMalloc(&d_w, std::max<size_t>(n, 1) * sizeof(float))); AHA_CUDA_CHECK(cudaMalloc(&d_t, B.taps.size() * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMalloc(&d_o, len_out * sizeof(float)));
-            AHA_CUDA_CHECK(cudaMemcpyAsync(d_w, wave, n * sizeof(float), cudaMemcpyHostToDevice, st));
-            const size_t smem = B.taps.size() * sizeof(float);
-            const unsigned blocks = (unsigned)((len_out + 255) / 256);
-            if (smem <= 96 * 1024) {   // the whole bank in shared memory
-                AHA_CUDA_CHECK(cudaMemcpyAsync(d_t, B.taps.data(), smem, cudaMemcpyHostToDevice, st));
-                if (smem > 48 * 1024) AHA_CUDA_CHECK(cudaFuncSetAttribute(sinc_resample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                sinc_resample_kernel<true><<<blocks, 256, smem, st>>>(d_w, (long long)n, d_t, B.orig, B.fresh, B.width, B.K, d_o, (long long)len_out);
-            } else {                   // 44.1 kHz and friends: hundreds of KB of taps, read from a transposed copy through the caches
-                std::vector<float> tT(B.taps.size());
-                for (int j = 0; j < B.fresh; ++j) for (int k = 0; k < B.K; ++k) tT[(size_t)k * B.fresh + j] = B.taps[(size_t)j * B.K + k];
-                AHA_CUDA_CHECK(cudaMemcpyAsync(d_t, tT.data(), smem, cudaMemcpyHostToDevice, st));
-                AHA_CUDA_CHECK(cudaStreamSynchronize(st));   // tT is a temporary
-                sinc_resample_kernel<false><<<blocks, 256, 0, st>>>(d_w, (long long)n, d_t, B.orig, B.fresh, B.width, B.K, d_o, (long long)len_out);
-            }
-            AHA_CUDA_CHECK(cudaGetLastError());
-            m->ctx.cnt.kernels++;
-            AHA_CUDA_CHECK(cudaMemcpyAsync(out, d_o, len_out * sizeof(float), cudaMemcpyDeviceToHost, st));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(st));
-        } catch (...) { cleanup(); throw; }
-        cleanup();
+        cudaStream_t st = m->ctx.stream;
+        Scratch mem;
+        float* d_w = mem.alloc<float>(std::max<size_t>(n, 1));
+        float* d_t = mem.alloc<float>(B.taps.size());
+        float* d_o = mem.alloc<float>(len_out);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_w, wave, n * sizeof(float), cudaMemcpyHostToDevice, st));
+        const size_t smem = B.taps.size() * sizeof(float);
+        const unsigned blocks = (unsigned)((len_out + 255) / 256);
+        if (smem <= 96 * 1024) {   // the whole bank in shared memory
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_t, B.taps.data(), smem, cudaMemcpyHostToDevice, st));
+            if (smem > 48 * 1024) AHA_CUDA_CHECK(cudaFuncSetAttribute(sinc_resample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            sinc_resample_kernel<true><<<blocks, 256, smem, st>>>(d_w, (long long)n, d_t, B.orig, B.fresh, B.width, B.K, d_o, (long long)len_out);
+        } else {                   // 44.1 kHz and friends: hundreds of KB of taps, read from a transposed copy through the caches
+            std::vector<float> tT(B.taps.size());
+            for (int j = 0; j < B.fresh; ++j) for (int k = 0; k < B.K; ++k) tT[(size_t)k * B.fresh + j] = B.taps[(size_t)j * B.K + k];
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_t, tT.data(), smem, cudaMemcpyHostToDevice, st));
+            AHA_CUDA_CHECK(cudaStreamSynchronize(st));   // tT is a temporary
+            sinc_resample_kernel<false><<<blocks, 256, 0, st>>>(d_w, (long long)n, d_t, B.orig, B.fresh, B.width, B.K, d_o, (long long)len_out);
+        }
+        AHA_CUDA_CHECK(cudaGetLastError());
+        m->ctx.cnt.kernels++;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(out, d_o, len_out * sizeof(float), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }
 
@@ -1871,100 +1860,72 @@ int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, 
         AHA_REQUIRE(x && w && out && M > 0 && N > 0 && K > 0, "x, w, out and positive sizes are required");
         AHA_REQUIRE((impl >= 1 && impl <= 3) || (impl >= 5 && impl <= 7), "impl must be 1 (SIMT), 2 / 3 (wgmma 128 x 128 / 128 x 256), 5 / 6 (batched GEMV) or 7 (wide batched GEMV)");
         Ctx& c = m->ctx;
-        float *dx = nullptr, *db = nullptr, *dr = nullptr, *dy = nullptr;
-        __half* dw = nullptr;
         const int Nout = epi == EPI_SWIGLU ? N / 2 : N;
-        auto cleanup = [&] { cudaFree(dx); cudaFree(db); cudaFree(dr); cudaFree(dy); cudaFree(dw); };
-        try {
-            AHA_CUDA_CHECK(cudaMalloc(&dx, (size_t)M * K * 4)); AHA_CUDA_CHECK(cudaMalloc(&dw, (size_t)N * K * 2)); AHA_CUDA_CHECK(cudaMalloc(&dy, (size_t)M * Nout * 4));
-            AHA_CUDA_CHECK(cudaMemcpy(dx, x, (size_t)M * K * 4, cudaMemcpyHostToDevice));
-            AHA_CUDA_CHECK(cudaMemcpy(dw, w, (size_t)N * K * 2, cudaMemcpyHostToDevice));
-            if (bias) { AHA_CUDA_CHECK(cudaMalloc(&db, (size_t)N * 4)); AHA_CUDA_CHECK(cudaMemcpy(db, bias, (size_t)N * 4, cudaMemcpyHostToDevice)); }
-            if (epi == EPI_RESID) {
-                AHA_REQUIRE(resid, "resid is required for the residual epilogue");
-                AHA_CUDA_CHECK(cudaMalloc(&dr, (size_t)M * N * 4)); AHA_CUDA_CHECK(cudaMemcpy(dr, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice));
-            }
-            LinearW W; W.w = dw; W.b = db; W.N = N; W.K = K;
-            if (impl == 7) {   // the wide decode projection (gemv_wide.cuh): M <= 64 rows split into fp16 hi / lo operand rows, then the kernel
-                AHA_REQUIRE(M <= kWideSeqs && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "wide batched GEMV: M <= 64, epilogue store / residual / SwiGLU");
-                AHA_REQUIRE(gemv_wide_supported(N, K), "wide batched GEMV: N and K must be multiples of 64");
-                const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
-                __half *hi = nullptr, *lo = nullptr;
-                float *ones = nullptr, *ws = nullptr;
-                int* cnt = nullptr;
-                auto free7 = [&] { cudaFree(hi); cudaFree(lo); cudaFree(ones); cudaFree(ws); cudaFree(cnt); };
-                try {
-                    const size_t xb = (size_t)kWideSeqs * K * sizeof(__half);
-                    AHA_CUDA_CHECK(cudaMalloc(&hi, xb)); AHA_CUDA_CHECK(cudaMalloc(&lo, xb));
-                    AHA_CUDA_CHECK(cudaMemset(hi, 0, xb)); AHA_CUDA_CHECK(cudaMemset(lo, 0, xb));   // rows M..63 stay zero
-                    const size_t wsf = wide_ws_floats(N, K, c.num_sms);
-                    const int tiles = wide_plan(N, K, c.num_sms).tiles;
-                    if (wsf) AHA_CUDA_CHECK(cudaMalloc(&ws, wsf * sizeof(float)));
-                    AHA_CUDA_CHECK(cudaMalloc(&cnt, (size_t)tiles * sizeof(int)));
-                    AHA_CUDA_CHECK(cudaMemset(cnt, 0, (size_t)tiles * sizeof(int)));
-                    if (gepi == GEPI_SWIGLU) {   // (behind a unit-gain RMSNorm prologue, as impl 5)
-                        std::vector<float> h1((size_t)K, 1.0f);
-                        AHA_CUDA_CHECK(cudaMalloc(&ones, (size_t)K * 4)); AHA_CUDA_CHECK(cudaMemcpy(ones, h1.data(), (size_t)K * 4, cudaMemcpyHostToDevice));
-                    }
-                    WideArgs a{};
-                    a.bias = db; a.resid = dr; a.ldr = N; a.out = dy; a.ldo = Nout; a.N = N; a.K = K; a.nb = M; a.ws = ws; a.counters = cnt;
-                    const CUtensorMap tm = make_tmap_f16(dw, (uint64_t)N, (uint64_t)K);
-                    auto run = [&] {
-                        if (ones) rmsnorm_split_kernel<<<M, 256, 0, c.stream>>>(dx, ones, 1e-6f, hi, lo, K);
-                        else split_f32_to_f16x2_kernel<<<(unsigned)(((size_t)M * K / 4 + 255) / 256), 256, 0, c.stream>>>(dx, K, hi, lo, M, K);
-                        gemv_wide(c.stream, gepi, tm, hi, lo, a, c.num_sms);
-                    };
-                    run();
-                    AHA_CUDA_CHECK(cudaEventRecord(m->ev0, c.stream));
-                    for (int i = 0; i < std::max(iters, 0); ++i) run();
-                    AHA_CUDA_CHECK(cudaEventRecord(m->ev1, c.stream));
-                    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-                } catch (...) { free7(); throw; }
-                free7();
-                if (device_ms) { float ms = 0.f; AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1)); *device_ms = ms; }
-                AHA_CUDA_CHECK(cudaMemcpy(out, dy, (size_t)M * Nout * 4, cudaMemcpyDeviceToHost));
-                cleanup();
-                return;
-            }
-            if (impl == 5 || impl == 6) {   // the batched decode GEMV (gemv_batch.cuh; 6 = the cp.async ring version): M <= 8 activation rows against every weight row
-                AHA_REQUIRE(M <= kGemvBatchMax && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "batched GEMV: M <= 8, epilogue store / residual / SwiGLU");
-                GemvBatchArgs a{};
-                a.W = dw; a.x = dx; a.ldx = K; a.bias = db; a.resid = dr; a.ldr = N; a.out = dy; a.ldo = Nout; a.N = N; a.K = K; a.nb = M; a.eps = 0.f;
-                const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
-                const int pro = epi == EPI_SWIGLU ? PRO_RMSNORM : PRO_NONE;   // (the SwiGLU instantiation carries the RMSNorm prologue: unit gain here)
-                float* ones = nullptr;
-                if (pro == PRO_RMSNORM) {
-                    std::vector<float> h1((size_t)K, 1.0f);
-                    AHA_CUDA_CHECK(cudaMalloc(&ones, (size_t)K * 4)); AHA_CUDA_CHECK(cudaMemcpy(ones, h1.data(), (size_t)K * 4, cudaMemcpyHostToDevice));
-                    a.norm_w = ones; a.eps = 1e-6f;
-                }
-                try {
-                    gemv_batch(c.stream, pro, gepi, a, impl == 6);
-                    AHA_CUDA_CHECK(cudaEventRecord(m->ev0, c.stream));
-                    for (int i = 0; i < std::max(iters, 0); ++i) gemv_batch(c.stream, pro, gepi, a, impl == 6);
-                    AHA_CUDA_CHECK(cudaEventRecord(m->ev1, c.stream));
-                    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-                } catch (...) { cudaFree(ones); throw; }
-                cudaFree(ones);
-                if (device_ms) { float ms = 0.f; AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1)); *device_ms = ms; }
-                AHA_CUDA_CHECK(cudaMemcpy(out, dy, (size_t)M * Nout * 4, cudaMemcpyDeviceToHost));
-                cleanup();
-                return;
-            }
+        Scratch mem;
+        float* dx = mem.alloc<float>((size_t)M * K);
+        __half* dw = mem.alloc<__half>((size_t)N * K);
+        float* dy = mem.alloc<float>((size_t)M * Nout);
+        float *db = nullptr, *dr = nullptr;
+        AHA_CUDA_CHECK(cudaMemcpy(dx, x, (size_t)M * K * 4, cudaMemcpyHostToDevice));
+        AHA_CUDA_CHECK(cudaMemcpy(dw, w, (size_t)N * K * 2, cudaMemcpyHostToDevice));
+        if (bias) { db = mem.alloc<float>(N); AHA_CUDA_CHECK(cudaMemcpy(db, bias, (size_t)N * 4, cudaMemcpyHostToDevice)); }
+        if (epi == EPI_RESID) {
+            AHA_REQUIRE(resid, "resid is required for the residual epilogue");
+            dr = mem.alloc<float>((size_t)M * N); AHA_CUDA_CHECK(cudaMemcpy(dr, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice));
+        }
+        LinearW W; W.w = dw; W.b = db; W.N = N; W.K = K;
+        auto unit_gain = [&] {   // the gain of a unit RMSNorm prologue (the SwiGLU instantiations of the batched GEMVs carry one)
+            std::vector<float> h1((size_t)K, 1.0f);
+            float* ones = mem.alloc<float>(K);
+            AHA_CUDA_CHECK(cudaMemcpy(ones, h1.data(), (size_t)K * 4, cudaMemcpyHostToDevice));
+            return ones;
+        };
+        const size_t n = (size_t)std::max(iters, 0);
+        float ms = 0.f;
+        if (impl == 7) {   // the wide decode projection (gemv_wide.cuh): M <= 64 rows split into fp16 hi / lo operand rows, then the kernel
+            AHA_REQUIRE(M <= kWideSeqs && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "wide batched GEMV: M <= 64, epilogue store / residual / SwiGLU");
+            AHA_REQUIRE(gemv_wide_supported(N, K), "wide batched GEMV: N and K must be multiples of 64");
+            const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
+            const size_t xh = (size_t)kWideSeqs * K;
+            __half* hi = mem.alloc<__half>(xh);
+            __half* lo = mem.alloc<__half>(xh);
+            AHA_CUDA_CHECK(cudaMemset(hi, 0, xh * sizeof(__half))); AHA_CUDA_CHECK(cudaMemset(lo, 0, xh * sizeof(__half)));   // rows M..63 stay zero
+            const size_t wsf = wide_ws_floats(N, K, c.num_sms);
+            const int tiles = wide_plan(N, K, c.num_sms).tiles;
+            float* ws = wsf ? mem.alloc<float>(wsf) : nullptr;
+            int* cnt = mem.alloc<int>(tiles);
+            AHA_CUDA_CHECK(cudaMemset(cnt, 0, (size_t)tiles * sizeof(int)));
+            const float* ones = gepi == GEPI_SWIGLU ? unit_gain() : nullptr;   // (behind a unit-gain RMSNorm prologue, as impl 5)
+            WideArgs a{};
+            a.bias = db; a.resid = dr; a.ldr = N; a.out = dy; a.ldo = Nout; a.N = N; a.K = K; a.nb = M; a.ws = ws; a.counters = cnt;
+            const CUtensorMap tm = make_tmap_f16(dw, (uint64_t)N, (uint64_t)K);
+            auto run = [&] {
+                if (ones) rmsnorm_split_kernel<<<M, 256, 0, c.stream>>>(dx, ones, 1e-6f, hi, lo, K);
+                else split_f32_to_f16x2_kernel<<<(unsigned)(((size_t)M * K / 4 + 255) / 256), 256, 0, c.stream>>>(dx, K, hi, lo, M, K);
+                gemv_wide(c.stream, gepi, tm, hi, lo, a, c.num_sms);
+            };
+            run();
+            ms = timed_ms(m, n, [&](size_t) { run(); });
+        } else if (impl == 5 || impl == 6) {   // the batched decode GEMV (gemv_batch.cuh; 6 = the cp.async ring version): M <= 8 activation rows against every weight row
+            AHA_REQUIRE(M <= kGemvBatchMax && (epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU), "batched GEMV: M <= 8, epilogue store / residual / SwiGLU");
+            GemvBatchArgs a{};
+            a.W = dw; a.x = dx; a.ldx = K; a.bias = db; a.resid = dr; a.ldr = N; a.out = dy; a.ldo = Nout; a.N = N; a.K = K; a.nb = M; a.eps = 0.f;
+            const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
+            const int pro = epi == EPI_SWIGLU ? PRO_RMSNORM : PRO_NONE;
+            if (pro == PRO_RMSNORM) { a.norm_w = unit_gain(); a.eps = 1e-6f; }
+            gemv_batch(c.stream, pro, gepi, a, impl == 6);
+            ms = timed_ms(m, n, [&](size_t) { gemv_batch(c.stream, pro, gepi, a, impl == 6); });
+        } else {
             const int saved = c.gemm_impl;
             c.gemm_impl = impl;
             try {
                 linear_gemm(c, epi, dx, K, W, dr, N, dy, Nout, M, act);   // warm-up + correctness run
-                AHA_CUDA_CHECK(cudaEventRecord(m->ev0, c.stream));
-                for (int i = 0; i < std::max(iters, 0); ++i) linear_gemm(c, epi, dx, K, W, dr, N, dy, Nout, M, act);
-                AHA_CUDA_CHECK(cudaEventRecord(m->ev1, c.stream));
-                AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+                ms = timed_ms(m, n, [&](size_t) { linear_gemm(c, epi, dx, K, W, dr, N, dy, Nout, M, act); });
             } catch (...) { c.gemm_impl = saved; throw; }
             c.gemm_impl = saved;
-            if (device_ms) { float ms = 0.f; AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1)); *device_ms = ms; }
-            AHA_CUDA_CHECK(cudaMemcpy(out, dy, (size_t)M * Nout * 4, cudaMemcpyDeviceToHost));
-        } catch (...) { cleanup(); throw; }
-        cleanup();
+        }
+        if (device_ms) *device_ms = ms;
+        AHA_CUDA_CHECK(cudaMemcpy(out, dy, (size_t)M * Nout * 4, cudaMemcpyDeviceToHost));
     });
 }
 
@@ -2223,19 +2184,10 @@ void bench_score(aha_model* m, const std::string& w, int iters, double* avg_ms, 
     cudaStream_t st = m->ctx.stream;
     AHA_CUDA_CHECK(cudaMemsetAsync(b.tgt, 0, (size_t)M * sizeof(uint32_t), st));
     AHA_CUDA_CHECK(cudaMemsetAsync(b.index, 0, (size_t)M * sizeof(uint32_t), st));
-    float* logits = nullptr;
-    if (impl == 1) AHA_CUDA_CHECK(cudaMalloc(&logits, (size_t)M * T.cfg.V * sizeof(float)));
-    try {
-        score_head_rows(m, impl, T.x, nullptr, M, n, b, logits);
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev0, st));
-        for (int i = 0; i < iters; ++i) score_head_rows(m, impl, T.x, nullptr, M, n, b, logits);
-        AHA_CUDA_CHECK(cudaEventRecord(m->ev1, st));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
-    } catch (...) { cudaFree(logits); throw; }
-    cudaFree(logits);
-    float ms = 0.f;
-    AHA_CUDA_CHECK(cudaEventElapsedTime(&ms, m->ev0, m->ev1));
-    *avg_ms = ms / iters;
+    Scratch mem;
+    float* logits = impl == 1 ? mem.alloc<float>((size_t)M * T.cfg.V) : nullptr;
+    score_head_rows(m, impl, T.x, nullptr, M, n, b, logits);
+    *avg_ms = timed_ms(m, (size_t)iters, [&](size_t) { score_head_rows(m, impl, T.x, nullptr, M, n, b, logits); }) / iters;
     *bytes = 2ull * T.cfg.V * T.cfg.H;
 }
 }  // namespace
@@ -2261,15 +2213,11 @@ int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_
         alloc_score_buffers(m);
         cudaStream_t st = m->ctx.stream;
         // scratch of this call only: the hidden rows, the buffers of M rows and (twin) the logits block
-        struct Scratch {
-            void* p = nullptr;
-            ~Scratch() { if (p) cudaFree(p); }
-        } mem;
         ScoreBufs b;
         const size_t o_x = (score_bufs_carve(nullptr, M, V, b) + 255) & ~(size_t)255;
         const size_t o_lg = (o_x + M * H * sizeof(float) + 255) & ~(size_t)255;
-        AHA_CUDA_CHECK(cudaMalloc(&mem.p, o_lg + (impl == 1 ? M * (size_t)V * sizeof(float) : 0)));
-        char* base = static_cast<char*>(mem.p);
+        Scratch mem;
+        char* base = mem.alloc<char>(o_lg + (impl == 1 ? M * (size_t)V * sizeof(float) : 0));
         score_bufs_carve(base, M, V, b);
         float* x = reinterpret_cast<float*>(base + o_x);
         std::vector<uint32_t> idx(M);
@@ -2310,24 +2258,19 @@ int aha_b200_rerank(aha_model* m, const uint32_t* query_ids, size_t query_len, c
 }
 
 int aha_b200_nccl_unique_id(uint8_t out[128]) {
-    try {
+    return guarded_host([&] {
         AHA_REQUIRE(out != nullptr, "out is required");
         NcclApi& n = NcclApi::get();
         NcclApi::unique_id id;
         n.check(n.GetUniqueId(&id), "ncclGetUniqueId");
         std::memcpy(out, &id, 128);
-        return 0;
-    } catch (const std::exception& e) {
-        std::lock_guard<std::mutex> lk(g_err_mu);
-        g_create_error = e.what();
-        return 1;
-    }
+    });
 }
 
 int aha_b200_rope_index_mm(const uint32_t* ids, size_t seq_len, const uint32_t* grid_thw, size_t n_images, const uint32_t* video_grid_thw, size_t n_videos,
                            uint32_t spatial_merge_size, uint32_t image_token_id, uint32_t video_token_id, uint32_t vision_start_token_id, int32_t* pos3_out,
                            int32_t* rope_delta_out) {
-    try {
+    return guarded_host([&] {
         AHA_REQUIRE(ids != nullptr && seq_len > 0 && pos3_out != nullptr && rope_delta_out != nullptr, "ids, pos3_out and rope_delta_out are required");
         AHA_REQUIRE(n_images == 0 || grid_thw != nullptr, "grid_thw is required when n_images > 0");
         AHA_REQUIRE(n_videos == 0 || video_grid_thw != nullptr, "video_grid_thw is required when n_videos > 0");
@@ -2341,12 +2284,7 @@ int aha_b200_rope_index_mm(const uint32_t* ids, size_t seq_len, const uint32_t* 
         get_rope_index(ids, (int)seq_len, grid, frames, (int)spatial_merge_size, (int)image_token_id, (int)video_token_id, (int)vision_start_token_id, pos3, delta);
         for (size_t i = 0; i < pos3.size(); ++i) pos3_out[i] = pos3[i];
         *rope_delta_out = delta;
-        return 0;
-    } catch (const std::exception& e) {
-        std::lock_guard<std::mutex> lk(g_err_mu);
-        g_create_error = e.what();
-        return 1;
-    }
+    });
 }
 int aha_b200_rope_index(const uint32_t* ids, size_t seq_len, const uint32_t* grid_thw, size_t n_images, uint32_t spatial_merge_size,
                         uint32_t image_token_id, uint32_t vision_start_token_id, int32_t* pos3_out, int32_t* rope_delta_out) {
@@ -2359,8 +2297,8 @@ void aha_b200_destroy(aha_model* m) {
     cudaSetDevice(m->ctx.device);
     if (m->ctx.stream) cudaStreamSynchronize(m->ctx.stream);
     m->text.destroy();
-    m->batch.clear_graphs();
-    m->wide_batch.clear_graphs();
+    m->batch.graphs.clear();
+    m->wide_batch.graphs.clear();
     m->spec.destroy();
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);

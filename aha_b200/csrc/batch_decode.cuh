@@ -68,12 +68,7 @@ struct BatchDecoder {
     bool use_graph = true;
     // one CUDA graph per (running count, any request asks for log-probabilities) (~170 launches per step become one); they outlive
     // composition changes
-    struct StepGraph { int width; bool lp; cudaGraphExec_t exec; uint64_t kernels; };
-    std::vector<StepGraph> graphs;
-    void clear_graphs() {
-        for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-        graphs.clear();
-    }
+    GraphCache<std::pair<int, bool>> graphs;
     // the set of running requests or a slot's sampler changed: the device copy of the composition is rebuilt before the next step
     void composition_changed() { table_for.clear(); }
     // no sequence holds a slot any more (a session opens or closes)
@@ -81,7 +76,7 @@ struct BatchDecoder {
         for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; }
         table_for.clear();
         lp_any = false;
-        clear_graphs();
+        graphs.clear();
     }
 
     // ---- wide mode
@@ -148,14 +143,13 @@ struct BatchDecoder {
         for (int i = 0; i < n; ++i) { slots[i].table.h.assign(t.num_pages, 0); slots[i].table.d = d_tables + (size_t)i * t.num_pages; }
     }
 
-    // after the prefill of slot i (the model's d_state / d_history / samp hold the request's state): move it into the slot
+    // after the first token of slot i: its decode state starts from that token (history[0]) at position seq_len
     void adopt(int i, uint32_t first_token, int seq_len, int rope_delta, uint32_t n_draws) {
         Ctx& c = *T->ctx;
         DecodeState st{first_token, seq_len, rope_delta, 1, n_draws, {0, 0, 0}};
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_states + i, &st, sizeof(st), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_hist + (size_t)i * T->hist_cap, &first_token, sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
-        bind_sampler(i);
     }
     void ensure_lp() {
         if (d_lp_rec) return;
@@ -167,17 +161,11 @@ struct BatchDecoder {
         lp_part_id = c.alloc<int>((size_t)cap * P * kLpMaxTop);
         AHA_CUDA_CHECK(cudaMemset(d_lp_on, 0, (size_t)cap * sizeof(int)));
     }
-    // the sampler set on the TextModel (set_sampler) becomes slot i's, with the slot's own state, history, token and scratch row
-    void bind_sampler(int i) {
-        BatchSlot& s = slots[i];
-        s.samp_active = T->samp_active;
-        if (s.samp_active) {
-            s.samp = T->samp;
-            s.samp.st = d_states + i;
-            s.samp.history = d_hist + (size_t)i * T->hist_cap;
-            s.samp.token_out = d_tok + i;
-            s.samp.work = workb + (size_t)i * T->cfg.V;
-        }
+    // the request's sampler becomes slot i's, with the slot's own state, history, token and scratch row
+    void bind_sampler(int i, const Sampler& s) {
+        BatchSlot& sl = slots[i];
+        sl.samp_active = s.active;
+        if (s.active) sl.samp = T->bind_sampler(s, d_states + i, d_hist + (size_t)i * T->hist_cap, d_tok + i, workb + (size_t)i * T->cfg.V);
     }
 
     // the device copy of the composition `act`: attention table, active list and every slot's sampler arguments
@@ -260,25 +248,7 @@ struct BatchDecoder {
         const int nb = (int)act.size();
         if (wide) zero_rows_from(nb);
         if (!use_graph) { launches(nb); return; }
-        StepGraph* g = nullptr;
-        for (auto& e : graphs) if (e.width == nb && e.lp == lp_any) { g = &e; break; }
-        if (!g) {
-            const uint64_t k0 = c.cnt.kernels;
-            cudaGraph_t cg = nullptr;
-            AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-            try { launches(nb); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
-            AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &cg));
-            StepGraph e{nb, lp_any, nullptr, c.cnt.kernels - k0};
-            c.cnt.kernels = k0;
-            const cudaError_t err = cudaGraphInstantiate(&e.exec, cg, 0);
-            cudaGraphDestroy(cg);
-            AHA_CUDA_CHECK(err);
-            graphs.push_back(e);
-            g = &graphs.back();
-        }
-        AHA_CUDA_CHECK(cudaGraphLaunch(g->exec, c.stream));
-        c.cnt.graphs++;
-        c.cnt.kernels += g->kernels;
+        graphs.run(c, {nb, lp_any}, [&] { launches(nb); });
     }
     void launches(int nb) {
         Ctx& c = *T->ctx;

@@ -13,6 +13,7 @@
 #pragma once
 #include <cstdint>
 
+#include "../../include/aha_b200.h"
 #include "common.cuh"
 #include "kernels_common.cuh"
 
@@ -348,6 +349,42 @@ __global__ void __launch_bounds__(kSampleThreads) sample_rows_kernel(const Sampl
     a.logits = logits + (size_t)blockIdx.x * ld;
     a.overwrite = overwrite;
     sample_dev(a, s);
+}
+
+// ----------------------------------------------------------------------------------------------------------------------- host side
+// A request's sampler.  inactive = plain ArgMax, which the step kernels compute themselves.  `args` holds the parameters only; the buffers
+// (logits, work, state, history, token, error flag) are filled where the sampler is bound to a row (TextModel::bind_sampler).
+struct Sampler {
+    bool active = false;
+    SampleArgs args{};
+};
+
+// get_logit_processor (sample.rs:7-38): the Sampling a request's parameters select, checked against what the device sampler supports
+inline Sampler make_sampler(const aha_gen_params& p, int V) {
+    const bool has_t = !(p.temperature < 1e-7f);
+    const bool has_k = p.top_k > 0, has_p = p.top_p > 0.f;
+    const int mode = !has_t ? SAMPLE_ARGMAX : !has_k ? (has_p ? SAMPLE_TOPP : SAMPLE_ALL) : (has_p ? SAMPLE_TOPK_TOPP : SAMPLE_TOPK);
+    const bool pen = !(p.repeat_penalty == 1.0f || p.repeat_last_n == 0);
+    Sampler s;
+    s.active = mode != SAMPLE_ARGMAX || pen;
+    if (!s.active) return s;
+    AHA_REQUIRE(V <= kSampleThreads * kSampleChunk, "vocabulary too large for the device sampler");
+    AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || p.top_k >= 1, "top_k must be >= 1");
+    AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || p.top_k >= V || p.top_k <= kSampleMaxTopK,
+                "top_k > 1024 is not supported by the device sampler");
+    SampleArgs& a = s.args;
+    a.V = V; a.mode = mode;
+    a.inv_temp = mode == SAMPLE_ARGMAX ? 1.0f : (float)(1.0 / (double)p.temperature);
+    a.top_p = p.top_p; a.top_k = p.top_k; a.penalty = p.repeat_penalty; a.last_n = p.repeat_last_n;
+    // rand_core::SeedableRng::seed_from_u64: eight PCG32 outputs fill the 32-byte ChaCha seed
+    uint64_t stt = p.seed;
+    for (int i = 0; i < 8; ++i) {
+        stt = stt * 6364136223846793005ull + 11634580027462260723ull;
+        const uint32_t xs = (uint32_t)(((stt >> 18) ^ stt) >> 27);
+        const uint32_t rot = (uint32_t)(stt >> 59);
+        a.key[i] = (xs >> rot) | (xs << ((32u - rot) & 31u));
+    }
+    return s;
 }
 
 }  // namespace aha

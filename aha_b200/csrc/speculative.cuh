@@ -336,14 +336,9 @@ struct SpecDecoder {
     SpecCtl* d_ctl = nullptr;
     float* partial = nullptr; int max_chunks = 0;
     uint32_t* d_buf = nullptr; size_t buf_cap = 0;     // prediction | prompt | stop ids of the current request
-    struct PassGraph { int R; cudaGraphExec_t exec; uint64_t kernels; };
-    std::vector<PassGraph> graphs;
-    void clear_graphs() {
-        for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-        graphs.clear();
-    }
+    GraphCache<int> graphs;                            // keyed by R
     void destroy() {
-        clear_graphs();
+        graphs.clear();
         if (d_buf) { cudaFree(d_buf); d_buf = nullptr; buf_cap = 0; }
     }
     void init(TextModel& t, BatchDecoder& b) {
@@ -359,8 +354,8 @@ struct SpecDecoder {
         AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<128>()));
     }
     // the request's control block, rows 0..R-1 of the decoder's active list / samplers / record flags (lp_on = 1 + top count, or 0)
-    void prepare(int R, const std::vector<uint32_t>& pred, const uint32_t* prompt, size_t n_prompt, const std::vector<uint32_t>& stop,
-                 int max_tokens, int ngram, int lp_on) {
+    void prepare(int R, const Sampler& samp, const std::vector<uint32_t>& pred, const uint32_t* prompt, size_t n_prompt,
+                 const std::vector<uint32_t>& stop, int max_tokens, int ngram, int lp_on) {
         Ctx& c = *T->ctx;
         const size_t need = pred.size() + n_prompt + stop.size();
         if (need > buf_cap) {
@@ -376,24 +371,20 @@ struct SpecDecoder {
         s.prompt = d_buf + pred.size(); s.n_prompt = (int)n_prompt;
         s.stop = d_buf + pred.size() + n_prompt; s.n_stop = (int)stop.size();
         s.max_tokens = max_tokens; s.ngram = ngram;
-        s.draw_step = T->samp_active && T->samp.mode != SAMPLE_ARGMAX ? 1u : 0u;
+        s.draw_step = samp.active && samp.args.mode != SAMPLE_ARGMAX ? 1u : 0u;
         s.lp = lp_on > 0 ? 1 : 0;
-        std::vector<int> act(kSpecMaxRows), on(kSpecMaxRows, T->samp_active ? 1 : 0), lp(kSpecMaxRows, lp_on);
-        std::vector<SampleArgs> samp(kSpecMaxRows);
+        std::vector<int> act(kSpecMaxRows), on(kSpecMaxRows, samp.active ? 1 : 0), lp(kSpecMaxRows, lp_on);
+        std::vector<SampleArgs> rows(kSpecMaxRows);
         for (int r = 0; r < kSpecMaxRows; ++r) {
             act[r] = r;
-            if (!T->samp_active) continue;
-            SampleArgs a = T->samp;           // the request's sampler; the shared history holds the emitted tokens followed by the drafts
-            a.st = B->d_states + r;
-            a.token_out = B->d_tok + r;
-            a.work = B->workb + (size_t)r * T->cfg.V;
-            samp[r] = a;
+            // the request's sampler on every row; the shared history holds the emitted tokens followed by the drafts
+            if (samp.active) rows[r] = T->bind_sampler(samp, B->d_states + r, T->d_history, B->d_tok + r, B->workb + (size_t)r * T->cfg.V);
         }
         if (!h.empty()) AHA_CUDA_CHECK(cudaMemcpyAsync(d_buf, h.data(), h.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_ctl, &s, sizeof(s), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(B->d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(B->d_samp_on, on.data(), on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(B->d_samp, samp.data(), samp.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(B->d_samp, rows.data(), rows.size() * sizeof(SampleArgs), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(B->d_lp_on, lp.data(), lp.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // host temporaries
         B->composition_changed();             // a later session rebuilds its own device copies
@@ -442,27 +433,8 @@ struct SpecDecoder {
         AHA_CUDA_CHECK(cudaGetLastError());
     }
     void pass(int R) {
-        Ctx& c = *T->ctx;
         if (!T->use_graph) { launches(R); return; }
-        PassGraph* g = nullptr;
-        for (auto& e : graphs) if (e.R == R) { g = &e; break; }
-        if (!g) {
-            const uint64_t k0 = c.cnt.kernels;
-            cudaGraph_t cg = nullptr;
-            AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-            try { launches(R); } catch (...) { cudaStreamEndCapture(c.stream, &cg); if (cg) cudaGraphDestroy(cg); throw; }
-            AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &cg));
-            PassGraph e{R, nullptr, c.cnt.kernels - k0};
-            c.cnt.kernels = k0;
-            const cudaError_t err = cudaGraphInstantiate(&e.exec, cg, 0);
-            cudaGraphDestroy(cg);
-            AHA_CUDA_CHECK(err);
-            graphs.push_back(e);
-            g = &graphs.back();
-        }
-        AHA_CUDA_CHECK(cudaGraphLaunch(g->exec, c.stream));
-        c.cnt.graphs++;
-        c.cnt.kernels += g->kernels;
+        graphs.run(*T->ctx, R, [&] { launches(R); });
     }
 };
 

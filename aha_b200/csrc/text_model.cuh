@@ -84,6 +84,43 @@ struct Ctx {  // per-handle launch context
     }
 };
 
+// CUDA graphs captured on first use, one per key: the first run of a key records `launches` under stream capture, every run replays the
+// graph.  The launch counters advance as if the captured kernels had run eagerly (aha_b200_get_stats).
+template <typename Key>
+struct GraphCache {
+    struct Entry { Key key; cudaGraphExec_t exec; uint64_t kernels; };
+    std::vector<Entry> entries;
+    size_t size() const { return entries.size(); }
+    void clear() {
+        for (auto& e : entries) if (e.exec) cudaGraphExecDestroy(e.exec);
+        entries.clear();
+    }
+    // returns the kernels the graph of `key` holds
+    template <typename F>
+    uint64_t run(Ctx& c, const Key& key, F&& launches) {
+        const Entry* e = nullptr;
+        for (const Entry& x : entries) if (x.key == key) { e = &x; break; }
+        if (!e) {
+            const uint64_t k0 = c.cnt.kernels;
+            cudaGraph_t g = nullptr;
+            AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
+            try { launches(); } catch (...) { cudaStreamEndCapture(c.stream, &g); if (g) cudaGraphDestroy(g); throw; }
+            AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &g));
+            Entry n{key, nullptr, c.cnt.kernels - k0};
+            c.cnt.kernels = k0;
+            const cudaError_t err = cudaGraphInstantiate(&n.exec, g, 0);
+            cudaGraphDestroy(g);
+            AHA_CUDA_CHECK(err);
+            entries.push_back(n);
+            e = &entries.back();
+        }
+        AHA_CUDA_CHECK(cudaGraphLaunch(e->exec, c.stream));
+        c.cnt.graphs++;
+        c.cnt.kernels += e->kernels;
+        return e->kernels;
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------
 // Host-side weight table (descs by name) + dtype conversion.
 inline float half_bits_to_float(uint16_t h) {
@@ -441,7 +478,7 @@ struct TextModel {
     DecodeState* d_state = nullptr;
     uint32_t* d_history = nullptr; int hist_cap = 0;
     uint32_t* d_argmax = nullptr;
-    cudaGraphExec_t step_graph = nullptr;
+    GraphCache<int> step_graph;          // the one decode-step graph (key 0)
     uint64_t step_graph_kernels = 0;
     bool use_graph = true;
     // fused persistent decode kernel (decode_fused.cuh)
@@ -927,48 +964,32 @@ struct TextModel {
         Ctx& c = *ctx;
         if (fused && !(full_logits && tp_world > 1)) { decode_step_fused(); return; }
         if (!use_graph) { decode_step_launches(); return; }
-        if (!step_graph) {
-            const uint64_t k0 = c.cnt.kernels;
-            cudaGraph_t g = nullptr;
-            AHA_CUDA_CHECK(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
-            try { decode_step_launches(); } catch (...) { cudaStreamEndCapture(c.stream, &g); if (g) cudaGraphDestroy(g); throw; }
-            AHA_CUDA_CHECK(cudaStreamEndCapture(c.stream, &g));
-            step_graph_kernels = c.cnt.kernels - k0;
-            c.cnt.kernels = k0;
-            AHA_CUDA_CHECK(cudaGraphInstantiate(&step_graph, g, 0));
-            AHA_CUDA_CHECK(cudaGraphDestroy(g));
-        }
-        AHA_CUDA_CHECK(cudaGraphLaunch(step_graph, c.stream));
-        c.cnt.graphs++;
-        c.cnt.kernels += step_graph_kernels;
+        const bool fresh = step_graph.size() == 0;
+        const uint64_t kernels = step_graph.run(c, 0, [&] { decode_step_launches(); });
+        if (fresh) step_graph_kernels = kernels;
     }
-    // ---- sampler.  mode / parameters follow get_logit_processor (sample.rs:7-38); `seed` keys the ChaCha12 stream.
-    void set_sampler(int mode, float temperature, float top_p, int top_k, float penalty, int last_n, uint64_t seed) {
-        const bool pen = !(penalty == 1.0f || last_n == 0);
-        samp_active = mode != SAMPLE_ARGMAX || pen;
+    // ---- sampler (sampling.cuh: make_sampler)
+    // the request's sampler on one row: its state, repeat-penalty history, token and [V] scratch row.  Every row samples the model's logits
+    // unless its kernel points it elsewhere, and raises the handle's one error flag.
+    SampleArgs bind_sampler(const Sampler& s, DecodeState* st, uint32_t* history, uint32_t* token_out, float* work) {
+        alloc_sampler();
+        SampleArgs a = s.args;
+        a.logits = logits; a.work = work;
+        a.st = st; a.history = history; a.hist_cap = hist_cap; a.token_out = token_out; a.error = d_sample_err;
+        return a;
+    }
+    // the sampler of the model's own decode loop
+    void set_sampler(const Sampler& s) {
+        samp_active = s.active;
         if (!samp_active) return;
-        AHA_REQUIRE(cfg.V <= kSampleThreads * kSampleChunk, "vocabulary too large for the device sampler");
-        AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || top_k >= 1, "top_k must be >= 1");
-        AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || top_k >= cfg.V || top_k <= kSampleMaxTopK,
-                    "top_k > 1024 is not supported by the device sampler");
-        if (!sample_work) {
-            sample_work = ctx->alloc<float>((size_t)cfg.V);
-            d_sample_err = ctx->alloc<int>(1);
-            AHA_CUDA_CHECK(cudaMemset(d_sample_err, 0, sizeof(int)));
-        }
-        samp = SampleArgs{};
-        samp.logits = logits; samp.work = sample_work; samp.V = cfg.V; samp.mode = mode;
-        samp.inv_temp = mode == SAMPLE_ARGMAX ? 1.0f : (float)(1.0 / (double)temperature);
-        samp.top_p = top_p; samp.top_k = top_k; samp.penalty = penalty; samp.last_n = last_n;
-        // rand_core::SeedableRng::seed_from_u64: eight PCG32 outputs fill the 32-byte ChaCha seed
-        uint64_t stt = seed;
-        for (int i = 0; i < 8; ++i) {
-            stt = stt * 6364136223846793005ull + 11634580027462260723ull;
-            const uint32_t xs = (uint32_t)(((stt >> 18) ^ stt) >> 27);
-            const uint32_t rot = (uint32_t)(stt >> 59);
-            samp.key[i] = (xs >> rot) | (xs << ((32u - rot) & 31u));
-        }
-        samp.st = d_state; samp.history = d_history; samp.hist_cap = hist_cap; samp.token_out = d_argmax; samp.error = d_sample_err;
+        alloc_sampler();
+        samp = bind_sampler(s, d_state, d_history, d_argmax, sample_work);
+    }
+    void alloc_sampler() {
+        if (sample_work) return;
+        sample_work = ctx->alloc<float>((size_t)cfg.V);
+        d_sample_err = ctx->alloc<int>(1);
+        AHA_CUDA_CHECK(cudaMemset(d_sample_err, 0, sizeof(int)));
     }
     void clear_sampler() { samp_active = false; }
     // overwrite = 1: the step kernel has already pushed its ArgMax token; the sampled token replaces it
@@ -1018,7 +1039,7 @@ struct TextModel {
     void destroy() {
         for (int w = 0; w < kFusedMaxTp; ++w)
             if (ll_peer_sym[w] && w != tp_rank) { cudaIpcCloseMemHandle(ll_peer_sym[w]); ll_peer_sym[w] = nullptr; }
-        if (step_graph) { cudaGraphExecDestroy(step_graph); step_graph = nullptr; }
+        step_graph.clear();
         if (comm) { NcclApi::get().CommDestroy(comm); comm = nullptr; }
     }
 };
