@@ -8,7 +8,9 @@
 //     layers -- weight row slabs and paged-KV half pages -- and issues TMA bulk copies
 //     (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes, SASS UBLKCP, L2 evict-first policy) into
 //     a ring of 16 KB shared-memory stages guarded by full/empty mbarriers.  It never waits for activations, so
-//     weights for the next phases keep streaming while the consumers sit in a grid barrier;
+//     weights for the next phase keep streaming while the consumers sit in a grid barrier -- but only up to a run-ahead
+//     budget past the end of the consumers' current phase (kFusedAheadBytes), so that the traffic of a phase end
+//     (barrier, activation loads) does not queue behind a full ring of next-phase copies from every SM;
 //   * the other 11 warps are CONSUMERS: per phase they stage the activation vector in shared memory (RMSNorm
 //     fused), and each warp consumes the ring slots it owns: a whole stage of weight rows is reduced by one warp
 //     with fp32 dot products (fp16 weights converted exactly) and the fused epilogue (residual add from the rows
@@ -54,6 +56,17 @@ constexpr int kFusedMergeChunk = 20;                     // splits merged per pa
 constexpr int kFusedMaxPages = 1024;                     // page-table entries staged in shared memory as uint16 (32K tokens; physical page ids < 65536)
 constexpr int kFusedMaxH = 4096;                         // residual stream kept per CTA in shared memory (LL mode)
 constexpr int kFusedMaxTp = 8;                           // tensor-parallel ranks on one NVSwitch domain
+// Run-ahead budget of the producer: stages of a phase the consumers have not entered yet may be issued only while they end at
+// most this many bytes past the end of the consumers' current phase (stages of the current phase are never held back).  Without
+// it every CTA keeps a full ring (176 KB) of the next phases' copies queued in the memory system while it sits in a phase end,
+// and the phase end's own traffic -- the barrier arrival and poll, the activation loads -- waits behind them.  96 KB is the
+// fastest of 0 / 16 / 32 / 48 / 64 / 96 / 128 / 176 KB on an H100 SXM (700 W) at the Qwen3-VL-2B decode shape (DESIGN §4.1):
+// less starves the next phase's first stages, more brings the queueing back.  -DAHA_FUSED_AHEAD_KB=N builds the sweep.
+#ifndef AHA_FUSED_AHEAD_KB
+#define AHA_FUSED_AHEAD_KB 96
+#endif
+constexpr uint32_t kFusedAheadBytes = AHA_FUSED_AHEAD_KB * 1024u;
+constexpr int kFusedGateWord = 28;                       // the gate's word in the `red` scratch ([0, 11) sums / argmax values, [16, 27) argmax indices, [31] last-CTA flag)
 
 struct __align__(8) LLPk { float v; uint32_t tag; };     // one tagged packet: 8-byte stores / loads are single-copy atomic
 struct LLPeerTab {                                       // device-resident table of the symmetric blocks of every tensor-parallel rank
@@ -385,6 +398,16 @@ struct Ring {
 };
 
 // ------------------------------------------------------------------------------------------------ producer
+// The run-ahead gate: `gate` holds (schedule bytes up to the end of the consumers' current phase) + kFusedAheadBytes, `issued`
+// counts the schedule bytes this producer has issued including the stage being acquired; the stage waits while it would end
+// past the gate.  No deadlock: consumers enter a phase (and raise the gate) without waiting on any ring slot -- they need only
+// the activations, which come from the other CTAs' consumers under the same rule -- and the stages of the phase they are in
+// always end below the gate.  Wrapping differences: a step's schedule is far below 2 GB per CTA.
+__device__ __forceinline__ uint32_t ld_volatile_shared_u32(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+    return v;
+}
 struct Producer {
     Ring ring;
     unsigned it = 0;
@@ -392,7 +415,12 @@ struct Producer {
     bool use_hint = false, hint_kv = false;
     uint64_t policy = 0;
     unsigned long long* st_trace = nullptr;
-    __device__ __forceinline__ void acquire(int& slot) {
+    const uint32_t* gate = nullptr;
+    uint32_t issued = 0, limit = 0;   // limit: the last value read from the gate (it only grows)
+    __device__ __forceinline__ void acquire(int& slot, uint32_t bytes) {
+        issued += bytes;
+        if ((int)(limit - issued) < 0)
+            while ((int)((limit = ld_volatile_shared_u32(gate)) - issued) < 0) __nanosleep(32);
         slot = it % ns;
         mbar_wait(&ring.empty[slot], ((it / ns) & 1u) ^ 1u);
         AHA_STAGE_STAMP(st_trace, it, 0);
@@ -403,9 +431,9 @@ struct Producer {
         const int R = rows_per_stage(K, N, gridDim.x);
         for (int r = r0; r < r1; r += R) {
             const int nr = min(R, r1 - r);
-            int slot;
-            acquire(slot);
             const uint32_t bytes = (uint32_t)nr * K * 2u;
+            int slot;
+            acquire(slot, bytes);
             mbar_expect_tx(&ring.full[slot], bytes);
             if (use_hint) tma_bulk_g2s_hint(ring.buf + (size_t)slot * kFusedStageBytes, W + (size_t)r * K, bytes, &ring.full[slot], policy);
             else tma_bulk_g2s(ring.buf + (size_t)slot * kFusedStageBytes, W + (size_t)r * K, bytes, &ring.full[slot]);
@@ -418,12 +446,12 @@ struct Producer {
         if (!attn_item(a, ctx, kvh, split, hp0, hp1)) return;
         const float* kbase = a.kv_pool + (size_t)layer * a.layer_stride;
         const size_t vofs = (size_t)a.nkv * kPage * a.hd;
+        const uint32_t half_bytes = kHalfPage * a.hd * 4u;  // 8 KB for hd = 128
         for (int hp = hp0; hp < hp1; ++hp) {
             int slot;
-            acquire(slot);
+            acquire(slot, 2u * half_bytes);
             const int page = pages[(hp * kHalfPage) >> kPageShift];
             const size_t off = (size_t)page * a.page_stride + (size_t)kvh * kPage * a.hd + (size_t)((hp * kHalfPage) & (kPage - 1)) * a.hd;
-            const uint32_t half_bytes = kHalfPage * a.hd * 4u;  // 8 KB for hd = 128
             uint8_t* dst = ring.buf + (size_t)slot * kFusedStageBytes;
             mbar_expect_tx(&ring.full[slot], 2u * half_bytes);
             if (hint_kv) {
@@ -439,8 +467,9 @@ struct Producer {
 };
 
 // ------------------------------------------------------------------------------------------------ consumer
-// Ring slots are OWNED by consumer warps: slot s is only ever consumed by warp s % 8, so each warp sees the uses
-// of its slots strictly in order (no cross-warp mbarrier phase hazards) and 8 stages are processed concurrently.
+// Ring slots are OWNED by consumer warps: slot s is only ever consumed by warp s % kFusedConsumers, so each warp sees the
+// uses of its slots strictly in order (no cross-warp mbarrier phase hazards) and up to kFusedConsumers stages are processed
+// concurrently.
 // A GEMV stage (R rows x K fp16) is reduced entirely by its owner warp against the activation vector staged in
 // shared memory; the epilogue is applied by the lanes of that warp -- no cross-warp partial sums.
 enum FusedEpi { FE_QKV = 0, FE_RESID = 1, FE_SWIGLU = 2, FE_LOGITS = 3 };
@@ -461,6 +490,12 @@ struct Consumer {
     bool sync_only = false;    // dbg bit9: no weight stream and no math, only the barriers and activation loads
     unsigned long long* sy_trace = nullptr;   // sync anatomy stamps (AHA_STAGE_TRACE builds, dbg bit10)
     unsigned n_loads = 0;
+    // Called once the phase's activations are staged, before its first wait_full: the producer may now run
+    // kFusedAheadBytes past the end of this phase.  A phase without stages leaves the gate where it is.  Only thread 0
+    // writes the gate word (no register of the hot loops holds it).
+    __device__ __forceinline__ void enter(uint32_t bytes) const {
+        if (threadIdx.x == 0) reinterpret_cast<volatile uint32_t*>(red)[kFusedGateWord] += bytes;
+    }
     __device__ __forceinline__ bool owns(unsigned i) const { return (int)((i % ns) % kFusedConsumers) == warp; }
     __device__ __forceinline__ const uint8_t* wait_full(unsigned i) {
         const int slot = i % ns;
@@ -706,6 +741,7 @@ struct Consumer {
         int r0, r1;
         cta_rows(N, EPI == FE_SWIGLU ? 2 : 1, r0, r1);
         const int R = rows_per_stage(K, N, gridDim.x);
+        enter((uint32_t)(r1 - r0) * K * 2u);
         if (sync_only) { consumer_bar_sync(); return; }
         unsigned i = it;
         for (int r = r0; r < r1; r += R, ++i) {
@@ -840,6 +876,7 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
         *reinterpret_cast<float4*>(s.vnew + lane * 4) = v;
     }
     consumer_bar_sync();
+    c.enter((uint32_t)(hp1 - hp0) * 2u * kHalfPage * HD * 4u);   // (a CTA without an item has no stages: its gate stays put)
     const int hp_new = t_new / kHalfPage;
     if (hp_new >= hp0 && hp_new < hp1 && tid < HD) {  // append K,V of the current token to the paged cache
         const int page = spages[t_new >> kPageShift];
@@ -1013,6 +1050,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
     uint64_t* full = reinterpret_cast<uint64_t*>(fused_smem_raw + (size_t)kFusedStages * kFusedStageBytes);
     uint64_t* empty = full + kFusedStages;
     float* red = reinterpret_cast<float*>(empty + kFusedStages);
+    uint32_t* gate = reinterpret_cast<uint32_t*>(red) + kFusedGateWord;   // the producer's run-ahead gate (Consumer::enter)
     float* xown = red + 32;                                     // [kFusedMaxOwnRows] (barrier mode only: LL mode keeps the whole stream in xres)
     float* cs = xown + (MODE != 0 ? 0 : kFusedMaxOwnRows);      // [128] cos | sin of the step's rotary angles
     float* xs = cs + 128;                                       // [kFusedMaxK] activations / attention scratch
@@ -1025,6 +1063,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
     if (tid == 0) {
         for (int i = 0; i < kFusedStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        *gate = kFusedAheadBytes;   // before the first phase the consumers are in an empty one
     }
     if ((a.dbg & 64) && tid == 0) { unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid)); a.trace[8192 + blockIdx.x * 256 + 255] = smid; }
     const int t_new = a.st->pos;
@@ -1050,6 +1089,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             p.hint_kv = (a.dbg & 32) == 0;       // bit5: same switch for the KV half-page copies
             p.policy = l2_evict_first_policy();
             p.pages = spages;
+            p.gate = gate;
 #ifdef AHA_STAGE_TRACE
             if ((a.dbg & 128) && (int)blockIdx.x == ((a.dbg >> 16) & 0xff)) p.st_trace = a.trace + 8192;
 #endif

@@ -501,7 +501,7 @@ struct TextModel {
     unsigned* d_sync = nullptr;   // [0] grid barrier, [1] final ticket, then kv tickets [nkv]
     unsigned long long* d_ftrace = nullptr;
     size_t sync_words = 0;
-    int fused_stages = kFusedStages;   // ring depth: re-measured on the final kernel of round 1, 11 slots 773 tok/s vs 8 slots 762 (profiles/README.md)
+    int fused_stages = kFusedStages;   // ring depth: on an H100 SXM (700 W), VL2 text stack at ctx 2554, 11 slots 1.96 ms/step vs 8 / 6 / 4 / 3 slots 2.02 / 2.03 / 2.03 / 2.15
     int fused_grid = 0, fused_nsplit = 0;
     size_t fused_smem = 0;
 
@@ -630,9 +630,9 @@ struct TextModel {
             AHA_REQUIRE(decode_impl < 2 || ok, "fused decode kernel unsupported for this model: " + why);
             AHA_REQUIRE(decode_impl != 3 || tp_world == 1, "the grid-barrier twin of the fused kernel is single-GPU only");
             fused = ok && decode_impl != 1;
-            // auto: one GPU -> the grid-barrier kernel (measured fastest there: 794 vs 690 (hybrid) / 637 (packets) tok/s on the Qwen3-VL-2B
-            // stack, profiles/README.md); tensor parallel -> the hybrid kernel: local grid barriers inside the layer, NVLink packets for the
-            // two residual-stream exchanges (no cross-GPU barrier anywhere)
+            // auto: one GPU -> the grid-barrier kernel (measured fastest there on a B200, before the H100 port: 794 vs 690 (hybrid) / 637
+            // (packets) tok/s on the Qwen3-VL-2B stack); tensor parallel -> the hybrid kernel: local grid barriers inside the layer, NVLink
+            // packets for the two residual-stream exchanges (no cross-GPU barrier anywhere)
             fused_mode = !fused ? 0 : (decode_impl == 2 ? 1 : (decode_impl == 4 ? 2 : (decode_impl == 3 ? 0 : (tp_world > 1 ? 2 : 0))));
             fused_ll = fused && fused_mode != 0;
         }

@@ -5,11 +5,18 @@
       SPEC = ';'-separated runs, each ','-separated key=value with keys impl, dbg, stages, ctx, tl (1 = print the phase
       timeline), st (1 = dump the per-stage trace of an AHA_STAGE_TRACE build to profile_out/stage_trace_<tag>.npy)
       e.g. --sweep "impl=0;impl=0,dbg=3;impl=3,tl=1"
-AHA_SHAPE = vl2 (default) | q0.6; AHA_LIB = path of an alternative libaha_b200.so (copied over the in-tree one by the caller)."""
+      key ahead=N runs the spec on variants/ahead<N>.so, a build of the library with the producer's run-ahead budget set to
+      N KB (decode_fused.cuh), loaded side by side with the other builds in this process (same weights, so repeated specs
+      alternate builds without process-to-process noise):
+        nvcc <aha_b200/build.py NVCC_FLAGS> -DAHA_FUSED_AHEAD_KB=N -o variants/aheadN.so aha_b200/csrc/api.cu -ldl
+      e.g. --sweep "ahead=0;ahead=64;impl=0;ahead=0;ahead=64;impl=0"
+AHA_SHAPE = vl2 (default) | q0.6; AHA_LIB = path of an alternative libaha_b200.so, loaded instead of the in-tree one."""
 import os, sys, time
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 import numpy as np
-from aha_b200 import B200Model, synth
+from aha_b200 import B200Model, _lib, synth
+DEFAULT_LIB = os.path.abspath(os.environ["AHA_LIB"]) if os.environ.get("AHA_LIB") else _lib.LIB_PATH
 
 
 def torch_sms():
@@ -59,11 +66,14 @@ def run(conf, models):
         os.environ["AHA_FUSED_STAGES"] = str(conf["stages"])
     else:
         os.environ.pop("AHA_FUSED_STAGES", None)
-    if impl not in models:
+    lib = os.path.join(ROOT, "variants", f"ahead{conf['ahead']}.so") if "ahead" in conf else DEFAULT_LIB
+    lib_tag = os.path.basename(lib)
+    if (lib, impl) not in models:
+        _lib._lib, _lib.LIB_PATH = None, lib   # every model keeps the library it was created on
         m = B200Model("qwen3", cfg, w, max_ctx=4096, max_prefill=64, decode_impl=impl)
         m.forward_initial(synth.synth_text_ids(8, 1000, 1), 0, want_logits=False)
-        models[impl] = m
-    m = models[impl]
+        models[(lib, impl)] = m
+    m = models[(lib, impl)]
     os.environ["AHA_FUSED_DBG"] = str(dbg)
     # decode at offset ctx: KV pages below ctx hold whatever is in the pool (timing only)
     m.decode_steps(5, ctx, steps, timed=True)
@@ -71,7 +81,7 @@ def run(conf, models):
     for _ in range(3):
         toks, ms = m.decode_steps(5, ctx, steps, timed=True)
         best = min(best, ms)
-    print(f"shape={shape} impl={impl} dbg={dbg} stages={conf.get('stages', '-')} ctx={ctx} steps={steps} ms/step={best/steps:.4f} tok/s={1e3*steps/best:.1f}", flush=True)
+    print(f"lib={lib_tag} shape={shape} impl={impl} dbg={dbg} stages={conf.get('stages', '-')} ctx={ctx} steps={steps} ms/step={best/steps:.4f} tok/s={1e3*steps/best:.1f}", flush=True)
     if int(conf.get("tl", 0)) or (sweep is None and dbg & 4):
         os.environ["AHA_FUSED_DBG"] = str(dbg | 4)
         timeline(m, ctx)
@@ -100,12 +110,18 @@ def run(conf, models):
             print(f"  cta {cta} barrier anatomy (us, mean over barriers 8..139): bar.sync {d[:,0].mean()/1e3:.2f} red.release {d[:,1].mean()/1e3:.2f} poll {d[:,2].mean()/1e3:.2f} fence {d[:,3].mean()/1e3:.2f} bar.sync {d[:,4].mean()/1e3:.2f}; polls/barrier {b[8:,6].mean():.1f}")
             dl = np.diff(l[8:], axis=1)
             print(f"  cta {cta} load_x anatomy: loads+sumsq {dl[:,0].mean()/1e3:.2f} bar.sync {dl[:,1].mean()/1e3:.2f} scale+sts+bar {dl[:,2].mean()/1e3:.2f}")
-    if sweep is None and dbg & 64:
+    if dbg & 64:
         m.decode_steps(5, ctx, 1)
         arr = np.stack([m.debug_read("fused_cta_trace", i, 256) for i in range(torch_sms())])
         os.makedirs("profile_out", exist_ok=True)
         np.save("profile_out/cta_trace.npy", arr)
         print("saved profile_out/cta_trace.npy", arr.shape)
+        # arrival skew at each grid barrier of layers 2.. (mode 0: 5 per layer): last CTA against the median and the first
+        b = arr[:, 10:5 * 28]
+        b = b[:, : b.shape[1] // 5 * 5]
+        last, med, first = b.max(0), np.median(b, 0), b.min(0)
+        for k, n in enumerate(["qkv", "attn", "o", "gate_up", "down"]):
+            print(f"    arrival skew after {n:8s} last-median {(last - med)[k::5].mean()/1e3:6.2f} us  last-first {(last - first)[k::5].mean()/1e3:6.2f} us")
     os.environ["AHA_FUSED_DBG"] = "0"
 
 
