@@ -26,7 +26,10 @@
 //     The same protocol carries the tensor-parallel exchange: o_proj / down partial sums are stored straight into
 //     every peer GPU's packet buffer over NVLink (8-byte stores are atomic there too) and summed in rank order by the
 //     reader -- a one-shot all-reduce with no collective call and no cross-GPU barrier.
-//     LL = false keeps the grid-barrier version (one counter in L2, release/acquire) as the A/B twin (decode_impl = 3).
+//     LL = false keeps the grid-barrier version (one counter in L2, release/acquire) as the A/B twin (decode_impl = 3).  Its
+//     qkv -> attention exchange is packets as well, but only inside each kv-head group: the nsplit CTAs that compute a group's
+//     q / k / v rows (qkv_slab) are the ones that run its attention, so that boundary costs one L2 round trip to data that is
+//     already there instead of a grid barrier + reload; four grid barriers per layer remain.
 // Phases per layer: [rmsnorm+qkv] -> [attention] -> [o_proj+residual] -> [rmsnorm+gate/up+SwiGLU] ->
 // [down+residual]; then [final norm + lm_head + argmax] and the on-device token feedback.
 //
@@ -91,7 +94,6 @@ struct FusedArgs {
     const float* inv_freq;
     DecodeState* st;
     float* x;          // [H]   residual stream
-    float* qkv1;       // [qkv_dim]
     float* h1;         // [I]
     float* logits;     // [V]
     float* partial;    // [nh][nsplit][kFusedPartialStride]
@@ -105,7 +107,8 @@ struct FusedArgs {
     int stages;        // ring slots in use (<= kFusedStages)
     int dbg;           // timing experiments only: bit0 = skip grid barriers, bit1 = skip the GEMV math, bit2 = timestamps, bit3 = old full-fence grid barrier, bit6 = per-CTA barrier arrival stamps, bit4 / bit5 = drop the L2 evict-first hint on weight / KV copies, bit7 = per-stage trace of CTA (dbg >> 16) & 0xff (AHA_STAGE_TRACE builds), bit8 = skip the activation / partial loads (streaming-rate experiments; results are garbage), bit9 = sync only (no weight stream, no math), bit10 = sync anatomy stamps of the traced CTA (AHA_STAGE_TRACE builds)
     unsigned long long* trace;  // [2][4096] globaltimer stamps of CTA 0 (consumer thread 0 / producer), dbg bit2
-    // ---- LL mode: packet buffers (device memory, zero-initialised once; tags make every step's data self-validating)
+    // ---- packet buffers (device memory, zero-initialised once; tags make every step's data self-validating).  ll_qkv, ll_tag and
+    // ll_abort serve every MODE (the qkv -> attention hand-off is always packets); the rest only MODEs 1 and 2.
     LLPk* ll_qkv;      // [qkv_dim]
     LLPk* ll_pb;       // [nh][nsplit][kFusedPartialStride] split-KV attention partials (acc[128], m, l)
     LLPk* ll_att;      // [nh * hd] merged attention output
@@ -119,7 +122,7 @@ struct FusedArgs {
     // "data is out" flags, one word per producing CTA and vector kind: written (relaxed, after the CTA's packets) by thread 0,
     // polled by ONE warp of a consumer that found packets missing -- the other 320 threads of every waiting CTA stay off the
     // memory system (every thread polling its own packets slows the weight stream of the CTAs still working: measured).
-    uint32_t* ll_flag;             // [4][256]: qkv | attention partials | merged attention | h, indexed by blockIdx.x
+    uint32_t* ll_flag;             // [4][256]: (unused) | attention partials | merged attention | h, indexed by blockIdx.x
     uint32_t* ll_flag_xp_local[2]; // this rank's own [tp_world][256] flags of the o_proj | down partial sums
     uint32_t ll_tag;   // tag of layer 0 of this launch; layer l uses ll_tag + l, the final phase ll_tag + L (never 0, never reused)
     int tp_rank, tp_world;
@@ -367,6 +370,43 @@ __device__ __forceinline__ void cta_rows(int N, int unit, int& r0, int& r1) {
     r0 = (int)((units * blockIdx.x) / gridDim.x) * unit;
     r1 = (int)((units * (blockIdx.x + 1)) / gridDim.x) * unit;
 }
+// The rows of one GEMV phase this CTA owns, as the share [j0, j1) of a sequence of rows made of up to three segments of
+// contiguous matrix rows (ends e0, e1; sequence position j sits at matrix row j + b[segment]).  The producer and the consumers
+// both walk it with Slab::stage, so a stage never straddles two segments and both sides cut the same stages.
+struct Slab {
+    int j0, j1;
+    int e0 = 0x7fffffff, e1 = 0x7fffffff;
+    int b0 = 0, b1 = 0, b2 = 0;
+    // the stage that starts at position j: its first matrix row and its row count (at most R)
+    __device__ __forceinline__ int stage(int j, int R, int& nr) const {
+        const int end = j < e0 ? e0 : (j < e1 ? e1 : 0x7fffffff);
+        nr = min(R, min(j1, end) - j);
+        return j + (j < e0 ? b0 : (j < e1 ? b1 : b2));
+    }
+};
+__device__ __forceinline__ Slab cta_slab(int N, int unit) {
+    Slab s;
+    cta_rows(N, unit, s.j0, s.j1);
+    return s;
+}
+// qkv rows by kv-head group: group g's sequence is the q rows of its heads gG .. gG+G-1, then the k rows and the v rows of kv
+// head g, (G + 2) * hd rows shared evenly by the group's nsplit attention CTAs (attn_item), so that the CTA (g, split) waits only
+// for the packets of its own group's CTAs before its attention.  CTAs past nkv * nsplit own no qkv rows.
+__device__ __forceinline__ Slab qkv_slab(int nh, int nkv, int hd, int nsplit) {
+    Slab s;
+    s.j0 = s.j1 = 0;
+    if ((int)blockIdx.x >= nkv * nsplit) return s;
+    const int g = blockIdx.x / nsplit, split = blockIdx.x % nsplit, G = nh / nkv;
+    const int n = (G + 2) * hd;
+    s.j0 = (n * split) / nsplit;
+    s.j1 = (n * (split + 1)) / nsplit;
+    s.e0 = G * hd;
+    s.e1 = (G + 1) * hd;
+    s.b0 = g * G * hd;
+    s.b1 = (nh + g) * hd - s.e0;
+    s.b2 = (nh + nkv + g) * hd - s.e1;
+    return s;
+}
 // Rows per ring stage.  Short phases (few rows per CTA) use smaller stages so that the slab spreads over more consumer
 // warps -- the per-stage latency of one warp is on the critical path of every phase.
 __host__ __device__ __forceinline__ int rows_per_stage(int K, int N, int grid) {
@@ -425,12 +465,10 @@ struct Producer {
         mbar_wait(&ring.empty[slot], ((it / ns) & 1u) ^ 1u);
         AHA_STAGE_STAMP(st_trace, it, 0);
     }
-    __device__ void rows(const __half* W, int N, int K, int unit) {
-        int r0, r1;
-        cta_rows(N, unit, r0, r1);
+    __device__ void rows(const __half* W, int N, int K, const Slab& s) {
         const int R = rows_per_stage(K, N, gridDim.x);
-        for (int r = r0; r < r1; r += R) {
-            const int nr = min(R, r1 - r);
+        for (int j = s.j0, nr; j < s.j1; j += nr) {
+            const int r = s.stage(j, R, nr);
             const uint32_t bytes = (uint32_t)nr * K * 2u;
             int slot;
             acquire(slot, bytes);
@@ -738,15 +776,15 @@ struct Consumer {
     // block `par` of every tensor-parallel peer, WITHOUT the residual: readers add it from their own copy of the stream).
     template <int EPI, bool LL = false>
     __device__ void gemv(const FusedArgs& a, int N, int K, const float* bias, float* out, float& best, int& bi, uint32_t tag = 0, int par = 0, int row_off = 0) {
-        int r0, r1;
-        cta_rows(N, EPI == FE_SWIGLU ? 2 : 1, r0, r1);
+        const Slab s = EPI == FE_QKV ? qkv_slab(a.nh, a.nkv, a.hd, a.nsplit) : cta_slab(N, EPI == FE_SWIGLU ? 2 : 1);
+        const int r0 = s.j0;
         const int R = rows_per_stage(K, N, gridDim.x);
-        enter((uint32_t)(r1 - r0) * K * 2u);
+        enter((uint32_t)(s.j1 - s.j0) * K * 2u);
         if (sync_only) { consumer_bar_sync(); return; }
         unsigned i = it;
-        for (int r = r0; r < r1; r += R, ++i) {
+        for (int j = s.j0, nr; j < s.j1; j += nr, ++i) {
+            const int r = s.stage(j, R, nr);
             if (!owns(i)) continue;
-            const int nr = min(R, r1 - r);
             const uint8_t* st = wait_full(i);
             float v[kFusedMaxRows];
 #pragma unroll
@@ -762,7 +800,11 @@ struct Consumer {
                 } else {   // tail stage of the slab: row by row
                     for (int q = 0; q < nr; ++q) {
                         float t[kFusedMaxRows];
-                        stage_dots<1, 4>(st + (size_t)q * K * 2, K, t);
+                        // a qkv row takes the accumulators of a full stage (NA 1 at R 8, else 2): its sum must not depend on where
+                        // the shares of its kv group end
+                        if (EPI == FE_QKV && R == 8) stage_dots<1, 1>(st + (size_t)q * K * 2, K, t);
+                        else if (EPI == FE_QKV) stage_dots<1, 2>(st + (size_t)q * K * 2, K, t);
+                        else stage_dots<1, 4>(st + (size_t)q * K * 2, K, t);
 #pragma unroll
                         for (int z = 0; z < kFusedMaxRows; ++z) if (z == q) v[z] = t[0];
                     }
@@ -805,8 +847,7 @@ struct Consumer {
         it = i;
         consumer_bar_sync();
         if (LL && threadIdx.x == 0) {   // every packet store of this CTA has been issued: raise its "data is out" flag
-            if (EPI == FE_QKV) ll_flag_store<false>(a.ll_flag + 0 * 256 + blockIdx.x, tag);
-            else if (EPI == FE_SWIGLU) ll_flag_store<false>(a.ll_flag + 3 * 256 + blockIdx.x, tag);
+            if (EPI == FE_SWIGLU) ll_flag_store<false>(a.ll_flag + 3 * 256 + blockIdx.x, tag);
             else if (EPI == FE_RESID) {
                 if (a.tp_world == 1) ll_flag_store<false>(a.ll_flag_xp_local[par] + blockIdx.x, tag);
                 else for (int w = 0; w < a.tp_world; ++w) ll_flag_store<true>(a.ll_peers->flag_xp[par][w] + (size_t)a.tp_rank * 256 + blockIdx.x, tag);
@@ -828,7 +869,7 @@ struct AttnSmem {
 };
 
 template <int G, bool LL = false>
-__device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s, const float* cs, const uint16_t* spages, int layer, const FusedLayer& Ly, int t_new, uint32_t tag = 0) {
+__device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s, const float* cs, const uint16_t* spages, int layer, const FusedLayer& Ly, int t_new, uint32_t tag) {
     constexpr int HD = 128;
     const int ctx = t_new + 1;
     const int lane = c.lane, warp = c.warp, tid = threadIdx.x;
@@ -836,19 +877,14 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
     const bool has_item = attn_item(a, ctx, kvh, split, hp0, hp1);
     if (!has_item || c.sync_only) return;  // this CTA's producer issued nothing for the phase either
     // ---- prologue: q heads (warps 0..G-1) and the new k (warp G): RMSNorm over hd then RoPE; v copy (warp G+1)
-    if (LL) {   // are this head's q / k / v rows out yet?  (fast path: yes; else one warp polls the qkv flags of the grid)
-        bool ok = true;
-        if (warp <= G + 1) {
-            const size_t src_off = (size_t)(warp < G ? (kvh * G + warp) : (warp == G ? (a.nh + kvh) : (a.nh + a.nkv + kvh))) * HD + lane * 4;
-            const uint4 pa = ll_load2<false>(a.ll_qkv + src_off), pb2 = ll_load2<false>(a.ll_qkv + src_off + 2);
-            ok = pa.y == tag && pa.w == tag && pb2.y == tag && pb2.w == tag;
-        }
-        if (!consumer_all(ok)) ll_wait_flags<false>(a.ll_flag, 1, 0, (int)gridDim.x, tag, c.ll_abort);
-    }
+    // Warps 0..G+1 each poll the 128 packets of their own row of q / k / v until they carry this layer's tag: one L2 round trip
+    // once the group's CTAs (qkv_slab) have stored them.  No "data is out" flag here: the flag poll, the CTA barrier after it and
+    // the re-read of the packets were three more dependent round trips (measured: 1.82 -> 1.75 ms per VL2 step on an H100 when
+    // dropped), and 512 polled floats per CTA are too little traffic to slow the weight streams of the CTAs still in qkv.
     if (warp <= G) {
         const bool is_q = warp < G;
         const size_t src_off = (size_t)(is_q ? (kvh * G + warp) : (a.nh + kvh)) * HD + lane * 4;
-        const float4 x = LL ? ll_wait4<false>(a.ll_qkv + src_off, tag, c.ll_abort) : __ldcg(reinterpret_cast<const float4*>(a.qkv1 + src_off));
+        const float4 x = ll_wait4<false>(a.ll_qkv + src_off, tag, c.ll_abort);
         float ss = x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
         ss = warp_sum(ss);
         const float inv = 1.0f / sqrtf(ss / (float)HD + a.eps);
@@ -869,7 +905,7 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
         *reinterpret_cast<float4*>(dst + lane * 4) = make_float4(o[0], o[1], o[2], o[3]);
     } else if (warp == G + 1) {
         const size_t src_off = (size_t)(a.nh + a.nkv + kvh) * HD + lane * 4;
-        float4 v = LL ? ll_wait4<false>(a.ll_qkv + src_off, tag, c.ll_abort) : __ldcg(reinterpret_cast<const float4*>(a.qkv1 + src_off));
+        float4 v = ll_wait4<false>(a.ll_qkv + src_off, tag, c.ll_abort);
 #ifdef AHA_KV_ROUND_FP16
         v = make_float4(kv_store_round(v.x), kv_store_round(v.y), kv_store_round(v.z), kv_store_round(v.w));
 #endif
@@ -1039,9 +1075,11 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// MODE 0: grid barriers between all phases.  MODE 1: every phase exchanges tagged packets.  MODE 2 (hybrid): grid barriers around the
-// attention and between gate/up and down (their exchanges are large or need an extra hop as packets: measured slower), tagged
-// packets for the two residual-stream exchanges per layer -- the ones that cross GPUs under tensor parallelism.
+// MODE 0: grid barriers between all other phases.  MODE 1: every phase exchanges tagged packets.  MODE 2 (hybrid): grid barriers
+// after the attention and between gate/up and down (their exchanges are large or need an extra hop as packets: measured slower),
+// tagged packets for the two residual-stream exchanges per layer -- the ones that cross GPUs under tensor parallelism.
+// In every MODE the qkv rows go to the attention as packets inside each kv-head group (qkv_slab): the attention CTA (g, split) needs
+// only its group's q / k / v rows, so it waits for the group's nsplit CTAs instead of a grid barrier behind all of them.
 template <int G, int MODE>
 __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(FusedArgs a) {
     constexpr bool LL = MODE == 1, PX = MODE != 0;   // PX: the residual stream lives in shared memory and its updates travel as packets
@@ -1100,15 +1138,15 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             for (int l = 0; l < a.L; ++l) {
                 const FusedLayer Ly = nxt;
                 if (l + 1 < a.L) nxt = a.layers[l + 1];   // pointer table one layer ahead: off the issue path
-                p.rows(Ly.qkv, a.qkv_dim, a.H, 1); AHA_STAMP(a, 1, pe);
+                p.rows(Ly.qkv, a.qkv_dim, a.H, qkv_slab(a.nh, a.nkv, a.hd, a.nsplit)); AHA_STAMP(a, 1, pe);
                 p.attn(a, l, ctx); AHA_STAMP(a, 1, pe);
-                p.rows(Ly.o, a.H, a.nh * a.hd, 1);
+                p.rows(Ly.o, a.H, a.nh * a.hd, cta_slab(a.H, 1));
                 AHA_STAMP(a, 1, pe);
-                p.rows(Ly.gu, 2 * a.I, a.H, 2); AHA_STAMP(a, 1, pe);
-                p.rows(Ly.down, a.H, a.I, 1);
+                p.rows(Ly.gu, 2 * a.I, a.H, cta_slab(2 * a.I, 2)); AHA_STAMP(a, 1, pe);
+                p.rows(Ly.down, a.H, a.I, cta_slab(a.H, 1));
                 AHA_STAMP(a, 1, pe);
             }
-            p.rows(a.lm_head + (size_t)a.v0 * a.H, a.V_l, a.H, 1); AHA_STAMP(a, 1, pe);
+            p.rows(a.lm_head + (size_t)a.v0 * a.H, a.V_l, a.H, cta_slab(a.V_l, 1)); AHA_STAMP(a, 1, pe);
         }
         return;
     }
@@ -1170,15 +1208,15 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             CSTAMP();
         } else if constexpr (MODE == 2) {
             const uint32_t tag = a.ll_tag + (uint32_t)l;
-            // P1: x = residual + down partial sums of layer l - 1 (packets, all ranks); qkv leaves as plain floats
+            // P1: x = residual + down partial sums of layer l - 1 (packets, all ranks); qkv leaves as packets to the kv group
             if (first) c.load_x(a.H, nullptr, emb_row, Ly.ln1, a.eps, true);
             else if (a.tp_world == 1) c.template load_ll<false, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
             CSTAMP();
-            c.template gemv<FE_QKV>(a, a.qkv_dim, a.H, Ly.qkv_b, a.qkv1, best, bi); CSTAMP();
-            grid_barrier(&a.sync[0], seq, a.dbg, a.trace, sy); CSTAMP();
+            c.template gemv<FE_QKV, true>(a, a.qkv_dim, a.H, Ly.qkv_b, nullptr, best, bi, tag); CSTAMP();
+            CSTAMP();
             // P2: attention (split partials as plain floats)
             CSTAMP();
-            fused_attention<G>(a, c, *as, cs, spages, l, Ly, t_new); CSTAMP();
+            fused_attention<G>(a, c, *as, cs, spages, l, Ly, t_new, tag); CSTAMP();
             grid_barrier(&a.sync[0], seq, a.dbg, a.trace, sy); CSTAMP();
             // P3: merge the splits, o_proj partial sums -> packets to every rank (no barrier: P4 polls them)
             c.load_attn(a); CSTAMP();
@@ -1194,14 +1232,16 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             c.template gemv<FE_RESID, true>(a, a.H, a.I, nullptr, nullptr, best, bi, tag, 1); CSTAMP();
             CSTAMP();
         } else {
-        // P1: qkv = Wqkv . rmsnorm(x)      (layer 0 reads the embedding row directly: Embedding::forward)
+        const uint32_t tag = a.ll_tag + (uint32_t)l;
+        // P1: qkv = Wqkv . rmsnorm(x)      (layer 0 reads the embedding row directly: Embedding::forward); the rows leave as
+        // packets that only the CTAs of their kv group wait for (qkv_slab): no grid barrier before the attention
         c.load_x(a.H, a.x, first ? emb_row : nullptr, Ly.ln1, a.eps);
         CSTAMP();
-        c.template gemv<FE_QKV>(a, a.qkv_dim, a.H, Ly.qkv_b, a.qkv1, best, bi); CSTAMP();
-        grid_barrier(&a.sync[0], seq, a.dbg, a.trace, sy); CSTAMP();
+        c.template gemv<FE_QKV, true>(a, a.qkv_dim, a.H, Ly.qkv_b, nullptr, best, bi, tag); CSTAMP();
+        CSTAMP();
         // P2: attention over the paged cache (+ q/k norm, RoPE, KV append)
         CSTAMP();
-        fused_attention<G>(a, c, *as, cs, spages, l, Ly, t_new); CSTAMP();
+        fused_attention<G>(a, c, *as, cs, spages, l, Ly, t_new, tag); CSTAMP();
         grid_barrier(&a.sync[0], seq, a.dbg, a.trace, sy); CSTAMP();
         // P3: x = resid + Wo . attn
         c.load_attn(a); CSTAMP();

@@ -666,9 +666,12 @@ struct TextModel {
                 fl[l] = FusedLayer{T.qkv.w, T.o.w, T.gu.w, T.down.w, T.qkv.b, T.o.b, T.ln1, T.ln2, T.qn, T.kn};
             }
             d_fused_layers = upload(c, fl);
+            auto zalloc = [&](size_t n) { LLPk* p = c.alloc<LLPk>(n); AHA_CUDA_CHECK(cudaMemset(p, 0, n * sizeof(LLPk))); return p; };
+            // every MODE hands q / k / v to the attention as packets (decode_fused.cuh: qkv_slab)
+            ll_qkv = zalloc((size_t)qkv_dim);
+            d_ll_abort = c.alloc<int>(1);
+            AHA_CUDA_CHECK(cudaMemset(d_ll_abort, 0, sizeof(int)));
             if (fused_ll) {
-                auto zalloc = [&](size_t n) { LLPk* p = c.alloc<LLPk>(n); AHA_CUDA_CHECK(cudaMemset(p, 0, n * sizeof(LLPk))); return p; };
-                ll_qkv = zalloc((size_t)qkv_dim);
                 ll_pb = zalloc((size_t)nh_l * fused_nsplit * kFusedPartialStride);
                 ll_att = zalloc((size_t)nh_l * cfg.hd);
                 ll_h = zalloc((size_t)I_l);
@@ -682,8 +685,6 @@ struct TextModel {
                 AHA_CUDA_CHECK(cudaMemset(ll_flag, 0, 4 * 256 * sizeof(uint32_t)));
                 AHA_REQUIRE(c.num_sms <= 256, "more than 256 SMs");
                 d_ll_peers = c.alloc<LLPeerTab>(1);
-                d_ll_abort = c.alloc<int>(1);
-                AHA_CUDA_CHECK(cudaMemset(d_ll_abort, 0, sizeof(int)));
             }
             d_ftrace = c.alloc<unsigned long long>(kFusedTraceWords);
             AHA_CUDA_CHECK(cudaMemset(d_ftrace, 0, kFusedTraceWords * sizeof(unsigned long long)));
@@ -755,7 +756,7 @@ struct TextModel {
         AHA_CUDA_CHECK(cudaMemcpy(&flag, d_ll_abort, sizeof(int), cudaMemcpyDeviceToHost));
         if (flag) {
             cudaMemset(d_ll_abort, 0, sizeof(int));
-            throw std::runtime_error("fused decode step: a packet never arrived (tensor-parallel peer not running the same step?)");
+            throw std::runtime_error("fused decode step: a packet never arrived (a CTA or a tensor-parallel peer did not run the same step)");
         }
     }
     // all-reduce(sum) of a partial projection over the tensor-parallel ranks, then x += sum (the residual add)
@@ -901,7 +902,7 @@ struct TextModel {
         fa.layers = d_fused_layers; fa.L = cfg.L; fa.H = cfg.H; fa.I = I_l; fa.nh = nh_l; fa.nkv = nkv_l; fa.hd = cfg.hd; fa.V = cfg.V; fa.qkv_dim = qkv_dim;
         fa.eps = cfg.eps; fa.scaling = (float)(1.0 / std::sqrt((double)cfg.hd));
         fa.embed = embed; fa.lm_head = lm_head; fa.final_norm = norm; fa.inv_freq = inv_freq; fa.st = d_state;
-        fa.x = x1; fa.qkv1 = qkv1; fa.h1 = h1; fa.logits = logits; fa.partial = partial;
+        fa.x = x1; fa.h1 = h1; fa.logits = logits; fa.partial = partial;
         fa.sync = d_sync; fa.pmax = pmax; fa.pidx = pidx; fa.argmax_out = d_argmax;
         fa.history = d_history; fa.hist_cap = hist_cap; fa.kv_pool = kv_pool; fa.layer_stride = layer_stride; fa.page_stride = page_stride;
         fa.page_table = table.d; fa.nsplit = fused_nsplit;
@@ -911,8 +912,15 @@ struct TextModel {
         fa.tp_rank = tp_rank; fa.tp_world = tp_world;
         fa.v0 = (int)(((long long)cfg.V * tp_rank) / tp_world);
         fa.V_l = (int)(((long long)cfg.V * (tp_rank + 1)) / tp_world) - fa.v0;
+        fa.ll_qkv = ll_qkv; fa.ll_abort = d_ll_abort;
+        // Packet tags are kernel parameters: fresh on every launch, which is why the fused step is launched directly and never
+        // replayed from a captured graph (decode_step_argmax).  After 2^26 launches the counter restarts at 1: 0 is the "never
+        // written" tag of the zeroed buffers, and the tags a launch finds in them are always those of the launch before.
+        if (++ll_launches == (1u << 26)) ll_launches = 1;
+        fa.ll_tag = ll_launches * 64u;   // layer l -> tag + l (L <= 62), the final phase tag + L
+        AHA_REQUIRE(cfg.L <= 62, "fused decode kernel: more than 62 layers");
         if (fused_ll) {
-            fa.ll_qkv = ll_qkv; fa.ll_pb = ll_pb; fa.ll_att = ll_att; fa.ll_h = ll_h; fa.ll_abort = d_ll_abort;
+            fa.ll_pb = ll_pb; fa.ll_att = ll_att; fa.ll_h = ll_h; fa.ll_flag = ll_flag;
             if (!ll_peers_ready) {
                 LLPeerTab tab{};
                 for (int w = 0; w < tp_world; ++w) {
@@ -937,10 +945,6 @@ struct TextModel {
                 fa.ll_flag_xp_local[0] = fl;
                 fa.ll_flag_xp_local[1] = fl + (size_t)tp_world * 256;
             }
-            fa.ll_flag = ll_flag;
-            ll_launches += 1;
-            fa.ll_tag = ll_launches * 64u;   // layer l -> tag + l (L <= 62); 0 is the "never written" tag of the zeroed buffers
-            AHA_REQUIRE(cfg.L <= 62, "fused decode kernel: more than 62 layers");
         } else {
             fa.v0 = 0; fa.V_l = cfg.V;
         }

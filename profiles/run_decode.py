@@ -10,6 +10,8 @@
       alternate builds without process-to-process noise):
         nvcc <aha_b200/build.py NVCC_FLAGS> -DAHA_FUSED_AHEAD_KB=N -o variants/aheadN.so aha_b200/csrc/api.cu -ldl
       e.g. --sweep "ahead=0;ahead=64;impl=0;ahead=0;ahead=64;impl=0"
+      key lib=PATH runs the spec on the library at PATH the same way, e.g. a build of the parent commit against this tree's:
+        --sweep "lib=/tmp/parent.so,tl=1;impl=0,tl=1;lib=/tmp/parent.so;impl=0"
 AHA_SHAPE = vl2 (default) | q0.6; AHA_LIB = path of an alternative libaha_b200.so, loaded instead of the in-tree one."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -36,6 +38,7 @@ cfg = synth.get_config("qwen3", "q0.6")
 if shape == "vl2":
     cfg.update(hidden_size=2048, intermediate_size=6144, rope_theta=5e6)   # Qwen3-VL-2B text stack shape (else: Qwen3-0.6B / ASR-0.6B)
 w = synth.make_weights("qwen3", cfg, 0)
+# "P1 bar" is empty where qkv goes to the attention as packets (every mode): the hand-off wait is the start of "P2 attn"
 NAMES = ["P1 load_x", "P1 gemv", "P1 bar", "P2 -", "P2 attn", "P2 bar", "P3 load_x", "P3 gemv", "P3 bar", "P4 load_x", "P4 gemv", "P4 bar", "P5 load_x", "P5 gemv", "P5 bar"]
 
 
@@ -67,6 +70,7 @@ def run(conf, models):
     else:
         os.environ.pop("AHA_FUSED_STAGES", None)
     lib = os.path.join(ROOT, "variants", f"ahead{conf['ahead']}.so") if "ahead" in conf else DEFAULT_LIB
+    lib = os.path.abspath(conf["lib"]) if "lib" in conf else lib
     lib_tag = os.path.basename(lib)
     if (lib, impl) not in models:
         _lib._lib, _lib.LIB_PATH = None, lib   # every model keeps the library it was created on
@@ -104,10 +108,10 @@ def run(conf, models):
             t = m.debug_read("fused_sync_trace", 0, 8192)
             tag = f"{shape}_impl{impl}_dbg{dbg}_cta{cta}"
             np.save(f"profile_out/sync_trace_{tag}.npy", t)
-            b = t[:4096].reshape(512, 8)[:140]
+            b = t[:4096].reshape(512, 8)[:112]
             l = t[4096:].reshape(1024, 4)[:112]
             d = np.diff(b[8:, :6], axis=1)
-            print(f"  cta {cta} barrier anatomy (us, mean over barriers 8..139): bar.sync {d[:,0].mean()/1e3:.2f} red.release {d[:,1].mean()/1e3:.2f} poll {d[:,2].mean()/1e3:.2f} fence {d[:,3].mean()/1e3:.2f} bar.sync {d[:,4].mean()/1e3:.2f}; polls/barrier {b[8:,6].mean():.1f}")
+            print(f"  cta {cta} barrier anatomy (us, mean over barriers 8..111): bar.sync {d[:,0].mean()/1e3:.2f} red.release {d[:,1].mean()/1e3:.2f} poll {d[:,2].mean()/1e3:.2f} fence {d[:,3].mean()/1e3:.2f} bar.sync {d[:,4].mean()/1e3:.2f}; polls/barrier {b[8:,6].mean():.1f}")
             dl = np.diff(l[8:], axis=1)
             print(f"  cta {cta} load_x anatomy: loads+sumsq {dl[:,0].mean()/1e3:.2f} bar.sync {dl[:,1].mean()/1e3:.2f} scale+sts+bar {dl[:,2].mean()/1e3:.2f}")
     if dbg & 64:
@@ -116,12 +120,12 @@ def run(conf, models):
         os.makedirs("profile_out", exist_ok=True)
         np.save("profile_out/cta_trace.npy", arr)
         print("saved profile_out/cta_trace.npy", arr.shape)
-        # arrival skew at each grid barrier of layers 2.. (mode 0: 5 per layer): last CTA against the median and the first
-        b = arr[:, 10:5 * 28]
-        b = b[:, : b.shape[1] // 5 * 5]
+        # arrival skew at each grid barrier of layers 2.. (mode 0: 4 per layer; qkv reaches the attention as packets inside each
+        # kv-head group): last CTA against the median and the first
+        b = arr[:, 8:4 * 28]
         last, med, first = b.max(0), np.median(b, 0), b.min(0)
-        for k, n in enumerate(["qkv", "attn", "o", "gate_up", "down"]):
-            print(f"    arrival skew after {n:8s} last-median {(last - med)[k::5].mean()/1e3:6.2f} us  last-first {(last - first)[k::5].mean()/1e3:6.2f} us")
+        for k, n in enumerate(["attn", "o", "gate_up", "down"]):
+            print(f"    arrival skew after {n:8s} last-median {(last - med)[k::4].mean()/1e3:6.2f} us  last-first {(last - first)[k::4].mean()/1e3:6.2f} us")
     os.environ["AHA_FUSED_DBG"] = "0"
 
 
