@@ -17,19 +17,24 @@
 //     of the residual stream the CTA keeps on chip, SwiGLU, argmax) is applied by its lanes; attention is split-KV
 //     with per-warp online softmax over the half pages the warp owns, q/k RMSNorm + RoPE + KV append fused in, and
 //     the merge of the splits folded into the o_proj input load;
-//   * phases exchange their (tiny) outputs through L2 as TAGGED PACKETS {value, tag} (template flag LL, the default): the
-//     producer of a value stores 8 bytes -- single-copy atomic, so the tag validates the value -- and the consumer of a
-//     vector polls the packets it needs until their tags carry this step's layer tag.  No fence, no counter, no separate
-//     load after a barrier: one store -> one (re)load per dependency instead of the four dependent L2 round trips of
-//     store-ack / release / poll / load that a grid barrier costs (measured: red.release 1.0 us + poll 0.7 us +
-//     fence.acq_rel 0.4 us + activation load 1.1 us per phase boundary, 5 boundaries per layer; profiles/README.md).
-//     The same protocol carries the tensor-parallel exchange: o_proj / down partial sums are stored straight into
-//     every peer GPU's packet buffer over NVLink (8-byte stores are atomic there too) and summed in rank order by the
-//     reader -- a one-shot all-reduce with no collective call and no cross-GPU barrier.
-//     LL = false keeps the grid-barrier version (one counter in L2, release/acquire) as the A/B twin (decode_impl = 3).  Its
-//     qkv -> attention exchange is packets as well, but only inside each kv-head group: the nsplit CTAs that compute a group's
-//     q / k / v rows (qkv_slab) are the ones that run its attention, so that boundary costs one L2 round trip to data that is
-//     already there instead of a grid barrier + reload; four grid barriers per layer remain.
+//   * some phase outputs travel through L2 as TAGGED PACKETS {value, tag}: the producer of a value stores 8 bytes --
+//     single-copy atomic, so the tag validates the value -- and the consumer of a vector polls the packets it needs until
+//     their tags carry this step's layer tag.  No fence, no counter, no separate load after a barrier: one store -> one
+//     (re)load per dependency instead of the four dependent L2 round trips of store-ack / release / poll / load that a grid
+//     barrier costs (measured: red.release 1.0 us + poll 0.7 us + fence.acq_rel 0.4 us + activation load 1.1 us per phase
+//     boundary; profiles/README.md).
+// The qkv -> attention exchange is packets in both modes of the kernel, but only inside each kv-head group: the nsplit CTAs
+// that compute a group's q / k / v rows (qkv_slab) are the ones that run its attention, so that boundary costs one L2 round
+// trip to data that is already there instead of a grid barrier + reload.  The other four boundaries per layer depend on the
+// template flag PACKET_RESID:
+//   * false (the default on one GPU, and decode_impl = 3): grid barriers (one counter in L2, release/acquire); the residual
+//     stream lives in global memory, each CTA keeping on chip the rows it updates;
+//   * true (the default under tensor parallelism, and decode_impl = 4 on one GPU): every CTA keeps the whole residual
+//     stream in shared memory, and its two updates per layer -- the o_proj and down partial sums -- travel as packets.
+//     Under tensor parallelism they are stored straight into every peer GPU's packet buffer over NVLink (8-byte stores are
+//     atomic there too) and summed in rank order by the reader -- a one-shot all-reduce with no collective call and no
+//     cross-GPU barrier.  The boundaries after the attention and after gate/up stay grid barriers: as packets their
+//     exchanges are large or need an extra hop (measured slower).
 // Phases per layer: [rmsnorm+qkv] -> [attention] -> [o_proj+residual] -> [rmsnorm+gate/up+SwiGLU] ->
 // [down+residual]; then [final norm + lm_head + argmax] and the on-device token feedback.
 //
@@ -57,7 +62,7 @@ constexpr int kFusedMaxOwnRows = 64;                     // residual-stream rows
 constexpr int kFusedPartialStride = 128 + 4;             // floats per (head, split) attention partial: acc[128], m, l, pad (16-byte rows)
 constexpr int kFusedMergeChunk = 20;                     // splits merged per pass when the o_proj input is assembled
 constexpr int kFusedMaxPages = 1024;                     // page-table entries staged in shared memory as uint16 (32K tokens; physical page ids < 65536)
-constexpr int kFusedMaxH = 4096;                         // residual stream kept per CTA in shared memory (LL mode)
+constexpr int kFusedMaxH = 4096;                         // residual stream kept per CTA in shared memory (PACKET_RESID)
 constexpr int kFusedMaxTp = 8;                           // tensor-parallel ranks on one NVSwitch domain
 // Run-ahead budget of the producer: stages of a phase the consumers have not entered yet may be issued only while they end at
 // most this many bytes past the end of the consumers' current phase (stages of the current phase are never held back).  Without
@@ -108,11 +113,8 @@ struct FusedArgs {
     int dbg;           // timing experiments only: bit0 = skip grid barriers, bit1 = skip the GEMV math, bit2 = timestamps, bit3 = old full-fence grid barrier, bit6 = per-CTA barrier arrival stamps, bit4 / bit5 = drop the L2 evict-first hint on weight / KV copies, bit7 = per-stage trace of CTA (dbg >> 16) & 0xff (AHA_STAGE_TRACE builds), bit8 = skip the activation / partial loads (streaming-rate experiments; results are garbage), bit9 = sync only (no weight stream, no math), bit10 = sync anatomy stamps of the traced CTA (AHA_STAGE_TRACE builds)
     unsigned long long* trace;  // [2][4096] globaltimer stamps of CTA 0 (consumer thread 0 / producer), dbg bit2
     // ---- packet buffers (device memory, zero-initialised once; tags make every step's data self-validating).  ll_qkv, ll_tag and
-    // ll_abort serve every MODE (the qkv -> attention hand-off is always packets); the rest only MODEs 1 and 2.
+    // ll_abort serve both modes (the qkv -> attention hand-off is always packets); the rest only PACKET_RESID.
     LLPk* ll_qkv;      // [qkv_dim]
-    LLPk* ll_pb;       // [nh][nsplit][kFusedPartialStride] split-KV attention partials (acc[128], m, l)
-    LLPk* ll_att;      // [nh * hd] merged attention output
-    LLPk* ll_h;        // [I]
     // Per-peer pointers live in a DEVICE table, not in this struct: indexing a kernel-parameter array with a runtime value makes the
     // compiler copy the whole parameter block to local memory, and then every `a.field` of the hot loops is a local load (measured:
     // all phases of the packet modes 1.5-4 us slower until this was moved out).
@@ -122,7 +124,6 @@ struct FusedArgs {
     // "data is out" flags, one word per producing CTA and vector kind: written (relaxed, after the CTA's packets) by thread 0,
     // polled by ONE warp of a consumer that found packets missing -- the other 320 threads of every waiting CTA stay off the
     // memory system (every thread polling its own packets slows the weight stream of the CTAs still working: measured).
-    uint32_t* ll_flag;             // [4][256]: (unused) | attention partials | merged attention | h, indexed by blockIdx.x
     uint32_t* ll_flag_xp_local[2]; // this rank's own [tp_world][256] flags of the o_proj | down partial sums
     uint32_t ll_tag;   // tag of layer 0 of this launch; layer l uses ll_tag + l, the final phase ll_tag + L (never 0, never reused)
     int tp_rank, tp_world;
@@ -290,6 +291,8 @@ __device__ __forceinline__ bool consumer_all(bool ok) {
     return r != 0;
 }
 // Warp 0 polls `rows` x `n` flags (row stride `stride`) until each carries `tag`; everybody meets at the CTA barrier after.
+// Every caller passes one row; the two arguments stay because dropping them moves the register allocation around the call
+// sites (CUDA 12.9: 40 more bytes of spill stores in decode_step_fused_kernel<2, true>).
 template <bool SYS>
 __device__ __noinline__ void ll_wait_flags(const uint32_t* f, int rows, int stride, int n, uint32_t tag, int* abort_flag) {
     if (threadIdx.x < 32) {
@@ -518,7 +521,7 @@ struct Consumer {
     float* xs;          // [K] activation vector (shared), also aliased by the attention scratch
     float* red;         // [32] scratch
     float* xown;        // [kFusedMaxOwnRows] this CTA's rows of the residual stream (never re-read from global memory; barrier mode)
-    float* xres = nullptr;   // [H] LL mode: the whole residual stream, kept by every CTA (thread t always touches the same elements)
+    float* xres = nullptr;   // [H] PACKET_RESID: the whole residual stream, kept by every CTA (thread t always touches the same elements)
     int* ll_abort = nullptr;
     int warp, lane;
 
@@ -607,31 +610,30 @@ struct Consumer {
         ++n_loads;
     }
 
-    // LL mode: stage x = [residual +] sum_r packets[r * vstride + e] in xs (optional RMSNorm).  The packets are polled until
-    // they carry `tag`; all loads of a vector are issued before the first tag is looked at, and the common case (data already
-    // there) costs one L2 round trip.  RESID: the sum is added into the residual stream this CTA keeps in shared memory
-    // (fixed rank order r = 0, 1, ... -> every CTA of every GPU forms bit-identical sums).
+    // PACKET_RESID: x = residual + sum_r packets[r * vstride + e] is added into the residual stream this CTA keeps in shared
+    // memory, and RMSNorm(x) is staged in xs.  The packets are polled until they carry `tag`; all loads of a vector are issued
+    // before the first tag is looked at, and the common case (data already there) costs one L2 round trip.  Fixed rank order
+    // r = 0, 1, ... -> every CTA of every GPU forms bit-identical sums.
     // flags / nflag: the "data is out" words of the CTAs that produce vector r (row r of `flags`, row stride 256).
-    template <bool SYS, bool RESID>
+    template <bool SYS>
     __device__ __forceinline__ void load_ll(int K, const LLPk* pk, int nvec, size_t vstride, uint32_t tag, const float* norm_w, float eps, const uint32_t* flags, int nflag) {
         constexpr int kChunk = kFusedConsumers * 32 * 4;   // elements one pass of the consumer threads covers
-        if (K <= 2 * kChunk) load_ll_n<SYS, RESID, RESID, 2>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
-        else if (K <= 3 * kChunk) load_ll_n<SYS, RESID, RESID, 3>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
-        else load_ll_n<SYS, RESID, RESID, (kFusedMaxK + kChunk - 1) / kChunk>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
+        if (K <= 2 * kChunk) load_ll_n<SYS, 2>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
+        else if (K <= 3 * kChunk) load_ll_n<SYS, 3>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
+        else load_ll_n<SYS, (kFusedMaxK + kChunk - 1) / kChunk>(K, pk, nvec, vstride, tag, norm_w, eps, flags, nflag);
     }
-    // NORM: RMSNorm of the vector (the residual-stream loads: RESID and NORM always come together; the o_proj / down inputs take neither)
-    template <bool SYS, bool RESID, bool NORM, int kPer>
+    template <bool SYS, int kPer>
     __device__ void load_ll_n(int K, const LLPk* pk, int nvec, size_t vstride, uint32_t tag, const float* norm_w, float eps, const uint32_t* flags, int nflag) {
         const int tid = threadIdx.x;
-        float4 v[kPer], w[NORM ? kPer : 1];
+        float4 v[kPer], w[kPer];
 #pragma unroll
         for (int j = 0; j < kPer; ++j) {
             const int e = (tid + j * kFusedConsumers * 32) * 4;
             v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (NORM) w[j] = v[j];
+            w[j] = v[j];
             if (e < K) {
-                if (NORM) w[j] = *reinterpret_cast<const float4*>(norm_w + e);
-                if (RESID) v[j] = *reinterpret_cast<const float4*>(xres + e);
+                w[j] = *reinterpret_cast<const float4*>(norm_w + e);
+                v[j] = *reinterpret_cast<const float4*>(xres + e);
             }
         }
         for (int r = 0; r < nvec; ++r) {
@@ -664,27 +666,23 @@ struct Consumer {
                 }
             }
         }
-        if (RESID) {
 #pragma unroll
-            for (int j = 0; j < kPer; ++j) {
-                const int e = (tid + j * kFusedConsumers * 32) * 4;
-                if (e < K) *reinterpret_cast<float4*>(xres + e) = v[j];
-            }
+        for (int j = 0; j < kPer; ++j) {
+            const int e = (tid + j * kFusedConsumers * 32) * 4;
+            if (e < K) *reinterpret_cast<float4*>(xres + e) = v[j];
         }
-        if (NORM) {
-            float ss = 0.f;
+        float ss = 0.f;
 #pragma unroll
-            for (int j = 0; j < kPer; ++j) ss += v[j].x * v[j].x + v[j].y * v[j].y + v[j].z * v[j].z + v[j].w * v[j].w;
-            ss = warp_sum(ss);
-            if (lane == 0) red[warp] = ss;
-            consumer_bar_sync();
-            float tot = 0.f;
+        for (int j = 0; j < kPer; ++j) ss += v[j].x * v[j].x + v[j].y * v[j].y + v[j].z * v[j].z + v[j].w * v[j].w;
+        ss = warp_sum(ss);
+        if (lane == 0) red[warp] = ss;
+        consumer_bar_sync();
+        float tot = 0.f;
 #pragma unroll
-            for (int q = 0; q < kFusedConsumers; ++q) tot += red[q];
-            const float inv = 1.0f / sqrtf(tot / (float)K + eps);
+        for (int q = 0; q < kFusedConsumers; ++q) tot += red[q];
+        const float inv = 1.0f / sqrtf(tot / (float)K + eps);
 #pragma unroll
-            for (int j = 0; j < kPer; ++j) { v[j].x *= inv * w[j].x; v[j].y *= inv * w[j].y; v[j].z *= inv * w[j].z; v[j].w *= inv * w[j].w; }
-        }
+        for (int j = 0; j < kPer; ++j) { v[j].x *= inv * w[j].x; v[j].y *= inv * w[j].y; v[j].z *= inv * w[j].z; v[j].w *= inv * w[j].w; }
 #pragma unroll
         for (int j = 0; j < kPer; ++j) {
             const int e = (tid + j * kFusedConsumers * 32) * 4;
@@ -772,8 +770,8 @@ struct Consumer {
 
     // One GEMV phase: y[r0:r1) = W[r0:r1, :] . xs  with the fused epilogue.  Ends with a consumer barrier so
     // that xs may be overwritten by the next phase.
-    // LL: the outputs leave as tagged packets (qkv -> ll_qkv, SwiGLU -> ll_h, o_proj / down partial sums -> the [rank][H]
-    // block `par` of every tensor-parallel peer, WITHOUT the residual: readers add it from their own copy of the stream).
+    // LL: the outputs leave as tagged packets (qkv -> ll_qkv, o_proj / down partial sums -> the [rank][H] block `par` of every
+    // tensor-parallel peer, WITHOUT the residual: readers add it from their own copy of the stream).
     template <int EPI, bool LL = false>
     __device__ void gemv(const FusedArgs& a, int N, int K, const float* bias, float* out, float& best, int& bi, uint32_t tag = 0, int par = 0, int row_off = 0) {
         const Slab s = EPI == FE_QKV ? qkv_slab(a.nh, a.nkv, a.hd, a.nsplit) : cta_slab(N, EPI == FE_SWIGLU ? 2 : 1);
@@ -823,11 +821,7 @@ struct Consumer {
             if (lane < nr) {
                 const int row = r + lane;
                 if (EPI == FE_SWIGLU) {
-                    if ((lane & 1) == 0) {   // rows (2i, 2i+1) = (gate_i, up_i)
-                        const float hval = silu_f(mine) * mate;
-                        if (LL) ll_store<false>(a.ll_h + (row >> 1), hval, tag);
-                        else out[row >> 1] = hval;
-                    }
+                    if ((lane & 1) == 0) out[row >> 1] = silu_f(mine) * mate;   // rows (2i, 2i+1) = (gate_i, up_i)
                 } else {
                     float y = mine;
                     if (bias) y += bias[row];
@@ -846,12 +840,9 @@ struct Consumer {
         }
         it = i;
         consumer_bar_sync();
-        if (LL && threadIdx.x == 0) {   // every packet store of this CTA has been issued: raise its "data is out" flag
-            if (EPI == FE_SWIGLU) ll_flag_store<false>(a.ll_flag + 3 * 256 + blockIdx.x, tag);
-            else if (EPI == FE_RESID) {
-                if (a.tp_world == 1) ll_flag_store<false>(a.ll_flag_xp_local[par] + blockIdx.x, tag);
-                else for (int w = 0; w < a.tp_world; ++w) ll_flag_store<true>(a.ll_peers->flag_xp[par][w] + (size_t)a.tp_rank * 256 + blockIdx.x, tag);
-            }
+        if (LL && EPI == FE_RESID && threadIdx.x == 0) {   // every packet store of this CTA has been issued: raise its "data is out" flag
+            if (a.tp_world == 1) ll_flag_store<false>(a.ll_flag_xp_local[par] + blockIdx.x, tag);
+            else for (int w = 0; w < a.tp_world; ++w) ll_flag_store<true>(a.ll_peers->flag_xp[par][w] + (size_t)a.tp_rank * 256 + blockIdx.x, tag);
         }
     }
 };
@@ -868,7 +859,7 @@ struct AttnSmem {
 
 };
 
-template <int G, bool LL = false>
+template <int G>
 __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s, const float* cs, const uint16_t* spages, int layer, const FusedLayer& Ly, int t_new, uint32_t tag) {
     constexpr int HD = 128;
     const int ctx = t_new + 1;
@@ -1020,80 +1011,32 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
                 O += s.acc[w][g][d] * e;
             }
         }
-        const size_t po = ((size_t)(kvh * G + g) * a.nsplit + split) * kFusedPartialStride;
-        if (LL) {
-            ll_store<false>(a.ll_pb + po + d, O, tag);
-            if (d == 0) { ll_store<false>(a.ll_pb + po + HD, M, tag); ll_store<false>(a.ll_pb + po + HD + 1, L, tag); }
-        } else {
-            float* p = a.partial + po;
-            p[d] = O;
-            if (d == 0) { p[HD] = M; p[HD + 1] = L; }
-        }
+        float* p = a.partial + ((size_t)(kvh * G + g) * a.nsplit + split) * kFusedPartialStride;
+        p[d] = O;
+        if (d == 0) { p[HD] = M; p[HD + 1] = L; }
     }
-    // barrier mode: the split partials are merged by the consumers of the next phase (Consumer::load_attn), after the grid barrier
-    if (!LL) return;
-    consumer_bar_sync();
-    const int item = kvh * a.nsplit + split;
-    if (tid == 0) ll_flag_store<false>(a.ll_flag + 1 * 256 + item, tag);
-    // LL mode: the nsplit CTAs of this kv head merge the partials among themselves -- CTA `split` owns the dims
-    // [d0, d1) of the group's G heads: warp g takes head g, lane s takes split s (all (m, l) pairs and value packets of a
-    // pass are in flight together), and the merged values leave as packets of the attention vector that o_proj reads.
-    // 150 KB of partials per reader (every CTA merging every head) becomes 2-3 KB here plus the 16 KB vector.
-    {   // fast path: the (m, l) packets of every split of the group are there
-        bool ok = true;
-        if (warp < G && lane < a.nsplit) {
-            const uint4 ml = ll_load2<false>(a.ll_pb + ((size_t)(kvh * G + warp) * a.nsplit + lane) * kFusedPartialStride + HD);
-            ok = ml.y == tag && ml.w == tag;
-        }
-        if (!consumer_all(ok)) ll_wait_flags<false>(a.ll_flag + 1 * 256 + kvh * a.nsplit, 1, 0, a.nsplit, tag, c.ll_abort);
-    }
-    if (warp < G) {
-        const int per = (HD + a.nsplit - 1) / a.nsplit;
-        const int d0 = split * per, d1 = min(HD, d0 + per);
-        const int h = kvh * G + warp;
-        const LLPk* pbase = a.ll_pb + ((size_t)h * a.nsplit + lane) * kFusedPartialStride;   // lane = split index
-        const bool on = lane < a.nsplit;
-        float m = -INFINITY, l = 0.f;
-        if (on) {
-            m = ll_wait1<false>(pbase + HD, tag, c.ll_abort);
-            l = ll_wait1<false>(pbase + HD + 1, tag, c.ll_abort);
-        }
-        float M = m;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, o));
-        const float e = (m == -INFINITY) ? 0.f : expf(m - M);
-        const float Ls = warp_sum(l * e);
-        for (int d = d0; d < d1; ++d) {
-            // the packets of a partial were stored by different threads: each one is validated on its own
-            const float val = on ? ll_wait1<false>(pbase + d, tag, c.ll_abort) : 0.f;
-            const float O = warp_sum(val * e) / Ls;
-            if (lane == 0) ll_store<false>(a.ll_att + (size_t)h * HD + d, O, tag);
-        }
-    }
-    consumer_bar_sync();
-    if (tid == 0) ll_flag_store<false>(a.ll_flag + 2 * 256 + item, tag);
+    // the split partials are merged by the consumers of the next phase (Consumer::load_attn), after the grid barrier
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// MODE 0: grid barriers between all other phases.  MODE 1: every phase exchanges tagged packets.  MODE 2 (hybrid): grid barriers
-// after the attention and between gate/up and down (their exchanges are large or need an extra hop as packets: measured slower),
+// PACKET_RESID = false: grid barriers after the attention, o_proj, gate/up and down.  PACKET_RESID = true: grid barriers after
+// the attention and between gate/up and down (their exchanges are large or need an extra hop as packets: measured slower),
 // tagged packets for the two residual-stream exchanges per layer -- the ones that cross GPUs under tensor parallelism.
-// In every MODE the qkv rows go to the attention as packets inside each kv-head group (qkv_slab): the attention CTA (g, split) needs
+// In both modes the qkv rows go to the attention as packets inside each kv-head group (qkv_slab): the attention CTA (g, split) needs
 // only its group's q / k / v rows, so it waits for the group's nsplit CTAs instead of a grid barrier behind all of them.
-template <int G, int MODE>
+template <int G, bool PACKET_RESID>
 __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(FusedArgs a) {
-    constexpr bool LL = MODE == 1, PX = MODE != 0;   // PX: the residual stream lives in shared memory and its updates travel as packets
     extern __shared__ __align__(1024) uint8_t fused_smem_raw[];
     uint8_t* ringbuf = fused_smem_raw;
     uint64_t* full = reinterpret_cast<uint64_t*>(fused_smem_raw + (size_t)kFusedStages * kFusedStageBytes);
     uint64_t* empty = full + kFusedStages;
     float* red = reinterpret_cast<float*>(empty + kFusedStages);
     uint32_t* gate = reinterpret_cast<uint32_t*>(red) + kFusedGateWord;   // the producer's run-ahead gate (Consumer::enter)
-    float* xown = red + 32;                                     // [kFusedMaxOwnRows] (barrier mode only: LL mode keeps the whole stream in xres)
-    float* cs = xown + (MODE != 0 ? 0 : kFusedMaxOwnRows);      // [128] cos | sin of the step's rotary angles
+    float* xown = red + 32;                                     // [kFusedMaxOwnRows] (barrier mode only: PACKET_RESID keeps the whole stream in xres)
+    float* cs = xown + (PACKET_RESID ? 0 : kFusedMaxOwnRows);   // [128] cos | sin of the step's rotary angles
     float* xs = cs + 128;                                       // [kFusedMaxK] activations / attention scratch
     uint16_t* spages = reinterpret_cast<uint16_t*>(xs + kFusedMaxK);   // [kFusedMaxPages] page table copy (physical page ids)
-    float* xres = reinterpret_cast<float*>(spages + kFusedMaxPages);   // [kFusedMaxH] LL mode: the residual stream (not carved in barrier mode)
+    float* xres = reinterpret_cast<float*>(spages + kFusedMaxPages);   // [kFusedMaxH] PACKET_RESID: the residual stream (not carved in barrier mode)
     AttnSmem<G>* as = reinterpret_cast<AttnSmem<G>*>(xs);
     static_assert(sizeof(AttnSmem<G>) <= kFusedMaxK * sizeof(float), "attention scratch must fit in the xs region");
 
@@ -1169,7 +1112,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
     const __half* emb_row = a.embed + (size_t)token * a.H;
     int own_r0, own_r1;
     cta_rows(a.H, 1, own_r0, own_r1);
-    if (!PX && tid < own_r1 - own_r0) xown[tid] = __half2float(emb_row[own_r0 + tid]);   // the rows of the residual stream this CTA owns start as the embedding row
+    if (!PACKET_RESID && tid < own_r1 - own_r0) xown[tid] = __half2float(emb_row[own_r0 + tid]);   // the rows of the residual stream this CTA owns start as the embedding row
     int ce = 0;
 #define CSTAMP() do { if (tid == 0) AHA_STAMP(a, 0, ce); } while (0)
     CSTAMP();
@@ -1178,39 +1121,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
         const FusedLayer Ly = nxtc;
         if (l + 1 < a.L) nxtc = a.layers[l + 1];
         const bool first = (l == 0);
-        if constexpr (LL) {
-            // Data-flow version: every phase polls the packets it needs (tag of this layer), no grid barrier anywhere.
-            const uint32_t tag = a.ll_tag + (uint32_t)l;
-            const LLPk* xp_o = a.ll_xp_local[0];     // this rank's [tp_world][H] blocks of o_proj / down partial sums
-            const LLPk* xp_d = a.ll_xp_local[1];
-            // P1: qkv = Wqkv . rmsnorm(x); x = residual + the down partial sums of layer l - 1 (layer 0: the embedding row)
-            if (first) c.load_x(a.H, nullptr, emb_row, Ly.ln1, a.eps, true);
-            else if (a.tp_world == 1) c.template load_ll<false, true>(a.H, xp_d, a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true, true>(a.H, xp_d, a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
-            CSTAMP();
-            c.template gemv<FE_QKV, true>(a, a.qkv_dim, a.H, Ly.qkv_b, nullptr, best, bi, tag); CSTAMP();
-            CSTAMP();
-            // P2: attention over the paged cache (+ q/k norm, RoPE, KV append), then the merge of the splits inside the kv group
-            CSTAMP();
-            fused_attention<G, true>(a, c, *as, cs, spages, l, Ly, t_new, tag); CSTAMP();
-            CSTAMP();
-            // P3: o_proj partial sums (this rank's heads) -> every rank
-            c.template load_ll<false, false>(a.nh * a.hd, a.ll_att, 1, 0, tag, nullptr, 0.f, a.ll_flag + 2 * 256, a.nkv * a.nsplit); CSTAMP();
-            c.template gemv<FE_RESID, true>(a, a.H, a.nh * a.hd, Ly.o_b, nullptr, best, bi, tag, 0); CSTAMP();
-            CSTAMP();
-            // P4: h = silu(gate) * up on rmsnorm(x), x = residual + sum over ranks of the o_proj partial sums
-            if (a.tp_world == 1) c.template load_ll<false, true>(a.H, xp_o, a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x); else c.template load_ll<true, true>(a.H, xp_o, a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x);
-            CSTAMP();
-            c.template gemv<FE_SWIGLU, true>(a, 2 * a.I, a.H, nullptr, nullptr, best, bi, tag); CSTAMP();
-            CSTAMP();
-            // P5: down partial sums (this rank's slice of the intermediate dimension) -> every rank
-            c.template load_ll<false, false>(a.I, a.ll_h, 1, 0, tag, nullptr, 0.f, a.ll_flag + 3 * 256, (int)gridDim.x); CSTAMP();
-            c.template gemv<FE_RESID, true>(a, a.H, a.I, nullptr, nullptr, best, bi, tag, 1); CSTAMP();
-            CSTAMP();
-        } else if constexpr (MODE == 2) {
+        if constexpr (PACKET_RESID) {
             const uint32_t tag = a.ll_tag + (uint32_t)l;
             // P1: x = residual + down partial sums of layer l - 1 (packets, all ranks); qkv leaves as packets to the kv group
             if (first) c.load_x(a.H, nullptr, emb_row, Ly.ln1, a.eps, true);
-            else if (a.tp_world == 1) c.template load_ll<false, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
+            else if (a.tp_world == 1) c.template load_ll<false>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, tag - 1u, Ly.ln1, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
             CSTAMP();
             c.template gemv<FE_QKV, true>(a, a.qkv_dim, a.H, Ly.qkv_b, nullptr, best, bi, tag); CSTAMP();
             CSTAMP();
@@ -1222,8 +1137,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             c.load_attn(a); CSTAMP();
             c.template gemv<FE_RESID, true>(a, a.H, a.nh * a.hd, Ly.o_b, nullptr, best, bi, tag, 0); CSTAMP();
             CSTAMP();
-            // P4
-            if (a.tp_world == 1) c.template load_ll<false, true>(a.H, a.ll_xp_local[0], a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x); else c.template load_ll<true, true>(a.H, a.ll_xp_local[0], a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x);
+            // P4: x = residual + o_proj partial sums (packets, all ranks); h = silu(gate) * up on rmsnorm(x)
+            if (a.tp_world == 1) c.template load_ll<false>(a.H, a.ll_xp_local[0], a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x); else c.template load_ll<true>(a.H, a.ll_xp_local[0], a.tp_world, (size_t)a.H, tag, Ly.ln2, a.eps, a.ll_flag_xp_local[0], (int)gridDim.x);
             CSTAMP();
             c.template gemv<FE_SWIGLU>(a, 2 * a.I, a.H, nullptr, a.h1, best, bi); CSTAMP();
             grid_barrier(&a.sync[0], seq, a.dbg, a.trace, sy); CSTAMP();
@@ -1259,7 +1174,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
         }
     }
     // final: logits = lm_head . rmsnorm(x) over this rank's vocabulary shard, per-CTA argmax candidate
-    if constexpr (PX) if (a.tp_world == 1) c.template load_ll<false, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, a.ll_tag + (uint32_t)a.L - 1u, a.final_norm, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true, true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, a.ll_tag + (uint32_t)a.L - 1u, a.final_norm, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
+    if constexpr (PACKET_RESID) if (a.tp_world == 1) c.template load_ll<false>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, a.ll_tag + (uint32_t)a.L - 1u, a.final_norm, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x); else c.template load_ll<true>(a.H, a.ll_xp_local[1], a.tp_world, (size_t)a.H, a.ll_tag + (uint32_t)a.L - 1u, a.final_norm, a.eps, a.ll_flag_xp_local[1], (int)gridDim.x);
     else c.load_x(a.H, a.x, nullptr, a.final_norm, a.eps);
     best = -INFINITY; bi = 0x7fffffff;
     c.template gemv<FE_LOGITS>(a, a.V_l, a.H, nullptr, a.logits + a.v0, best, bi, 0, 0, a.v0); CSTAMP();
@@ -1296,7 +1211,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             const int oi = __shfl_xor_sync(0xffffffffu, gi, o);
             if (ov > gb || (ov == gb && oi < gi)) { gb = ov; gi = oi; }
         }
-        if (PX && a.tp_world > 1) {
+        if (PACKET_RESID && a.tp_world > 1) {
             // vocabulary shards: every rank publishes its (value, index) candidate to every rank and picks the same winner
             // (largest value, lowest index on ties)
             const uint32_t ftag = a.ll_tag + (uint32_t)a.L;
@@ -1330,8 +1245,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
 }
 
 template <int G>
-inline size_t fused_smem_bytes(bool ll) {
-    return (ll ? (size_t)kFusedMaxH * sizeof(float) : (size_t)kFusedMaxOwnRows * sizeof(float)) + (size_t)kFusedStages * kFusedStageBytes + 2 * kFusedStages * sizeof(uint64_t) + (32 + 128) * sizeof(float) + (size_t)kFusedMaxK * sizeof(float) +
+inline size_t fused_smem_bytes(bool packet_resid) {
+    return (packet_resid ? (size_t)kFusedMaxH * sizeof(float) : (size_t)kFusedMaxOwnRows * sizeof(float)) + (size_t)kFusedStages * kFusedStageBytes + 2 * kFusedStages * sizeof(uint64_t) + (32 + 128) * sizeof(float) + (size_t)kFusedMaxK * sizeof(float) +
            (size_t)kFusedMaxPages * sizeof(uint16_t) + 64;
 }
 

@@ -483,17 +483,15 @@ struct TextModel {
     bool use_graph = true;
     // fused persistent decode kernel (decode_fused.cuh)
     bool fused = false;
-    bool fused_ll = false;               // the fused kernel keeps the residual stream on chip and exchanges packets (modes 1 and 2)
-    int fused_mode = 0;                  // decode_fused.cuh MODE: 0 grid barriers, 1 packets everywhere, 2 hybrid
+    bool fused_packet_resid = false;     // decode_fused.cuh PACKET_RESID: the residual stream on chip, its two exchanges per layer as packets
     int decode_impl = 0;
     // LL packet buffers.  The blocks a tensor-parallel peer writes (partial sums, argmax candidates) live in ONE separate
     // allocation per rank so that a single CUDA IPC handle maps them into the peers.
-    LLPk *ll_qkv = nullptr, *ll_pb = nullptr, *ll_att = nullptr, *ll_h = nullptr;
+    LLPk* ll_qkv = nullptr;
     LLPk* ll_sym = nullptr;                         // [2][W][H] partial sums | [W][2] candidates   (this rank's copy)
     LLPk* ll_peer_sym[kFusedMaxTp] = {};            // the same block of every rank (own entry = ll_sym)
     int* d_ll_abort = nullptr;
     uint32_t ll_launches = 0;
-    uint32_t* ll_flag = nullptr;                    // [4][256] local "data is out" flags
     LLPeerTab* d_ll_peers = nullptr;                // device copy of the per-peer pointer table (built once the peers are attached)
     bool ll_peers_ready = false;
     size_t ll_sym_packets() const { return (size_t)2 * tp_world * cfg.H + (size_t)tp_world * 2 + (size_t)tp_world * 256; }   // + [2][W][256] u32 flags = W * 256 packets
@@ -607,11 +605,11 @@ struct TextModel {
     }
     template <int G>
     void (*fused_kernel() const)(FusedArgs) {
-        return fused_mode == 1 ? decode_step_fused_kernel<G, 1> : (fused_mode == 2 ? decode_step_fused_kernel<G, 2> : decode_step_fused_kernel<G, 0>);
+        return fused_packet_resid ? decode_step_fused_kernel<G, true> : decode_step_fused_kernel<G, false>;
     }
     template <int G>
     void fused_prepare() {
-        fused_smem = fused_smem_bytes<G>(fused_ll);
+        fused_smem = fused_smem_bytes<G>(fused_packet_resid);
         auto prep = [&](auto kernel) {
             AHA_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fused_smem));
             int nb = 0;
@@ -626,15 +624,14 @@ struct TextModel {
         {
             std::string why;
             const bool ok = fused_supported(&why);
-            AHA_REQUIRE(decode_impl >= 0 && decode_impl <= 4, "decode_impl must be 0 (auto), 1 (per-op kernels), 2 (fused, packets), 3 (fused, grid barriers) or 4 (fused, hybrid)");
+            AHA_REQUIRE(decode_impl == 0 || decode_impl == 1 || decode_impl == 3 || decode_impl == 4,
+                        "decode_impl must be 0 (auto), 1 (per-op kernels), 3 (fused, grid barriers) or 4 (fused, packets for the residual stream)");
             AHA_REQUIRE(decode_impl < 2 || ok, "fused decode kernel unsupported for this model: " + why);
             AHA_REQUIRE(decode_impl != 3 || tp_world == 1, "the grid-barrier twin of the fused kernel is single-GPU only");
             fused = ok && decode_impl != 1;
-            // auto: one GPU -> the grid-barrier kernel (measured fastest there on a B200, before the H100 port: 794 vs 690 (hybrid) / 637
-            // (packets) tok/s on the Qwen3-VL-2B stack); tensor parallel -> the hybrid kernel: local grid barriers inside the layer, NVLink
-            // packets for the two residual-stream exchanges (no cross-GPU barrier anywhere)
-            fused_mode = !fused ? 0 : (decode_impl == 2 ? 1 : (decode_impl == 4 ? 2 : (decode_impl == 3 ? 0 : (tp_world > 1 ? 2 : 0))));
-            fused_ll = fused && fused_mode != 0;
+            // auto: one GPU -> grid barriers (measured fastest there on an H100 80GB HBM3 at 700 W; BASELINE §4); tensor parallel ->
+            // local grid barriers inside the layer, NVLink packets for the two residual-stream exchanges (no cross-GPU barrier anywhere)
+            fused_packet_resid = decode_impl == 4 || (decode_impl == 0 && fused && tp_world > 1);
         }
         num_pages = ceil_div(max_ctx, kPage);
         page_stride = (size_t)2 * nkv_l * kPage * cfg.hd;
@@ -667,22 +664,17 @@ struct TextModel {
             }
             d_fused_layers = upload(c, fl);
             auto zalloc = [&](size_t n) { LLPk* p = c.alloc<LLPk>(n); AHA_CUDA_CHECK(cudaMemset(p, 0, n * sizeof(LLPk))); return p; };
-            // every MODE hands q / k / v to the attention as packets (decode_fused.cuh: qkv_slab)
+            // both modes hand q / k / v to the attention as packets (decode_fused.cuh: qkv_slab)
             ll_qkv = zalloc((size_t)qkv_dim);
             d_ll_abort = c.alloc<int>(1);
             AHA_CUDA_CHECK(cudaMemset(d_ll_abort, 0, sizeof(int)));
-            if (fused_ll) {
-                ll_pb = zalloc((size_t)nh_l * fused_nsplit * kFusedPartialStride);
-                ll_att = zalloc((size_t)nh_l * cfg.hd);
-                ll_h = zalloc((size_t)I_l);
+            if (fused_packet_resid) {
                 void* sym = nullptr;   // its own allocation: the IPC handle of a pointer covers the whole cudaMalloc block
                 AHA_CUDA_CHECK(cudaMalloc(&sym, ll_sym_packets() * sizeof(LLPk)));
                 c.allocs.push_back(sym);
                 AHA_CUDA_CHECK(cudaMemset(sym, 0, ll_sym_packets() * sizeof(LLPk)));
                 ll_sym = reinterpret_cast<LLPk*>(sym);
                 ll_peer_sym[tp_rank] = ll_sym;
-                ll_flag = c.alloc<uint32_t>(4 * 256);
-                AHA_CUDA_CHECK(cudaMemset(ll_flag, 0, 4 * 256 * sizeof(uint32_t)));
                 AHA_REQUIRE(c.num_sms <= 256, "more than 256 SMs");
                 d_ll_peers = c.alloc<LLPeerTab>(1);
             }
@@ -730,7 +722,7 @@ struct TextModel {
         NcclApi::unique_id id;
         std::memcpy(&id, unique_id, sizeof(id));
         n.check(n.CommInitRank(&comm, tp_world, id, tp_rank), "ncclCommInitRank");
-        if (!fused_ll) return;
+        if (!fused_packet_resid) return;
         // Map every rank's packet block into this process (CUDA IPC; NVLink / NVSwitch peer access): the handles travel
         // through the communicator itself, so the C ABI needs nothing beyond the unique id it already takes.
         cudaIpcMemHandle_t mine;
@@ -919,8 +911,7 @@ struct TextModel {
         if (++ll_launches == (1u << 26)) ll_launches = 1;
         fa.ll_tag = ll_launches * 64u;   // layer l -> tag + l (L <= 62), the final phase tag + L
         AHA_REQUIRE(cfg.L <= 62, "fused decode kernel: more than 62 layers");
-        if (fused_ll) {
-            fa.ll_pb = ll_pb; fa.ll_att = ll_att; fa.ll_h = ll_h; fa.ll_flag = ll_flag;
+        if (fused_packet_resid) {
             if (!ll_peers_ready) {
                 LLPeerTab tab{};
                 for (int w = 0; w < tp_world; ++w) {

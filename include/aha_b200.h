@@ -67,9 +67,9 @@ typedef struct aha_options {
     int32_t max_frames;    /* largest mel frame count (0 = 3000); Qwen3-ASR only */
     int32_t use_graph;     /* 1 = replay the decode step from a CUDA graph (default), 0 = eager launches */
     int32_t decode_impl;   /* 0 = auto (persistent fused step kernel where the model shape allows: grid-barrier version on one GPU,
-                            * tagged-packet version under tensor parallelism), 1 = per-op kernels under a CUDA graph (validation twin),
-                            * 2 = fused, tagged-packet (data-flow) version, 3 = fused, grid-barrier version (single GPU only), 4 = fused hybrid (grid
-                            * barriers inside the layer, tagged packets for the two residual-stream exchanges) */
+                            * hybrid version under tensor parallelism), 1 = per-op kernels under a CUDA graph (validation twin),
+                            * 3 = fused, grid-barrier version (single GPU only), 4 = fused hybrid (grid barriers inside the layer, tagged
+                            * packets for the two residual-stream exchanges).  2 is refused. */
     int32_t gemm_impl;     /* 0 = auto, 1 = SIMT fp32, 2 = wgmma 128x128 tiles (split-fp16, fp32-exact), 3 = wgmma 128x256 tiles */
     const void* tp_comm;   /* opaque: ncclUniqueId bytes (128) when tp_world > 1, else NULL */
     int32_t reserved[8];   /* reserved[0]: prefill attention, 0 = tensor cores (wgmma kernel; split-fp16), 1 = fp32 SIMT twin, 2 = mma.sync kernel everywhere */

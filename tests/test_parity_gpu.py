@@ -81,12 +81,11 @@ def test_qwen3_greedy_generate_matches_oracle(q3):
 
 
 def test_qwen3_decode_implementations_agree(q3):
-    """fused persistent kernel (default: grid-barrier version; 2 = tagged-packet version) == per-op kernels under a CUDA graph
-    == per-op eager launches."""
+    """fused persistent kernel (default: grid-barrier version; 3 = the same, asked for; 4 = hybrid version) == per-op kernels under
+    a CUDA graph == per-op eager launches."""
     cfg, w, m, o = q3
     others = [make_model("qwen3", "tiny", max_ctx=512, decode_impl=1)[2],
               make_model("qwen3", "tiny", max_ctx=512, decode_impl=1, use_graph=False)[2],
-              make_model("qwen3", "tiny", max_ctx=512, decode_impl=2)[2],
               make_model("qwen3", "tiny", max_ctx=512, decode_impl=3)[2],
               make_model("qwen3", "tiny", max_ctx=512, decode_impl=4)[2]]
     try:
@@ -108,7 +107,7 @@ def test_qwen3_decode_implementations_agree(q3):
             m2.close()
 
 
-@pytest.mark.parametrize("impl", [1, 2, 3, 4])
+@pytest.mark.parametrize("impl", [1, 3, 4])
 def test_qwen3_long_context_decode(impl):
     """decode far past the prompt: many KV pages, every split of the attention busy."""
     cfg, w, m = make_model("qwen3", "tiny", max_ctx=2048, decode_impl=impl)
@@ -126,10 +125,10 @@ def test_qwen3_long_context_decode(impl):
         m.close()
 
 
-@pytest.mark.parametrize("impl", [1, 2, 3, 4])
+@pytest.mark.parametrize("impl", [1, 3, 4])
 def test_qwen3_production_row_shapes(impl):
     """Qwen3-VL-2B text-stack row shapes (H=2048, I=6144; 2 layers): the 4-row / 1-row tensor-core stage paths of the
-    fused kernel (impl 2) and the per-op kernels (impl 1) against the oracle, teacher-forced over page boundaries."""
+    fused kernel (impl 3, 4) and the per-op kernels (impl 1) against the oracle, teacher-forced over page boundaries."""
     cfg, w, m = make_model("qwen3", "mid", max_ctx=512, decode_impl=impl)
     try:
         o = make_oracle("qwen3", cfg, w)
@@ -198,6 +197,13 @@ def test_error_behaviour(q3):
     # the handle stays usable after an error
     m.clear_cache()
     assert m.forward_initial(_ids(4, cfg["vocab_size"], 1), 0).shape == (1, 1, cfg["vocab_size"])
+
+
+def test_removed_decode_impl_is_refused_at_create():
+    """decode_impl 2 is not a decode path: create fails and the message names the values that are."""
+    from aha_b200 import B200Error
+    with pytest.raises(B200Error, match=r"decode_impl must be 0 \(auto\), 1 \(per-op kernels\), 3 \(fused, grid barriers\) or 4 "):
+        make_model("qwen3", "tiny", max_ctx=512, decode_impl=2)
 
 
 def test_clear_cache_resets_state(q3):
@@ -463,7 +469,7 @@ def _rand_ids(n, vocab, seed):
 
 # GQA groups other than 2 (every shipped Qwen3 size has nh / nkv = 2): MHA and a group of 4, fused and per-op decode
 @pytest.mark.parametrize("preset", ["tiny-g1", "tiny-g4"])
-@pytest.mark.parametrize("impl", [1, 2, 3, 4])
+@pytest.mark.parametrize("impl", [1, 3, 4])
 def test_decode_with_other_gqa_groups(preset, impl):
     cfg, w, m = make_model("qwen3", preset, max_ctx=512, decode_impl=impl)
     o = make_oracle("qwen3", cfg, w)
