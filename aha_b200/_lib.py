@@ -176,6 +176,10 @@ SYMBOLS = {
     "aha_b200_batch_add": (C.c_int, [_P, C.POINTER(BatchRequest), C.POINTER(C.c_int32), _U32P, C.POINTER(C.c_int32), C.POINTER(Usage)]),
     "aha_b200_batch_add_many": (C.c_int, [_P, C.POINTER(BatchRequest), C.c_size_t, C.POINTER(C.c_int32), _U32P, C.POINTER(C.c_int32),
                                           C.POINTER(Usage)]),
+    "aha_b200_batch_add_n": (C.c_int, [_P, C.POINTER(BatchRequest), C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), _U32P,
+                                       C.POINTER(C.c_int32), C.POINTER(Usage)]),
+    "aha_b200_generate_n": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), C.c_size_t, C.POINTER(C.c_uint64), _U32P,
+                                      C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
     "aha_b200_batch_step": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.POINTER(C.c_size_t)]),
     "aha_b200_batch_close": (C.c_int, [_P]),
     "aha_b200_batch_open_wide": (C.c_int, [_P, C.c_size_t]),

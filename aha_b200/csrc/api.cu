@@ -1005,6 +1005,25 @@ void session_release(aha_model* m, int slot) {
     m->session.used[slot] = false;
     m->sess().composition_changed();
 }
+// the bookkeeping of a request admitted into slot s with its first token: true (and the slot released) when that token is also its last
+bool session_admitted(aha_model* m, int s, size_t sample_len, int lp_n, uint32_t flags, uint32_t tok) {
+    m->session.budget[s] = sample_len;
+    m->session.produced[s] = 1;
+    m->session.lp_valid[s] = lp_n >= 0;
+    bool stop = sample_len == 1;
+    if ((flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok) stop = true;
+    if (stop) session_release(m, s);
+    return stop;
+}
+struct AdmitGuard {   // a failed admission leaves the session as it was: every slot the call took is released with its pages
+    aha_model* m; const std::vector<int>& slots;
+    bool ok = false;
+    ~AdmitGuard() {
+        if (ok) return;
+        for (int s : slots) { session_release(m, s); m->session.lp_valid[s] = false; }
+        m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
+    }
+};
 // width 0: the narrow session (8 slots, batched CUDA-core GEMV); 1..64: a wide session (gemv_wide.cuh)
 void session_open(aha_model* m, int width) {
     TextModel& T = m->text;
@@ -1080,15 +1099,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     }
     const auto t0 = clk::now();
-    struct Guard {   // a failure leaves the session as it was: every slot this call took is released with its pages
-        aha_model* m; const std::vector<int>& slots;
-        bool ok = false;
-        ~Guard() {
-            if (ok) return;
-            for (int s : slots) { session_release(m, s); m->session.lp_valid[s] = false; }
-            m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
-        }
-    } guard{m, slot};
+    AdmitGuard guard{m, slot};
     for (int s : slot) m->session.used[s] = true;
     std::vector<uint32_t> tok(n);
     std::vector<double> secs(n), vision(n, 0.0);
@@ -1159,18 +1170,97 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     T.clear_sampler();
     B.composition_changed();
     for (size_t i = 0; i < n; ++i) {
-        const int s = slot[i];
-        m->session.budget[s] = sample_len[i];
-        m->session.produced[s] = 1;
-        m->session.lp_valid[s] = lp_n[i] >= 0;
-        bool stop = sample_len[i] == 1;
-        if ((reqs[i].params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[i]) stop = true;
+        const bool stop = session_admitted(m, slot[i], sample_len[i], lp_n[i], reqs[i].params.flags, tok[i]);
         if (usage) {
             usage[i] = aha_usage{};
             add_usage(&usage[i], reqs[i].seq_len, 1, secs[i], 0.0, vision[i]);
         }
-        if (stop) session_release(m, s);
-        slots_out[i] = s; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
+        slots_out[i] = slot[i]; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
+    }
+}
+
+// OpenAI `n` (aha_b200_batch_add_n): n choices of one request in the n lowest free slots.  The prompt is prefilled once, into choice 0's
+// slot, by batch_prefill_slot (tower, M-RoPE, deepstack, chunks beyond max_prefill: whatever batch_add does); its pages are copied into the
+// other choices' own pages by one kv_fork launch.  Every other choice then draws its first token from the prefill logits, still in
+// TextModel::logits, with the single-row kernels forward_any draws with -- finish_argmax, the choice's sampler against an empty state at draw
+// index 0, its record -- so each choice yields exactly what batch_add yields for the request with its seed.  Nothing between two draws
+// writes logits, pmax or pidx (the sampler works in sample_work, the records in their own partials).  After the call every choice is an
+// ordinary slot that owns its pages.
+void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const uint64_t* seeds, int32_t* slots_out, uint32_t* first_tokens,
+                   int32_t* finished, aha_usage* usage) {
+    TextModel& T = m->text;
+    BatchDecoder& B = m->sess();
+    Ctx& c = m->ctx;
+    const std::string who = "batch_add_n: ";
+    // ---- every check before any device work: a refused call leaves the session untouched
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    AHA_REQUIRE(n >= 1, who + "n must be at least 1");
+    std::vector<int> slot;
+    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) slot.push_back(i);
+    AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " choices, but only " + std::to_string(slot.size()) + " of the " +
+                                      std::to_string(m->session.width) + " slots are free (step until requests finish)");
+    slot.resize(n);
+    AHA_REQUIRE(req.ids && req.seq_len >= 1, who + "the request needs input_ids");
+    const int lp_n = logprob_request(req.params, T, who);
+    for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
+    AHA_REQUIRE((req.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+    require_mm_arity(m, req.mm);
+    const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len;
+    AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+    const size_t pages = n * (size_t)ceil_div((int)ctx, kPage);
+    AHA_REQUIRE(pages <= T.pages.free_count(), who + std::to_string(n) + " choices need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
+                                                   std::to_string(T.pages.free_count() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+    std::vector<aha_batch_request> r(n, req);
+    std::vector<Sampler> samp(n);
+    for (size_t i = 0; i < n; ++i) {
+        r[i].params.seed = seeds ? seeds[i] : req.params.seed + i;
+        samp[i] = make_sampler(r[i].params, T.cfg.V);
+    }
+    const auto t0 = clk::now();
+    AdmitGuard guard{m, slot};
+    for (int s : slot) m->session.used[s] = true;
+    std::vector<uint32_t> tok(n);
+    tok[0] = batch_prefill_slot(m, slot[0], r[0], sample_len, lp_n);
+    if (n > 1) {
+        const std::vector<int> dst(slot.begin() + 1, slot.end());
+        for (int s : dst) T.pages.map(B.slots[s].table, (int)ctx);
+        B.fork(slot[0], dst, (int)req.seq_len);
+        const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};   // first_token's state: empty history, draw index 0
+        for (size_t i = 1; i < n; ++i) {
+            const int s = slot[i];
+            T.set_sampler(samp[i]);
+            AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_state, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
+            T.finish_argmax(0);
+            T.sample(0);
+            if (lp_n >= 0) T.logprobs(true, B.d_lp_rec + s, false);
+            // the draw's token and draw count, collected in the slot's own rows and read back once below
+            AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_tok + s, T.d_argmax, sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, T.d_state, sizeof(DecodeState), cudaMemcpyDeviceToDevice, c.stream));
+            B.slots[s].lp = lp_n + 1;
+            B.bind_sampler(s, samp[i]);
+        }
+        std::vector<uint32_t> h_tok((size_t)B.cap);
+        std::vector<DecodeState> h_st((size_t)B.cap);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        T.check_sample_error();
+        for (size_t i = 1; i < n; ++i) {
+            tok[i] = h_tok[slot[i]];
+            B.adopt(slot[i], tok[i], (int)req.seq_len, decode_rope_delta(m), h_st[slot[i]].n_draws);
+        }
+    }
+    const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
+    guard.ok = true;
+    T.clear_sampler();
+    B.composition_changed();
+    for (size_t i = 0; i < n; ++i) {
+        const bool stop = session_admitted(m, slot[i], sample_len, lp_n, req.params.flags, tok[i]);
+        if (usage) {
+            usage[i] = aha_usage{};
+            add_usage(&usage[i], req.seq_len, 1, secs, 0.0, vision);
+        }
+        slots_out[i] = slot[i]; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
     }
 }
 // tokens_out / status_out: [cap] entries, cap >= the session width (8 for batch_step)
@@ -1248,6 +1338,67 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
     }
     if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
 }
+
+// per slot of the open session, the record of the last token its request delivered (a zero record where there is none)
+std::vector<aha_logprobs> session_records(aha_model* m) {
+    const int width = m->session.width;
+    BatchDecoder& B = m->sess();
+    std::vector<aha_logprobs> h((size_t)width);
+    if (B.d_lp_rec) {
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h.data(), B.d_lp_rec, h.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+    }
+    for (int i = 0; i < width; ++i) if (!m->session.lp_valid[i]) h[i] = aha_logprobs{};
+    return h;
+}
+
+// n choices of one request (OpenAI `n`, 1..8): a narrow session, one batch_add_n, steps until every choice has finished.  Choice i yields
+// exactly what aha_b200_generate yields for the request with its seed, and with AHA_GEN_LOGPROBS the records generate_logprobs yields.
+void generate_n_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params& params, size_t n,
+                     const uint64_t* seeds, uint32_t* out_tokens, aha_logprobs* out_lp, size_t cap, size_t* n_out, aha_usage* usage) {
+    TextModel& T = m->text;
+    const std::string who = "generate_n: ";
+    require_no_session(m);
+    AHA_REQUIRE(n >= 1 && n <= (size_t)kGemvBatchMax, who + "n must be 1 to 8 (more choices: batch_add_n on a wide session)");
+    AHA_REQUIRE(cap >= token_budget(params), who + "out_tokens capacity (per choice) is smaller than max_tokens");
+    const bool lp = logprob_request(params, T, who) >= 0;
+    AHA_REQUIRE(!lp || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
+    for (size_t i = 0; i < n; ++i) n_out[i] = 0;
+    session_open(m, 0);
+    struct Close {   // whatever happens, the handle is left as after clear_cache()
+        aha_model* m;
+        ~Close() { session_close(m); }
+    } close{m};
+    const aha_batch_request req{ids, seq_len, mm, params};
+    std::vector<int32_t> slot(n), fin(n);
+    std::vector<uint32_t> first(n);
+    session_add_n(m, req, n, seeds, slot.data(), first.data(), fin.data(), usage);
+    std::vector<int> choice_of(kGemvBatchMax, -1);   // slot -> choice
+    auto take = [&](int s, size_t i, uint32_t t, const std::vector<aha_logprobs>& rec) {
+        out_tokens[i * cap + n_out[i]] = t;
+        if (lp) out_lp[i * cap + n_out[i]] = rec[s];
+        ++n_out[i];
+    };
+    const std::vector<aha_logprobs> none;
+    std::vector<aha_logprobs> rec = lp ? session_records(m) : none;
+    for (size_t i = 0; i < n; ++i) {
+        take(slot[i], i, first[i], rec);
+        if (!fin[i]) choice_of[slot[i]] = (int)i;
+    }
+    const auto t_dec = clk::now();
+    uint32_t tok[kGemvBatchMax];
+    int32_t status[kGemvBatchMax];
+    while (session_step(m, tok, status, kGemvBatchMax, true) > 0) {
+        if (lp) rec = session_records(m);
+        for (int s = 0; s < kGemvBatchMax; ++s) {
+            if (!status[s]) continue;
+            const int i = choice_of[s];
+            take(s, (size_t)i, tok[s], rec);
+            if (status[s] == 2 && usage) usage[i].completion_secs = seconds(clk::now() - t_dec);
+        }
+    }
+    if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
+}
 }  // namespace
 
 int aha_b200_batch_open(aha_model* m) { return guarded(m, [&] { session_open(m, 0); }); }
@@ -1274,6 +1425,22 @@ int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t 
     });
 }
 
+int aha_b200_batch_add_n(aha_model* m, const aha_batch_request* req, size_t n, const uint64_t* seeds, int32_t* slots_out, uint32_t* first_tokens_out,
+                         int32_t* finished_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(req && slots_out && first_tokens_out && finished_out, "req, slots_out, first_tokens_out and finished_out are required");
+        session_add_n(m, *req, n, seeds, slots_out, first_tokens_out, finished_out, usage);
+    });
+}
+
+int aha_b200_generate_n(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params, size_t n,
+                        const uint64_t* seeds, uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap, size_t* n_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(params && out_tokens && n_out, "params, out_tokens and n_out are required");
+        generate_n_impl(m, ids, seq_len, mm, *params, n, seeds, out_tokens, out_logprobs, cap, n_out, usage);
+    });
+}
+
 int aha_b200_batch_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t* n_stepped_out) {
     return guarded(m, [&] {
         AHA_REQUIRE(tokens_out && status_out, "tokens_out[8] and status_out[8] are required");
@@ -1296,13 +1463,8 @@ int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out, size_t cap) {
         AHA_REQUIRE(out, "batch_logprobs: out[cap] is required");
         const int width = m->session.width;
         AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-        BatchDecoder& B = m->sess();
-        std::vector<aha_logprobs> h((size_t)width);
-        if (B.d_lp_rec) {
-            AHA_CUDA_CHECK(cudaMemcpyAsync(h.data(), B.d_lp_rec, h.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
-            AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        }
-        for (size_t i = 0; i < cap; ++i) out[i] = (i < (size_t)width && m->session.lp_valid[i]) ? h[i] : aha_logprobs{};
+        const std::vector<aha_logprobs> h = session_records(m);
+        for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? h[i] : aha_logprobs{};
     });
 }
 
@@ -1537,6 +1699,28 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
 
 namespace {
 void bench_score(aha_model* m, const std::string& w, int iters, double* avg_ms, uint64_t* bytes);   // the score_head timings, defined with scoring
+
+// kernel timing "kv_fork:P:n": P pages of every layer copied from one table row to n - 1 others, over pool pages no sequence holds at the
+// time (rows of a scratch table, row r taking pages r * P .. r * P + P - 1); bytes are the algorithmic read + writes, n * P pages
+void bench_fork(aha_model* m, const std::string& w, int iters, double* avg_ms, uint64_t* bytes) {
+    TextModel& T = m->text;
+    int P = 0, n = 0;
+    AHA_REQUIRE(std::sscanf(w.c_str(), "kv_fork:%d:%d", &P, &n) == 2 && P >= 1 && n >= 2 && n <= kForkMaxDst + 1,
+                "the fork kernel is named kv_fork:P:n with P >= 1 pages and 2 <= n <= 64 choices");
+    AHA_REQUIRE((size_t)P * n <= (size_t)T.num_pages, "kv_fork bench: P * n pages exceed the pool (max_ctx / 32 = " + std::to_string(T.num_pages) + ")");
+    require_no_session(m);
+    drop_cache(m);
+    std::vector<int> h((size_t)n * T.num_pages, 0), dst;
+    for (int r = 0; r < n; ++r) for (int p = 0; p < P; ++p) h[(size_t)r * T.num_pages + p] = r * P + p;
+    for (int r = 1; r < n; ++r) dst.push_back(r);
+    Scratch mem;
+    int* tables = mem.alloc<int>(h.size());
+    AHA_CUDA_CHECK(cudaMemcpy(tables, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice));
+    auto launch = [&] { kv_fork(m->ctx, T.kv_pool, T.layer_stride, T.page_stride, T.cfg.L, tables, T.num_pages, 0, dst.data(), n - 1, P); };
+    for (int i = 0; i < 3; ++i) launch();
+    *avg_ms = timed_ms(m, (size_t)iters, [&](size_t) { launch(); }) / iters;
+    *bytes = (uint64_t)n * P * T.cfg.L * T.page_stride * sizeof(float);
+}
 }  // namespace
 
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch) {
@@ -1547,6 +1731,7 @@ int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* av
         cudaStream_t st = m->ctx.stream;
         const int L = T.cfg.L;
         if (w.rfind("score_", 0) == 0) { bench_score(m, w, iters, avg_ms, bytes_per_launch); return; }
+        if (w.rfind("kv_fork:", 0) == 0) { bench_fork(m, w, iters, avg_ms, bytes_per_launch); return; }
         uint64_t bytes = 0;
         auto launch = [&](int i) {
             TextLayer& Y = T.layers[i % L];

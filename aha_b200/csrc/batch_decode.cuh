@@ -28,6 +28,7 @@
 #pragma once
 #include "gemv_batch.cuh"
 #include "gemv_wide.cuh"
+#include "kv_fork.cuh"
 #include "text_model.cuh"
 
 namespace aha {
@@ -150,6 +151,11 @@ struct BatchDecoder {
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_states + i, &st, sizeof(st), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_hist + (size_t)i * T->hist_cap, &first_token, sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
+    }
+    // the K/V of positions [0, n_tokens) of slot src copied into slots dst, whose tables already map those pages (kv_fork.cuh)
+    void fork(int src, const std::vector<int>& dst, int n_tokens) {
+        kv_fork(*T->ctx, T->kv_pool, T->layer_stride, T->page_stride, T->cfg.L, d_tables, T->num_pages, src, dst.data(), (int)dst.size(),
+                ceil_div(n_tokens, kPage));
     }
     void ensure_lp() {
         if (d_lp_rec) return;

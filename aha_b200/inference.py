@@ -324,6 +324,64 @@ class B200Model:
         res = [(int(slots[i]), int(toks[i]), bool(fins[i])) for i in range(n)]
         return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
 
+    @staticmethod
+    def _seeds(n, seeds):
+        """per-choice seeds -> (uint64 array or None, the pointer argument)"""
+        if seeds is None:
+            return None, None
+        s = np.ascontiguousarray(np.asarray(seeds, dtype=np.uint64).reshape(-1))
+        if s.size != n:
+            raise ValueError(f"seeds must hold n = {n} seeds, got {s.size}")
+        return s, s.ctypes.data_as(C.POINTER(C.c_uint64))
+
+    def batch_add_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
+                    repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, return_usage=False):
+        """OpenAI `n` (aha_b200_batch_add_n): n choices of one request in the n lowest free slots, the prompt prefilled once and its K/V
+        copied into every other choice's own pages.  Choice i samples with seeds[i] (None: seed + i) and yields exactly what batch_add
+        yields for the request with that seed.  All or nothing.  -> [(slot, first token, finished), ...] per choice, and with
+        return_usage=True also the prompt-side usage dicts."""
+        n = int(n)
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
+        ids = self._ids(input_ids)
+        mm, _keep = self._mm(data)
+        _s, seeds_p = self._seeds(n, seeds)
+        req = L.BatchRequest()
+        req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
+        req.seq_len = ids.size
+        req.mm = C.pointer(mm) if mm is not None else None
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        k = max(n, 1)
+        slots, toks, fins, us = (C.c_int32 * k)(), (C.c_uint32 * k)(), (C.c_int32 * k)(), (L.Usage * k)()
+        self._check(self._lib.aha_b200_batch_add_n(self._h, C.byref(req), n, seeds_p, slots, toks, fins, us))
+        res = [(int(slots[i]), int(toks[i]), bool(fins[i])) for i in range(n)]
+        return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
+
+    def generate_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
+                   repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0):
+        """OpenAI `n` in one call (aha_b200_generate_n, 1 <= n <= 8): the prompt prefilled once, the choices decoded in lockstep.
+        -> [(ids, usage), ...] per choice, [(ids, usage, records), ...] with logprobs=True; choice i is exactly what generate()
+        returns for seeds[i] (None: seed + i)."""
+        n = int(n)
+        ids = self._ids(input_ids)
+        mm, _keep = self._mm(data)
+        _s, seeds_p = self._seeds(n, seeds)
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        cap, k = max(max_tokens, 1), max(n, 1)
+        out = (C.c_uint32 * (k * cap))()
+        recs = (L.Logprobs * (k * cap))() if logprobs else None
+        n_out, us = (C.c_size_t * k)(), (L.Usage * k)()
+        self._check(self._lib.aha_b200_generate_n(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint32)), ids.size,
+                                                  C.byref(mm) if mm is not None else None, C.byref(p), n, seeds_p, out, recs, cap, n_out, us))
+        res = []
+        for i in range(n):
+            toks = [int(out[i * cap + j]) for j in range(n_out[i])]
+            if logprobs:
+                res.append((toks, self._usage(us[i]), [L.logprobs_record(recs[i * cap + j]) for j in range(n_out[i])]))
+            else:
+                res.append((toks, self._usage(us[i])))
+        return res
+
     def batch_step(self):
         """One decode step of every running request -> {slot: (token, finished)} (empty when nothing is running)."""
         w = getattr(self, "_batch_width", 8)

@@ -214,6 +214,15 @@ typedef struct aha_batch_request {
 } aha_batch_request;
 int aha_b200_generate_batch(aha_model* m, const aha_batch_request* reqs, size_t n, uint32_t* out_tokens, size_t cap,
                             size_t* n_out, aha_usage* usage);
+/* OpenAI `n` in one call: n (1..8) choices of one request through a narrow session (aha_b200_batch_add_n, then steps until every choice has
+ * finished; the session is closed on every path, and the call is refused while one is open).  Choice i returns exactly what
+ * aha_b200_generate returns for the request with seed seeds[i] (NULL: params->seed + i).  Unlike generate_batch it accepts AHA_GEN_LOGPROBS /
+ * TOP_LOGPROBS: out_logprobs[i][k] is the record of out_tokens[i][k] as the narrow session's aha_b200_batch_logprobs gives it -- with the
+ * per-op decode step (aha_options.decode_impl = 1) bit for bit aha_b200_generate_logprobs' records (NULL otherwise).
+ * out_tokens: [n][cap], out_logprobs: [n][cap] or NULL, n_out: [n], usage: [n] or NULL.  More than 8 choices: batch_add_n on a wide session. */
+int aha_b200_generate_n(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params* params, size_t n,
+                        const uint64_t* seeds, uint32_t* out_tokens /* [n][cap] */, aha_logprobs* out_logprobs /* [n][cap] or NULL */,
+                        size_t cap, size_t* n_out /* [n] */, aha_usage* usage /* [n] or NULL */);
 
 /* Continuous batching on the same slots and the same lockstep step (new design): requests join and leave a running batch BETWEEN steps.
  *   batch_open                      clear_cache, enter batch mode (the single-request entries are refused until batch_close / clear_cache)
@@ -235,6 +244,17 @@ int aha_b200_batch_add(aha_model* m, const aha_batch_request* req, int32_t* slot
  * exactly the ids batch_add gives it.  slots_out / first_tokens_out / finished_out: [n]; usage: [n] or NULL (prompt side only). */
 int aha_b200_batch_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out,
                             uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage);
+/* OpenAI `n`: n choices of one request in n free slots of the open session (narrow or wide).  The prompt is prefilled ONCE (tower included),
+ * its K/V pages are copied into the other choices' pages, and every choice draws its first token from the same prefill logits with its own
+ * sampler.  Choice i uses seed seeds[i] (seeds == NULL: req->params.seed + i, so choice 0 is the request itself).  Each choice yields exactly
+ * the ids (and log-probability records) batch_add yields for the request with that seed, in the same session kind.  All or nothing, like
+ * batch_add_many: the checks (1 <= n <= free slots, n * ceil((seq_len + max_tokens) / 32) free pages, ids, multimodal arity, flags) run
+ * before any device work.  Choices take the n lowest free slots, in order; after the call each is an ordinary request that owns its pages
+ * (the copy is not shared), finishes on its own and releases them.  Greedy choices (temperature 0, no repeat penalty) are identical, as
+ * they are with n batch_add calls.  slots_out / first_tokens_out / finished_out: [n]; usage: [n] or NULL (prompt side; prompt_tokens =
+ * seq_len each). */
+int aha_b200_batch_add_n(aha_model* m, const aha_batch_request* req, size_t n, const uint64_t* seeds,
+                         int32_t* slots_out, uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage);
 int aha_b200_batch_step(aha_model* m, uint32_t* tokens_out /* [8] */, int32_t* status_out /* [8] */, size_t* n_stepped_out /* may be NULL */);
 int aha_b200_batch_close(aha_model* m);
 /* Wide continuous batching: a session of max_seqs (1..64) slots whose decode step runs every projection and the lm_head on the tensor
@@ -460,7 +480,9 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
  * layers' weights so that consecutive launches never hit L2.  which = "gemv_gate_up" | "gemv_qkv" |
  * "gemv_down" | "gemv_o" | "gemv_lm_head" | "decode_attn", or the scoring head over rows 0 .. M-1 of the last prefill with n
  * alternatives: "score_head:M:n" (score_head_kernel) | "score_twin:M:n" (gemm_tc + logprob_partial_rows_kernel), each with its final
- * RMSNorm and stage 2.  bytes_per_launch = algorithmic bytes (the score entries: the lm_head's). */
+ * RMSNorm and stage 2; or "kv_fork:P:n" (kv_fork_kernel: P KV pages of every layer copied to n - 1 other page tables, as batch_add_n
+ * does; needs P * n <= max_ctx / 32 and no open session, and clears the single-request cache).  bytes_per_launch = algorithmic bytes (the
+ * score entries: the lm_head's; kv_fork: P pages read and (n - 1) * P written). */
 /* the device sampler on a given logits row (tests): context = tokens generated so far, draw_index = draws already consumed */
 int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_params* params, const uint32_t* context,
                           size_t n_context, uint32_t draw_index, uint32_t* token_out);

@@ -247,6 +247,26 @@ public:
         }
         return res;
     }
+    // OpenAI `n` (aha_b200_generate_n): n (1..8) choices of one request, the prompt prefilled once; choice i is what generate() with the
+    // same params returns for seed seeds[i] (seeds empty: params.seed + i).  params carries the sampler (temperature, top_k, top_p, ...).
+    std::vector<std::vector<uint32_t>> generate_n(const std::vector<uint32_t>& ids, const MultiModalData* data, const aha_gen_params& params, size_t n,
+                                                  const std::vector<uint64_t>& seeds = {}, std::vector<Usage>* usage = nullptr) {
+        if (!seeds.empty() && seeds.size() != n) throw Error("generate_n: seeds must be empty or hold n seeds");
+        const size_t cap = std::max<size_t>(params.max_tokens, 1);
+        std::vector<uint32_t> out(n * cap);
+        std::vector<size_t> n_out(n);
+        std::vector<aha_usage> us(n);
+        const aha_mm mm = data ? data->view() : aha_mm{nullptr, 0};
+        check(aha_b200_generate_n(h_, ids.data(), ids.size(), data ? &mm : nullptr, &params, n, seeds.empty() ? nullptr : seeds.data(), out.data(),
+                                  nullptr, cap, n_out.data(), us.data()));
+        std::vector<std::vector<uint32_t>> res(n);
+        for (size_t i = 0; i < n; ++i) res[i].assign(out.begin() + (std::ptrdiff_t)(i * cap), out.begin() + (std::ptrdiff_t)(i * cap + n_out[i]));
+        if (usage) {
+            usage->clear();
+            for (const aha_usage& u : us) usage->push_back(Usage{u.prompt_tokens, u.completion_tokens, u.prompt_secs, u.completion_secs, u.vision_secs});
+        }
+        return res;
+    }
     // Speculative decoding of one greedy request (aha_b200_generate_speculative): verify passes of max_draft + 1 rows drafted from
     // `prediction` and, with prompt_lookup, from the prompt and the output so far.  The ids do not depend on the drafts.
     std::vector<uint32_t> generate_speculative(const std::vector<uint32_t>& ids, const MultiModalData* data, const GenerationContext& ctx,
