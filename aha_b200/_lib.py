@@ -148,6 +148,7 @@ class Stats(C.Structure):
 _P = C.c_void_p
 _U32P = C.POINTER(C.c_uint32)
 _F32P = C.POINTER(C.c_float)
+_I32P = C.POINTER(C.c_int32)
 SYMBOLS = {
     "aha_b200_abi_version": (C.c_int, []),
     "aha_b200_create": (C.c_int, [C.c_char_p, C.c_char_p, C.POINTER(TensorDesc), C.c_size_t, _U32P, C.c_size_t,
@@ -170,6 +171,10 @@ SYMBOLS = {
     "aha_b200_generate_speculative": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), C.POINTER(SpecParams), _U32P,
                                                 C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage), C.POINTER(SpecStats)]),
     "aha_b200_debug_verify_attn": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _F32P, _F32P, _F32P]),
+    "aha_b200_debug_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, _I32P, C.c_size_t,
+                                           _I32P, C.c_int, _F32P, _F32P, _F32P, _F32P]),
+    "aha_b200_debug_decode_attn": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _I32P, _I32P, _F32P, _F32P, _I32P, C.c_size_t,
+                                             _F32P, _F32P, C.c_float, C.c_float, _F32P, _F32P, _F32P]),
     "aha_b200_debug_logprobs": (C.c_int, [_P, _F32P, C.c_size_t, C.c_uint32, C.c_uint32, C.POINTER(Logprobs)]),
     "aha_b200_generate_batch": (C.c_int, [_P, C.POINTER(BatchRequest), C.c_size_t, _U32P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
     "aha_b200_batch_open": (C.c_int, [_P]),

@@ -6,6 +6,7 @@
 #include <chrono>
 #include <cstdio>
 #include <functional>
+#include <limits>
 #include <mutex>
 #include <system_error>
 #include <thread>
@@ -1505,6 +1506,70 @@ int aha_b200_generate_speculative(aha_model* m, const uint32_t* ids, size_t seq_
     });
 }
 
+extern "C++" {
+namespace {
+// Host staging of the debug attention entries: a paged KV pool laid out like the model's ([page][K|V][kv_head][kPage][hd]), filled with NaN,
+// into which each sequence's tokens 0 .. ctx - 1 are written through its page table.  Every slot no table references, and every slot past a
+// context inside its last page, stays NaN: a kernel that reads pool memory its sequence does not own, even under a mask or with a zero
+// probability, returns NaN.
+struct HostPool {
+    int nkv, hd;
+    size_t page_stride;
+    std::vector<float> data;
+    HostPool(int n_pages, int nkv_, int hd_)
+        : nkv(nkv_), hd(hd_), page_stride((size_t)2 * nkv_ * kPage * hd_), data((size_t)n_pages * page_stride, std::numeric_limits<float>::quiet_NaN()) {}
+    int pages() const { return (int)(data.size() / page_stride); }
+    // k, v: [ctx][nkv][hd]; table: ceil(ctx / kPage) distinct physical pages
+    void put(const int* table, int ctx, const float* k, const float* v) {
+        for (int p = 0; p < ceil_div(ctx, kPage); ++p)
+            AHA_REQUIRE(table[p] >= 0 && table[p] < pages(), "page table entry " + std::to_string(table[p]) + " is outside the pool");
+        for (int t = 0; t < ctx; ++t)
+            for (int h = 0; h < nkv; ++h) {
+                const size_t base = (size_t)table[t / kPage] * page_stride + (size_t)h * kPage * hd + (size_t)(t % kPage) * hd;
+                std::memcpy(&data[base], k + ((size_t)t * nkv + h) * hd, hd * sizeof(float));
+                std::memcpy(&data[base + (size_t)nkv * kPage * hd], v + ((size_t)t * nkv + h) * hd, hd * sizeof(float));
+            }
+    }
+    // layer view of the device copy `d` through the device page table `d_table`
+    KVSrc src(float* d, const int* d_table) const {
+        KVSrc s;
+        s.k = d; s.v = d + (size_t)nkv * kPage * hd; s.page_table = d_table; s.page_shift = kPageShift;
+        s.page_stride = page_stride; s.tok_stride = hd; s.head_stride = (size_t)kPage * hd;
+        return s;
+    }
+};
+// copies and fills on the model's stream, ordered with the launches that follow
+template <typename T>
+T* upload_scratch(Scratch& mem, cudaStream_t st, const T* h, size_t n) {
+    T* d = mem.alloc<T>(std::max<size_t>(n, 1));
+    if (n) AHA_CUDA_CHECK(cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, st));
+    return d;
+}
+template <typename T>
+void fill_nan(cudaStream_t st, T* d, size_t n) { AHA_CUDA_CHECK(cudaMemsetAsync(d, 0xff, n * sizeof(T), st)); }   // all-ones words: NaN
+template <int HD>
+void debug_attention_run(Ctx& c, const FlashArgs& fa, int nh, bool causal, const std::vector<std::pair<int, int>>& segs, const int* d_work, int n_work) {
+    if (segs.empty()) { flash_dispatch<HD>(c, fa, nh, causal); return; }
+    if (causal) {   // a packed prefill (embed_batch, batch_add_many)
+        PrefillSegments sg;
+        sg.segs = segs; sg.d_work = d_work; sg.n_work = n_work;
+        flash_dispatch_segments(c, fa, nh, sg);
+        return;
+    }
+    for (const auto& s : segs) {   // the ViT / audio encoder: one launch per segment, keys and queries both from the segment
+        FlashArgs f = fa;
+        f.Sq = f.Skv = s.second; f.q0 = f.kv0 = s.first;
+        flash_dispatch<HD>(c, f, nh, false);
+    }
+}
+template <int G>
+void debug_decode_launch(cudaStream_t st, int B, int nkv, const DecodeAttnArgs& a0, const DecodeAttnArgs* d_table) {
+    if (B == 1) decode_attn_kernel<128, G><<<dim3(kDecodeSplits, nkv), 256, 0, st>>>(a0);
+    else decode_attn_batch_kernel<128, G><<<dim3(kDecodeSplits, nkv, B), 256, 0, st>>>(d_table);
+}
+}  // namespace
+}  // extern "C++"
+
 int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
                                const float* v, float* out) {
     return guarded(m, [&] {
@@ -1515,36 +1580,25 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
         Ctx& c = m->ctx;
         const int R = (int)rows, nh = (int)n_heads, nkv = (int)n_kv_heads;
         const int ctx = (int)pos0 + R;
-        // a paged pool with the pages in reverse order, laid out like the model's ([page][K|V][kv_head][kPage][hd])
+        // a paged pool with the pages in reverse order and one page no table references
         const int np = ceil_div(ctx, kPage);
-        const size_t page_stride = (size_t)2 * nkv * kPage * HD;
-        std::vector<float> pool((size_t)np * page_stride);
+        HostPool pool(np + 1, nkv, HD);
         std::vector<int> table(np);
-        for (int p = 0; p < np; ++p) table[p] = np - 1 - p;
-        for (int t = 0; t < ctx; ++t)
-            for (int h = 0; h < nkv; ++h) {
-                const size_t base = (size_t)table[t / kPage] * page_stride + (size_t)h * kPage * HD + (size_t)(t % kPage) * HD;
-                std::memcpy(&pool[base], k + ((size_t)t * nkv + h) * HD, HD * sizeof(float));
-                std::memcpy(&pool[base + (size_t)nkv * kPage * HD], v + ((size_t)t * nkv + h) * HD, HD * sizeof(float));
-            }
+        for (int p = 0; p < np; ++p) table[p] = np - p;
+        pool.put(table.data(), ctx, k, v);
         std::vector<DecodeState> st(R);
         for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, {0, 0, 0}};
         const int max_chunks = ceil_div(ctx, kSpecChunk);
         Scratch mem;
-        float* d_pool = mem.alloc<float>(pool.size());
-        float* d_q = mem.alloc<float>((size_t)R * nh * HD);
+        float* d_pool = upload_scratch(mem, c.stream, pool.data.data(), pool.data.size());
+        float* d_q = upload_scratch(mem, c.stream, q, (size_t)R * nh * HD);
         float* d_out = mem.alloc<float>((size_t)R * nh * HD);
         float* d_part = mem.alloc<float>((size_t)R * nh * max_chunks * spec_part_stride(HD));
-        int* d_table = mem.alloc<int>(np);
-        DecodeState* d_st = mem.alloc<DecodeState>(R);
-        AHA_CUDA_CHECK(cudaMemcpy(d_pool, pool.data(), pool.size() * sizeof(float), cudaMemcpyHostToDevice));
-        AHA_CUDA_CHECK(cudaMemcpy(d_q, q, (size_t)R * nh * HD * sizeof(float), cudaMemcpyHostToDevice));
-        AHA_CUDA_CHECK(cudaMemcpy(d_table, table.data(), np * sizeof(int), cudaMemcpyHostToDevice));
-        AHA_CUDA_CHECK(cudaMemcpy(d_st, st.data(), R * sizeof(DecodeState), cudaMemcpyHostToDevice));
+        const int* d_table = upload_scratch(mem, c.stream, table.data(), table.size());
+        DecodeState* d_st = upload_scratch(mem, c.stream, st.data(), st.size());
         SpecAttnArgs a{};
         a.q = d_q; a.ldq = nh * HD;
-        a.kv.k = d_pool; a.kv.v = d_pool + (size_t)nkv * kPage * HD; a.kv.page_table = d_table; a.kv.page_shift = kPageShift;
-        a.kv.page_stride = page_stride; a.kv.tok_stride = HD; a.kv.head_stride = (size_t)kPage * HD;
+        a.kv = pool.src(d_pool, d_table);
         a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
         a.R = R; a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
         AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
@@ -1554,6 +1608,158 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
         AHA_CUDA_CHECK(cudaGetLastError());
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
         AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)R * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
+    });
+}
+
+int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_heads, size_t n_kv_heads, size_t sq, size_t skv, int causal,
+                             const int32_t* segments, size_t n_segments, const int32_t* page_order, int split_out, const float* q, const float* k,
+                             const float* v, float* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(q && k && v && out, "q, k, v and out are required");
+        AHA_REQUIRE(impl >= 0 && impl <= 2, "impl must be 0 (wgmma), 1 (SIMT) or 2 (mma.sync)");
+        AHA_REQUIRE(head_dim == 64 || head_dim == 128, "head_dim must be 64 or 128");
+        AHA_REQUIRE(n_kv_heads >= 1 && n_heads % n_kv_heads == 0 && n_heads <= 64, "debug_attention: bad head counts");
+        AHA_REQUIRE(sq >= 1 && skv >= 1 && skv <= (1u << 20), "debug_attention: bad lengths");
+        AHA_REQUIRE(!causal || skv >= sq, "causal attention needs skv >= sq (skv - sq tokens already cached)");
+        AHA_REQUIRE(!split_out || impl == 0, "the split hi / lo output is written by the wgmma kernel only");
+        Ctx& c = m->ctx;
+        const int hd = head_dim, nh = (int)n_heads, nkv = (int)n_kv_heads, Sq = (int)sq, Skv = (int)skv;
+        std::vector<std::pair<int, int>> segs;
+        std::vector<int> work;
+        if (n_segments) {
+            AHA_REQUIRE(segments && Sq == Skv, "segments split one sequence: sq == skv");
+            AHA_REQUIRE(!causal || hd == 128, "packed causal segments are head_dim 128");
+            int end = 0;
+            for (size_t i = 0; i < n_segments; ++i) {
+                const int s0 = segments[2 * i], len = segments[2 * i + 1];
+                AHA_REQUIRE(s0 >= end && len >= 1 && s0 + len <= Sq, "segments must be non-empty, in order, disjoint and inside [0, sq)");
+                segs.emplace_back(s0, len);
+                for (int q0 = 0; q0 < len; q0 += kFaBQ) { work.push_back(s0); work.push_back(len); work.push_back(q0); }   // as plan_pack builds it
+                end = s0 + len;
+            }
+        }
+        Scratch mem;
+        FlashArgs fa;
+        fa.q = upload_scratch(mem, c.stream, q, (size_t)Sq * nh * hd); fa.q_tok_stride = (size_t)nh * hd; fa.q_head_stride = hd;
+        if (causal) {   // the LLM prefill: K / V in a paged pool through the caller's page order
+            const int np = ceil_div(Skv, kPage);
+            std::vector<int> table(np);
+            for (int p = 0; p < np; ++p) table[p] = page_order ? page_order[p] : p;
+            std::vector<char> seen(*std::max_element(table.begin(), table.end()) + 1, 0);
+            for (int p : table) { AHA_REQUIRE(p >= 0 && !seen[p], "page_order must hold distinct non-negative pages"); seen[p] = 1; }
+            HostPool pool((int)seen.size(), nkv, hd);
+            pool.put(table.data(), Skv, k, v);
+            fa.kv = pool.src(upload_scratch(mem, c.stream, pool.data.data(), pool.data.size()), upload_scratch(mem, c.stream, table.data(), table.size()));
+        } else {        // the encoders: contiguous [token][kv_head][hd], followed by a page of NaN tokens
+            const size_t n = (size_t)Skv * nkv * hd, pad = (size_t)kPage * nkv * hd;
+            float* dk = mem.alloc<float>(n + pad);
+            float* dv = mem.alloc<float>(n + pad);
+            fill_nan(c.stream, dk + n, pad); fill_nan(c.stream, dv + n, pad);
+            AHA_CUDA_CHECK(cudaMemcpyAsync(dk, k, n * sizeof(float), cudaMemcpyHostToDevice, c.stream));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(dv, v, n * sizeof(float), cudaMemcpyHostToDevice, c.stream));
+            fa.kv.k = dk; fa.kv.v = dv; fa.kv.page_table = nullptr; fa.kv.page_shift = 0; fa.kv.page_stride = 0;
+            fa.kv.tok_stride = (size_t)nkv * hd; fa.kv.head_stride = hd;
+        }
+        const size_t n_out = (size_t)Sq * nh * hd;
+        fa.out = mem.alloc<float>(n_out); fa.o_tok_stride = (size_t)nh * hd; fa.o_head_stride = hd;
+        fill_nan(c.stream, fa.out, n_out);   // rows no segment covers stay NaN
+        if (split_out) {
+            fa.out_hi = mem.alloc<__half>(n_out); fa.out_lo = mem.alloc<__half>(n_out);
+            fill_nan(c.stream, fa.out_hi, n_out); fill_nan(c.stream, fa.out_lo, n_out);
+        }
+        fa.Sq = Sq; fa.Skv = Skv; fa.q0 = 0; fa.kv0 = 0; fa.groups = nh / nkv; fa.scaling = (float)(1.0 / std::sqrt((double)hd));
+        const int* d_work = upload_scratch(mem, c.stream, work.data(), work.size());
+        const int saved = c.attn_impl;
+        c.attn_impl = impl;
+        try {
+            if (hd == 64) debug_attention_run<64>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / 3);
+            else debug_attention_run<128>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / 3);
+        } catch (...) { c.attn_impl = saved; throw; }
+        c.attn_impl = saved;
+        AHA_CUDA_CHECK(cudaGetLastError());
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        if (!split_out) {
+            AHA_CUDA_CHECK(cudaMemcpy(out, fa.out, n_out * sizeof(float), cudaMemcpyDeviceToHost));
+            return;
+        }
+        std::vector<__half> hi(n_out), lo(n_out);
+        AHA_CUDA_CHECK(cudaMemcpy(hi.data(), fa.out_hi, n_out * sizeof(__half), cudaMemcpyDeviceToHost));
+        AHA_CUDA_CHECK(cudaMemcpy(lo.data(), fa.out_lo, n_out * sizeof(__half), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n_out; ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);   // exact in fp32
+    });
+}
+
+int aha_b200_debug_decode_attn(aha_model* m, size_t batch, size_t n_heads, size_t n_kv_heads, const float* qkv, const int32_t* pos,
+                               const int32_t* rope_delta, const float* k_cache, const float* v_cache, const int32_t* tables, size_t n_pool_pages,
+                               const float* q_norm, const float* k_norm, float eps, float rope_theta, float* out, float* out_repeat,
+                               float* pool_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(qkv && pos && rope_delta && tables && q_norm && k_norm && out, "qkv, pos, rope_delta, tables, the norm weights and out are required");
+        AHA_REQUIRE(batch >= 1 && batch <= 64, "debug_decode_attn: batch must be 1 to 64");
+        AHA_REQUIRE(n_kv_heads >= 1 && n_heads % n_kv_heads == 0, "debug_decode_attn: bad head counts");
+        const int G = (int)(n_heads / n_kv_heads);
+        AHA_REQUIRE(G == 1 || G == 2 || G == 4 || G == 6, "debug_decode_attn: GQA group must be 1, 2, 4 or 6");
+        constexpr int HD = 128;
+        Ctx& c = m->ctx;
+        const int B = (int)batch, nh = (int)n_heads, nkv = (int)n_kv_heads, row = (nh + 2 * nkv) * HD;
+        HostPool pool((int)n_pool_pages, nkv, HD);
+        std::vector<char> used(n_pool_pages, 0);
+        std::vector<int> t_off(B), c_off(B);
+        int nt = 0, nc = 0;
+        for (int b = 0; b < B; ++b) {
+            AHA_REQUIRE(pos[b] >= 0, "debug_decode_attn: negative position");
+            t_off[b] = nt; c_off[b] = nc;
+            for (int p = 0; p < ceil_div(pos[b] + 1, kPage); ++p) {
+                const int pg = tables[nt + p];
+                AHA_REQUIRE(pg >= 0 && pg < (int)n_pool_pages && !used[pg], "tables must hold distinct pages of the pool");
+                used[pg] = 1;
+            }
+            AHA_REQUIRE(pos[b] == 0 || (k_cache && v_cache), "k_cache and v_cache are required");
+            if (pos[b]) pool.put(tables + nt, pos[b], k_cache + (size_t)nc * nkv * HD, v_cache + (size_t)nc * nkv * HD);
+            nt += ceil_div(pos[b] + 1, kPage);
+            nc += pos[b];
+        }
+        Scratch mem;
+        float* d_pool = upload_scratch(mem, c.stream, pool.data.data(), pool.data.size());
+        const int* d_tables = upload_scratch(mem, c.stream, tables, (size_t)nt);
+        const float* d_qkv = upload_scratch(mem, c.stream, qkv, (size_t)B * row);
+        const float* d_qw = upload_scratch(mem, c.stream, q_norm, HD);
+        const float* d_kw = upload_scratch(mem, c.stream, k_norm, HD);
+        const float* d_inv = upload_scratch(mem, c.stream, rope_inv_freq(rope_theta, HD).data(), HD / 2);
+        std::vector<DecodeState> st(B);
+        for (int b = 0; b < B; ++b) st[b] = DecodeState{0, pos[b], rope_delta[b], 0, 0, {0, 0, 0}};
+        const DecodeState* d_st = upload_scratch(mem, c.stream, st.data(), st.size());
+        const size_t part = (size_t)nh * kDecodeSplits * (HD + 2), n_out = (size_t)B * nh * HD;
+        float* d_part = mem.alloc<float>((size_t)B * part);
+        int* d_cnt = mem.alloc<int>((size_t)B * nkv);
+        AHA_CUDA_CHECK(cudaMemsetAsync(d_cnt, 0, (size_t)B * nkv * sizeof(int), c.stream));
+        float* d_out = mem.alloc<float>(n_out);
+        std::vector<DecodeAttnArgs> args(B);
+        for (int b = 0; b < B; ++b) {
+            DecodeAttnArgs& d = args[b];
+            d = DecodeAttnArgs{};
+            d.qkv = d_qkv + (size_t)b * row; d.qw = d_qw; d.kw = d_kw; d.eps = eps; d.inv_freq = d_inv; d.st = d_st + b;
+            d.kv = pool.src(d_pool, d_tables + t_off[b]);
+            d.kbase = d_pool; d.vbase = const_cast<float*>(d.kv.v);
+            d.partial = d_part + (size_t)b * part; d.counters = d_cnt + (size_t)b * nkv; d.out = d_out + (size_t)b * nh * HD;
+            d.nh = nh; d.nkv = nkv; d.nsplit = kDecodeSplits; d.scaling = (float)(1.0 / std::sqrt((double)HD));
+        }
+        const DecodeAttnArgs* d_args = upload_scratch(mem, c.stream, args.data(), args.size());
+        // Run 1 sees the pool as a decode step does: the new token's slot does not hold its K / V yet.  Run 2 (out_repeat) goes again on the
+        // same partials and counters over the pool run 1 left, so a counter run 1 did not reset leaves its output NaN.
+        for (int run = 0; run < (out_repeat ? 2 : 1); ++run) {
+            fill_nan(c.stream, d_out, n_out);
+            switch (G) {
+                case 1: debug_decode_launch<1>(c.stream, B, nkv, args[0], d_args); break;
+                case 2: debug_decode_launch<2>(c.stream, B, nkv, args[0], d_args); break;
+                case 4: debug_decode_launch<4>(c.stream, B, nkv, args[0], d_args); break;
+                default: debug_decode_launch<6>(c.stream, B, nkv, args[0], d_args); break;
+            }
+            AHA_CUDA_CHECK(cudaGetLastError());
+            AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+            AHA_CUDA_CHECK(cudaMemcpy(run == 0 ? out : out_repeat, d_out, n_out * sizeof(float), cudaMemcpyDeviceToHost));
+        }
+        if (pool_out) AHA_CUDA_CHECK(cudaMemcpy(pool_out, d_pool, pool.data.size() * sizeof(float), cudaMemcpyDeviceToHost));
     });
 }
 

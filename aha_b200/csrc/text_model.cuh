@@ -404,6 +404,13 @@ struct TextLayer {
 
 constexpr int kDecodeSplits = 16;        // split-KV factor of the decode attention
 
+// RoPE frequencies inv_freq[j] = 1 / theta^(2j / hd), in f32 powf like rope.rs:7-13
+inline std::vector<float> rope_inv_freq(float theta, int hd) {
+    std::vector<float> inv(hd / 2);
+    for (int j = 0; j < hd / 2; ++j) inv[j] = 1.0f / powf(theta, (float)(2 * j) / (float)hd);
+    return inv;
+}
+
 // One sequence's logical -> physical map over the paged KV pool: entry p of `h` is the pool page of the sequence's tokens
 // [p * kPage, (p + 1) * kPage); entries 0 .. mapped-1 hold pages, and `d` is the device copy the kernels read.
 struct PageTable {
@@ -573,9 +580,7 @@ struct TextModel {
                                    4ull * (2 * H + 2 * hd);
         decode_weight_bytes += 4ull * H + 2ull * (size_t)cfg.V * H;
         // RoPE tables: inv_freq in f32 powf like rope.rs:7-13; M-RoPE row selector per frequency (rope.rs:454-476 / 478-500)
-        std::vector<float> inv(hd / 2);
-        for (int j = 0; j < hd / 2; ++j) inv[j] = 1.0f / powf(cfg.theta, (float)(2 * j) / (float)hd);
-        inv_freq = upload(c, inv);
+        inv_freq = upload(c, rope_inv_freq(cfg.theta, hd));
         std::vector<uint8_t> sel(hd / 2, 0);
         if (cfg.mrope) {
             for (int dim = 1; dim < 3; ++dim) {

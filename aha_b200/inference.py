@@ -257,6 +257,60 @@ class B200Model:
         self._check(self._lib.aha_b200_debug_verify_attn(self._h, R, nh, nkv, int(pos0), f(q), f(k), f(v), f(out)))
         return out
 
+    def debug_attention(self, q, k, v, impl, causal, segments=None, page_order=None, split_out=False):
+        """The prefill attention on host data (aha_b200_debug_attention): q [Sq][nh][hd], k / v [Skv][nkv][hd] with hd 64 or 128 ->
+        [Sq][nh][hd].  impl 0 = wgmma, 1 = SIMT, 2 = mma.sync.  causal: query i sees keys 0 .. Skv - Sq + i, K / V on a paged pool
+        (logical page p at physical page page_order[p]).  segments: [(start, len), ...] attending only to themselves (Sq == Skv).
+        split_out: the wgmma kernel's fp16 hi + lo output, summed."""
+        q = np.ascontiguousarray(q, np.float32)
+        k = np.ascontiguousarray(k, np.float32)
+        v = np.ascontiguousarray(v, np.float32)
+        Sq, nh, hd = q.shape
+        Skv, nkv = k.shape[:2]
+        if k.shape != (Skv, nkv, hd) or v.shape != k.shape:
+            raise ValueError("q [Sq][nh][hd], k and v [Skv][nkv][hd]")
+        seg = np.ascontiguousarray(np.asarray(segments if segments is not None else [], np.int32).reshape(-1, 2))
+        po = None if page_order is None else np.ascontiguousarray(page_order, np.int32)
+        if po is not None and po.size != -(-Skv // 32):
+            raise ValueError("page_order needs one entry per 32-token page")
+        out = np.empty_like(q)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32)) if a is not None and a.size else None
+        self._check(self._lib.aha_b200_debug_attention(self._h, int(impl), hd, nh, nkv, Sq, Skv, 1 if causal else 0, i32(seg), len(seg),
+                                                       i32(po), 1 if split_out else 0, f(q), f(k), f(v), f(out)))
+        return out
+
+    def debug_decode_attn(self, qkv, pos, rope_delta, k_cache, v_cache, tables, n_pool_pages, q_norm, k_norm, n_heads, n_kv_heads,
+                          eps=1e-6, rope_theta=1e6):
+        """The decode attention on host data (aha_b200_debug_decode_attn) for B sequences: qkv [B][(nh + 2 nkv) * 128] raw
+        projections, pos / rope_delta [B], k_cache / v_cache lists of [pos[b]][nkv][128], tables a list of B page tables
+        (ceil((pos[b] + 1) / 32) distinct pages of a pool of n_pool_pages).  -> (out [B][nh][128] of a run on the pool as a decode step
+        finds it, out of a second run on the same partials and counters, pool after the call [n_pool_pages][2][nkv][32][128])."""
+        qkv = np.ascontiguousarray(qkv, np.float32)
+        B = qkv.shape[0]
+        if qkv.shape != (B, (n_heads + 2 * n_kv_heads) * 128) or len(pos) != B or len(rope_delta) != B or len(tables) != B:
+            raise ValueError("qkv [B][(nh + 2 nkv) * 128]; pos, rope_delta, k_cache, v_cache and tables one per sequence")
+        for b in range(B):
+            if np.shape(tables[b]) != (-(-(int(pos[b]) + 1) // 32),) or np.shape(k_cache[b]) != (pos[b], n_kv_heads, 128) or \
+                    np.shape(v_cache[b]) != np.shape(k_cache[b]):
+                raise ValueError(f"sequence {b}: k_cache / v_cache [pos][nkv][128], table of ceil((pos + 1) / 32) pages")
+        kc = np.ascontiguousarray(np.concatenate([np.reshape(x, (-1, n_kv_heads, 128)) for x in k_cache]), np.float32)
+        vc = np.ascontiguousarray(np.concatenate([np.reshape(x, (-1, n_kv_heads, 128)) for x in v_cache]), np.float32)
+        tb = np.ascontiguousarray(np.concatenate([np.asarray(t, np.int32) for t in tables]), np.int32)
+        p = np.ascontiguousarray(pos, np.int32)
+        rd = np.ascontiguousarray(rope_delta, np.int32)
+        qn = np.ascontiguousarray(q_norm, np.float32)
+        kn = np.ascontiguousarray(k_norm, np.float32)
+        out = np.empty((B, n_heads, 128), np.float32)
+        again = np.empty_like(out)
+        pool = np.empty((n_pool_pages, 2, n_kv_heads, 32, 128), np.float32)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self._check(self._lib.aha_b200_debug_decode_attn(self._h, B, n_heads, n_kv_heads, f(qkv), i32(p), i32(rd), f(kc), f(vc), i32(tb),
+                                                         n_pool_pages, f(qn), f(kn), float(eps), float(rope_theta), f(out), f(again),
+                                                         f(pool)))
+        return out, again, pool
+
     def generate_batch(self, requests):
         """Static batching (aha_b200_generate_batch): requests = [dict(input_ids=..., data=None, max_tokens=..., temperature=..., top_p=...,
         top_k=..., repeat_penalty=..., repeat_last_n=..., seed=...), ...] (at most 8) decoded in lockstep on this handle.

@@ -495,9 +495,34 @@ int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_
                               aha_logprobs* out);
 /* the verify attention of speculative decoding on host data (tests): `rows` query rows at positions pos0 .. pos0 + rows - 1 over K / V of
  * pos0 + rows positions (laid out on a paged pool with the pages in reverse order), head_dim 128.  q, out: [rows][n_heads][128] (q
- * normalised and rotated); k, v: [pos0 + rows][n_kv_heads][128].  Row r attends to positions 0 .. pos0 + r. */
+ * normalised and rotated); k, v: [pos0 + rows][n_kv_heads][128].  Row r attends to positions 0 .. pos0 + r.
+ * In this entry and the two below, every pool slot no page table references, and every slot past a context inside its last page, holds NaN. */
 int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
                                const float* v, float* out);
+/* the prefill attention on host data (tests), through the dispatch the models use: impl 0 = wgmma (flash_attn_tc_kernel), 1 = fp32 SIMT,
+ * 2 = mma.sync; head_dim 64 or 128.  q, out: [sq][n_heads][head_dim] (q normalised and rotated); k, v: [skv][n_kv_heads][head_dim].
+ *   causal, no segments: the LLM prefill; query i attends to keys 0 .. skv - sq + i, K / V on a paged pool whose logical page p is physical
+ *     page page_order[p] (NULL: p).
+ *   causal with segments: a packed prefill (head_dim 128, sq == skv, K / V paged as above); segment (start, len) attends causally to itself,
+ *     starts are multiples of 16 for impl 0.
+ *   not causal: K / V contiguous; without segments every query attends to all skv keys, with segments (sq == skv) each segment to itself.
+ * segments: [n_segments][2] = (start, len), in order and disjoint; rows outside every segment come back NaN.  split_out (impl 0): the kernel
+ * writes fp16 hi + lo halves, and out = hi + lo (exact in fp32). */
+int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_heads, size_t n_kv_heads, size_t sq, size_t skv, int causal,
+                             const int32_t* segments, size_t n_segments, const int32_t* page_order, int split_out, const float* q,
+                             const float* k, const float* v, float* out);
+/* the decode attention on host data (tests): `batch` sequences, head_dim 128, n_heads / n_kv_heads in {1, 2, 4, 6}.  batch 1 runs
+ * decode_attn_kernel, more run decode_attn_batch_kernel, both over kDecodeSplits splits.  Sequence b: qkv row b of
+ * [batch][(n_heads + 2 n_kv_heads) * 128] (raw projections), position pos[b] (tokens already cached), rope_delta[b]; its cached K / V are the
+ * next pos[b] rows of k_cache / v_cache ([sum pos][n_kv_heads][128], rotated K), its page table the next ceil((pos[b] + 1) / 32) entries of
+ * `tables`, pages of one pool of n_pool_pages pages ([page][K|V][kv_head][32][128]; the tables' pages must be distinct).  q_norm, k_norm
+ * [128]: the per-head RMSNorm weights; rope_theta: the RoPE base.  out: [batch][n_heads][128], the output of a run on the pool as a decode
+ * step finds it (the new token's slot not yet written).  out_repeat (may be NULL): the output of a second run on the same partial buffers and
+ * counters, over the pool the first run left.  pool_out (may be NULL): the pool after the call. */
+int aha_b200_debug_decode_attn(aha_model* m, size_t batch, size_t n_heads, size_t n_kv_heads, const float* qkv, const int32_t* pos,
+                               const int32_t* rope_delta, const float* k_cache, const float* v_cache, const int32_t* tables, size_t n_pool_pages,
+                               const float* q_norm, const float* k_norm, float eps, float rope_theta, float* out, float* out_repeat,
+                               float* pool_out);
 /* Run ONE Linear layer y = epilogue(x W^T + b) through the library's GEMM dispatch on host data (unit tests of the
  * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 5 = the batched decode GEMV (M <= 8; its SwiGLU
  * instantiation runs with a unit-gain RMSNorm prologue), 6 = the same with the cp.async weight ring, 7 = the wide batched decode GEMV

@@ -5,9 +5,12 @@ F32 = np.float32
 
 
 def compute_default_rope_parameters(dim, base):
-    """rope.rs:7-13: inv_freq[i] = 1 / base.powf(i / dim) for even i, all in f32."""
+    """rope.rs:7-13: inv_freq[i] = 1 / base.powf(i / dim) for even i, all in f32.  f32::powf calls the C library's powf, as the library's
+    rope_inv_freq does.  numpy's float32 power can differ from it by 1 ulp (at 15 of the 64 frequencies of base 1e6, dim 128); the power
+    taken in f64 and rounded to f32 matches the C powf (tests/test_attn_ref.py checks it)."""
     i = np.arange(0, dim, 2, dtype=F32)
-    return (F32(1.0) / np.power(F32(base), i / F32(dim), dtype=F32)).astype(F32)
+    p = np.power(np.float64(F32(base)), (i / F32(dim)).astype(np.float64)).astype(F32)
+    return (F32(1.0) / p).astype(F32)
 
 
 def rotate_half(x):

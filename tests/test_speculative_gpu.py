@@ -8,6 +8,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from attn_ref import attention
 from conftest import make_model, make_oracle
 from spec_ref import simulate
 from test_batch_wide_gpu import SAMPLERS, _check_oracle_ids
@@ -34,19 +35,6 @@ def tiny():
     m.close()
 
 
-def _attn_ref(q, k, v, pos0):
-    R, nh, hd = q.shape
-    G = nh // k.shape[1]
-    out = np.zeros((R, nh, hd))
-    for r in range(R):
-        for h in range(nh):
-            K, V = k[:pos0 + r + 1, h // G].astype(np.float64), v[:pos0 + r + 1, h // G].astype(np.float64)
-            s = K @ q[r, h].astype(np.float64) / np.sqrt(hd)
-            p = np.exp(s - s.max())
-            out[r, h] = p @ V / p.sum()
-    return out
-
-
 @pytest.mark.parametrize("G", [1, 2, 4, 6])
 @pytest.mark.parametrize("R", [1, 2, 8, 16])
 def test_verify_attention_against_float64(tiny, G, R):
@@ -58,7 +46,7 @@ def test_verify_attention_against_float64(tiny, G, R):
         k = rng.standard_normal((pos0 + R, nkv, 128)).astype(np.float32)
         v = rng.standard_normal((pos0 + R, nkv, 128)).astype(np.float32)
         got = m.debug_verify_attn(q, k, v, pos0)
-        assert np.abs(got - _attn_ref(q, k, v, pos0)).max() <= 1e-5, pos0
+        assert np.abs(got - attention(q, k, v, causal=True)).max() <= 1e-5, pos0   # row r sees positions 0 .. pos0 + r
         for r in {0, R // 2, R - 1}:            # row r alone (R = 1 at its position) gives the same bits
             alone = m.debug_verify_attn(q[r:r + 1], k[:pos0 + r + 1], v[:pos0 + r + 1], pos0 + r)
             assert np.array_equal(alone[0], got[r]), (pos0, r)
