@@ -193,7 +193,8 @@ SYMBOLS = {
                                            C.POINTER(Usage)]),
     "aha_b200_asr_generate": (C.c_int, [_P, C.POINTER(AsrChunk), C.c_size_t, C.POINTER(GenParams), _U32P, C.c_size_t,
                                         C.POINTER(C.c_size_t), TOKEN_CALLBACK, C.c_void_p, C.POINTER(Usage)]),
-    "aha_b200_debug_sample": (C.c_int, [_P, _F32P, C.POINTER(GenParams), _U32P, C.c_size_t, C.c_uint32, _U32P]),
+    "aha_b200_debug_sample": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _F32P, C.c_size_t, C.POINTER(GenParams), _U32P, _U32P, _U32P,
+                                        C.c_int, _I32P, _I32P, _U32P, _U32P, _U32P]),
     "aha_b200_mel_spectrogram": (C.c_int, [_P, _F32P, C.c_size_t, _F32P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_image_patchify": (C.c_int, [_P, C.POINTER(C.c_uint8), C.c_size_t, C.c_size_t, _F32P, C.c_size_t, _U32P]),
     "aha_b200_img_smart_resize": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, _U32P, _U32P]),

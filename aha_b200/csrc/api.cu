@@ -1834,23 +1834,86 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
     });
 }
 
-int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_params* params, const uint32_t* context, size_t n_context,
-                          uint32_t draw_index, uint32_t* token_out) {
+int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                          const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                          const int32_t* on, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out) {
     return guarded(m, [&] {
-        AHA_REQUIRE(logits && params && token_out && (context || n_context == 0), "logits, params and token_out are required");
-        TextModel& T = m->text;
-        AHA_REQUIRE(n_context <= (size_t)T.hist_cap, "context longer than the history buffer");
-        T.set_sampler(make_sampler(*params, T.cfg.V));
-        AHA_REQUIRE(T.samp_active, "plain ArgMax needs no sampler (temperature < 1e-7 and no repeat penalty)");
-        AHA_CUDA_CHECK(cudaMemcpyAsync(T.logits, logits, (size_t)T.cfg.V * sizeof(float), cudaMemcpyHostToDevice, m->ctx.stream));
-        if (n_context) AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_history, context, n_context * sizeof(uint32_t), cudaMemcpyHostToDevice, m->ctx.stream));
-        T.set_state(0, 0, 0, (int)n_context, draw_index);
-        T.sample(0);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_pin, T.d_argmax, sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-        T.check_sample_error();
-        T.clear_sampler();
-        *token_out = m->h_pin[0];
+        AHA_REQUIRE(logits && params && n_context && draw_index && token_out && state_out && hist_out,
+                    "logits, params, n_context, draw_index, token_out, state_out and hist_out are required");
+        AHA_REQUIRE(kernel == 0 || kernel == 1, "kernel must be 0 (sample_kernel) or 1 (sample_rows_kernel)");
+        AHA_REQUIRE(rows >= 1 && rows <= (size_t)kSampleMaxRows, "rows must be 1 to " + std::to_string(kSampleMaxRows));
+        AHA_REQUIRE(V >= 1 && V <= (size_t)kSampleThreads * kSampleChunk, "V must be 1 to " + std::to_string(kSampleThreads * kSampleChunk));
+        AHA_REQUIRE(ld == 0 || (ld >= V && ld <= (size_t)INT32_MAX), "ld must be 0 or V to 2^31 - 1");
+        AHA_REQUIRE(kernel == 0 || (act && on), "sample_rows_kernel needs act and on");
+        // row r runs as slot slot[r]: its own state, history, token and [V] scratch row
+        std::vector<int> slot(rows);
+        std::vector<char> used(kSampleMaxRows, 0);
+        size_t n_ctx_total = 0, cap = 1;
+        for (size_t r = 0; r < rows; ++r) {
+            slot[r] = kernel == 0 ? (int)r : act[r];
+            AHA_REQUIRE(slot[r] >= 0 && slot[r] < kSampleMaxRows && !used[slot[r]], "act must map the rows to distinct slots 0 to 63");
+            used[slot[r]] = 1;
+            AHA_REQUIRE(!overwrite || n_context[r] >= 1, "overwrite needs a context of at least one token (the pushed ArgMax token)");
+            n_ctx_total += n_context[r];
+            cap = std::max(cap, (size_t)n_context[r]);
+        }
+        AHA_REQUIRE(context || n_ctx_total == 0, "context is required");
+        std::vector<SampleArgs> args(kSampleMaxRows, SampleArgs{});
+        for (size_t r = 0; r < rows; ++r) {
+            const Sampler s = make_sampler(params[r], (int)V);
+            AHA_REQUIRE(s.active, "row " + std::to_string(r) + ": plain ArgMax needs no sampler (temperature < 1e-7 and no repeat penalty)");
+            args[slot[r]] = s.args;
+        }
+        cudaStream_t st = m->ctx.stream;
+        const size_t n_logits = ld ? rows * ld : V;
+        Scratch mem;
+        float* d_logits = mem.alloc<float>(n_logits);
+        float* d_work = mem.alloc<float>(rows * V);
+        DecodeState* d_st = mem.alloc<DecodeState>(rows);
+        uint32_t* d_hist = mem.alloc<uint32_t>(rows * cap);
+        uint32_t* d_tok = mem.alloc<uint32_t>(rows);
+        int* d_err = mem.alloc<int>(1);
+        std::vector<DecodeState> hs(rows);
+        std::vector<uint32_t> hh(rows * cap, 0xffffffffu);
+        for (size_t r = 0, off = 0; r < rows; off += n_context[r], ++r) {
+            const uint32_t n = n_context[r];
+            std::copy(context + off, context + off + n, hh.begin() + r * cap);
+            hs[r] = DecodeState{n ? context[off + n - 1] : 0u, 0, 0, (int32_t)n, draw_index[r], {0, 0, 0}};
+            SampleArgs& a = args[slot[r]];
+            a.logits = d_logits + r * ld; a.work = d_work + r * V;
+            a.st = d_st + r; a.history = d_hist + r * cap; a.hist_cap = (int)cap; a.token_out = d_tok + r; a.error = d_err;
+            a.overwrite = overwrite;
+        }
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_logits, logits, n_logits * sizeof(float), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_st, hs.data(), rows * sizeof(DecodeState), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_hist, hh.data(), hh.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        AHA_CUDA_CHECK(cudaMemsetAsync(d_tok, 0xff, rows * sizeof(uint32_t), st));
+        AHA_CUDA_CHECK(cudaMemsetAsync(d_err, 0, sizeof(int), st));
+        if (kernel == 0) {
+            for (size_t r = 0; r < rows; ++r) sample_kernel<<<1, kSampleThreads, 0, st>>>(args[r]);
+            m->ctx.cnt.kernels += rows;
+        } else {
+            SampleArgs* d_args = mem.alloc<SampleArgs>(kSampleMaxRows);
+            int* d_on = mem.alloc<int>(kSampleMaxRows);
+            int* d_act = mem.alloc<int>(rows);
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_args, args.data(), kSampleMaxRows * sizeof(SampleArgs), cudaMemcpyHostToDevice, st));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_on, on, kSampleMaxRows * sizeof(int), cudaMemcpyHostToDevice, st));
+            AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, slot.data(), rows * sizeof(int), cudaMemcpyHostToDevice, st));
+            sample_rows_kernel<<<(unsigned)rows, kSampleThreads, 0, st>>>(d_args, d_on, d_act, d_logits, (int)ld, overwrite);
+            m->ctx.cnt.kernels++;
+        }
+        AHA_CUDA_CHECK(cudaGetLastError());
+        int err = 0;
+        AHA_CUDA_CHECK(cudaMemcpyAsync(token_out, d_tok, rows * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(hs.data(), d_st, rows * sizeof(DecodeState), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(hh.data(), d_hist, hh.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, st));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(st));
+        if (err) throw std::runtime_error(kSampleWeightsError);
+        for (size_t r = 0; r < rows; ++r) {
+            state_out[3 * r] = hs[r].token; state_out[3 * r + 1] = (uint32_t)hs[r].n_hist; state_out[3 * r + 2] = hs[r].n_draws;
+            hist_out[r] = n_context[r] ? hh[r * cap + n_context[r] - 1] : 0xffffffffu;
+        }
     });
 }
 

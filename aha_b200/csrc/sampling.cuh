@@ -22,6 +22,9 @@ namespace aha {
 constexpr int kSampleThreads = 1024;
 constexpr int kSampleChunk = 256;
 constexpr int kSampleMaxTopK = 1024;
+constexpr int kSampleMaxRows = 64;          // rows of one sample_rows_kernel launch: the widest batch session
+constexpr const char* kSampleWeightsError =
+    "sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)";
 
 enum SampleMode { SAMPLE_ARGMAX = 0, SAMPLE_ALL = 1, SAMPLE_TOPP = 2, SAMPLE_TOPK = 3, SAMPLE_TOPK_TOPP = 4 };
 
@@ -196,8 +199,11 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
         __syncthreads();
         const float u01 = uniform01_from_word(chacha12_word(a.key, draw >> 4, (int)(draw & 15u)));
         const uint32_t* key = reinterpret_cast<const uint32_t*>(p);      // p >= 0: the bit pattern orders like the value
-        const bool plain = a.mode == SAMPLE_ALL || ((a.mode == SAMPLE_TOPP || a.mode == SAMPLE_TOPK_TOPP) && a.top_k >= V && (a.top_p <= 0.f || a.top_p >= 1.f)) ||
-                           (a.mode == SAMPLE_TOPP && (a.top_p <= 0.f || a.top_p >= 1.f)) || (a.mode == SAMPLE_TOPK && a.top_k >= V);
+        // candle's own shortcuts to the plain multinomial: TopP with p outside (0, 1) (the TopP arm of LogitsProcessor::sample_f) and
+        // TopK with k >= V (sample_topk).  TopKThenTopP with k >= V has none: sample_topk_topp runs sample_topp, which with p = 1 still
+        // drops the smallest entries once the fp32 sum of the kept ones reaches 1 (and keeps every entry when p > 1).
+        const bool plain = a.mode == SAMPLE_ALL || (a.mode == SAMPLE_TOPP && (a.top_p <= 0.f || a.top_p >= 1.f)) ||
+                           (a.mode == SAMPLE_TOPK && a.top_k >= V);
         const bool nucleus = !plain && (a.mode == SAMPLE_TOPP || (a.mode == SAMPLE_TOPK_TOPP && a.top_k >= V));
         if (plain) {
             token = blocked_pick_dev(s, V, [&](int i) { return p[i]; }, u01, a.error);
@@ -229,7 +235,8 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
                 for (int i = i0; i < i1; ++i) {
                     const uint32_t k = key[i];
                     if (k < T) p[i] = 0.f;
-                    else if (k == T) { if (!(A + (float)j * tv < a.top_p)) p[i] = 0.f; ++j; }
+                    // product and sum rounded separately, as the oracle states them (a contracted FMA rounds once and can decide a tie differently)
+                    else if (k == T) { if (!(__fadd_rn(A, __fmul_rn((float)j, tv)) < a.top_p)) p[i] = 0.f; ++j; }
                 }
             }
             __syncthreads();

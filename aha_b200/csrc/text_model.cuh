@@ -1008,7 +1008,7 @@ struct TextModel {
         AHA_CUDA_CHECK(cudaMemcpy(&e, d_sample_err, sizeof(int), cudaMemcpyDeviceToHost));
         if (e) {
             cudaMemset(d_sample_err, 0, sizeof(int));
-            throw std::runtime_error("sampler: the token weights are all zero or not finite (rand::distr::weighted::WeightedIndex::new fails in the reference)");
+            throw std::runtime_error(kSampleWeightsError);
         }
     }
     // ---- log-probabilities: the request asks for n_top alternatives per record

@@ -511,14 +511,44 @@ class B200Model:
 
     def debug_sample(self, logits, context=(), draw_index=0, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
                      repeat_last_n=64, seed=299792458):
-        """The device sampler on a given logits row (tests)."""
-        lg = np.ascontiguousarray(logits, np.float32).reshape(-1)
-        ctx = np.ascontiguousarray(np.asarray(list(context), dtype=np.uint32))
-        p = self._gen_params(1, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed)
-        tok = C.c_uint32(0)
-        self._check(self._lib.aha_b200_debug_sample(self._h, lg.ctypes.data_as(C.POINTER(C.c_float)), C.byref(p),
-                                                    ctx.ctypes.data_as(C.POINTER(C.c_uint32)), ctx.size, int(draw_index), C.byref(tok)))
-        return int(tok.value)
+        """The device sampler (sample_kernel) on a given logits row of any length (tests) -> token."""
+        params = dict(temperature=temperature, top_p=top_p, top_k=top_k, repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, seed=seed)
+        return int(self.debug_sample_rows(logits, [params], [context], draw_index)["token"][0])
+
+    def debug_sample_rows(self, logits, params, contexts=None, draw_index=0, overwrite=False, kernel=0, act=None, on=None):
+        """The device sampler on given logits, one call for len(params) rows (1 to 64; tests).
+        logits: [V] (every row reads it) or [rows, ld] with V = ld.  params: per row a dict of generate()'s sampling keywords
+        (temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed).  contexts: per row the tokens generated so far;
+        draw_index: per row (or one for all) the draws already consumed.  overwrite: the last context token stands for the ArgMax token a
+        decode step pushed; the sampled token replaces it.  kernel 0: sample_kernel per row; 1: sample_rows_kernel, row r as slot act[r]
+        (default r), on: [64] flags per slot (default all on).
+        -> dict of uint32 arrays [rows]: token (0xffffffff where the row did not sample), state_token, n_hist, n_draws (the DecodeState
+        after the call) and last_hist (the last history word, 0xffffffff without a context)."""
+        rows = len(params)
+        lg = np.ascontiguousarray(logits, np.float32)
+        V, ld = (lg.size, 0) if lg.ndim == 1 else (lg.shape[1], lg.shape[1])
+        if lg.ndim not in (1, 2) or (lg.ndim == 2 and lg.shape[0] != rows):
+            raise ValueError(f"logits must be [V] or [{rows}, V], got {lg.shape}")
+        ps = (L.GenParams * rows)()
+        for r, q in enumerate(params):
+            q = dict(dict(temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64, seed=299792458), **q)
+            ps[r] = self._gen_params(1, q["temperature"], q["top_p"], q["top_k"], q["repeat_penalty"], q["repeat_last_n"], q["seed"])
+        ctxs = [np.asarray(c, np.uint32).reshape(-1) for c in (contexts if contexts is not None else [()] * rows)]
+        if len(ctxs) != rows:
+            raise ValueError(f"{len(ctxs)} contexts for {rows} rows")
+        cat = np.ascontiguousarray(np.concatenate(ctxs + [np.zeros(0, np.uint32)]))
+        n_ctx = np.array([c.size for c in ctxs], np.uint32)
+        draws = np.ascontiguousarray(np.broadcast_to(np.asarray(draw_index, np.uint32), (rows,)))
+        act = np.ascontiguousarray(np.arange(rows) if act is None else act, np.int32)
+        on = np.ascontiguousarray(np.ones(64) if on is None else on, np.int32)
+        if act.size != rows or on.size != 64:
+            raise ValueError("act needs one slot per row and on one flag per slot (64)")
+        tok, state, hist = np.zeros(rows, np.uint32), np.zeros((rows, 3), np.uint32), np.zeros(rows, np.uint32)
+        u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self._check(self._lib.aha_b200_debug_sample(self._h, int(kernel), rows, V, lg.ctypes.data_as(C.POINTER(C.c_float)), ld, ps, u32(cat),
+                                                    u32(n_ctx), u32(draws), 1 if overwrite else 0, i32(act), i32(on), u32(tok), u32(state), u32(hist)))
+        return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist)
 
     def debug_logprobs(self, logits, token, n_top=0):
         """The log-probability kernels on a given logits row of any length (tests) -> record dict."""

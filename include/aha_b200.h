@@ -483,9 +483,17 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
  * RMSNorm and stage 2; or "kv_fork:P:n" (kv_fork_kernel: P KV pages of every layer copied to n - 1 other page tables, as batch_add_n
  * does; needs P * n <= max_ctx / 32 and no open session, and clears the single-request cache).  bytes_per_launch = algorithmic bytes (the
  * score entries: the lm_head's; kv_fork: P pages read and (n - 1) * P written). */
-/* the device sampler on a given logits row (tests): context = tokens generated so far, draw_index = draws already consumed */
-int aha_b200_debug_sample(aha_model* m, const float* logits, const aha_gen_params* params, const uint32_t* context,
-                          size_t n_context, uint32_t draw_index, uint32_t* token_out);
+/* the device sampler on given logits (tests), in scratch of this call: `rows` (1 to 64) independent rows over a vocabulary of V (1 to
+ * 262144) entries.  Row r reads logits[r * ld ..] (ld = 0: every row reads the one row), samples with params[r], its context is the next
+ * n_context[r] tokens of `context` (the tokens generated so far) and it has consumed draw_index[r] draws.  overwrite = 1: the last context
+ * token stands for the ArgMax token a decode step pushed; it is kept out of the repeat penalty and the sampled token replaces it.
+ * kernel 0 runs sample_kernel once per row; kernel 1 runs sample_rows_kernel once over all rows, row r as slot act[r] (distinct, 0 to 63),
+ * and a row whose slot has on[slot] == 0 ([64] flags) does not sample: its outputs keep their initial values.
+ * Out, per row: token_out (initially 0xffffffff), state_out [3] = the DecodeState's token, n_hist and n_draws after the call (initially
+ * the last context token or 0, n_context[r], draw_index[r]), hist_out = the last history word (0xffffffff without a context). */
+int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                          const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                          const int32_t* on, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out);
 /* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
 int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);

@@ -66,6 +66,23 @@ def test_blocked_pick_is_a_weighted_index():
     assert counts[0] == 0 and counts[2] == 0 and abs(counts[1] / 2000 - 0.5) < 0.05
 
 
+def test_topk_then_topp_with_k_over_the_vocabulary_is_a_nucleus_even_at_p_1():
+    """candle's sample_topk_topp with k >= V runs sample_topp, which has no p >= 1 shortcut: where the fp32 sum of the softmax rounds
+    to >= 1 the smallest entries are dropped and the pick moves.  These are the values the device sampler test pins at V = 151936."""
+    lg = (np.random.default_rng(7).standard_normal(151936) * 1.5).astype(np.float32)
+    p = S.softmax_blocked(lg, 0.9)
+    assert S.blocked_sum(p) >= 1
+    w = S.topp_weights(p, 1.0)
+    assert np.count_nonzero(p) == 151936 and np.count_nonzero(w == 0) == 68
+    assert np.count_nonzero(S.topp_weights(p, 1.5)) == 151936                 # p > 1 keeps everything
+    r = S.StdRng(77)
+    for draw, nucleus, plain in ((90, 106616, 106615), (384, 57439, 57440)):
+        assert S.sample(lg, 0.9, 1.0, 151936, r, draw) == nucleus and S.blocked_pick(p, r.uniform01(draw)) == plain
+        assert S.sample(lg, 0.9, 1.0, None, r, draw) == plain                   # TopP alone keeps candle's p >= 1 shortcut
+        assert S.sample(lg, 0.9, None, 151936, r, draw) == plain                # and so does TopK with k >= V
+    assert all(S.blocked_pick(w, r.uniform01(d)) == S.blocked_pick(p, r.uniform01(d)) for d in range(90))   # draw 90 is the first to move
+
+
 def test_topk_then_topp_and_penalty():
     rng = np.random.default_rng(1)
     lg = rng.standard_normal(300).astype(np.float32)
