@@ -34,7 +34,7 @@ class GenParams(C.Structure):
                 ("flags", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX, GEN_LOGPROBS = 1, 2, 4, 8
+GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX, GEN_LOGPROBS, GEN_CONSTRAINED = 1, 2, 4, 8, 16
 MAX_TOP_LOGPROBS = 20
 TOKEN_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32)
 
@@ -58,6 +58,24 @@ def logprob_flags(logprobs=False, top_logprobs=0, vocab_size=None):
     if vocab_size is not None and n > vocab_size:
         raise ValueError(f"top_logprobs {n} exceeds the vocabulary of {vocab_size}")
     return GEN_LOGPROBS | gen_top_logprobs(n)
+
+
+class TokenFsm(C.Structure):
+    _fields_ = [("n_states", C.c_uint32), ("start", C.c_uint32), ("offsets", C.POINTER(C.c_uint64)), ("tokens", C.POINTER(C.c_uint32)),
+                ("next", C.POINTER(C.c_uint32))]
+
+
+def token_fsm(offsets, tokens, next, start=0):
+    """(TokenFsm, arrays it points into) of a token automaton in CSR form: state s allows tokens[offsets[s]:offsets[s + 1]] (ascending)
+    and next[j] is the state after tokens[j].  The library checks the rest (aha_b200_fsm_check)."""
+    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.uint64))
+    tok = np.ascontiguousarray(np.asarray(tokens, np.int64).reshape(-1).astype(np.uint32))
+    nxt = np.ascontiguousarray(np.asarray(next, np.int64).reshape(-1).astype(np.uint32))
+    if off.size < 1 or tok.size != nxt.size:
+        raise ValueError("offsets needs n_states + 1 entries, and tokens and next one entry per transition each")
+    ptr = lambda a, t: a.ctypes.data_as(C.POINTER(t)) if a.size else None
+    f = TokenFsm(n_states=off.size - 1, start=int(start), offsets=ptr(off, C.c_uint64), tokens=ptr(tok, C.c_uint32), next=ptr(nxt, C.c_uint32))
+    return f, (off, tok, nxt)
 
 
 class Logprobs(C.Structure):
@@ -195,6 +213,11 @@ SYMBOLS = {
                                         C.POINTER(C.c_size_t), TOKEN_CALLBACK, C.c_void_p, C.POINTER(Usage)]),
     "aha_b200_debug_sample": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _F32P, C.c_size_t, C.POINTER(GenParams), _U32P, _U32P, _U32P,
                                         C.c_int, _I32P, _I32P, _U32P, _U32P, _U32P]),
+    "aha_b200_debug_sample_fsm": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _F32P, C.c_size_t, C.POINTER(GenParams), _U32P, _U32P, _U32P,
+                                            C.c_int, _I32P, _I32P, C.POINTER(TokenFsm), _I32P, _U32P, _U32P, _U32P, _U32P, _U32P]),
+    "aha_b200_fsm_check": (C.c_int, [C.POINTER(TokenFsm), C.c_size_t]),
+    "aha_b200_fsm_create": (C.c_int, [_P, C.POINTER(TokenFsm), _U32P]),
+    "aha_b200_fsm_destroy": (C.c_int, [_P, C.c_uint32]),
     "aha_b200_mel_spectrogram": (C.c_int, [_P, _F32P, C.c_size_t, _F32P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_image_patchify": (C.c_int, [_P, C.POINTER(C.c_uint8), C.c_size_t, C.c_size_t, _F32P, C.c_size_t, _U32P]),
     "aha_b200_img_smart_resize": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, _U32P, _U32P]),

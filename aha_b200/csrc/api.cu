@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <functional>
 #include <limits>
+#include <map>
 #include <mutex>
 #include <system_error>
 #include <thread>
@@ -95,6 +96,13 @@ struct aha_model {
     } score;
     CUtensorMap score_tm_w{};
     bool score_ready = false;
+    // token automata of constrained requests (aha_b200_fsm_create): id -> one device allocation holding offsets | tokens | next
+    struct Fsm {
+        void* mem = nullptr;
+        TokenFsmDev dev;
+    };
+    std::map<uint32_t, Fsm> fsms;
+    uint32_t next_fsm_id = 1;
 };
 
 namespace {
@@ -385,6 +393,64 @@ int logprob_request(const aha_gen_params& p, const TextModel& T, const std::stri
 void refuse_logprobs(const aha_gen_params& p, const std::string& who, const std::string& instead) {
     AHA_REQUIRE((p.flags & AHA_GEN_LOGPROBS) == 0 && (p.flags >> 8) == 0, who + " returns no log-probabilities: use " + instead);
 }
+// Everything aha_token_fsm promises, checked on the host before an automaton reaches the device: the kernels index with these values
+// unchecked (sampling.cuh), and a state without a token would leave a request nothing to draw.
+void fsm_validate(const aha_token_fsm* f, size_t vocab) {
+    AHA_REQUIRE(f, "token automaton: fsm is NULL");
+    AHA_REQUIRE(f->n_states >= 1, "token automaton: n_states must be at least 1");
+    AHA_REQUIRE(f->offsets, "token automaton: offsets is NULL");
+    const uint64_t n_trans = f->offsets[f->n_states];
+    AHA_REQUIRE(n_trans == 0 || (f->tokens && f->next), "token automaton: tokens and next are required");
+    AHA_REQUIRE(f->start < f->n_states, "token automaton: start " + std::to_string(f->start) + " is not below n_states " + std::to_string(f->n_states));
+    AHA_REQUIRE(f->offsets[0] == 0, "token automaton: offsets[0] must be 0");
+    for (uint32_t st = 0; st < f->n_states; ++st) {
+        const uint64_t a = f->offsets[st], b = f->offsets[st + 1];
+        AHA_REQUIRE(a <= b && b <= n_trans, "token automaton: offsets must be non-decreasing up to offsets[n_states] (state " + std::to_string(st) + ")");
+        AHA_REQUIRE(b > a, "token automaton: state " + std::to_string(st) + " allows no token");
+        for (uint64_t j = a; j < b; ++j) {
+            AHA_REQUIRE(f->tokens[j] < vocab, "token automaton: state " + std::to_string(st) + " allows token " + std::to_string(f->tokens[j]) +
+                                                  ", outside the vocabulary of " + std::to_string(vocab));
+            AHA_REQUIRE(j == a || f->tokens[j] > f->tokens[j - 1], "token automaton: the tokens of state " + std::to_string(st) +
+                                                                       " are not strictly ascending");
+            AHA_REQUIRE(f->next[j] < f->n_states, "token automaton: next[" + std::to_string(j) + "] = " + std::to_string(f->next[j]) +
+                                                      " is not below n_states " + std::to_string(f->n_states));
+        }
+    }
+}
+// bytes of an automaton's device copy: offsets [n_states + 1] (u64), then tokens and next [transitions] (u32)
+size_t fsm_bytes(const aha_token_fsm& f) { return (size_t)(f.n_states + 1) * sizeof(uint64_t) + (size_t)f.offsets[f.n_states] * 2 * sizeof(uint32_t); }
+// a validated automaton copied into `mem` (fsm_bytes(f) bytes of device memory)
+TokenFsmDev fsm_upload(const aha_token_fsm& f, void* mem) {
+    const size_t n_off = (size_t)f.n_states + 1, n = (size_t)f.offsets[f.n_states];
+    TokenFsmDev d;
+    char* p = static_cast<char*>(mem);
+    d.off = reinterpret_cast<const uint64_t*>(p);
+    d.tok = reinterpret_cast<const uint32_t*>(p + n_off * sizeof(uint64_t));
+    d.next = d.tok + n;
+    d.start = f.start;
+    AHA_CUDA_CHECK(cudaMemcpy(p, f.offsets, n_off * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    if (n) {
+        AHA_CUDA_CHECK(cudaMemcpy(const_cast<uint32_t*>(d.tok), f.tokens, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        AHA_CUDA_CHECK(cudaMemcpy(const_cast<uint32_t*>(d.next), f.next, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    }
+    return d;
+}
+// AHA_GEN_CONSTRAINED: the request's automaton (nullptr without the flag), refused where constrained decoding does not run
+const aha_model::Fsm* request_fsm(const aha_model* m, const aha_gen_params& p, const std::string& who) {
+    if (!(p.flags & AHA_GEN_CONSTRAINED)) return nullptr;
+    AHA_REQUIRE(m->text.tp_world == 1, who + "constrained decoding is single-GPU (under tensor parallelism the decode step holds only a vocabulary shard)");
+    const auto it = m->fsms.find(p.reserved);
+    AHA_REQUIRE(it != m->fsms.end(), who + "AHA_GEN_CONSTRAINED: no token automaton has id " + std::to_string(p.reserved) + " on this handle");
+    return &it->second;
+}
+// the request's sampler (make_sampler), constrained by its automaton when it asks
+Sampler request_sampler(const aha_model* m, const aha_gen_params& p, const std::string& who) {
+    const aha_model::Fsm* f = request_fsm(m, p, who);
+    Sampler s = make_sampler(p, m->text.cfg.V, f ? &f->dev : nullptr);
+    if (f) s.fsm_id = p.reserved;
+    return s;
+}
+
 // AHA_BATCH_GEMV's default (BatchDecoder::gemv).  The two batched GEMVs are bit-identical on every tested shape and neither wins everywhere: on
 // one H100 80GB HBM3 at 400 W (profiles/run_batch.py, ms per step at 1 / 8 requests) v2 takes 2.25 / 4.68-4.76 against v1's 2.22 / 4.17 on the
 // VL2 text stack, and 1.30 / 2.71 against 1.33 / 2.63-2.64 on the Qwen3-0.6B shape.
@@ -640,7 +706,7 @@ uint32_t first_token(aha_model* m, PageTable& pt, const uint32_t* ids, size_t se
                      uint32_t draws0) {
     TextModel& T = m->text;
     T.set_sampler(samp);
-    T.set_state(0, 0, 0, 0, draws0);    // empty history: the first token sees no repeat-penalty context
+    T.set_state(0, 0, 0, 0, draws0, samp.fsm_start);    // empty history: the first token sees no repeat-penalty context
     uint32_t tok = 0;
     if (hit > 0) forward_any(m, pt, ids + hit, seq_len - hit, hit, nullptr, false, nullptr, &tok, true);   // only the tokens the cache does not hold yet
     else forward_any(m, pt, ids, seq_len, 0, mm, true, nullptr, &tok);
@@ -650,17 +716,17 @@ uint32_t first_token(aha_model* m, PageTable& pt, const uint32_t* ids, size_t se
 
 // The handoff to decode after first_token: every page positions [0, ctx) can touch is mapped on `pt` (the step kernels only read the
 // table), and the decode state starts from `tok` at position seq_len, with history[0] = tok and the draw index the first token left.  The
-// state is the model's own, or batch slot `slot`'s.
+// state is the model's own, or batch slot `slot`'s; the automaton state the first token left travels with it.
 void handoff(aha_model* m, PageTable& pt, size_t ctx, uint32_t tok, size_t seq_len, int slot = -1) {
     TextModel& T = m->text;
     T.pages.map(pt, (int)ctx);
     DecodeState cur;
     AHA_CUDA_CHECK(cudaMemcpy(&cur, T.d_state, sizeof(cur), cudaMemcpyDeviceToHost));
     if (slot >= 0) {
-        m->sess().adopt(slot, tok, (int)seq_len, decode_rope_delta(m), cur.n_draws);
+        m->sess().adopt(slot, tok, (int)seq_len, decode_rope_delta(m), cur.n_draws, cur.fsm_state);
         return;
     }
-    T.set_state(tok, (int)seq_len, decode_rope_delta(m), 1, cur.n_draws);
+    T.set_state(tok, (int)seq_len, decode_rope_delta(m), 1, cur.n_draws, cur.fsm_state);
     AHA_CUDA_CHECK(cudaMemcpy(T.d_history, &tok, sizeof(uint32_t), cudaMemcpyHostToDevice));
 }
 
@@ -818,6 +884,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
                    aha_usage* usage, size_t* n_generated, int lp_n = -1) {
     TextModel& T = m->text;
     require_no_session(m);
+    request_fsm(m, params, "");
     const bool lp = lp_n >= 0;
     request_logprobs(m, lp_n);
     const size_t sample_len = token_budget(params);
@@ -847,7 +914,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
         draws0 = cur.n_draws;
     }
     auto is_eos = [&](uint32_t t) { for (uint32_t e : m->stop_ids) if (e == t) return true; return false; };
-    const uint32_t tok = first_token(m, T.table, ids, seq_len, hit, mm, make_sampler(params, T.cfg.V), draws0);
+    const uint32_t tok = first_token(m, T.table, ids, seq_len, hit, mm, request_sampler(m, params, ""), draws0);
     if (lp) {   // the first token's record, from the prefill logits
         T.logprobs(true, T.d_lp, true);
         AHA_CUDA_CHECK(cudaMemcpyAsync(m->h_lp_pin, T.d_lp, sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
@@ -923,6 +990,8 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
     for (size_t i = 0; i < sp.n_prediction; ++i) AHA_REQUIRE(sp.prediction[i] < (uint32_t)T.cfg.V, who + "prediction token id out of range");
     AHA_REQUIRE((params.flags & (AHA_GEN_REUSE_PREFIX | AHA_GEN_CONTINUE_RNG | AHA_GEN_EOS_ON_FIRST)) == 0,
                 who + "REUSE_PREFIX, CONTINUE_RNG and EOS_ON_FIRST are not supported with speculative decoding");
+    AHA_REQUIRE((params.flags & AHA_GEN_CONSTRAINED) == 0,
+                who + "AHA_GEN_CONSTRAINED is not supported with speculative decoding (a verify row's mask would depend on the drafts before it)");
     const int lp_n = logprob_request(params, T, who);
     AHA_REQUIRE(lp_n < 0 || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
     const size_t sample_len = token_budget(params);
@@ -982,7 +1051,7 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
     BatchDecoder& B = m->sess();
     PageTable& pt = B.slots[slot].table;
     m->have_rope_delta = false; m->rope_delta = 0;
-    const Sampler samp = make_sampler(r.params, T.cfg.V);
+    const Sampler samp = request_sampler(m, r.params, "");
     const uint32_t tok = first_token(m, pt, r.ids, r.seq_len, 0, r.mm, samp, 0);
     if (lp_n >= 0) {   // the first token's record goes straight into the slot's record row
         T.set_logprobs(lp_n);
@@ -1086,6 +1155,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         lp_n[i] = logprob_request(r.params, T, who + "request " + std::to_string(i) + ": ");
         for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
         AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+        request_fsm(m, r.params, who + "request " + std::to_string(i) + ": ");
         require_mm_arity(m, r.mm);
         sample_len[i] = token_budget(r.params);
         pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
@@ -1138,14 +1208,16 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         }
         // first tokens: batched lm_head over the gathered rows, then each request's ArgMax / sampler against an empty state (forward_any's draw)
         std::vector<int> act;
+        std::vector<DecodeState> empty((size_t)B.cap, DecodeState{0, 0, 0, 0, 0, 0, {0, 0}});   // per slot: empty history, draw index 0
         for (size_t i : pk) {
-            B.bind_sampler(slot[i], make_sampler(reqs[i].params, T.cfg.V));
+            const Sampler samp = request_sampler(m, reqs[i].params, who);
+            B.bind_sampler(slot[i], samp);
+            empty[slot[i]].fsm_state = samp.fsm_start;
             B.slots[slot[i]].lp = lp_n[i] + 1;
             if (lp_n[i] >= 0) B.ensure_lp();
             act.push_back(slot[i]);
         }
-        const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};
-        for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
+        for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty[s], sizeof(DecodeState), cudaMemcpyHostToDevice, c.stream));
         B.head_rows(act, true);
         std::vector<uint32_t> h_tok((size_t)B.cap);
         std::vector<DecodeState> h_st((size_t)B.cap);
@@ -1155,7 +1227,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         T.check_sample_error();
         const double t_first = seconds(clk::now() - t0);
         for (size_t i : pk) {   // (their pages were mapped before the prefill)
-            B.adopt(slot[i], h_tok[slot[i]], (int)reqs[i].seq_len, 0, h_st[slot[i]].n_draws);
+            B.adopt(slot[i], h_tok[slot[i]], (int)reqs[i].seq_len, 0, h_st[slot[i]].n_draws, h_st[slot[i]].fsm_state);
             tok[i] = h_tok[slot[i]];
             secs[i] = t_first;
         }
@@ -1205,6 +1277,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     const int lp_n = logprob_request(req.params, T, who);
     for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
     AHA_REQUIRE((req.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+    request_fsm(m, req.params, who);
     require_mm_arity(m, req.mm);
     const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len;
     AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
@@ -1215,7 +1288,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     std::vector<Sampler> samp(n);
     for (size_t i = 0; i < n; ++i) {
         r[i].params.seed = seeds ? seeds[i] : req.params.seed + i;
-        samp[i] = make_sampler(r[i].params, T.cfg.V);
+        samp[i] = request_sampler(m, r[i].params, who);
     }
     const auto t0 = clk::now();
     AdmitGuard guard{m, slot};
@@ -1226,7 +1299,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
         const std::vector<int> dst(slot.begin() + 1, slot.end());
         for (int s : dst) T.pages.map(B.slots[s].table, (int)ctx);
         B.fork(slot[0], dst, (int)req.seq_len);
-        const DecodeState empty{0, 0, 0, 0, 0, {0, 0, 0}};   // first_token's state: empty history, draw index 0
+        const DecodeState empty{0, 0, 0, 0, 0, samp[0].fsm_start, {0, 0}};   // first_token's state: empty history, draw index 0, start state
         for (size_t i = 1; i < n; ++i) {
             const int s = slot[i];
             T.set_sampler(samp[i]);
@@ -1248,7 +1321,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
         T.check_sample_error();
         for (size_t i = 1; i < n; ++i) {
             tok[i] = h_tok[slot[i]];
-            B.adopt(slot[i], tok[i], (int)req.seq_len, decode_rope_delta(m), h_st[slot[i]].n_draws);
+            B.adopt(slot[i], tok[i], (int)req.seq_len, decode_rope_delta(m), h_st[slot[i]].n_draws, h_st[slot[i]].fsm_state);
         }
     }
     const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
@@ -1506,6 +1579,42 @@ int aha_b200_generate_speculative(aha_model* m, const uint32_t* ids, size_t seq_
     });
 }
 
+int aha_b200_fsm_check(const aha_token_fsm* fsm, size_t vocab) {
+    return guarded_host([&] { fsm_validate(fsm, vocab); });
+}
+
+int aha_b200_fsm_create(aha_model* m, const aha_token_fsm* fsm, uint32_t* id_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(id_out, "fsm_create: id_out is required");
+        fsm_validate(fsm, (size_t)m->text.cfg.V);
+        AHA_REQUIRE(m->next_fsm_id != 0, "fsm_create: the handle has used every automaton id");
+        aha_model::Fsm f;
+        AHA_CUDA_CHECK(cudaMalloc(&f.mem, fsm_bytes(*fsm)));
+        try {
+            f.dev = fsm_upload(*fsm, f.mem);
+        } catch (...) {
+            cudaFree(f.mem);
+            throw;
+        }
+        const uint32_t id = m->next_fsm_id++;
+        m->fsms[id] = f;
+        *id_out = id;
+    });
+}
+
+int aha_b200_fsm_destroy(aha_model* m, uint32_t id) {
+    return guarded(m, [&] {
+        const auto it = m->fsms.find(id);
+        AHA_REQUIRE(it != m->fsms.end(), "fsm_destroy: no token automaton has id " + std::to_string(id) + " on this handle");
+        for (int i = 0; m->session.open && i < m->session.width; ++i)
+            AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].fsm_id == id),
+                        "fsm_destroy: token automaton " + std::to_string(id) + " constrains the running request in slot " + std::to_string(i));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+        AHA_CUDA_CHECK(cudaFree(it->second.mem));
+        m->fsms.erase(it);
+    });
+}
+
 extern "C++" {
 namespace {
 // Host staging of the debug attention entries: a paged KV pool laid out like the model's ([page][K|V][kv_head][kPage][hd]), filled with NaN,
@@ -1587,7 +1696,7 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
         for (int p = 0; p < np; ++p) table[p] = np - p;
         pool.put(table.data(), ctx, k, v);
         std::vector<DecodeState> st(R);
-        for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, {0, 0, 0}};
+        for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, 0, {0, 0}};
         const int max_chunks = ceil_div(ctx, kSpecChunk);
         Scratch mem;
         float* d_pool = upload_scratch(mem, c.stream, pool.data.data(), pool.data.size());
@@ -1727,7 +1836,7 @@ int aha_b200_debug_decode_attn(aha_model* m, size_t batch, size_t n_heads, size_
         const float* d_kw = upload_scratch(mem, c.stream, k_norm, HD);
         const float* d_inv = upload_scratch(mem, c.stream, rope_inv_freq(rope_theta, HD).data(), HD / 2);
         std::vector<DecodeState> st(B);
-        for (int b = 0; b < B; ++b) st[b] = DecodeState{0, pos[b], rope_delta[b], 0, 0, {0, 0, 0}};
+        for (int b = 0; b < B; ++b) st[b] = DecodeState{0, pos[b], rope_delta[b], 0, 0, 0, {0, 0}};
         const DecodeState* d_st = upload_scratch(mem, c.stream, st.data(), st.size());
         const size_t part = (size_t)nh * kDecodeSplits * (HD + 2), n_out = (size_t)B * nh * HD;
         float* d_part = mem.alloc<float>((size_t)B * part);
@@ -1807,6 +1916,7 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
         AHA_REQUIRE(m->kind == aha_model::QWEN3_ASR, "asr_generate needs a qwen3_asr handle");
         AHA_REQUIRE(chunks && n_chunks >= 1 && params && out_tokens && n_out, "chunks, params, out_tokens and n_out are required");
         refuse_logprobs(*params, "asr_generate", "aha_b200_generate_logprobs on each chunk's prompt");
+        AHA_REQUIRE((params->flags & AHA_GEN_CONSTRAINED) == 0, "asr_generate: AHA_GEN_CONSTRAINED is not supported on the ASR loop");
         if (usage) *usage = aha_usage{};
         // Qwen3AsrGenerateModel::generate (qwen3_asr/generate.rs:130-186): ONE LogitsProcessor for the whole request (its RNG
         // stream runs on across the chunks), no repeat penalty, every token -- the first included -- is EOS-checked, the KV
@@ -1837,6 +1947,14 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
 int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
                           const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
                           const int32_t* on, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out) {
+    return aha_b200_debug_sample_fsm(m, kernel, rows, V, logits, ld, params, context, n_context, draw_index, overwrite, act, on, nullptr, nullptr,
+                                     nullptr, token_out, state_out, hist_out, nullptr);
+}
+
+int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                              const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                              const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
+                              uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out, uint32_t* fsm_state_out) {
     return guarded(m, [&] {
         AHA_REQUIRE(logits && params && n_context && draw_index && token_out && state_out && hist_out,
                     "logits, params, n_context, draw_index, token_out, state_out and hist_out are required");
@@ -1858,15 +1976,21 @@ int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const
             cap = std::max(cap, (size_t)n_context[r]);
         }
         AHA_REQUIRE(context || n_ctx_total == 0, "context is required");
+        AHA_REQUIRE(!fsm || (constrained && fsm_state_in && fsm_state_out), "an automaton needs constrained, fsm_state_in and fsm_state_out");
+        if (fsm) fsm_validate(fsm, V);
+        for (size_t r = 0; fsm && r < rows; ++r)
+            AHA_REQUIRE(!constrained[r] || fsm_state_in[r] < fsm->n_states, "row " + std::to_string(r) + ": fsm_state_in is not below n_states");
+        Scratch mem;
+        TokenFsmDev dev;
+        if (fsm) dev = fsm_upload(*fsm, mem.alloc<char>(fsm_bytes(*fsm)));
         std::vector<SampleArgs> args(kSampleMaxRows, SampleArgs{});
         for (size_t r = 0; r < rows; ++r) {
-            const Sampler s = make_sampler(params[r], (int)V);
+            const Sampler s = make_sampler(params[r], (int)V, fsm && constrained[r] ? &dev : nullptr);
             AHA_REQUIRE(s.active, "row " + std::to_string(r) + ": plain ArgMax needs no sampler (temperature < 1e-7 and no repeat penalty)");
             args[slot[r]] = s.args;
         }
         cudaStream_t st = m->ctx.stream;
         const size_t n_logits = ld ? rows * ld : V;
-        Scratch mem;
         float* d_logits = mem.alloc<float>(n_logits);
         float* d_work = mem.alloc<float>(rows * V);
         DecodeState* d_st = mem.alloc<DecodeState>(rows);
@@ -1878,7 +2002,7 @@ int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const
         for (size_t r = 0, off = 0; r < rows; off += n_context[r], ++r) {
             const uint32_t n = n_context[r];
             std::copy(context + off, context + off + n, hh.begin() + r * cap);
-            hs[r] = DecodeState{n ? context[off + n - 1] : 0u, 0, 0, (int32_t)n, draw_index[r], {0, 0, 0}};
+            hs[r] = DecodeState{n ? context[off + n - 1] : 0u, 0, 0, (int32_t)n, draw_index[r], fsm ? fsm_state_in[r] : 0u, {0, 0}};
             SampleArgs& a = args[slot[r]];
             a.logits = d_logits + r * ld; a.work = d_work + r * V;
             a.st = d_st + r; a.history = d_hist + r * cap; a.hist_cap = (int)cap; a.token_out = d_tok + r; a.error = d_err;
@@ -1913,6 +2037,7 @@ int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const
         for (size_t r = 0; r < rows; ++r) {
             state_out[3 * r] = hs[r].token; state_out[3 * r + 1] = (uint32_t)hs[r].n_hist; state_out[3 * r + 2] = hs[r].n_draws;
             hist_out[r] = n_context[r] ? hh[r * cap + n_context[r] - 1] : 0xffffffffu;
+            if (fsm) fsm_state_out[r] = hs[r].fsm_state;
         }
     });
 }
@@ -1926,7 +2051,7 @@ int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_
         cudaStream_t st = m->ctx.stream;
         const int P = lp_parts((int)V);
         const int on = 1 + (int)n_top;
-        const DecodeState ds{token, 0, 0, 0, 0, {0, 0, 0}};
+        const DecodeState ds{token, 0, 0, 0, 0, 0, {0, 0}};
         // scratch of this call only: [V] logits, the candidate lists, the on flag, the token, a state and the record
         const size_t o_part = V * sizeof(float), o_id = o_part + (size_t)P * kLpPartFloats * sizeof(float), o_on = o_id + (size_t)P * kLpMaxTop * sizeof(int);
         const size_t o_tok = o_on + 16, o_st = o_tok + 16, o_rec = o_st + sizeof(DecodeState), bytes = o_rec + sizeof(aha_logprobs);
@@ -2754,6 +2879,7 @@ void aha_b200_destroy(aha_model* m) {
     m->batch.graphs.clear();
     m->wide_batch.graphs.clear();
     m->spec.destroy();
+    for (auto& f : m->fsms) cudaFree(f.second.mem);
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
     if (m->h_lp_pin) cudaFreeHost(m->h_lp_pin);

@@ -38,6 +38,7 @@ struct BatchSlot {                       // one sequence of the batch
     bool samp_active = false;
     SampleArgs samp{};                   // sampler of the request with the pointers of this slot
     int lp = 0;                          // 0: the request asked for no log-probabilities, else 1 + its top count
+    uint32_t fsm_id = 0;                 // the token automaton the request is constrained by (0: none); it cannot be destroyed while the slot runs
 };
 
 struct BatchDecoder {
@@ -144,10 +145,11 @@ struct BatchDecoder {
         for (int i = 0; i < n; ++i) { slots[i].table.h.assign(t.num_pages, 0); slots[i].table.d = d_tables + (size_t)i * t.num_pages; }
     }
 
-    // after the first token of slot i: its decode state starts from that token (history[0]) at position seq_len
-    void adopt(int i, uint32_t first_token, int seq_len, int rope_delta, uint32_t n_draws) {
+    // after the first token of slot i: its decode state starts from that token (history[0]) at position seq_len, with the draw index and
+    // automaton state the first token left
+    void adopt(int i, uint32_t first_token, int seq_len, int rope_delta, uint32_t n_draws, uint32_t fsm_state) {
         Ctx& c = *T->ctx;
-        DecodeState st{first_token, seq_len, rope_delta, 1, n_draws, {0, 0, 0}};
+        DecodeState st{first_token, seq_len, rope_delta, 1, n_draws, fsm_state, {0, 0}};
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_states + i, &st, sizeof(st), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_hist + (size_t)i * T->hist_cap, &first_token, sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // stack temporaries
@@ -171,6 +173,7 @@ struct BatchDecoder {
     void bind_sampler(int i, const Sampler& s) {
         BatchSlot& sl = slots[i];
         sl.samp_active = s.active;
+        sl.fsm_id = s.fsm_id;
         if (s.active) sl.samp = T->bind_sampler(s, d_states + i, d_hist + (size_t)i * T->hist_cap, d_tok + i, workb + (size_t)i * T->cfg.V);
     }
 

@@ -175,7 +175,8 @@ struct DecodeState {
     int32_t rope_delta;  // Qwen3-VL rope_deltas (0 for text / ASR)
     int32_t n_hist;      // tokens written to history
     uint32_t n_draws;    // random draws the request's sampler has consumed (index into its ChaCha12 stream)
-    uint32_t pad_[3];
+    uint32_t fsm_state;  // state of the request's token automaton (sampling.cuh; 0 and unused without one)
+    uint32_t pad_[2];
 };
 __device__ __forceinline__ void argmax_final_dev(const float* __restrict__ pmax, const int* __restrict__ pidx, int n,
                                                  uint32_t* __restrict__ argmax_out, DecodeState* __restrict__ st,

@@ -45,6 +45,11 @@ struct SampleArgs {
     uint32_t* token_out;
     int overwrite;           // 1: the step kernel already pushed its argmax token (history[n_hist - 1], st->token): replace it
     int* error;              // set to 1 when the weights are all zero / not finite (WeightedIndex::new fails in the reference)
+    // token automaton of a constrained request (aha_b200_fsm_create; null: unconstrained): state s allows the ascending tokens
+    // fsm_tok[fsm_off[s] .. fsm_off[s + 1]), and fsm_next[j] is the state after fsm_tok[j].  The current state is st->fsm_state.
+    const uint64_t* fsm_off;
+    const uint32_t* fsm_tok;
+    const uint32_t* fsm_next;
 };
 
 // ---- StdRng: ChaCha12 block `counter` of the stream keyed by `key`, word `w` (rand_chacha: 64-bit counter in words 12-13, stream 0)
@@ -151,16 +156,29 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
     const int n_hist = a.st->n_hist;
     const int n_ctx = a.overwrite ? n_hist - 1 : n_hist;     // tokens generated before this one
     const unsigned draw = a.st->n_draws;
-    // ---- penalised logits (use_repeat_penalty: every distinct token of the last `last_n` generated ones, once)
-    for (int i = tid; i < V; i += kSampleThreads) p[i] = a.logits[i];
+    const bool fsm = a.fsm_off != nullptr;
+    if (!fsm) {
+        for (int i = tid; i < V; i += kSampleThreads) p[i] = a.logits[i];
+    } else {
+        // masked logits: -inf, then the allowed entries scattered from the state's row (O(V + allowed), no per-state bitmap)
+        const uint32_t fs = a.st->fsm_state;
+        const uint64_t f0 = a.fsm_off[fs], f1 = a.fsm_off[fs + 1];
+        for (int i = tid; i < V; i += kSampleThreads) p[i] = -INFINITY;
+        __syncthreads();
+        for (uint64_t j = f0 + tid; j < f1; j += kSampleThreads) { const uint32_t t = a.fsm_tok[j]; p[t] = a.logits[t]; }
+    }
     __syncthreads();
+    // ---- penalised logits (use_repeat_penalty: every distinct token of the last `last_n` generated ones, once; a masked entry stays -inf)
     if (!(a.penalty == 1.0f || a.last_n == 0) && n_ctx > 0) {
         const int start = max(0, n_ctx - a.last_n);
         for (int t = start + tid; t < n_ctx; t += kSampleThreads) {
             const uint32_t tok = a.history[t];
             bool first = true;
             for (int u = start; u < t; ++u) if (a.history[u] == tok) { first = false; break; }
-            if (first && tok < (uint32_t)V) { const float x = p[tok]; p[tok] = x >= 0.f ? x / a.penalty : x * a.penalty; }
+            if (first && tok < (uint32_t)V) {
+                const float x = p[tok];
+                if (!(fsm && x == -INFINITY)) p[tok] = x >= 0.f ? x / a.penalty : x * a.penalty;
+            }
         }
         __syncthreads();
     }
@@ -179,6 +197,7 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
         if (tid == 0) {
             for (int w = 1; w < kSampleThreads / 32; ++w) if (s.redf[w] > best || (s.redf[w] == best && s.redi[w] < bi)) { best = s.redf[w]; bi = s.redi[w]; }
             s.bc_i[1] = (bi < 0 || bi >= V) ? 0 : bi;
+            if (fsm && !(best > -INFINITY)) *a.error = 1;      // no allowed token has a finite logit
         }
         __syncthreads();
         token = s.bc_i[1];
@@ -336,6 +355,14 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
             st->token = (uint32_t)token;
             if (n_hist >= 1 && n_hist - 1 < a.hist_cap) a.history[n_hist - 1] = (uint32_t)token;
         }
+        if (fsm) {   // advance: the token's entry in the state's sorted row; a token the state does not allow is an error, never a transition
+            const uint32_t fs = st->fsm_state;
+            const uint64_t f1 = a.fsm_off[fs + 1];
+            uint64_t lo = a.fsm_off[fs], hi = f1;
+            while (lo < hi) { const uint64_t mid = lo + ((hi - lo) >> 1); if (a.fsm_tok[mid] < (uint32_t)token) lo = mid + 1; else hi = mid; }
+            if (lo < f1 && a.fsm_tok[lo] == (uint32_t)token) st->fsm_state = a.fsm_next[lo];
+            else *a.error = 1;
+        }
     }
 }
 
@@ -364,16 +391,27 @@ __global__ void __launch_bounds__(kSampleThreads) sample_rows_kernel(const Sampl
 struct Sampler {
     bool active = false;
     SampleArgs args{};
+    uint32_t fsm_start = 0;      // the automaton's start state: a first token is drawn from it
+    uint32_t fsm_id = 0;         // the automaton's id on the handle (0: unconstrained)
+};
+
+// a token automaton in device memory (aha_b200_fsm_create)
+struct TokenFsmDev {
+    const uint64_t* off = nullptr;
+    const uint32_t* tok = nullptr;
+    const uint32_t* next = nullptr;
+    uint32_t start = 0;
 };
 
 // get_logit_processor (sample.rs:7-38): the Sampling a request's parameters select, checked against what the device sampler supports
-inline Sampler make_sampler(const aha_gen_params& p, int V) {
+// A constrained request (fsm != null) always samples on the device, greedy included: ArgMax over its allowed tokens.
+inline Sampler make_sampler(const aha_gen_params& p, int V, const TokenFsmDev* fsm = nullptr) {
     const bool has_t = !(p.temperature < 1e-7f);
     const bool has_k = p.top_k > 0, has_p = p.top_p > 0.f;
     const int mode = !has_t ? SAMPLE_ARGMAX : !has_k ? (has_p ? SAMPLE_TOPP : SAMPLE_ALL) : (has_p ? SAMPLE_TOPK_TOPP : SAMPLE_TOPK);
     const bool pen = !(p.repeat_penalty == 1.0f || p.repeat_last_n == 0);
     Sampler s;
-    s.active = mode != SAMPLE_ARGMAX || pen;
+    s.active = mode != SAMPLE_ARGMAX || pen || fsm != nullptr;
     if (!s.active) return s;
     AHA_REQUIRE(V <= kSampleThreads * kSampleChunk, "vocabulary too large for the device sampler");
     AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || p.top_k >= 1, "top_k must be >= 1");
@@ -383,6 +421,7 @@ inline Sampler make_sampler(const aha_gen_params& p, int V) {
     a.V = V; a.mode = mode;
     a.inv_temp = mode == SAMPLE_ARGMAX ? 1.0f : (float)(1.0 / (double)p.temperature);
     a.top_p = p.top_p; a.top_k = p.top_k; a.penalty = p.repeat_penalty; a.last_n = p.repeat_last_n;
+    if (fsm) { a.fsm_off = fsm->off; a.fsm_tok = fsm->tok; a.fsm_next = fsm->next; s.fsm_start = fsm->start; }
     // rand_core::SeedableRng::seed_from_u64: eight PCG32 outputs fill the 32-byte ChaCha seed
     uint64_t stt = p.seed;
     for (int i = 0; i < 8; ++i) {

@@ -1031,8 +1031,8 @@ struct TextModel {
         AHA_CUDA_CHECK(cudaGetLastError());
         ctx->cnt.kernels += 2;
     }
-    void set_state(uint32_t token, int pos, int rope_delta, int n_hist, uint32_t n_draws = 0) {
-        DecodeState s{token, pos, rope_delta, n_hist, n_draws, {0, 0, 0}};
+    void set_state(uint32_t token, int pos, int rope_delta, int n_hist, uint32_t n_draws = 0, uint32_t fsm_state = 0) {
+        DecodeState s{token, pos, rope_delta, n_hist, n_draws, fsm_state, {0, 0}};
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_state, &s, sizeof(s), cudaMemcpyHostToDevice, ctx->stream));
         AHA_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));  // `s` is a stack temporary
     }

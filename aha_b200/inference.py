@@ -63,6 +63,15 @@ def prefix_match(cached_ids, ids, mm_token_ids=(), same_mm=True):
     return int(lib.aha_b200_prefix_match(u32(a), a.size, u32(b), b.size, u32(t), t.size, 1 if same_mm else 0))
 
 
+def fsm_check(offsets, tokens, next, start=0, vocab_size=None):
+    """Check a token automaton (CSR: state s allows tokens[offsets[s]:offsets[s + 1]], next[j] follows tokens[j]) the way
+    fsm_create checks it, over a vocabulary of vocab_size tokens (host only, aha_b200_fsm_check).  Raises B200Error."""
+    lib = L.load()
+    f, _keep = L.token_fsm(offsets, tokens, next, start)
+    if lib.aha_b200_fsm_check(C.byref(f), int(vocab_size)) != 0:
+        raise B200Error(lib.aha_b200_last_error(None).decode())
+
+
 def mm_fingerprint(data):
     """64-bit fingerprint of a MultiModalData list (0 = no tensor): what decides whether two requests carry the same images / audio."""
     lib = L.load()
@@ -181,9 +190,13 @@ class B200Model:
 
     # ------------------------------------------------------------------ generate_generic / generate_stream_generic
     @staticmethod
-    def _gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags=0):
+    def _gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags=0, fsm=None):
+        """fsm: the id of a token automaton (fsm_create) that constrains the request (AHA_GEN_CONSTRAINED), or None"""
+        if fsm is not None:
+            flags |= L.GEN_CONSTRAINED
         return L.GenParams(temperature=temperature or 0.0, repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n,
-                           max_tokens=max_tokens, seed=seed, top_p=top_p or 0.0, top_k=top_k or 0, flags=flags)
+                           max_tokens=max_tokens, seed=seed, top_p=top_p or 0.0, top_k=top_k or 0, flags=flags,
+                           reserved=0 if fsm is None else int(fsm))
 
     @staticmethod
     def _usage(u):
@@ -191,18 +204,19 @@ class B200Model:
                     completion_secs=u.completion_secs, vision_secs=u.vision_secs)
 
     def generate(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False, logprobs=False, top_logprobs=0):
+                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None):
         """-> (generated ids, usage dict).  temperature < 1e-7: ArgMax; else the device sampler (TopK / TopKThenTopP / TopP /
         All exactly as get_logit_processor picks them from temperature, top_p, top_k).  reuse_prefix: keep this request's K/V
         and prefill only what follows the prefix shared with the cache (multi-turn chats; same tokens as without it).
         logprobs=True (aha_b200_generate_logprobs): -> (ids, usage, records), one record dict per token (token, index, logprob,
-        top_ids, top_logprobs with top_logprobs alternatives; raw model log-probabilities, before penalty and temperature)."""
+        top_ids, top_logprobs with top_logprobs alternatives; raw model log-probabilities, before penalty and temperature).
+        fsm: the id of a token automaton (fsm_create); every token is drawn from the tokens its current state allows."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         if reuse_prefix:
             flags |= L.GEN_REUSE_PREFIX
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
         cap = max(max_tokens, 1)
         out = (C.c_uint32 * cap)()
         n = C.c_size_t(0)
@@ -313,7 +327,7 @@ class B200Model:
 
     def generate_batch(self, requests):
         """Static batching (aha_b200_generate_batch): requests = [dict(input_ids=..., data=None, max_tokens=..., temperature=..., top_p=...,
-        top_k=..., repeat_penalty=..., repeat_last_n=..., seed=...), ...] (at most 8) decoded in lockstep on this handle.
+        top_k=..., repeat_penalty=..., repeat_last_n=..., seed=..., fsm=...), ...] (at most 8) decoded in lockstep on this handle.
         -> [(generated ids, usage dict), ...]: per request exactly what generate() returns for it alone."""
         n = len(requests)
         arr, _keep = self._batch_requests(requests)
@@ -337,8 +351,22 @@ class B200Model:
             arr[i].mm = C.pointer(mm) if mm is not None else None
             flags = r.get("flags", 0) | L.logprob_flags(r.get("logprobs", False), r.get("top_logprobs", 0), self.vocab_size)
             arr[i].params = self._gen_params(r.get("max_tokens", 1024), r.get("temperature", 0.0), r.get("top_p"), r.get("top_k"),
-                                             r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), flags)
+                                             r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), flags,
+                                             r.get("fsm"))
         return arr, keep
+
+    # ---- constrained decoding: token automata on the handle
+    def fsm_create(self, offsets, tokens, next, start=0):
+        """Copy a token automaton to the device (aha_b200_fsm_create) -> its id, the `fsm` argument of the generation entries.
+        State s allows tokens[offsets[s]:offsets[s + 1]] (strictly ascending, at least one) and next[j] is the state after tokens[j]."""
+        f, _keep = L.token_fsm(offsets, tokens, next, start)
+        i = C.c_uint32(0)
+        self._check(self._lib.aha_b200_fsm_create(self._h, C.byref(f), C.byref(i)))
+        return int(i.value)
+
+    def fsm_destroy(self, fsm):
+        """Free a token automaton (refused while a running batch slot uses it)."""
+        self._check(self._lib.aha_b200_fsm_destroy(self._h, int(fsm)))
 
     # ---- continuous batching: requests join / leave a running batch between steps (aha_b200_batch_open / _add / _step / _close)
     def batch_open(self):
@@ -351,7 +379,7 @@ class B200Model:
         self._batch_width = int(max_seqs)
 
     def batch_add(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64,
-                  seed=299792458, flags=0, logprobs=False, top_logprobs=0):
+                  seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None):
         """Prefill one request into a free slot -> (slot, first token, finished).  logprobs / top_logprobs: batch_logprobs() holds the
         record of each token it delivers."""
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
@@ -361,7 +389,7 @@ class B200Model:
         req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
         req.seq_len = ids.size
         req.mm = C.pointer(mm) if mm is not None else None
-        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
         slot, fin, tok = C.c_int32(-1), C.c_int32(0), C.c_uint32(0)
         u = L.Usage()
         self._check(self._lib.aha_b200_batch_add(self._h, C.byref(req), C.byref(slot), C.byref(tok), C.byref(fin), C.byref(u)))
@@ -389,7 +417,7 @@ class B200Model:
         return s, s.ctypes.data_as(C.POINTER(C.c_uint64))
 
     def batch_add_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                    repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, return_usage=False):
+                    repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, return_usage=False, fsm=None):
         """OpenAI `n` (aha_b200_batch_add_n): n choices of one request in the n lowest free slots, the prompt prefilled once and its K/V
         copied into every other choice's own pages.  Choice i samples with seeds[i] (None: seed + i) and yields exactly what batch_add
         yields for the request with that seed.  All or nothing.  -> [(slot, first token, finished), ...] per choice, and with
@@ -403,7 +431,7 @@ class B200Model:
         req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
         req.seq_len = ids.size
         req.mm = C.pointer(mm) if mm is not None else None
-        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
         k = max(n, 1)
         slots, toks, fins, us = (C.c_int32 * k)(), (C.c_uint32 * k)(), (C.c_int32 * k)(), (L.Usage * k)()
         self._check(self._lib.aha_b200_batch_add_n(self._h, C.byref(req), n, seeds_p, slots, toks, fins, us))
@@ -411,7 +439,7 @@ class B200Model:
         return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
 
     def generate_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                   repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0):
+                   repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None):
         """OpenAI `n` in one call (aha_b200_generate_n, 1 <= n <= 8): the prompt prefilled once, the choices decoded in lockstep.
         -> [(ids, usage), ...] per choice, [(ids, usage, records), ...] with logprobs=True; choice i is exactly what generate()
         returns for seeds[i] (None: seed + i)."""
@@ -420,7 +448,7 @@ class B200Model:
         mm, _keep = self._mm(data)
         _s, seeds_p = self._seeds(n, seeds)
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
         cap, k = max(max_tokens, 1), max(n, 1)
         out = (C.c_uint32 * (k * cap))()
         recs = (L.Logprobs * (k * cap))() if logprobs else None
@@ -461,13 +489,13 @@ class B200Model:
         self._check(self._lib.aha_b200_batch_close(self._h))
 
     def generate_stream(self, input_ids, on_token, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None,
-                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0):
+                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None):
         """generate_stream_generic: on_token(token, index) is called per generated token as its step completes; a truthy
         return value ends the request.  logprobs=True: on_token(token, index, record).  -> usage dict."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         flags = (L.GEN_REUSE_PREFIX if reuse_prefix else 0) | L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
         err = []
 
         def _cb(_user, token, index, *lp):
@@ -515,15 +543,18 @@ class B200Model:
         params = dict(temperature=temperature, top_p=top_p, top_k=top_k, repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n, seed=seed)
         return int(self.debug_sample_rows(logits, [params], [context], draw_index)["token"][0])
 
-    def debug_sample_rows(self, logits, params, contexts=None, draw_index=0, overwrite=False, kernel=0, act=None, on=None):
+    def debug_sample_rows(self, logits, params, contexts=None, draw_index=0, overwrite=False, kernel=0, act=None, on=None, fsm=None,
+                          constrained=None, fsm_states=None):
         """The device sampler on given logits, one call for len(params) rows (1 to 64; tests).
         logits: [V] (every row reads it) or [rows, ld] with V = ld.  params: per row a dict of generate()'s sampling keywords
         (temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed).  contexts: per row the tokens generated so far;
         draw_index: per row (or one for all) the draws already consumed.  overwrite: the last context token stands for the ArgMax token a
         decode step pushed; the sampled token replaces it.  kernel 0: sample_kernel per row; 1: sample_rows_kernel, row r as slot act[r]
         (default r), on: [64] flags per slot (default all on).
+        fsm: (offsets, tokens, next) of a token automaton (aha_b200_debug_sample_fsm); the rows with constrained[r] (default all) are
+        constrained by it from state fsm_states[r] (default 0).
         -> dict of uint32 arrays [rows]: token (0xffffffff where the row did not sample), state_token, n_hist, n_draws (the DecodeState
-        after the call) and last_hist (the last history word, 0xffffffff without a context)."""
+        after the call), last_hist (the last history word, 0xffffffff without a context) and, with fsm, fsm_state (after the call)."""
         rows = len(params)
         lg = np.ascontiguousarray(logits, np.float32)
         V, ld = (lg.size, 0) if lg.ndim == 1 else (lg.shape[1], lg.shape[1])
@@ -546,9 +577,20 @@ class B200Model:
         tok, state, hist = np.zeros(rows, np.uint32), np.zeros((rows, 3), np.uint32), np.zeros(rows, np.uint32)
         u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
         i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
-        self._check(self._lib.aha_b200_debug_sample(self._h, int(kernel), rows, V, lg.ctypes.data_as(C.POINTER(C.c_float)), ld, ps, u32(cat),
-                                                    u32(n_ctx), u32(draws), 1 if overwrite else 0, i32(act), i32(on), u32(tok), u32(state), u32(hist)))
-        return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist)
+        lg_p = lg.ctypes.data_as(C.POINTER(C.c_float))
+        if fsm is None:
+            self._check(self._lib.aha_b200_debug_sample(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
+                                                        1 if overwrite else 0, i32(act), i32(on), u32(tok), u32(state), u32(hist)))
+            return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist)
+        f, _keep = L.token_fsm(*fsm)
+        con = np.ascontiguousarray(np.broadcast_to(np.asarray(True if constrained is None else constrained, np.int32), (rows,)))
+        fin = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if fsm_states is None else fsm_states, np.uint32), (rows,)))
+        fout = np.zeros(rows, np.uint32)
+        self._check(self._lib.aha_b200_debug_sample_fsm(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
+                                                        1 if overwrite else 0, i32(act), i32(on), C.byref(f), i32(con), u32(fin), u32(tok),
+                                                        u32(state), u32(hist), u32(fout)))
+        return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist,
+                    fsm_state=fout)
 
     def debug_logprobs(self, logits, token, n_top=0):
         """The log-probability kernels on a given logits row of any length (tests) -> record dict."""

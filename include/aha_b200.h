@@ -97,6 +97,24 @@ typedef struct aha_gen_params {      /* ChatCompletionParameters subset used by 
                                   * Not masked: a count above AHA_MAX_TOP_LOGPROBS (or above the vocabulary) is refused, never wrapped.
                                   * Needs AHA_GEN_LOGPROBS. */
 #define AHA_MAX_TOP_LOGPROBS 20
+#define AHA_GEN_CONSTRAINED 16u  /* constrained decoding: params.reserved holds the id of a token automaton from aha_b200_fsm_create (read
+                                  * only when this flag is set).  Every drawn token, the first included, is drawn with the tokens the current
+                                  * state does not allow at logit -inf (before the repeat penalty, which leaves them there), and the state then
+                                  * follows the drawn token.  Log-probability records stay raw (taken before the mask).  Accepted by generate,
+                                  * generate_stream, generate_logprobs, generate_stream_logprobs, generate_batch, generate_n and the batch
+                                  * session entries; refused by generate_speculative, asr_generate and under tensor parallelism. */
+
+/* A token automaton (constrained decoding): a deterministic automaton over token ids, e.g. a grammar, regex or JSON schema compiled by
+ * the caller against its tokenizer.  State s allows tokens[offsets[s] .. offsets[s + 1]) (strictly ascending, at least one per state), and
+ * next[j] is the state after tokens[j].  A request starts in `start`; the automaton ends a request by allowing only a stop id (the first
+ * token is never EOS-checked, so a final state should loop on EOS). */
+typedef struct aha_token_fsm {
+    uint32_t n_states;            /* >= 1 */
+    uint32_t start;               /* < n_states */
+    const uint64_t* offsets;      /* [n_states + 1], offsets[0] = 0, non-decreasing, offsets[n_states] = the number of transitions */
+    const uint32_t* tokens;       /* strictly ascending within a state, each < the vocabulary */
+    const uint32_t* next;         /* next[j] = the state after tokens[j], < n_states */
+} aha_token_fsm;
 
 /* The log-probability record of one generated token (new design; the reference's responses carry `logprobs: None`).
  *   logprob = x[token] - (M + log sum_j exp(x[j] - M)), x = the fp32 logits row the step computed, M = its maximum: the model's own
@@ -440,6 +458,14 @@ int aha_b200_score_batch(aha_model* m, const uint32_t* ids, const size_t* lens, 
  * o_proj and down_proj. */
 int aha_b200_nccl_unique_id(uint8_t out[128]);
 
+/* Token automata (AHA_GEN_CONSTRAINED).  aha_b200_fsm_check (host only, no handle): 0 when `fsm` is well formed over a vocabulary of
+ * `vocab` tokens, else 1 with the reason in aha_b200_last_error(NULL).  aha_b200_fsm_create checks it against the handle's vocabulary and
+ * copies it to device memory: *id_out (>= 1) names it in params.reserved until aha_b200_fsm_destroy or aha_b200_destroy frees it.
+ * aha_b200_fsm_destroy refuses an id that a running batch slot uses. */
+int aha_b200_fsm_check(const aha_token_fsm* fsm, size_t vocab);
+int aha_b200_fsm_create(aha_model* m, const aha_token_fsm* fsm, uint32_t* id_out);
+int aha_b200_fsm_destroy(aha_model* m, uint32_t id);
+
 void aha_b200_destroy(aha_model* m);
 
 /* Host-only helper (no device work, usable without a GPU): Qwen3VLModel::get_rope_index, image branch
@@ -494,6 +520,13 @@ int aha_b200_decode_steps(aha_model* m, uint32_t first_token, size_t seqlen_offs
 int aha_b200_debug_sample(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
                           const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
                           const int32_t* on, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out);
+/* aha_b200_debug_sample with a token automaton (tests): `fsm` (checked against V) is copied to scratch of this call; row r is constrained
+ * by it when constrained[r] != 0, starting in state fsm_state_in[r], and fsm_state_out[r] receives its state after the call (the input
+ * state for an unconstrained row or one that did not sample). */
+int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                              const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                              const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
+                              uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out, uint32_t* fsm_state_out);
 /* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
 int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);
