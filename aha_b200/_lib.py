@@ -34,7 +34,7 @@ class GenParams(C.Structure):
                 ("flags", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX, GEN_LOGPROBS, GEN_CONSTRAINED = 1, 2, 4, 8, 16
+GEN_EOS_ON_FIRST, GEN_CONTINUE_RNG, GEN_REUSE_PREFIX, GEN_LOGPROBS, GEN_CONSTRAINED, GEN_LOGIT_RULES = 1, 2, 4, 8, 16, 32
 MAX_TOP_LOGPROBS = 20
 TOKEN_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32)
 
@@ -76,6 +76,23 @@ def token_fsm(offsets, tokens, next, start=0):
     ptr = lambda a, t: a.ctypes.data_as(C.POINTER(t)) if a.size else None
     f = TokenFsm(n_states=off.size - 1, start=int(start), offsets=ptr(off, C.c_uint64), tokens=ptr(tok, C.c_uint32), next=ptr(nxt, C.c_uint32))
     return f, (off, tok, nxt)
+
+
+class LogitRules(C.Structure):
+    _fields_ = [("presence_penalty", C.c_float), ("frequency_penalty", C.c_float), ("bias_ids", C.POINTER(C.c_uint32)),
+                ("bias_values", C.POINTER(C.c_float)), ("n_bias", C.c_size_t), ("fsm", C.c_uint32), ("reserved", C.c_uint32 * 3)]
+
+
+def logit_rules(presence_penalty=0.0, frequency_penalty=0.0, logit_bias=None, fsm=None):
+    """(LogitRules, arrays it points into).  logit_bias: OpenAI's map of token id (int or decimal string) -> bias, or (id, bias) pairs;
+    fsm: the id of a token automaton on the handle, or None.  The library checks ranges and ids (aha_b200_rules_check)."""
+    items = list((logit_bias or {}).items()) if isinstance(logit_bias, dict) else list(logit_bias or [])
+    ids = np.ascontiguousarray(np.array([int(k) for k, _ in items], np.int64).astype(np.uint32))
+    vals = np.ascontiguousarray(np.array([float(v) for _, v in items], np.float32))
+    ptr = lambda a, t: a.ctypes.data_as(C.POINTER(t)) if a.size else None
+    r = LogitRules(presence_penalty=float(presence_penalty), frequency_penalty=float(frequency_penalty), bias_ids=ptr(ids, C.c_uint32),
+                   bias_values=ptr(vals, C.c_float), n_bias=ids.size, fsm=0 if fsm is None else int(fsm))
+    return r, (ids, vals)
 
 
 class Logprobs(C.Structure):
@@ -215,6 +232,12 @@ SYMBOLS = {
                                         C.c_int, _I32P, _I32P, _U32P, _U32P, _U32P]),
     "aha_b200_debug_sample_fsm": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _F32P, C.c_size_t, C.POINTER(GenParams), _U32P, _U32P, _U32P,
                                             C.c_int, _I32P, _I32P, C.POINTER(TokenFsm), _I32P, _U32P, _U32P, _U32P, _U32P, _U32P]),
+    "aha_b200_debug_sample_rules": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _F32P, C.c_size_t, C.POINTER(GenParams), _U32P, _U32P, _U32P,
+                                              C.c_int, _I32P, _I32P, C.POINTER(TokenFsm), _I32P, _U32P, C.POINTER(LogitRules), _I32P, _U32P, _U32P,
+                                              _U32P, _U32P]),
+    "aha_b200_rules_check": (C.c_int, [C.POINTER(LogitRules), C.c_size_t]),
+    "aha_b200_rules_create": (C.c_int, [_P, C.POINTER(LogitRules), _U32P]),
+    "aha_b200_rules_destroy": (C.c_int, [_P, C.c_uint32]),
     "aha_b200_fsm_check": (C.c_int, [C.POINTER(TokenFsm), C.c_size_t]),
     "aha_b200_fsm_create": (C.c_int, [_P, C.POINTER(TokenFsm), _U32P]),
     "aha_b200_fsm_destroy": (C.c_int, [_P, C.c_uint32]),

@@ -103,6 +103,15 @@ struct aha_model {
     };
     std::map<uint32_t, Fsm> fsms;
     uint32_t next_fsm_id = 1;
+    // logit-rules objects (aha_b200_rules_create): id -> the penalties, one device allocation holding bias ids | values, and the automaton
+    // the object names (0: none)
+    struct Rules {
+        void* mem = nullptr;
+        LogitRulesDev dev;
+        uint32_t fsm = 0;
+    };
+    std::map<uint32_t, Rules> rules;
+    uint32_t next_rules_id = 1;
 };
 
 namespace {
@@ -435,19 +444,76 @@ TokenFsmDev fsm_upload(const aha_token_fsm& f, void* mem) {
     }
     return d;
 }
-// AHA_GEN_CONSTRAINED: the request's automaton (nullptr without the flag), refused where constrained decoding does not run
-const aha_model::Fsm* request_fsm(const aha_model* m, const aha_gen_params& p, const std::string& who) {
-    if (!(p.flags & AHA_GEN_CONSTRAINED)) return nullptr;
-    AHA_REQUIRE(m->text.tp_world == 1, who + "constrained decoding is single-GPU (under tensor parallelism the decode step holds only a vocabulary shard)");
-    const auto it = m->fsms.find(p.reserved);
-    AHA_REQUIRE(it != m->fsms.end(), who + "AHA_GEN_CONSTRAINED: no token automaton has id " + std::to_string(p.reserved) + " on this handle");
-    return &it->second;
+// Everything aha_logit_rules promises, checked on the host: the kernel scatters the bias by id unchecked and relies on distinct ids (one
+// thread per entry), and the ranges are OpenAI's.
+void rules_validate(const aha_logit_rules* r, size_t vocab) {
+    AHA_REQUIRE(r, "logit rules: rules is NULL");
+    auto in = [](float x, float lim) { return std::isfinite(x) && x >= -lim && x <= lim; };
+    AHA_REQUIRE(in(r->presence_penalty, 2.f), "logit rules: presence_penalty " + std::to_string(r->presence_penalty) + " is not a finite value in [-2, 2]");
+    AHA_REQUIRE(in(r->frequency_penalty, 2.f), "logit rules: frequency_penalty " + std::to_string(r->frequency_penalty) + " is not a finite value in [-2, 2]");
+    AHA_REQUIRE(r->reserved[0] == 0 && r->reserved[1] == 0 && r->reserved[2] == 0, "logit rules: reserved must be 0");
+    AHA_REQUIRE(r->n_bias <= vocab, "logit rules: n_bias " + std::to_string(r->n_bias) + " exceeds the vocabulary of " + std::to_string(vocab));
+    if (r->n_bias == 0) return;
+    AHA_REQUIRE(r->bias_ids && r->bias_values, "logit rules: bias_ids and bias_values are required when n_bias > 0");
+    std::vector<char> seen(vocab, 0);
+    for (size_t j = 0; j < r->n_bias; ++j) {
+        const uint32_t t = r->bias_ids[j];
+        AHA_REQUIRE(t < vocab, "logit rules: bias id " + std::to_string(t) + " is outside the vocabulary of " + std::to_string(vocab));
+        AHA_REQUIRE(!seen[t], "logit rules: bias id " + std::to_string(t) + " is listed twice");
+        seen[t] = 1;
+        AHA_REQUIRE(in(r->bias_values[j], 100.f), "logit rules: the bias of token " + std::to_string(t) + " (" + std::to_string(r->bias_values[j]) +
+                                                       ") is not a finite value in [-100, 100]");
+    }
 }
-// the request's sampler (make_sampler), constrained by its automaton when it asks
+// a validated rules object's bias list copied into `mem` (n_bias ids, then n_bias values)
+LogitRulesDev rules_upload(const aha_logit_rules& r, void* mem) {
+    LogitRulesDev d;
+    d.n_bias = (int)r.n_bias; d.presence = r.presence_penalty; d.frequency = r.frequency_penalty;
+    if (r.n_bias == 0) return d;
+    uint32_t* ids = static_cast<uint32_t*>(mem);
+    float* vals = reinterpret_cast<float*>(ids + r.n_bias);
+    AHA_CUDA_CHECK(cudaMemcpy(ids, r.bias_ids, r.n_bias * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    AHA_CUDA_CHECK(cudaMemcpy(vals, r.bias_values, r.n_bias * sizeof(float), cudaMemcpyHostToDevice));
+    d.ids = ids; d.vals = vals;
+    return d;
+}
+// What a request's AHA_GEN_CONSTRAINED / AHA_GEN_LOGIT_RULES resolve to on the handle: its automaton (directly, or the one its rules name)
+// and its rules, each with its id (0 and null: none).  Refused where neither runs.
+struct RequestRules {
+    const TokenFsmDev* fsm = nullptr;
+    uint32_t fsm_id = 0;
+    const LogitRulesDev* rules = nullptr;
+    uint32_t rules_id = 0;
+};
+RequestRules request_rules(const aha_model* m, const aha_gen_params& p, const std::string& who) {
+    RequestRules q;
+    const bool con = (p.flags & AHA_GEN_CONSTRAINED) != 0, lr = (p.flags & AHA_GEN_LOGIT_RULES) != 0;
+    if (!con && !lr) return q;
+    AHA_REQUIRE(!(con && lr), who + "AHA_GEN_CONSTRAINED and AHA_GEN_LOGIT_RULES exclude each other (params.reserved holds one id): name the "
+                                    "automaton in the logit-rules object (aha_logit_rules.fsm) instead");
+    uint32_t fsm_id = p.reserved;
+    if (lr) {
+        AHA_REQUIRE(m->text.tp_world == 1, who + "logit rules are single-GPU (under tensor parallelism the decode step holds only a vocabulary shard)");
+        const auto it = m->rules.find(p.reserved);
+        AHA_REQUIRE(it != m->rules.end(), who + "AHA_GEN_LOGIT_RULES: no logit-rules object has id " + std::to_string(p.reserved) + " on this handle");
+        q.rules = &it->second.dev;
+        q.rules_id = p.reserved;
+        fsm_id = it->second.fsm;
+        if (fsm_id == 0) return q;
+    }
+    AHA_REQUIRE(m->text.tp_world == 1, who + "constrained decoding is single-GPU (under tensor parallelism the decode step holds only a vocabulary shard)");
+    const auto it = m->fsms.find(fsm_id);
+    AHA_REQUIRE(it != m->fsms.end(), who + "AHA_GEN_CONSTRAINED: no token automaton has id " + std::to_string(fsm_id) + " on this handle");
+    q.fsm = &it->second.dev;
+    q.fsm_id = fsm_id;
+    return q;
+}
+// the request's sampler (make_sampler), constrained by its automaton and transformed by its logit rules when it asks
 Sampler request_sampler(const aha_model* m, const aha_gen_params& p, const std::string& who) {
-    const aha_model::Fsm* f = request_fsm(m, p, who);
-    Sampler s = make_sampler(p, m->text.cfg.V, f ? &f->dev : nullptr);
-    if (f) s.fsm_id = p.reserved;
+    const RequestRules q = request_rules(m, p, who);
+    Sampler s = make_sampler(p, m->text.cfg.V, q.fsm, q.rules);
+    s.fsm_id = q.fsm_id;
+    s.rules_id = q.rules_id;
     return s;
 }
 
@@ -884,7 +950,7 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
                    aha_usage* usage, size_t* n_generated, int lp_n = -1) {
     TextModel& T = m->text;
     require_no_session(m);
-    request_fsm(m, params, "");
+    request_rules(m, params, "");
     const bool lp = lp_n >= 0;
     request_logprobs(m, lp_n);
     const size_t sample_len = token_budget(params);
@@ -992,6 +1058,9 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
                 who + "REUSE_PREFIX, CONTINUE_RNG and EOS_ON_FIRST are not supported with speculative decoding");
     AHA_REQUIRE((params.flags & AHA_GEN_CONSTRAINED) == 0,
                 who + "AHA_GEN_CONSTRAINED is not supported with speculative decoding (a verify row's mask would depend on the drafts before it)");
+    AHA_REQUIRE(request_rules(m, params, who).fsm == nullptr,
+                who + "logit rules that name a token automaton are not supported with speculative decoding (a verify row's mask would depend on "
+                      "the drafts before it)");
     const int lp_n = logprob_request(params, T, who);
     AHA_REQUIRE(lp_n < 0 || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
     const size_t sample_len = token_budget(params);
@@ -1006,7 +1075,7 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
     drop_cache(m);
     m->last_prefix_hit = 0;
     RequestReset reset{m};
-    const Sampler samp = make_sampler(params, T.cfg.V);
+    const Sampler samp = request_sampler(m, params, who);
     const uint32_t tok = first_token(m, T.table, ids, seq_len, 0, mm, samp, 0);
     if (lp_n >= 0) T.logprobs(true, T.d_lp, true);   // record 0, from the prefill logits
     const auto t1 = clk::now();
@@ -1155,7 +1224,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         lp_n[i] = logprob_request(r.params, T, who + "request " + std::to_string(i) + ": ");
         for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
         AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-        request_fsm(m, r.params, who + "request " + std::to_string(i) + ": ");
+        request_rules(m, r.params, who + "request " + std::to_string(i) + ": ");
         require_mm_arity(m, r.mm);
         sample_len[i] = token_budget(r.params);
         pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
@@ -1277,7 +1346,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     const int lp_n = logprob_request(req.params, T, who);
     for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
     AHA_REQUIRE((req.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-    request_fsm(m, req.params, who);
+    request_rules(m, req.params, who);
     require_mm_arity(m, req.mm);
     const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len;
     AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
@@ -1609,9 +1678,50 @@ int aha_b200_fsm_destroy(aha_model* m, uint32_t id) {
         for (int i = 0; m->session.open && i < m->session.width; ++i)
             AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].fsm_id == id),
                         "fsm_destroy: token automaton " + std::to_string(id) + " constrains the running request in slot " + std::to_string(i));
+        for (const auto& r : m->rules)
+            AHA_REQUIRE(r.second.fsm != id, "fsm_destroy: token automaton " + std::to_string(id) + " is named by logit-rules object " +
+                                                std::to_string(r.first) + " (destroy that first)");
         AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         AHA_CUDA_CHECK(cudaFree(it->second.mem));
         m->fsms.erase(it);
+    });
+}
+
+int aha_b200_rules_check(const aha_logit_rules* r, size_t vocab) {
+    return guarded_host([&] { rules_validate(r, vocab); });
+}
+
+int aha_b200_rules_create(aha_model* m, const aha_logit_rules* r, uint32_t* id_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(id_out, "rules_create: id_out is required");
+        rules_validate(r, (size_t)m->text.cfg.V);
+        AHA_REQUIRE(r->fsm == 0 || m->fsms.count(r->fsm), "rules_create: no token automaton has id " + std::to_string(r->fsm) + " on this handle");
+        AHA_REQUIRE(m->next_rules_id != 0, "rules_create: the handle has used every logit-rules id");
+        aha_model::Rules x;
+        x.fsm = r->fsm;
+        if (r->n_bias) AHA_CUDA_CHECK(cudaMalloc(&x.mem, r->n_bias * (sizeof(uint32_t) + sizeof(float))));
+        try {
+            x.dev = rules_upload(*r, x.mem);
+        } catch (...) {
+            cudaFree(x.mem);
+            throw;
+        }
+        const uint32_t id = m->next_rules_id++;
+        m->rules[id] = x;
+        *id_out = id;
+    });
+}
+
+int aha_b200_rules_destroy(aha_model* m, uint32_t id) {
+    return guarded(m, [&] {
+        const auto it = m->rules.find(id);
+        AHA_REQUIRE(it != m->rules.end(), "rules_destroy: no logit-rules object has id " + std::to_string(id) + " on this handle");
+        for (int i = 0; m->session.open && i < m->session.width; ++i)
+            AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].rules_id == id),
+                        "rules_destroy: logit-rules object " + std::to_string(id) + " applies to the running request in slot " + std::to_string(i));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+        if (it->second.mem) AHA_CUDA_CHECK(cudaFree(it->second.mem));
+        m->rules.erase(it);
     });
 }
 
@@ -1917,6 +2027,7 @@ int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_ch
         AHA_REQUIRE(chunks && n_chunks >= 1 && params && out_tokens && n_out, "chunks, params, out_tokens and n_out are required");
         refuse_logprobs(*params, "asr_generate", "aha_b200_generate_logprobs on each chunk's prompt");
         AHA_REQUIRE((params->flags & AHA_GEN_CONSTRAINED) == 0, "asr_generate: AHA_GEN_CONSTRAINED is not supported on the ASR loop");
+        AHA_REQUIRE((params->flags & AHA_GEN_LOGIT_RULES) == 0, "asr_generate: AHA_GEN_LOGIT_RULES is not supported on the ASR loop");
         if (usage) *usage = aha_usage{};
         // Qwen3AsrGenerateModel::generate (qwen3_asr/generate.rs:130-186): ONE LogitsProcessor for the whole request (its RNG
         // stream runs on across the chunks), no repeat penalty, every token -- the first included -- is EOS-checked, the KV
@@ -1955,6 +2066,15 @@ int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, c
                               const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
                               const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
                               uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out, uint32_t* fsm_state_out) {
+    return aha_b200_debug_sample_rules(m, kernel, rows, V, logits, ld, params, context, n_context, draw_index, overwrite, act, on, fsm, constrained,
+                                       fsm_state_in, nullptr, nullptr, token_out, state_out, hist_out, fsm_state_out);
+}
+
+int aha_b200_debug_sample_rules(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                                const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                                const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
+                                const aha_logit_rules* rules, const int32_t* ruled, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out,
+                                uint32_t* fsm_state_out) {
     return guarded(m, [&] {
         AHA_REQUIRE(logits && params && n_context && draw_index && token_out && state_out && hist_out,
                     "logits, params, n_context, draw_index, token_out, state_out and hist_out are required");
@@ -1980,16 +2100,26 @@ int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, c
         if (fsm) fsm_validate(fsm, V);
         for (size_t r = 0; fsm && r < rows; ++r)
             AHA_REQUIRE(!constrained[r] || fsm_state_in[r] < fsm->n_states, "row " + std::to_string(r) + ": fsm_state_in is not below n_states");
+        AHA_REQUIRE(!rules || ruled, "logit rules need ruled");
+        if (rules) {
+            rules_validate(rules, V);
+            AHA_REQUIRE(rules->fsm == 0, "the automaton of a debug call is passed as fsm, not named in rules");
+        }
         Scratch mem;
         TokenFsmDev dev;
         if (fsm) dev = fsm_upload(*fsm, mem.alloc<char>(fsm_bytes(*fsm)));
+        LogitRulesDev rdev;
+        if (rules) rdev = rules_upload(*rules, mem.alloc<char>(std::max<size_t>(1, rules->n_bias * (sizeof(uint32_t) + sizeof(float)))));
+        int* d_cnt = rules ? mem.alloc<int>(rows * V) : nullptr;       // row r's count row
         std::vector<SampleArgs> args(kSampleMaxRows, SampleArgs{});
         for (size_t r = 0; r < rows; ++r) {
-            const Sampler s = make_sampler(params[r], (int)V, fsm && constrained[r] ? &dev : nullptr);
+            const Sampler s = make_sampler(params[r], (int)V, fsm && constrained[r] ? &dev : nullptr, rules && ruled[r] ? &rdev : nullptr);
             AHA_REQUIRE(s.active, "row " + std::to_string(r) + ": plain ArgMax needs no sampler (temperature < 1e-7 and no repeat penalty)");
             args[slot[r]] = s.args;
+            if (s.counts) args[slot[r]].cnt = d_cnt + r * V;
         }
         cudaStream_t st = m->ctx.stream;
+        if (d_cnt) AHA_CUDA_CHECK(cudaMemsetAsync(d_cnt, 0, rows * V * sizeof(int), st));
         const size_t n_logits = ld ? rows * ld : V;
         float* d_logits = mem.alloc<float>(n_logits);
         float* d_work = mem.alloc<float>(rows * V);
@@ -2032,8 +2162,13 @@ int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, c
         AHA_CUDA_CHECK(cudaMemcpyAsync(hs.data(), d_st, rows * sizeof(DecodeState), cudaMemcpyDeviceToHost, st));
         AHA_CUDA_CHECK(cudaMemcpyAsync(hh.data(), d_hist, hh.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
         AHA_CUDA_CHECK(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, st));
+        std::vector<int> cnt_after(d_cnt ? rows * V : 0);
+        if (d_cnt) AHA_CUDA_CHECK(cudaMemcpyAsync(cnt_after.data(), d_cnt, rows * V * sizeof(int), cudaMemcpyDeviceToHost, st));
         AHA_CUDA_CHECK(cudaStreamSynchronize(st));
         if (err) throw std::runtime_error(kSampleWeightsError);
+        for (size_t i = 0; i < cnt_after.size(); ++i)
+            AHA_REQUIRE(cnt_after[i] == 0, "row " + std::to_string(i / V) + ": the sampler left count " + std::to_string(cnt_after[i]) + " for token " +
+                                               std::to_string(i % V) + " (count rows must be zero after every draw)");
         for (size_t r = 0; r < rows; ++r) {
             state_out[3 * r] = hs[r].token; state_out[3 * r + 1] = (uint32_t)hs[r].n_hist; state_out[3 * r + 2] = hs[r].n_draws;
             hist_out[r] = n_context[r] ? hh[r * cap + n_context[r] - 1] : 0xffffffffu;
@@ -2880,6 +3015,7 @@ void aha_b200_destroy(aha_model* m) {
     m->wide_batch.graphs.clear();
     m->spec.destroy();
     for (auto& f : m->fsms) cudaFree(f.second.mem);
+    for (auto& r : m->rules) cudaFree(r.second.mem);
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
     if (m->h_lp_pin) cudaFreeHost(m->h_lp_pin);

@@ -39,6 +39,7 @@ struct BatchSlot {                       // one sequence of the batch
     SampleArgs samp{};                   // sampler of the request with the pointers of this slot
     int lp = 0;                          // 0: the request asked for no log-probabilities, else 1 + its top count
     uint32_t fsm_id = 0;                 // the token automaton the request is constrained by (0: none); it cannot be destroyed while the slot runs
+    uint32_t rules_id = 0;               // the request's logit-rules object (0: none); it cannot be destroyed while the slot runs
 };
 
 struct BatchDecoder {
@@ -56,6 +57,7 @@ struct BatchDecoder {
     SampleArgs* d_samp = nullptr;        // [cap] per-slot sampler arguments
     int* d_samp_on = nullptr;            // [cap]
     float* workb = nullptr;              // [cap][V] sampler scratch, one row per slot (the rows sample concurrently)
+    int* cntb = nullptr;                 // [cap][V] count rows of frequency / presence penalties, allocated when a request of the handle first asks
     // log-probabilities (logprobs.cuh), allocated when a request of the session first asks: per slot the on flag and the record of its
     // latest token; the candidate lists of every row
     int* d_lp_on = nullptr;              // [cap] BatchSlot::lp
@@ -174,7 +176,14 @@ struct BatchDecoder {
         BatchSlot& sl = slots[i];
         sl.samp_active = s.active;
         sl.fsm_id = s.fsm_id;
-        if (s.active) sl.samp = T->bind_sampler(s, d_states + i, d_hist + (size_t)i * T->hist_cap, d_tok + i, workb + (size_t)i * T->cfg.V);
+        sl.rules_id = s.rules_id;
+        if (s.active) sl.samp = T->bind_sampler(s, d_states + i, d_hist + (size_t)i * T->hist_cap, d_tok + i, workb + (size_t)i * T->cfg.V, counts(s, i));
+    }
+    // slot i's count row when the request has frequency or presence penalties (else null)
+    int* counts(const Sampler& s, int i) {
+        if (!s.counts) return nullptr;
+        if (!cntb) cntb = T->alloc_counts(cap);
+        return cntb + (size_t)i * T->cfg.V;
     }
 
     // the device copy of the composition `act`: attention table, active list and every slot's sampler arguments

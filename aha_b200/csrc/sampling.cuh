@@ -50,6 +50,14 @@ struct SampleArgs {
     const uint64_t* fsm_off;
     const uint32_t* fsm_tok;
     const uint32_t* fsm_next;
+    // logit rules (aha_b200_rules_create): bias_vals[j] is added to the logit of bias_ids[j] (distinct ids); with a count row `cnt` ([V],
+    // zero between draws; null: no penalties), every token generated before this draw loses frequency per occurrence and presence once
+    const uint32_t* bias_ids;
+    const float* bias_vals;
+    int n_bias;
+    float presence;
+    float frequency;
+    int* cnt;
 };
 
 // ---- StdRng: ChaCha12 block `counter` of the stream keyed by `key`, word `w` (rand_chacha: 64-bit counter in words 12-13, stream 0)
@@ -168,6 +176,15 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
         for (uint64_t j = f0 + tid; j < f1; j += kSampleThreads) { const uint32_t t = a.fsm_tok[j]; p[t] = a.logits[t]; }
     }
     __syncthreads();
+    // ---- logit bias: one fp32 add per listed token (a masked entry stays -inf: the values are finite)
+    if (a.n_bias > 0) {
+        for (int j = tid; j < a.n_bias; j += kSampleThreads) { const uint32_t t = a.bias_ids[j]; p[t] = __fadd_rn(p[t], a.bias_vals[j]); }
+        __syncthreads();
+    }
+    // occurrence counts of the generated tokens, scattered now and consumed after the repeat penalty (frequency / presence)
+    const bool counts = a.cnt != nullptr && n_ctx > 0;
+    if (counts)
+        for (int t = tid; t < n_ctx; t += kSampleThreads) { const uint32_t tok = a.history[t]; if (tok < (uint32_t)V) atomicAdd(&a.cnt[tok], 1); }
     // ---- penalised logits (use_repeat_penalty: every distinct token of the last `last_n` generated ones, once; a masked entry stays -inf)
     if (!(a.penalty == 1.0f || a.last_n == 0) && n_ctx > 0) {
         const int start = max(0, n_ctx - a.last_n);
@@ -179,6 +196,18 @@ __device__ __forceinline__ void sample_dev(const SampleArgs& a, SampleSmem& s) {
                 const float x = p[tok];
                 if (!(fsm && x == -INFINITY)) p[tok] = x >= 0.f ? x / a.penalty : x * a.penalty;
             }
+        }
+        __syncthreads();
+    }
+    // ---- frequency and presence: the first position to take a token's count applies y - c * frequency - presence once (product and
+    // differences rounded separately, as the oracle states them), and the exchange leaves the count row zero for the next draw
+    if (counts) {
+        __syncthreads();
+        for (int t = tid; t < n_ctx; t += kSampleThreads) {
+            const uint32_t tok = a.history[t];
+            if (tok >= (uint32_t)V) continue;
+            const int c = atomicExch(&a.cnt[tok], 0);
+            if (c > 0) p[tok] = __fsub_rn(__fsub_rn(p[tok], __fmul_rn((float)c, a.frequency)), a.presence);
         }
         __syncthreads();
     }
@@ -393,6 +422,8 @@ struct Sampler {
     SampleArgs args{};
     uint32_t fsm_start = 0;      // the automaton's start state: a first token is drawn from it
     uint32_t fsm_id = 0;         // the automaton's id on the handle (0: unconstrained)
+    uint32_t rules_id = 0;       // the logit-rules object's id on the handle (0: none)
+    bool counts = false;         // frequency or presence penalty: the row it is bound to needs a count row
 };
 
 // a token automaton in device memory (aha_b200_fsm_create)
@@ -403,15 +434,25 @@ struct TokenFsmDev {
     uint32_t start = 0;
 };
 
+// the logit rules of a request with the bias list in device memory (aha_b200_rules_create)
+struct LogitRulesDev {
+    const uint32_t* ids = nullptr;
+    const float* vals = nullptr;
+    int n_bias = 0;
+    float presence = 0.f;
+    float frequency = 0.f;
+};
+
 // get_logit_processor (sample.rs:7-38): the Sampling a request's parameters select, checked against what the device sampler supports
-// A constrained request (fsm != null) always samples on the device, greedy included: ArgMax over its allowed tokens.
-inline Sampler make_sampler(const aha_gen_params& p, int V, const TokenFsmDev* fsm = nullptr) {
+// A constrained request (fsm != null) or one with logit rules always samples on the device, greedy included: ArgMax over its
+// allowed tokens and transformed logits.
+inline Sampler make_sampler(const aha_gen_params& p, int V, const TokenFsmDev* fsm = nullptr, const LogitRulesDev* rules = nullptr) {
     const bool has_t = !(p.temperature < 1e-7f);
     const bool has_k = p.top_k > 0, has_p = p.top_p > 0.f;
     const int mode = !has_t ? SAMPLE_ARGMAX : !has_k ? (has_p ? SAMPLE_TOPP : SAMPLE_ALL) : (has_p ? SAMPLE_TOPK_TOPP : SAMPLE_TOPK);
     const bool pen = !(p.repeat_penalty == 1.0f || p.repeat_last_n == 0);
     Sampler s;
-    s.active = mode != SAMPLE_ARGMAX || pen || fsm != nullptr;
+    s.active = mode != SAMPLE_ARGMAX || pen || fsm != nullptr || rules != nullptr;
     if (!s.active) return s;
     AHA_REQUIRE(V <= kSampleThreads * kSampleChunk, "vocabulary too large for the device sampler");
     AHA_REQUIRE(!(mode == SAMPLE_TOPK || mode == SAMPLE_TOPK_TOPP) || p.top_k >= 1, "top_k must be >= 1");
@@ -422,6 +463,12 @@ inline Sampler make_sampler(const aha_gen_params& p, int V, const TokenFsmDev* f
     a.inv_temp = mode == SAMPLE_ARGMAX ? 1.0f : (float)(1.0 / (double)p.temperature);
     a.top_p = p.top_p; a.top_k = p.top_k; a.penalty = p.repeat_penalty; a.last_n = p.repeat_last_n;
     if (fsm) { a.fsm_off = fsm->off; a.fsm_tok = fsm->tok; a.fsm_next = fsm->next; s.fsm_start = fsm->start; }
+    if (rules) {
+        a.bias_ids = rules->ids; a.bias_vals = rules->vals; a.n_bias = rules->n_bias;
+        a.presence = rules->presence; a.frequency = rules->frequency;
+        // both zero: y - fl(c * 0) - 0 = y, so the counting pass is skipped and no count row is needed
+        s.counts = rules->presence != 0.f || rules->frequency != 0.f;
+    }
     // rand_core::SeedableRng::seed_from_u64: eight PCG32 outputs fill the 32-byte ChaCha seed
     uint64_t stt = p.seed;
     for (int i = 0; i < 8; ++i) {

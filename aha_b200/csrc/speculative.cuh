@@ -377,8 +377,9 @@ struct SpecDecoder {
         std::vector<SampleArgs> rows(kSpecMaxRows);
         for (int r = 0; r < kSpecMaxRows; ++r) {
             act[r] = r;
-            // the request's sampler on every row; the shared history holds the emitted tokens followed by the drafts
-            if (samp.active) rows[r] = T->bind_sampler(samp, B->d_states + r, T->d_history, B->d_tok + r, B->workb + (size_t)r * T->cfg.V);
+            // the request's sampler on every row; the shared history holds the emitted tokens followed by the drafts, so row r's counts
+            // (frequency / presence, each row its own count row) cover the context a sequential decode would see at that draw
+            if (samp.active) rows[r] = T->bind_sampler(samp, B->d_states + r, T->d_history, B->d_tok + r, B->workb + (size_t)r * T->cfg.V, B->counts(samp, r));
         }
         if (!h.empty()) AHA_CUDA_CHECK(cudaMemcpyAsync(d_buf, h.data(), h.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_ctl, &s, sizeof(s), cudaMemcpyHostToDevice, c.stream));

@@ -515,6 +515,7 @@ struct TextModel {
     SampleArgs samp{};
     float* sample_work = nullptr;
     int* d_sample_err = nullptr;
+    int* sample_counts = nullptr;    // [V] count row of the model's own sampler (alloc_counts)
 
     // log-probability records of the request (logprobs.cuh), allocated the first time a request asks: d_lp_on = 1 + its top count,
     // d_lp[i] = the record of generated token i
@@ -970,12 +971,15 @@ struct TextModel {
     }
     // ---- sampler (sampling.cuh: make_sampler)
     // the request's sampler on one row: its state, repeat-penalty history, token and [V] scratch row.  Every row samples the model's logits
-    // unless its kernel points it elsewhere, and raises the handle's one error flag.
-    SampleArgs bind_sampler(const Sampler& s, DecodeState* st, uint32_t* history, uint32_t* token_out, float* work) {
+    // unless its kernel points it elsewhere, and raises the handle's one error flag.  `cnt`: the row's zeroed count row of V entries, used
+    // when the request has frequency or presence penalties (Sampler::counts).
+    SampleArgs bind_sampler(const Sampler& s, DecodeState* st, uint32_t* history, uint32_t* token_out, float* work, int* cnt) {
         alloc_sampler();
         SampleArgs a = s.args;
         a.logits = logits; a.work = work;
         a.st = st; a.history = history; a.hist_cap = hist_cap; a.token_out = token_out; a.error = d_sample_err;
+        AHA_REQUIRE(!s.counts || cnt, "sampler: a request with frequency or presence penalties needs a count row");
+        a.cnt = s.counts ? cnt : nullptr;
         return a;
     }
     // the sampler of the model's own decode loop
@@ -983,7 +987,15 @@ struct TextModel {
         samp_active = s.active;
         if (!samp_active) return;
         alloc_sampler();
-        samp = bind_sampler(s, d_state, d_history, d_argmax, sample_work);
+        if (s.counts && !sample_counts) sample_counts = alloc_counts(1);
+        samp = bind_sampler(s, d_state, d_history, d_argmax, sample_work, sample_counts);
+    }
+    // zeroed count rows [rows][V] (frequency / presence penalties); the sampler leaves them zero after every draw.  Allocated the first time a
+    // request with penalties arrives, so a handle that never sees one holds none.
+    int* alloc_counts(int rows) {
+        int* p = ctx->alloc<int>((size_t)rows * cfg.V);
+        AHA_CUDA_CHECK(cudaMemset(p, 0, (size_t)rows * cfg.V * sizeof(int)));
+        return p;
     }
     void alloc_sampler() {
         if (sample_work) return;

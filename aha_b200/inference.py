@@ -63,6 +63,15 @@ def prefix_match(cached_ids, ids, mm_token_ids=(), same_mm=True):
     return int(lib.aha_b200_prefix_match(u32(a), a.size, u32(b), b.size, u32(t), t.size, 1 if same_mm else 0))
 
 
+def rules_check(presence_penalty=0.0, frequency_penalty=0.0, logit_bias=None, vocab_size=None):
+    """Check a logit-rules object (OpenAI presence_penalty, frequency_penalty, logit_bias) the way rules_create checks it, over a
+    vocabulary of vocab_size tokens (host only, aha_b200_rules_check).  Raises B200Error."""
+    lib = L.load()
+    r, _keep = L.logit_rules(presence_penalty, frequency_penalty, logit_bias)
+    if lib.aha_b200_rules_check(C.byref(r), int(vocab_size)) != 0:
+        raise B200Error(lib.aha_b200_last_error(None).decode())
+
+
 def fsm_check(offsets, tokens, next, start=0, vocab_size=None):
     """Check a token automaton (CSR: state s allows tokens[offsets[s]:offsets[s + 1]], next[j] follows tokens[j]) the way
     fsm_create checks it, over a vocabulary of vocab_size tokens (host only, aha_b200_fsm_check).  Raises B200Error."""
@@ -190,13 +199,17 @@ class B200Model:
 
     # ------------------------------------------------------------------ generate_generic / generate_stream_generic
     @staticmethod
-    def _gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags=0, fsm=None):
-        """fsm: the id of a token automaton (fsm_create) that constrains the request (AHA_GEN_CONSTRAINED), or None"""
+    def _gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags=0, fsm=None, rules=None):
+        """fsm: the id of a token automaton (fsm_create) that constrains the request (AHA_GEN_CONSTRAINED), or None.
+        rules: the id of a logit-rules object (rules_create, AHA_GEN_LOGIT_RULES), or None.  params.reserved holds one id: with both,
+        the library refuses the request (an automaton goes into the rules object instead)."""
         if fsm is not None:
             flags |= L.GEN_CONSTRAINED
+        if rules is not None:
+            flags |= L.GEN_LOGIT_RULES
         return L.GenParams(temperature=temperature or 0.0, repeat_penalty=repeat_penalty, repeat_last_n=repeat_last_n,
                            max_tokens=max_tokens, seed=seed, top_p=top_p or 0.0, top_k=top_k or 0, flags=flags,
-                           reserved=0 if fsm is None else int(fsm))
+                           reserved=int(rules) if rules is not None else (0 if fsm is None else int(fsm)))
 
     @staticmethod
     def _usage(u):
@@ -204,19 +217,20 @@ class B200Model:
                     completion_secs=u.completion_secs, vision_secs=u.vision_secs)
 
     def generate(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None):
+                 repeat_last_n=64, seed=299792458, flags=0, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None, rules=None):
         """-> (generated ids, usage dict).  temperature < 1e-7: ArgMax; else the device sampler (TopK / TopKThenTopP / TopP /
         All exactly as get_logit_processor picks them from temperature, top_p, top_k).  reuse_prefix: keep this request's K/V
         and prefill only what follows the prefix shared with the cache (multi-turn chats; same tokens as without it).
         logprobs=True (aha_b200_generate_logprobs): -> (ids, usage, records), one record dict per token (token, index, logprob,
         top_ids, top_logprobs with top_logprobs alternatives; raw model log-probabilities, before penalty and temperature).
-        fsm: the id of a token automaton (fsm_create); every token is drawn from the tokens its current state allows."""
+        fsm: the id of a token automaton (fsm_create); every token is drawn from the tokens its current state allows.
+        rules: the id of a logit-rules object (rules_create): logit bias, frequency and presence penalties on every draw."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         if reuse_prefix:
             flags |= L.GEN_REUSE_PREFIX
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm, rules)
         cap = max(max_tokens, 1)
         out = (C.c_uint32 * cap)()
         n = C.c_size_t(0)
@@ -231,16 +245,17 @@ class B200Model:
 
     def generate_speculative(self, input_ids, data=None, prediction=None, prompt_lookup=False, max_draft=7, ngram=3, max_tokens=1024,
                              temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64, seed=299792458, flags=0,
-                             logprobs=False, top_logprobs=0):
+                             logprobs=False, top_logprobs=0, rules=None):
         """Speculative decoding of one request (aha_b200_generate_speculative): verify passes of max_draft + 1 rows, drafted from
         `prediction` (token ids the answer will largely repeat) and, with prompt_lookup, from the prompt and the output so far.
         -> (ids, usage, stats) with stats = dict(passes, drafted, accepted); (ids, usage, stats, records) with logprobs=True.
-        The ids and records do not depend on the drafts; they follow the model as wide batch sessions do."""
+        The ids and records do not depend on the drafts; they follow the model as wide batch sessions do.  rules: a logit-rules id whose
+        object names no automaton."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         sp, _pred = L.spec_params(prediction, prompt_lookup, max_draft, ngram, self.vocab_size)
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, rules=rules)
         cap = max(max_tokens, 1)
         out = (C.c_uint32 * cap)()
         recs = (L.Logprobs * cap)() if logprobs else None
@@ -327,7 +342,7 @@ class B200Model:
 
     def generate_batch(self, requests):
         """Static batching (aha_b200_generate_batch): requests = [dict(input_ids=..., data=None, max_tokens=..., temperature=..., top_p=...,
-        top_k=..., repeat_penalty=..., repeat_last_n=..., seed=..., fsm=...), ...] (at most 8) decoded in lockstep on this handle.
+        top_k=..., repeat_penalty=..., repeat_last_n=..., seed=..., fsm=..., rules=...), ...] (at most 8) decoded in lockstep on this handle.
         -> [(generated ids, usage dict), ...]: per request exactly what generate() returns for it alone."""
         n = len(requests)
         arr, _keep = self._batch_requests(requests)
@@ -352,7 +367,7 @@ class B200Model:
             flags = r.get("flags", 0) | L.logprob_flags(r.get("logprobs", False), r.get("top_logprobs", 0), self.vocab_size)
             arr[i].params = self._gen_params(r.get("max_tokens", 1024), r.get("temperature", 0.0), r.get("top_p"), r.get("top_k"),
                                              r.get("repeat_penalty", 1.0), r.get("repeat_last_n", 64), r.get("seed", 299792458), flags,
-                                             r.get("fsm"))
+                                             r.get("fsm"), r.get("rules"))
         return arr, keep
 
     # ---- constrained decoding: token automata on the handle
@@ -365,8 +380,22 @@ class B200Model:
         return int(i.value)
 
     def fsm_destroy(self, fsm):
-        """Free a token automaton (refused while a running batch slot uses it)."""
+        """Free a token automaton (refused while a running batch slot uses it or a logit-rules object names it)."""
         self._check(self._lib.aha_b200_fsm_destroy(self._h, int(fsm)))
+
+    # ---- OpenAI presence_penalty / frequency_penalty / logit_bias: logit-rules objects on the handle
+    def rules_create(self, presence_penalty=0.0, frequency_penalty=0.0, logit_bias=None, fsm=None):
+        """A logit-rules object (aha_b200_rules_create) -> its id, the `rules` argument of the generation entries.  Penalties in [-2, 2];
+        logit_bias: {token id (int or decimal string): bias in [-100, 100]} or (id, bias) pairs; fsm: a token automaton id (fsm_create)
+        that constrains the request too."""
+        r, _keep = L.logit_rules(presence_penalty, frequency_penalty, logit_bias, fsm)
+        i = C.c_uint32(0)
+        self._check(self._lib.aha_b200_rules_create(self._h, C.byref(r), C.byref(i)))
+        return int(i.value)
+
+    def rules_destroy(self, rules):
+        """Free a logit-rules object (refused while a running batch slot uses it)."""
+        self._check(self._lib.aha_b200_rules_destroy(self._h, int(rules)))
 
     # ---- continuous batching: requests join / leave a running batch between steps (aha_b200_batch_open / _add / _step / _close)
     def batch_open(self):
@@ -379,7 +408,7 @@ class B200Model:
         self._batch_width = int(max_seqs)
 
     def batch_add(self, input_ids, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64,
-                  seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None):
+                  seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None, rules=None):
         """Prefill one request into a free slot -> (slot, first token, finished).  logprobs / top_logprobs: batch_logprobs() holds the
         record of each token it delivers."""
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
@@ -389,7 +418,7 @@ class B200Model:
         req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
         req.seq_len = ids.size
         req.mm = C.pointer(mm) if mm is not None else None
-        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm, rules)
         slot, fin, tok = C.c_int32(-1), C.c_int32(0), C.c_uint32(0)
         u = L.Usage()
         self._check(self._lib.aha_b200_batch_add(self._h, C.byref(req), C.byref(slot), C.byref(tok), C.byref(fin), C.byref(u)))
@@ -417,7 +446,7 @@ class B200Model:
         return s, s.ctypes.data_as(C.POINTER(C.c_uint64))
 
     def batch_add_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                    repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, return_usage=False, fsm=None):
+                    repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, return_usage=False, fsm=None, rules=None):
         """OpenAI `n` (aha_b200_batch_add_n): n choices of one request in the n lowest free slots, the prompt prefilled once and its K/V
         copied into every other choice's own pages.  Choice i samples with seeds[i] (None: seed + i) and yields exactly what batch_add
         yields for the request with that seed.  All or nothing.  -> [(slot, first token, finished), ...] per choice, and with
@@ -431,7 +460,7 @@ class B200Model:
         req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
         req.seq_len = ids.size
         req.mm = C.pointer(mm) if mm is not None else None
-        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm, rules)
         k = max(n, 1)
         slots, toks, fins, us = (C.c_int32 * k)(), (C.c_uint32 * k)(), (C.c_int32 * k)(), (L.Usage * k)()
         self._check(self._lib.aha_b200_batch_add_n(self._h, C.byref(req), n, seeds_p, slots, toks, fins, us))
@@ -439,7 +468,7 @@ class B200Model:
         return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
 
     def generate_n(self, input_ids, n, seeds=None, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0,
-                   repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None):
+                   repeat_last_n=64, seed=299792458, flags=0, logprobs=False, top_logprobs=0, fsm=None, rules=None):
         """OpenAI `n` in one call (aha_b200_generate_n, 1 <= n <= 8): the prompt prefilled once, the choices decoded in lockstep.
         -> [(ids, usage), ...] per choice, [(ids, usage, records), ...] with logprobs=True; choice i is exactly what generate()
         returns for seeds[i] (None: seed + i)."""
@@ -448,7 +477,7 @@ class B200Model:
         mm, _keep = self._mm(data)
         _s, seeds_p = self._seeds(n, seeds)
         flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm, rules)
         cap, k = max(max_tokens, 1), max(n, 1)
         out = (C.c_uint32 * (k * cap))()
         recs = (L.Logprobs * (k * cap))() if logprobs else None
@@ -489,13 +518,14 @@ class B200Model:
         self._check(self._lib.aha_b200_batch_close(self._h))
 
     def generate_stream(self, input_ids, on_token, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None,
-                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None):
+                        repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None,
+                        rules=None):
         """generate_stream_generic: on_token(token, index) is called per generated token as its step completes; a truthy
         return value ends the request.  logprobs=True: on_token(token, index, record).  -> usage dict."""
         ids = self._ids(input_ids)
         mm, _keep = self._mm(data)
         flags = (L.GEN_REUSE_PREFIX if reuse_prefix else 0) | L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
-        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm)
+        p = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, fsm, rules)
         err = []
 
         def _cb(_user, token, index, *lp):
@@ -544,7 +574,7 @@ class B200Model:
         return int(self.debug_sample_rows(logits, [params], [context], draw_index)["token"][0])
 
     def debug_sample_rows(self, logits, params, contexts=None, draw_index=0, overwrite=False, kernel=0, act=None, on=None, fsm=None,
-                          constrained=None, fsm_states=None):
+                          constrained=None, fsm_states=None, rules=None, ruled=None):
         """The device sampler on given logits, one call for len(params) rows (1 to 64; tests).
         logits: [V] (every row reads it) or [rows, ld] with V = ld.  params: per row a dict of generate()'s sampling keywords
         (temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed).  contexts: per row the tokens generated so far;
@@ -553,6 +583,8 @@ class B200Model:
         (default r), on: [64] flags per slot (default all on).
         fsm: (offsets, tokens, next) of a token automaton (aha_b200_debug_sample_fsm); the rows with constrained[r] (default all) are
         constrained by it from state fsm_states[r] (default 0).
+        rules: dict(presence_penalty, frequency_penalty, logit_bias) (aha_b200_debug_sample_rules), applied by the rows with ruled[r]
+        (default all); the call checks that every row's count row is zero again afterwards.
         -> dict of uint32 arrays [rows]: token (0xffffffff where the row did not sample), state_token, n_hist, n_draws (the DecodeState
         after the call), last_hist (the last history word, 0xffffffff without a context) and, with fsm, fsm_state (after the call)."""
         rows = len(params)
@@ -578,19 +610,28 @@ class B200Model:
         u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
         i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
         lg_p = lg.ctypes.data_as(C.POINTER(C.c_float))
-        if fsm is None:
+        if fsm is None and rules is None:
             self._check(self._lib.aha_b200_debug_sample(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
                                                         1 if overwrite else 0, i32(act), i32(on), u32(tok), u32(state), u32(hist)))
             return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist)
-        f, _keep = L.token_fsm(*fsm)
+        f, _keep = L.token_fsm(*fsm) if fsm is not None else (None, None)
         con = np.ascontiguousarray(np.broadcast_to(np.asarray(True if constrained is None else constrained, np.int32), (rows,)))
         fin = np.ascontiguousarray(np.broadcast_to(np.asarray(0 if fsm_states is None else fsm_states, np.uint32), (rows,)))
         fout = np.zeros(rows, np.uint32)
-        self._check(self._lib.aha_b200_debug_sample_fsm(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
-                                                        1 if overwrite else 0, i32(act), i32(on), C.byref(f), i32(con), u32(fin), u32(tok),
-                                                        u32(state), u32(hist), u32(fout)))
-        return dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist,
-                    fsm_state=fout)
+        if rules is None:
+            self._check(self._lib.aha_b200_debug_sample_fsm(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
+                                                            1 if overwrite else 0, i32(act), i32(on), C.byref(f), i32(con), u32(fin), u32(tok),
+                                                            u32(state), u32(hist), u32(fout)))
+        else:
+            rl, _rkeep = L.logit_rules(**rules)
+            rd = np.ascontiguousarray(np.broadcast_to(np.asarray(True if ruled is None else ruled, np.int32), (rows,)))
+            self._check(self._lib.aha_b200_debug_sample_rules(self._h, int(kernel), rows, V, lg_p, ld, ps, u32(cat), u32(n_ctx), u32(draws),
+                                                              1 if overwrite else 0, i32(act), i32(on), C.byref(f) if f is not None else None,
+                                                              i32(con), u32(fin), C.byref(rl), i32(rd), u32(tok), u32(state), u32(hist), u32(fout)))
+        out = dict(token=tok, state_token=state[:, 0].copy(), n_hist=state[:, 1].copy(), n_draws=state[:, 2].copy(), last_hist=hist)
+        if fsm is not None:
+            out["fsm_state"] = fout
+        return out
 
     def debug_logprobs(self, logits, token, n_top=0):
         """The log-probability kernels on a given logits row of any length (tests) -> record dict."""

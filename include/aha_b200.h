@@ -102,7 +102,29 @@ typedef struct aha_gen_params {      /* ChatCompletionParameters subset used by 
                                   * state does not allow at logit -inf (before the repeat penalty, which leaves them there), and the state then
                                   * follows the drawn token.  Log-probability records stay raw (taken before the mask).  Accepted by generate,
                                   * generate_stream, generate_logprobs, generate_stream_logprobs, generate_batch, generate_n and the batch
-                                  * session entries; refused by generate_speculative, asr_generate and under tensor parallelism. */
+                                  * session entries; refused by generate_speculative, asr_generate and under tensor parallelism.
+                                  * params.reserved holds one id, so CONSTRAINED together with AHA_GEN_LOGIT_RULES is refused: a request
+                                  * with both names its automaton in the logit-rules object (aha_logit_rules.fsm). */
+#define AHA_GEN_LOGIT_RULES 32u  /* OpenAI frequency_penalty / presence_penalty / logit_bias: params.reserved holds the id of a logit-rules
+                                  * object from aha_b200_rules_create (read only when this flag is set).  Every draw, the first included, takes
+                                  * the raw logits x through: the automaton's mask (when the object names one), y[t] = x[t] + bias[t], the
+                                  * repeat penalty, then for every token t that occurs c[t] > 0 times among the tokens generated before this
+                                  * draw (the whole output, not only the last repeat_last_n; the prompt does not count)
+                                  *   y[t] = (y[t] - (float)c[t] * frequency_penalty) - presence_penalty   (each step rounded separately),
+                                  * then temperature, top-k and top-p; a greedy request draws the ArgMax of y (ties: lowest id).  Log-probability
+                                  * records stay raw.  Accepted by every entry that accepts CONSTRAINED and by generate_speculative (rules
+                                  * without an automaton); refused by asr_generate and under tensor parallelism. */
+
+/* Frequency / presence penalties and logit bias (AHA_GEN_LOGIT_RULES), ranges as OpenAI states them. */
+typedef struct aha_logit_rules {
+    float presence_penalty;       /* finite, [-2, 2]: subtracted once from every token already generated */
+    float frequency_penalty;      /* finite, [-2, 2]: subtracted once per occurrence */
+    const uint32_t* bias_ids;     /* [n_bias], distinct, each < the vocabulary */
+    const float* bias_values;     /* [n_bias], finite, [-100, 100]: added to the logit (-100 bans a token, +100 forces it) */
+    size_t n_bias;                /* 0 .. the vocabulary */
+    uint32_t fsm;                 /* 0, or the id of a token automaton on the handle (aha_b200_fsm_create) that constrains the request too */
+    uint32_t reserved[3];         /* 0 */
+} aha_logit_rules;
 
 /* A token automaton (constrained decoding): a deterministic automaton over token ids, e.g. a grammar, regex or JSON schema compiled by
  * the caller against its tokenizer.  State s allows tokens[offsets[s] .. offsets[s + 1]) (strictly ascending, at least one per state), and
@@ -466,6 +488,16 @@ int aha_b200_fsm_check(const aha_token_fsm* fsm, size_t vocab);
 int aha_b200_fsm_create(aha_model* m, const aha_token_fsm* fsm, uint32_t* id_out);
 int aha_b200_fsm_destroy(aha_model* m, uint32_t id);
 
+/* Logit-rules objects (AHA_GEN_LOGIT_RULES).  aha_b200_rules_check (host only, no handle): 0 when `r` is well formed over a vocabulary of
+ * `vocab` tokens, else 1 with the reason in aha_b200_last_error(NULL) (r->fsm is not looked up).  aha_b200_rules_create also checks that
+ * r->fsm names an automaton on the handle, and copies the bias list to device memory: *id_out (>= 1) names it in params.reserved until
+ * aha_b200_rules_destroy or aha_b200_destroy frees it.  aha_b200_rules_destroy refuses an id that a running batch slot uses, and
+ * aha_b200_fsm_destroy refuses an automaton that a live rules object names.  A server creates the rules of a request and destroys them
+ * after it. */
+int aha_b200_rules_check(const aha_logit_rules* r, size_t vocab);
+int aha_b200_rules_create(aha_model* m, const aha_logit_rules* r, uint32_t* id_out);
+int aha_b200_rules_destroy(aha_model* m, uint32_t id);
+
 void aha_b200_destroy(aha_model* m);
 
 /* Host-only helper (no device work, usable without a GPU): Qwen3VLModel::get_rope_index, image branch
@@ -527,6 +559,14 @@ int aha_b200_debug_sample_fsm(aha_model* m, int kernel, size_t rows, size_t V, c
                               const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
                               const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
                               uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out, uint32_t* fsm_state_out);
+/* aha_b200_debug_sample_fsm with logit rules (tests): `rules` (checked against V; its fsm must be 0, the automaton is `fsm`) is copied to
+ * scratch of this call, and row r applies it when ruled[r] != 0.  Each ruled row counts in a zeroed count row of its own, and the call
+ * fails unless every count row is zero again afterwards.  fsm may be NULL (constrained and fsm_state_in are then ignored). */
+int aha_b200_debug_sample_rules(aha_model* m, int kernel, size_t rows, size_t V, const float* logits, size_t ld, const aha_gen_params* params,
+                                const uint32_t* context, const uint32_t* n_context, const uint32_t* draw_index, int overwrite, const int32_t* act,
+                                const int32_t* on, const aha_token_fsm* fsm, const int32_t* constrained, const uint32_t* fsm_state_in,
+                                const aha_logit_rules* rules, const int32_t* ruled, uint32_t* token_out, uint32_t* state_out, uint32_t* hist_out,
+                                uint32_t* fsm_state_out);
 /* the log-probability kernels on a given logits row of V entries (tests): `token` is taken as the row's final token, index 0 */
 int aha_b200_debug_logprobs(aha_model* m, const float* logits, size_t V, uint32_t token, uint32_t n_top, aha_logprobs* out);
 int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* avg_ms, uint64_t* bytes_per_launch);

@@ -210,16 +210,26 @@ public:
         return id;
     }
     void fsm_destroy(uint32_t id) { check(aha_b200_fsm_destroy(h_, id)); }
+    // Logit-rules objects (OpenAI presence_penalty / frequency_penalty / logit_bias, aha_b200_rules_create): the id goes into generate() /
+    // BatchRequest::rules_id.  An automaton named in the object (aha_logit_rules::fsm) constrains the request too.
+    uint32_t rules_create(const aha_logit_rules& rules) {
+        uint32_t id = 0;
+        check(aha_b200_rules_create(h_, &rules, &id));
+        return id;
+    }
+    void rules_destroy(uint32_t id) { check(aha_b200_rules_destroy(h_, id)); }
     // The whole request with the decode loop on the device (generate_generic semantics, aha_b200_generate).
     // reuse_prefix (new design; the reference clears the cache after every request, generate.rs:147): keep the K/V of this request and
     // prefill only what follows the prefix the prompt shares with the cache -- same tokens, shorter time to the first one.
     // fsm_id (non-zero): every token is drawn from the tokens that automaton allows (AHA_GEN_CONSTRAINED).
+    // rules_id (non-zero): the logit rules of that object apply to every draw (AHA_GEN_LOGIT_RULES); give at most one of the two ids.
     std::vector<uint32_t> generate(const std::vector<uint32_t>& ids, const MultiModalData* data, const GenerationContext& ctx, Usage* usage = nullptr,
-                                   bool reuse_prefix = false, uint32_t fsm_id = 0) {
+                                   bool reuse_prefix = false, uint32_t fsm_id = 0, uint32_t rules_id = 0) {
         aha_gen_params p{};
         p.temperature = 0.f; p.repeat_penalty = ctx.repeat_penalty; p.repeat_last_n = (int32_t)ctx.repeat_last_n; p.max_tokens = (uint32_t)ctx.sample_len;
         if (reuse_prefix) p.flags |= AHA_GEN_REUSE_PREFIX;
         if (fsm_id) { p.flags |= AHA_GEN_CONSTRAINED; p.reserved = fsm_id; }
+        if (rules_id) { p.flags |= AHA_GEN_LOGIT_RULES; p.reserved = rules_id; }
         std::vector<uint32_t> out(ctx.sample_len);
         size_t n = 0;
         aha_usage u{};
@@ -230,7 +240,7 @@ public:
         return out;
     }
     // Static batching (aha_b200_generate_batch): up to 8 requests decoded in lockstep; result i is what generate() returns for request i alone.
-    struct BatchRequest { std::vector<uint32_t> ids; const MultiModalData* data = nullptr; GenerationContext ctx; uint32_t fsm_id = 0; };
+    struct BatchRequest { std::vector<uint32_t> ids; const MultiModalData* data = nullptr; GenerationContext ctx; uint32_t fsm_id = 0; uint32_t rules_id = 0; };
     std::vector<std::vector<uint32_t>> generate_batch(const std::vector<BatchRequest>& reqs, std::vector<Usage>* usage = nullptr) {
         const size_t n = reqs.size();
         std::vector<aha_batch_request> r(n);
@@ -243,6 +253,7 @@ public:
             r[i].params.repeat_penalty = reqs[i].ctx.repeat_penalty; r[i].params.repeat_last_n = (int32_t)reqs[i].ctx.repeat_last_n;
             r[i].params.max_tokens = (uint32_t)reqs[i].ctx.sample_len;
             if (reqs[i].fsm_id) { r[i].params.flags |= AHA_GEN_CONSTRAINED; r[i].params.reserved = reqs[i].fsm_id; }
+            if (reqs[i].rules_id) { r[i].params.flags |= AHA_GEN_LOGIT_RULES; r[i].params.reserved = reqs[i].rules_id; }
             cap = std::max(cap, reqs[i].ctx.sample_len);
         }
         std::vector<uint32_t> out(n * cap);
