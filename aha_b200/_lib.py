@@ -179,6 +179,11 @@ class Stats(C.Structure):
                 ("kv_bytes_per_token", C.c_uint64), ("decode_bytes_per_step_fixed", C.c_uint64)]
 
 
+class PrefixStats(C.Structure):
+    _fields_ = [("cached_pages", C.c_uint64), ("shared_pages", C.c_uint64), ("hit_tokens", C.c_uint64), ("lookups", C.c_uint64),
+                ("evicted_pages", C.c_uint64), ("max_pages", C.c_uint64), ("free_pages", C.c_uint64)]
+
+
 # every symbol include/aha_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 _U32P = C.POINTER(C.c_uint32)
@@ -222,6 +227,9 @@ SYMBOLS = {
                                       C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage)]),
     "aha_b200_batch_step": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.POINTER(C.c_size_t)]),
     "aha_b200_batch_close": (C.c_int, [_P]),
+    "aha_b200_batch_prefix_cache": (C.c_int, [_P, C.c_size_t]),
+    "aha_b200_batch_prefix_stats": (C.c_int, [_P, C.POINTER(PrefixStats), C.POINTER(C.c_size_t), C.c_size_t]),
+    "aha_b200_debug_prefix_attention": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _I32P, C.c_size_t, _I32P, _F32P, _F32P, _F32P, _F32P]),
     "aha_b200_batch_open_wide": (C.c_int, [_P, C.c_size_t]),
     "aha_b200_batch_step_n": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_generate_stream": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), TOKEN_CALLBACK, C.c_void_p,

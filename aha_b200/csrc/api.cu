@@ -3,12 +3,15 @@
 // Qwen3Model (src/models/qwen3/model.rs:94-214), Qwen3VLModel (qwen3vl/model.rs:837-1324),
 // Qwen3ASRModel (qwen3_asr/model.rs:308-425) and generate_generic (common/generate.rs:115-159).
 #include <array>
+#include <cassert>
 #include <chrono>
 #include <cstdio>
 #include <functional>
 #include <limits>
 #include <map>
 #include <mutex>
+#include <set>
+#include <unordered_map>
 #include <system_error>
 #include <thread>
 #include <type_traits>
@@ -38,6 +41,109 @@ int guarded_host(F&& f) {   // host-only entries (no handle)
 }
 }  // namespace
 
+// A batch session's prefix cache (aha_b200_batch_prefix_cache): full 32-token pages of admitted prompts, keyed by their token ids and their
+// parent page, so that a later request whose prompt starts with the same pages maps them into its table instead of prefilling them.  Every
+// block holds one reference on its page (PagePool::refs); the blocks form a tree from the prompts' first pages.  A key's hash only narrows
+// the search: a match is confirmed on the 32 ids.
+struct PrefixIndex {
+    struct Block {
+        uint32_t ids[kPage];
+        int parent = -1;     // page of the block before it in the prompt (-1: the prompt's first page)
+        int children = 0;    // cached blocks whose parent this is
+        uint64_t used = 0;   // LRU clock of the last admission that hit or inserted it
+    };
+    size_t max_pages = 0;                          // 0: off
+    std::unordered_map<int, Block> blocks;         // by page
+    std::unordered_multimap<uint64_t, int> by_key; // hash(parent, ids) -> page
+    uint64_t clock = 0, hit_tokens = 0, lookups = 0, evicted = 0;
+    bool on() const { return max_pages > 0; }
+    static uint64_t key(int parent, const uint32_t* ids) {
+        uint64_t h = 0x9e3779b97f4a7c15ull ^ (uint64_t)(uint32_t)parent;
+        for (int i = 0; i < kPage; ++i) { h = (h ^ ids[i]) * 0xff51afd7ed558ccdull; h ^= h >> 29; }
+        return h;
+    }
+    // the page caching ids[0, kPage) after `parent`, or -1
+    int find(int parent, const uint32_t* ids) const {
+        auto r = by_key.equal_range(key(parent, ids));
+        for (auto it = r.first; it != r.second; ++it) {
+            const Block& b = blocks.at(it->second);
+            if (b.parent == parent && std::equal(ids, ids + kPage, b.ids)) return it->second;
+        }
+        return -1;
+    }
+    // the pages of the longest cached chain of full pages that starts ids[0, n)
+    std::vector<int> chain(const uint32_t* ids, size_t n) const {
+        std::vector<int> pages;
+        int parent = -1;
+        for (size_t t = 0; t + kPage <= n; t += kPage) {
+            const int p = find(parent, ids + t);
+            if (p < 0) break;
+            pages.push_back(p);
+            parent = p;
+        }
+        return pages;
+    }
+    // pages the index alone holds, outside `keep`: every one can be evicted, leaves first (a page a table holds keeps its ancestors held too)
+    size_t evictable(const PagePool& pool, const std::set<int>& keep) const {
+        size_t k = 0;
+        for (const auto& e : blocks) k += pool.refs[e.first] == 1 && !keep.count(e.first);
+        return k;
+    }
+    // drop the least recently used leaf only the index holds, outside `keep`; false when there is none
+    bool evict_one(PagePool& pool, const std::set<int>& keep) {
+        int victim = -1;
+        uint64_t best = 0;
+        for (const auto& e : blocks)
+            if (pool.refs[e.first] == 1 && e.second.children == 0 && !keep.count(e.first) && (victim < 0 || e.second.used < best)) {
+                victim = e.first;
+                best = e.second.used;
+            }
+        if (victim < 0) return false;
+        erase(pool, victim);
+        ++evicted;
+        return true;
+    }
+    void erase(PagePool& pool, int page) {
+        const Block& b = blocks.at(page);
+        auto r = by_key.equal_range(key(b.parent, b.ids));
+        for (auto it = r.first; it != r.second; ++it) if (it->second == page) { by_key.erase(it); break; }
+        if (b.parent >= 0) blocks.at(b.parent).children -= 1;
+        blocks.erase(page);
+        pool.unref(page);
+    }
+    // The full pages of an admitted prompt that the table `t` holds (its first hit / kPage of them are the cached chain it hit), in prompt
+    // order.  Inserting beyond max_pages evicts LRU leaves first; the chain stops at the first page that cannot be inserted.
+    void insert(PagePool& pool, const uint32_t* ids, size_t n, const PageTable& t) {
+        ++clock;
+        int parent = -1;
+        for (size_t b = 0; (b + 1) * kPage <= n; ++b) {
+            const int page = t.h[b];
+            const int have = find(parent, ids + b * kPage);
+            if (have >= 0) {   // the chain this request hit, or the same ids inserted earlier in this call from another request's pages
+                blocks.at(have).used = clock;
+                if (have != page) return;
+                parent = page;
+                continue;
+            }
+            while (blocks.size() >= max_pages) if (!evict_one(pool, {})) return;
+            Block& nb = blocks[page];
+            std::copy(ids + b * kPage, ids + (b + 1) * kPage, nb.ids);
+            nb.parent = parent;
+            nb.used = clock;
+            if (parent >= 0) blocks.at(parent).children += 1;
+            by_key.emplace(key(parent, nb.ids), page);
+            pool.ref(page);
+            parent = page;
+        }
+    }
+    // max_tokens 0: every block lets go of its page
+    void clear(PagePool& pool) {
+        for (const auto& e : blocks) pool.unref(e.first);
+        blocks.clear();
+        by_key.clear();
+    }
+};
+
 struct aha_model {
     enum Kind { QWEN3, QWEN3VL, QWEN3_ASR } kind = QWEN3;
     Ctx ctx;
@@ -53,9 +159,10 @@ struct aha_model {
     int audio_token_id = -1;
     int* d_scatter_idx = nullptr;
     int max_scatter = 0;
-    int* d_pack_work = nullptr;   // packed prefills (embed_batch, batch_add_many): varlen attention work list ([max_prefill][3]), the rows
+    int* d_pack_work = nullptr;   // packed prefills (embed_batch, batch_add_many): varlen attention work list ([max_prefill][kFaWork]), the rows
     int* d_pack_rows = nullptr;   // taken from the pack ([max_prefill]) and the pack's page table ([num_pages]); allocated on first use
     int* d_pack_table = nullptr;
+    int* d_pack_read = nullptr;   // the read table of a pack with cached prefixes ([num_pages]); allocated when a batch_add_many first hits
     double last_vision_secs = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // pinned staging for the host<->device scalars of a step / the tokens of a burst
@@ -79,6 +186,8 @@ struct aha_model {
         bool used[kWideSeqs] = {};
         size_t budget[kWideSeqs] = {}, produced[kWideSeqs] = {};
         bool lp_valid[kWideSeqs] = {};  // the slot's record row holds the record of the last token its request delivered
+        size_t hit[kWideSeqs] = {};     // prompt tokens the slot's request took from the prefix cache
+        PrefixIndex prefix;             // aha_b200_batch_prefix_cache; dropped with the session
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
     SpecDecoder spec;                   // speculative single requests (aha_b200_generate_speculative) on wide_batch's buffers
@@ -549,7 +658,7 @@ void session_close(aha_model* m) {
 void alloc_pack_buffers(aha_model* m) {
     if (m->d_pack_work) return;
     const TextModel& T = m->text;
-    m->d_pack_work = m->ctx.alloc<int>((size_t)3 * T.max_prefill);
+    m->d_pack_work = m->ctx.alloc<int>((size_t)kFaWork * T.max_prefill);
     m->d_pack_rows = m->ctx.alloc<int>((size_t)T.max_prefill);
     m->d_pack_table = m->ctx.alloc<int>((size_t)T.num_pages);
 }
@@ -561,34 +670,46 @@ void alloc_pack_buffers(aha_model* m) {
 struct Pack {
     size_t first = 0, last = 0;
     size_t S = 0;                    // tokens in the pack
+    size_t KV = 0;                   // key rows of the pack: S plus the cached prefixes of its inputs
     std::vector<size_t> start;
+    std::vector<size_t> kv_start;    // where each input's keys (its prefix, then its own rows) start among the KV rows
     std::vector<uint32_t> ids;       // [S]
-    std::vector<int> pos3;           // [3][S]: positions restart at 0 in every segment
+    std::vector<int> pos3;           // [3][S]: positions restart at the input's prefix length (0 without one) in every segment
     PrefillSegments sg;              // (start, length) of every segment; the work list's device copy is set by upload_pack
-    std::vector<int> work;           // [n_work][3] work list of flash_attn_tc_varlen
+    std::vector<int> work;           // [n_work][kFaWork] work list of flash_attn_tc_varlen
     std::vector<int> rows;           // the last row of every input
 };
-// the pack that begins at input `first`: as many inputs as fit `cap` tokens, each starting on a multiple of `align`
-Pack plan_pack(const std::vector<const uint32_t*>& ids, const std::vector<size_t>& lens, size_t first, size_t align, size_t cap) {
+// The pack that begins at input `first`: as many inputs as fit `cap` tokens, each starting on a multiple of `align`.  pre (optional): the
+// cached prefix of every input, a multiple of `align` tokens that the pack does not run but its attention reads; then the pack's key rows
+// (every input's prefix and segment, laid end to end) must also fit `kv_cap`.
+Pack plan_pack(const std::vector<const uint32_t*>& ids, const std::vector<size_t>& lens, size_t first, size_t align, size_t cap,
+               const std::vector<size_t>& pre = {}, size_t kv_cap = 0) {
     Pack p;
     p.first = p.last = first;
+    auto pre_of = [&](size_t j) { return pre.empty() ? (size_t)0 : pre[j]; };
     while (p.last < lens.size()) {
         const size_t s0 = p.last == first ? 0 : (p.S + align - 1) / align * align;
+        const size_t kv0 = p.last == first ? 0 : p.kv_start.back() + pre_of(p.last - 1) + (s0 - p.start.back());
         if (s0 + lens[p.last] > cap) break;
+        if (!pre.empty() && kv0 + pre[p.last] + lens[p.last] > kv_cap) break;
         p.start.push_back(s0);
-        p.S = s0 + lens[p.last++];
+        p.kv_start.push_back(kv0);
+        p.S = s0 + lens[p.last];
+        p.KV = kv0 + pre_of(p.last) + lens[p.last];
+        ++p.last;
     }
     AHA_REQUIRE(p.last > first, "packed prefill: an input of " + std::to_string(lens[first]) + " tokens exceeds the pack capacity of " + std::to_string(cap));
     const size_t S = p.S;
     p.ids.assign(S, 0);
     p.pos3.resize((size_t)3 * S);
     for (size_t j = p.first; j < p.last; ++j) {
-        const int s0 = (int)p.start[j - first], len = (int)lens[j];
+        const int s0 = (int)p.start[j - first], len = (int)lens[j], pj = (int)pre_of(j), kv0 = (int)p.kv_start[j - first];
         const int seg = (j + 1 < p.last ? (int)p.start[j + 1 - first] : (int)S) - s0;   // the input and the filler behind it
         std::memcpy(p.ids.data() + s0, ids[j], (size_t)len * sizeof(uint32_t));
-        for (int k = 0; k < 3; ++k) for (int i = 0; i < seg; ++i) p.pos3[(size_t)k * S + s0 + i] = i;
+        for (int k = 0; k < 3; ++k) for (int i = 0; i < seg; ++i) p.pos3[(size_t)k * S + s0 + i] = pj + i;
         p.sg.segs.emplace_back(s0, seg);
-        for (int q = 0; q < seg; q += kFaBQ) { p.work.push_back(s0); p.work.push_back(seg); p.work.push_back(q); }
+        if (!pre.empty()) p.sg.kv.emplace_back(kv0, pj + seg);
+        for (int q = 0; q < seg; q += kFaBQ) p.work.insert(p.work.end(), {s0, seg, kv0, pj + seg, q});
         p.rows.push_back(s0 + len - 1);
     }
     return p;
@@ -597,7 +718,7 @@ Pack plan_pack(const std::vector<const uint32_t*>& ids, const std::vector<size_t
 void upload_pack(aha_model* m, Pack& p) {
     cudaStream_t st = m->ctx.stream;
     p.sg.d_work = m->d_pack_work;
-    p.sg.n_work = (int)(p.work.size() / 3);
+    p.sg.n_work = (int)(p.work.size() / kFaWork);
     AHA_CUDA_CHECK(cudaMemcpyAsync(m->text.d_ids, p.ids.data(), p.S * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_work, p.work.data(), p.work.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_rows, p.rows.data(), p.rows.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -1114,14 +1235,16 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
 namespace {
 // One request into slot `slot` of the batch decoder: the reference's forward_initial + sample_and_push on the slot's own page table (the
 // single-request code, so tower / M-RoPE / deepstack / sampler-on-prefill are shared), then its decode state, history and sampler move into the
-// slot.  If this throws, the slot's table holds whatever pages it took and the caller releases them with the slot.
-uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int lp_n) {
+// slot.  hit > 0: the table already starts with the prefix cache's pages of ids[0, hit) and only the rest is prefilled, as a continuation (a
+// text-only prompt, so on Qwen3-VL its positions are the plain ones, rope_delta 0).  If this throws, the slot's table holds whatever pages it
+// took and the caller releases them with the slot.
+uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, size_t sample_len, int lp_n, size_t hit = 0) {
     TextModel& T = m->text;
     BatchDecoder& B = m->sess();
     PageTable& pt = B.slots[slot].table;
-    m->have_rope_delta = false; m->rope_delta = 0;
+    m->have_rope_delta = hit > 0; m->rope_delta = 0;
     const Sampler samp = request_sampler(m, r.params, "");
-    const uint32_t tok = first_token(m, pt, r.ids, r.seq_len, 0, r.mm, samp, 0);
+    const uint32_t tok = first_token(m, pt, r.ids, r.seq_len, hit, r.mm, samp, 0);
     if (lp_n >= 0) {   // the first token's record goes straight into the slot's record row
         T.set_logprobs(lp_n);
         B.ensure_lp();
@@ -1133,6 +1256,44 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
     return tok;
 }
 
+// The hit rule of every admission path: the longest cached chain of full pages that starts the prompt, capped at seq_len - 1 tokens and,
+// unless every GEMM runs on the SIMT kernel, at seq_len - kPage, so that the rows still prefilled run on the wgmma GEMM as the cold prefill of
+// the same rows does (gemm_on_tc: M < 32 takes SIMT).  The pages it returns hold ids[0, kPage * size()).  Multimodal requests never hit.
+std::vector<int> prefix_hit(const aha_model* m, const uint32_t* ids, size_t seq_len, bool has_mm) {
+    const PrefixIndex& X = m->session.prefix;
+    if (!X.on() || has_mm) return {};
+    const size_t cap = m->ctx.gemm_impl == 1 ? seq_len - 1 : (seq_len >= (size_t)kPage ? seq_len - kPage : 0);
+    return X.chain(ids, cap / kPage * kPage);
+}
+// Admission's page check: `pages` fresh pages must fit the free list plus the pages only the prefix cache holds, less those this call hits
+// (`keep`).  Once the call has passed every check, prefix_make_room evicts LRU leaves only as far as the call needs.
+void prefix_check_room(const aha_model* m, size_t pages, const std::set<int>& keep, const std::string& what) {
+    const TextModel& T = m->text;
+    const PrefixIndex& X = m->session.prefix;
+    const size_t avail = T.pages.free_count() + (X.on() ? X.evictable(T.pages, keep) : 0);
+    AHA_REQUIRE(pages <= avail, what + std::to_string(pages * kPage) + " tokens of KV capacity, " + std::to_string(avail * kPage) +
+                                    " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+}
+void prefix_make_room(aha_model* m, size_t pages, const std::set<int>& keep) {
+    while (m->text.pages.free_count() < pages) AHA_REQUIRE(m->session.prefix.evict_one(m->text.pages, keep), "prefix cache: no page left to evict");
+}
+// the shared pages first in the (empty) table of each admitted request that hit; the debug assert states why no step ever writes them:
+// decode writes positions >= seq_len, and the hit ends at or before seq_len - 1
+void prefix_share(aha_model* m, int slot, const std::vector<int>& pages, size_t seq_len) {
+    assert(pages.size() * kPage < seq_len);
+    if (!pages.empty()) m->text.pages.share(m->sess().slots[slot].table, pages);
+    (void)seq_len;
+}
+// after a successful admission: the request's full prompt pages enter the index, and the statistics count its lookup
+void prefix_admitted(aha_model* m, int slot, const uint32_t* ids, size_t seq_len, size_t hit) {
+    PrefixIndex& X = m->session.prefix;
+    m->session.hit[slot] = hit;
+    if (!X.on()) return;
+    X.lookups += 1;
+    X.hit_tokens += hit;
+    X.insert(m->text.pages, ids, seq_len, m->sess().slots[slot].table);
+}
+
 // ---- continuous batching: the same slots and the same step, with requests joining and leaving between steps -------------------------
 // (new design; the reference's server holds ONE request behind a write lock, server/api.rs:117.)  A finished request's pages go back to the
 // free list at once, so a waiting request can take its place while the others keep decoding.
@@ -1142,6 +1303,7 @@ void session_release(aha_model* m, int slot) {
     sl.samp_active = false;
     sl.lp = 0;
     m->session.used[slot] = false;
+    m->session.hit[slot] = 0;
     m->sess().composition_changed();
 }
 // the bookkeeping of a request admitted into slot s with its first token: true (and the slot released) when that token is also its last
@@ -1214,9 +1376,11 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) + " of the " + width +
                                       " slots are free (step until requests finish)");
     slot.resize(n);
-    std::vector<size_t> sample_len(n);
-    std::vector<bool> packed(n);
+    std::vector<size_t> sample_len(n), hit(n);
+    std::vector<bool> packed(n), text_only(n);
     std::vector<int> lp_n(n);
+    std::vector<std::vector<int>> hit_pages(n);
+    std::set<int> keep;   // pages this call hits: never evicted by it
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
         const aha_batch_request& r = reqs[i];
@@ -1227,48 +1391,69 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
         request_rules(m, r.params, who + "request " + std::to_string(i) + ": ");
         require_mm_arity(m, r.mm);
         sample_len[i] = token_budget(r.params);
-        pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage;
         bool has_mm = false;   // (a qwen3 handle ignores the tensors)
         for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
+        text_only[i] = !has_mm;
+        hit_pages[i] = prefix_hit(m, r.ids, r.seq_len, has_mm);
+        hit[i] = hit_pages[i].size() * kPage;
+        keep.insert(hit_pages[i].begin(), hit_pages[i].end());
+        pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage - hit_pages[i].size();
         packed[i] = pack && !has_mm && r.seq_len <= (size_t)T.max_prefill;
     }
-    AHA_REQUIRE(pages <= T.pages.free_count(), who + "the requests need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
-                                                   std::to_string(T.pages.free_count() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+    prefix_check_room(m, pages, keep, who + "the requests need ");
     for (size_t i = 0; i < n; ++i) {   // (only reachable when max_ctx is not a multiple of the page)
         const size_t ctx = reqs[i].seq_len + sample_len[i];
         AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     }
+    prefix_make_room(m, pages, keep);
     const auto t0 = clk::now();
     AdmitGuard guard{m, slot};
     for (int s : slot) m->session.used[s] = true;
+    for (size_t i = 0; i < n; ++i) prefix_share(m, slot[i], hit_pages[i], reqs[i].seq_len);
     std::vector<uint32_t> tok(n);
     std::vector<double> secs(n), vision(n, 0.0);
     // ---- packed requests: map every page each can touch (as batch_prefill_slot does after its prefill), then prefill them pack by pack
-    std::vector<size_t> pk;
+    // With prefix hits a request's pack segment is the part of its prompt the cache does not hold: ids[hit, seq_len) at positions hit ..
+    std::vector<size_t> pk, pk_pre;
     std::vector<const uint32_t*> pk_ids;
     std::vector<size_t> pk_lens;
+    bool any_hit = false;
     for (size_t i = 0; i < n; ++i) {
         if (!packed[i]) continue;
-        pk.push_back(i); pk_ids.push_back(reqs[i].ids); pk_lens.push_back(reqs[i].seq_len);
+        pk.push_back(i); pk_ids.push_back(reqs[i].ids + hit[i]); pk_lens.push_back(reqs[i].seq_len - hit[i]); pk_pre.push_back(hit[i]);
+        any_hit = any_hit || hit[i] > 0;
         T.pages.map(B.slots[slot[i]].table, (int)(reqs[i].seq_len + sample_len[i]));
     }
+    if (!any_hit) pk_pre.clear();
     if (!pk.empty()) {
         alloc_pack_buffers(m);
+        if (any_hit && !m->d_pack_read) m->d_pack_read = c.alloc<int>((size_t)T.num_pages);
         const int H = T.cfg.H;
         const size_t cap = (size_t)std::min(T.max_prefill, T.max_ctx);
         for (size_t first = 0; first < pk.size();) {
-            Pack p = plan_pack(pk_ids, pk_lens, first, kPage, cap);
-            // the pack's table: the requests' own pages laid end to end, all mapped above, so the prefill takes no page from the pool
-            PageTable pt;
+            // (key rows: the split workspace of the attention holds max_ctx of them, as for a continuation prefill)
+            Pack p = plan_pack(pk_ids, pk_lens, first, kPage, cap, pk_pre, (size_t)T.max_ctx);
+            // The pack's table: the requests' own pages laid end to end, all mapped above, so the prefill takes no page from the pool and
+            // writes only pages no other table holds.  With prefixes, the attention reads a second table: every request's pages from its
+            // first, the shared ones included, laid end to end the same way (every segment but the last ends on a page boundary).
+            PageTable pt, rd;
             for (size_t j = p.first; j < p.last; ++j) {
                 const std::vector<int>& own = B.slots[slot[pk[j]]].table.h;
-                pt.h.insert(pt.h.end(), own.begin(), own.begin() + ceil_div(p.sg.segs[j - p.first].second, kPage));
+                const int pre = any_hit ? (int)pk_pre[j] / kPage : 0, seg = p.sg.segs[j - p.first].second;
+                pt.h.insert(pt.h.end(), own.begin() + pre, own.begin() + pre + ceil_div(seg, kPage));
+                if (any_hit) rd.h.insert(rd.h.end(), own.begin(), own.begin() + pre + ceil_div(seg, kPage));
             }
             pt.mapped = (int)pt.h.size();
             AHA_REQUIRE(ceil_div((int)p.S, kPage) <= pt.mapped, "batch_add_many: the pack's page table does not cover the pack");
             pt.h.resize(T.num_pages, 0);
             pt.d = m->d_pack_table;
             AHA_CUDA_CHECK(cudaMemcpyAsync(pt.d, pt.h.data(), (size_t)pt.mapped * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+            if (any_hit) {
+                AHA_REQUIRE(ceil_div((int)p.KV, kPage) <= (int)rd.h.size() && rd.h.size() <= (size_t)T.num_pages, "batch_add_many: the pack's read table does not cover its keys");
+                AHA_CUDA_CHECK(cudaMemcpyAsync(m->d_pack_read, rd.h.data(), rd.h.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+                p.sg.d_read = m->d_pack_read;
+                p.sg.kv_rows = (int)p.KV;
+            }
             upload_pack(m, p);
             T.prefill(pt, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
             gather_rows_kernel<<<(unsigned)(p.last - p.first), 256, 0, c.stream>>>(m->d_pack_rows, T.x, B.xb + p.first * H, H);
@@ -1304,11 +1489,12 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     // ---- the others: one prefill each, on the slot's own table
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
-        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i]);
+        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i], hit[i]);
         secs[i] = seconds(clk::now() - t0);
         vision[i] = m->last_vision_secs;
     }
     guard.ok = true;
+    for (size_t i = 0; i < n; ++i) if (text_only[i]) prefix_admitted(m, slot[i], reqs[i].ids, reqs[i].seq_len, hit[i]);
     T.clear_sampler();
     B.composition_changed();
     for (size_t i = 0; i < n; ++i) {
@@ -1350,20 +1536,26 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     require_mm_arity(m, req.mm);
     const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len;
     AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
-    const size_t pages = n * (size_t)ceil_div((int)ctx, kPage);
-    AHA_REQUIRE(pages <= T.pages.free_count(), who + std::to_string(n) + " choices need " + std::to_string(pages * kPage) + " tokens of KV capacity, " +
-                                                   std::to_string(T.pages.free_count() * kPage) + " are free (max_ctx " + std::to_string(T.max_ctx) + ")");
+    bool has_mm = false;
+    for (size_t k = 0; m->kind != aha_model::QWEN3 && k < req.mm->n; ++k) has_mm = has_mm || mm_entry(req.mm, k) != nullptr;
+    const std::vector<int> hit_pages = prefix_hit(m, req.ids, req.seq_len, has_mm);   // choice 0's table starts with them
+    const size_t hit = hit_pages.size() * kPage;
+    const size_t pages = n * (size_t)ceil_div((int)ctx, kPage) - hit_pages.size();
+    const std::set<int> keep(hit_pages.begin(), hit_pages.end());
+    prefix_check_room(m, pages, keep, who + std::to_string(n) + " choices need ");
     std::vector<aha_batch_request> r(n, req);
     std::vector<Sampler> samp(n);
     for (size_t i = 0; i < n; ++i) {
         r[i].params.seed = seeds ? seeds[i] : req.params.seed + i;
         samp[i] = request_sampler(m, r[i].params, who);
     }
+    prefix_make_room(m, pages, keep);
     const auto t0 = clk::now();
     AdmitGuard guard{m, slot};
     for (int s : slot) m->session.used[s] = true;
     std::vector<uint32_t> tok(n);
-    tok[0] = batch_prefill_slot(m, slot[0], r[0], sample_len, lp_n);
+    prefix_share(m, slot[0], hit_pages, req.seq_len);
+    tok[0] = batch_prefill_slot(m, slot[0], r[0], sample_len, lp_n, hit);
     if (n > 1) {
         const std::vector<int> dst(slot.begin() + 1, slot.end());
         for (int s : dst) T.pages.map(B.slots[s].table, (int)ctx);
@@ -1395,6 +1587,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     }
     const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
     guard.ok = true;
+    if (!has_mm) prefix_admitted(m, slot[0], req.ids, req.seq_len, hit);
     T.clear_sampler();
     B.composition_changed();
     for (size_t i = 0; i < n; ++i) {
@@ -1608,6 +1801,33 @@ int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out, size_t cap) {
         AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
         const std::vector<aha_logprobs> h = session_records(m);
         for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? h[i] : aha_logprobs{};
+    });
+}
+
+int aha_b200_batch_prefix_cache(aha_model* m, size_t max_tokens) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        PrefixIndex& X = m->session.prefix;
+        TextModel& T = m->text;
+        X.max_pages = max_tokens / kPage;
+        if (!X.on()) { X.clear(T.pages); return; }
+        while (X.blocks.size() > X.max_pages && X.evict_one(T.pages, {})) {}
+    });
+}
+
+int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hits_out, size_t cap) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        AHA_REQUIRE(out, "batch_prefix_stats: out is required");
+        const int width = m->session.width;
+        AHA_REQUIRE(!hits_out || cap >= (size_t)width, "batch_prefix_stats: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+        const PrefixIndex& X = m->session.prefix;
+        *out = aha_prefix_stats{};
+        out->cached_pages = X.blocks.size();
+        for (const auto& e : X.blocks) out->shared_pages += m->text.pages.refs[e.first] > 1;
+        out->hit_tokens = X.hit_tokens; out->lookups = X.lookups; out->evicted_pages = X.evicted; out->max_pages = X.max_pages;
+        out->free_pages = m->text.pages.free_count();
+        if (hits_out) for (size_t i = 0; i < cap; ++i) hits_out[i] = i < (size_t)width ? m->session.hit[i] : 0;
     });
 }
 
@@ -1830,6 +2050,56 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
     });
 }
 
+int aha_b200_debug_prefix_attention(aha_model* m, int impl, size_t n_heads, size_t n_kv_heads, const int32_t* segments, size_t n_segments,
+                                    const int32_t* page_order, const float* q, const float* k, const float* v, float* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(q && k && v && out && segments && n_segments >= 1, "q, k, v, out and at least one segment are required");
+        AHA_REQUIRE(impl >= 0 && impl <= 2, "impl must be 0 (wgmma), 1 (SIMT) or 2 (mma.sync)");
+        AHA_REQUIRE(n_kv_heads >= 1 && n_heads % n_kv_heads == 0 && n_heads <= 64, "debug_prefix_attention: bad head counts");
+        constexpr int HD = 128;
+        Ctx& c = m->ctx;
+        const int nh = (int)n_heads, nkv = (int)n_kv_heads;
+        // segment j: its queries follow the previous segment's, its keys (prefix, then one per query) follow the previous segment's keys
+        PrefillSegments sg;
+        std::vector<int> work;
+        int Sq = 0, Skv = 0;
+        for (size_t j = 0; j < n_segments; ++j) {
+            const int pre = segments[2 * j], len = segments[2 * j + 1];
+            AHA_REQUIRE(pre >= 0 && len >= 1 && Skv + pre + len <= (1 << 20), "debug_prefix_attention: segments need prefix >= 0 and rows >= 1");
+            AHA_REQUIRE(Skv % 16 == 0, "debug_prefix_attention: every segment's keys must start on a multiple of 16 rows");
+            sg.segs.emplace_back(Sq, len);
+            sg.kv.emplace_back(Skv, pre + len);
+            for (int q0 = 0; q0 < len; q0 += kFaBQ) work.insert(work.end(), {Sq, len, Skv, pre + len, q0});   // as plan_pack builds it
+            Sq += len;
+            Skv += pre + len;
+        }
+        const int np = ceil_div(Skv, kPage);
+        std::vector<int> table(np);
+        for (int p = 0; p < np; ++p) table[p] = page_order ? page_order[p] : p;
+        std::vector<char> seen(*std::max_element(table.begin(), table.end()) + 1, 0);
+        for (int p : table) { AHA_REQUIRE(p >= 0 && !seen[p], "page_order must hold distinct non-negative pages"); seen[p] = 1; }
+        HostPool pool((int)seen.size(), nkv, HD);
+        pool.put(table.data(), Skv, k, v);
+        Scratch mem;
+        FlashArgs fa;
+        fa.q = upload_scratch(mem, c.stream, q, (size_t)Sq * nh * HD); fa.q_tok_stride = (size_t)nh * HD; fa.q_head_stride = HD;
+        fa.kv = pool.src(upload_scratch(mem, c.stream, pool.data.data(), pool.data.size()), upload_scratch(mem, c.stream, table.data(), table.size()));
+        const size_t n_out = (size_t)Sq * nh * HD;
+        fa.out = mem.alloc<float>(n_out); fa.o_tok_stride = (size_t)nh * HD; fa.o_head_stride = HD;
+        fill_nan(c.stream, fa.out, n_out);
+        fa.Sq = Sq; fa.Skv = Skv; fa.q0 = 0; fa.kv0 = 0; fa.groups = nh / nkv; fa.scaling = (float)(1.0 / std::sqrt((double)HD));
+        sg.d_work = upload_scratch(mem, c.stream, work.data(), work.size());
+        sg.n_work = (int)(work.size() / kFaWork);
+        const int saved = c.attn_impl;
+        c.attn_impl = impl;
+        try { flash_dispatch_segments(c, fa, nh, sg); } catch (...) { c.attn_impl = saved; throw; }
+        c.attn_impl = saved;
+        AHA_CUDA_CHECK(cudaGetLastError());
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        AHA_CUDA_CHECK(cudaMemcpy(out, fa.out, n_out * sizeof(float), cudaMemcpyDeviceToHost));
+    });
+}
+
 int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_heads, size_t n_kv_heads, size_t sq, size_t skv, int causal,
                              const int32_t* segments, size_t n_segments, const int32_t* page_order, int split_out, const float* q, const float* k,
                              const float* v, float* out) {
@@ -1853,7 +2123,7 @@ int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_head
                 const int s0 = segments[2 * i], len = segments[2 * i + 1];
                 AHA_REQUIRE(s0 >= end && len >= 1 && s0 + len <= Sq, "segments must be non-empty, in order, disjoint and inside [0, sq)");
                 segs.emplace_back(s0, len);
-                for (int q0 = 0; q0 < len; q0 += kFaBQ) { work.push_back(s0); work.push_back(len); work.push_back(q0); }   // as plan_pack builds it
+                for (int q0 = 0; q0 < len; q0 += kFaBQ) work.insert(work.end(), {s0, len, s0, len, q0});   // as plan_pack builds it
                 end = s0 + len;
             }
         }
@@ -1891,8 +2161,8 @@ int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_head
         const int saved = c.attn_impl;
         c.attn_impl = impl;
         try {
-            if (hd == 64) debug_attention_run<64>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / 3);
-            else debug_attention_run<128>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / 3);
+            if (hd == 64) debug_attention_run<64>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / kFaWork);
+            else debug_attention_run<128>(c, fa, nh, causal != 0, segs, d_work, (int)work.size() / kFaWork);
         } catch (...) { c.attn_impl = saved; throw; }
         c.attn_impl = saved;
         AHA_CUDA_CHECK(cudaGetLastError());

@@ -23,6 +23,7 @@
 namespace aha {
 
 constexpr int kFaBQ = 128, kFaBKV = 64, kFaThreads = 288;
+constexpr int kFaWork = 5;   // ints per work item of the varlen kernel
 
 // fp16 row-major [rows, cols] matrix, box = box_rows x 64 halfs (128 bytes), 128-byte swizzle, OOB reads as zero
 inline CUtensorMap make_tmap_f16_box(const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows) {
@@ -96,7 +97,7 @@ struct FlashTcArgs {
     __half *out_hi, *out_lo;   // when set: the output goes out as fp16 hi + lo halves (operand format of the next GEMM) instead of fp32
     int Sq, Skv, q0, groups;
     float scaling;
-    const int* work = nullptr;   // VARLEN: [gridDim.x][3] = (seg_start, seg_len, qt0), one 128-query tile of one packed segment per item
+    const int* work = nullptr;   // VARLEN: [gridDim.x][kFaWork] = (q_start, q_len, kv_start, kv_len, qt0), one 128-query tile of one segment per item
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {   // 2^x on the MUFU, flush-to-zero (inputs here are <= 0; -inf -> 0)
@@ -112,11 +113,12 @@ __device__ __forceinline__ void fa_mma_pv(float (&o)[HD / 2], const uint32_t (&a
     else wgmma_rs_n128(o, a, db);
 }
 
-// VARLEN: independent segments packed back to back in one tensor (Sq = Skv = the pack's length T).  blockIdx.x picks a work item; inside it
-// Sq = Skv = seg_len and every tensor row / column and the output row is offset by seg_start, while the KV tile grid and the masks stay
-// relative to the segment.  So each query row goes through the same operations in the same order as when its segment runs alone: keys of the
-// next segment that enter the last tile are masked (kj >= seg_len or kj > qi) and their V rows are multiplied by P = 0.  seg_start must be a
-// multiple of 16 tokens (flash_attn_tc_varlen).
+// VARLEN: independent segments packed back to back (Sq: the pack's query rows, Skv: its gathered key rows).  blockIdx.x picks a work item;
+// inside it the queries are rows [q_start, q_start + q_len) and the keys rows [kv_start, kv_start + kv_len), so Sq = q_len, Skv = kv_len and
+// the causal diagonal shifts by kv_len - q_len (a segment whose first kv_len - q_len keys are a cached prefix), while the KV tile grid and the
+// masks stay relative to the segment.  So each query row goes through the same operations in the same order as when its segment runs alone:
+// keys of the next segment that enter the last tile are masked (kj >= kv_len or kj > qi + shift) and their V rows are multiplied by P = 0.
+// kv_start must be a multiple of 16 tokens (flash_attn_tc_varlen).
 template <int HD, bool CAUSAL, bool VARLEN = false>
 __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __grid_constant__ CUtensorMap tm_qh, const __grid_constant__ CUtensorMap tm_ql,
                                                                      const __grid_constant__ CUtensorMap tm_kh, const __grid_constant__ CUtensorMap tm_kl,
@@ -135,10 +137,10 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int head = blockIdx.y, kvh = head / a.groups;
-    int seg0 = 0, Sq = a.Sq, Skv = a.Skv, qt0 = blockIdx.x * BQ;
+    int q_start = 0, kv_start = 0, Sq = a.Sq, Skv = a.Skv, qt0 = blockIdx.x * BQ;
     if constexpr (VARLEN) {
-        const int* w = a.work + 3 * blockIdx.x;
-        seg0 = __ldg(w); Sq = Skv = __ldg(w + 1); qt0 = __ldg(w + 2);
+        const int* w = a.work + kFaWork * blockIdx.x;
+        q_start = __ldg(w); Sq = __ldg(w + 1); kv_start = __ldg(w + 2); Skv = __ldg(w + 3); qt0 = __ldg(w + 4);
     }
     const int causal_shift = Skv - Sq;
     int kv_end = Skv;
@@ -155,7 +157,7 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
     if (warp == 8) {
         // ======================= producer lane: Q once, then the K / V^T tiles through the two-stage ring
         if (lane == 0) {
-            const int qrow = head * a.Sq + seg0 + qt0, krow = kvh * a.Skv + seg0, vrow = kvh * HD;
+            const int qrow = head * a.Sq + q_start + qt0, krow = kvh * a.Skv + kv_start, vrow = kvh * HD;
             mbar_expect_tx(bar_q, 2 * kQBytes);
 #pragma unroll
             for (int kb = 0; kb < KB; ++kb) {
@@ -172,8 +174,8 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
                     tma_load_2d(st + kb * kKBlk, &tm_kh, kb * 64, krow + t * BKV, &full[s]);
                     tma_load_2d(st + kKBytes + kb * kKBlk, &tm_kl, kb * 64, krow + t * BKV, &full[s]);
                 }
-                tma_load_2d(st + 2 * kKBytes, &tm_vh, seg0 + t * BKV, vrow, &full[s]);
-                tma_load_2d(st + 2 * kKBytes + kVBytes, &tm_vl, seg0 + t * BKV, vrow, &full[s]);
+                tma_load_2d(st + 2 * kKBytes, &tm_vh, kv_start + t * BKV, vrow, &full[s]);
+                tma_load_2d(st + 2 * kKBytes + kVBytes, &tm_vl, kv_start + t * BKV, vrow, &full[s]);
             }
         }
         return;
@@ -268,8 +270,8 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
         if (lane == 0) mbar_arrive(&empty[s]);   // this warp's reads of the stage have retired
     }
     if constexpr (VARLEN) {   // read again rather than held through the KV loop (keeps the register count of the plain kernel)
-        const int* w = a.work + 3 * blockIdx.x;
-        asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(seg0) : "l"(w));
+        const int* w = a.work + kFaWork * blockIdx.x;
+        asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(q_start) : "l"(w));
         asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(Sq) : "l"(w + 1));
     }
 #pragma unroll
@@ -279,7 +281,7 @@ __global__ void __launch_bounds__(kFaThreads, 1) flash_attn_tc_kernel(const __gr
         const int qi = qt0 + r0 + 8 * r;
         if (qi >= Sq) continue;
         const float inv = 1.0f / l[r];
-        const size_t off = (size_t)(a.q0 + seg0 + qi) * a.o_tok_stride + (size_t)head * a.o_head_stride + c0;
+        const size_t off = (size_t)(a.q0 + q_start + qi) * a.o_tok_stride + (size_t)head * a.o_head_stride + c0;
 #pragma unroll
         for (int j = 0; j < HD / 8; ++j) {
             const float x = o[4 * j + 2 * r] * inv, y = o[4 * j + 2 * r + 1] * inv;
@@ -345,14 +347,14 @@ inline void flash_attn_tc(cudaStream_t st, const FlashArgs& a, int nheads, bool 
     else flash_attn_tc_kernel<HD, false><<<grid, kFaThreads, smem, st>>>(L.tqh, L.tql, L.tkh, L.tkl, L.tvh, L.tvl, L.m);
     AHA_CUDA_CHECK(cudaGetLastError());
 }
-// Causal attention over independent segments packed back to back (head_dim 128; packed embeddings).  `a` covers the whole pack
-// (Sq = Skv = T, q0 = kv0 = 0): the split pass runs once over it, then one launch of (n_work, nheads) CTAs.  work: device
-// [n_work][3] = (seg_start, seg_len, qt0), one item per 128-query tile of every segment.  `ws`: at least flash_tc_ws_halfs<128>(a) halfs.
-// seg_start is the innermost TMA coordinate of the V^T tiles, so it must keep them on a 16-byte boundary: callers pack segments on
-// multiples of 16 tokens.
+// Causal attention over independent segments packed back to back (head_dim 128; packed embeddings, packed admission).  `a` covers the
+// whole pack (Sq query rows, Skv key rows; q0 = kv0 = 0): the split pass runs once over it, then one launch of (n_work, nheads) CTAs.  work:
+// device [n_work][kFaWork] = (q_start, q_len, kv_start, kv_len, qt0), one item per 128-query tile of every segment; a segment without a
+// cached prefix has q_start = kv_start and q_len = kv_len.  `ws`: at least flash_tc_ws_halfs<128>(a) halfs.  kv_start is the innermost TMA
+// coordinate of the V^T tiles, so it must keep them on a 16-byte boundary: callers lay segments out on multiples of 16 tokens.
 inline void flash_attn_tc_varlen(cudaStream_t st, const FlashArgs& a, int nheads, const int* work, int n_work, __half* ws, int num_sms) {
     if (n_work == 0) return;
-    AHA_REQUIRE(a.Sq == a.Skv && a.q0 == 0 && a.kv0 == 0, "flash_attn_tc_varlen: the pack is its own key range");
+    AHA_REQUIRE(a.Sq <= a.Skv && a.q0 == 0 && a.kv0 == 0, "flash_attn_tc_varlen: the pack's key rows start at 0 and hold at least its query rows");
     FlashTcLaunch L = flash_tc_prepare<128>(st, a, nheads, ws, num_sms);
     L.m.work = work;
     flash_attn_tc_kernel<128, true, true><<<dim3(n_work, nheads), kFaThreads, flash_tc_smem_bytes<128>(), st>>>(L.tqh, L.tql, L.tkh, L.tkl, L.tvh, L.tvl, L.m);

@@ -222,27 +222,33 @@ inline void flash_dispatch(Ctx& c, const FlashArgs& a, int nheads, bool causal) 
     c.cnt.kernels++;
 }
 
-// Independent texts packed into one prefill (aha_b200_embed_batch, aha_b200_batch_add_many): each text attends only to itself, its RoPE
-// positions restart at 0 and its K/V take the packed cache slots [start, start + len) (which the pack's page table maps to the text's own pages
-// when batch_add_many composes it from the requests' slots).
+// Independent texts packed into one prefill (aha_b200_embed_batch, aha_b200_batch_add_many): each text attends only to itself and its K/V
+// take the packed cache slots [start, start + len) (which the pack's page table maps to the text's own pages when batch_add_many composes it
+// from the requests' slots).  Its RoPE positions restart at 0, or at its prefix length when batch_add_many found a cached prefix for it: then
+// the attention reads a second table, `d_read`, where the text's keys are its prefix pages followed by its own pages, at rows `kv`.
 struct PrefillSegments {
-    std::vector<std::pair<int, int>> segs;   // (start, len) of every text, in pack order
-    const int* d_work = nullptr;             // device [n_work][3] = (seg_start, seg_len, qt0): the work list of flash_attn_tc_varlen
+    std::vector<std::pair<int, int>> segs;   // (start, len) of every text's query rows, in pack order
+    std::vector<std::pair<int, int>> kv;     // (start, len) of every text's key rows in the read table; empty: the same as segs
+    const int* d_work = nullptr;             // device [n_work][kFaWork] = (q_start, q_len, kv_start, kv_len, qt0): flash_attn_tc_varlen's list
     int n_work = 0;
+    const int* d_read = nullptr;             // device page table of the key rows (kv non-empty), null: the pack's own table
+    int kv_rows = 0;                         // key rows of the read table (kv non-empty)
     bool empty() const { return segs.empty(); }
 };
-// Causal attention inside every segment of a pack (`a` covers the whole pack: Sq = Skv = T, q0 = kv0 = 0).  attn_impl 0: one launch of the
-// varlen wgmma kernel; the SIMT and mma.sync twins run one flash_dispatch per segment, as the ViT runs its segments.
+// Causal attention inside every segment of a pack (`a` covers the whole pack: Sq query rows, Skv key rows, q0 = kv0 = 0).  attn_impl 0: one
+// launch of the varlen wgmma kernel; the SIMT and mma.sync twins run one flash_dispatch per segment, as the ViT runs its segments.
 inline void flash_dispatch_segments(Ctx& c, const FlashArgs& a, int nheads, const PrefillSegments& sg) {
+    const std::vector<std::pair<int, int>>& kv = sg.kv.empty() ? sg.segs : sg.kv;
     if (c.attn_impl == 0) {
-        for (const auto& s : sg.segs) AHA_REQUIRE(s.first % 16 == 0, "packed segments must start on multiples of 16 tokens");
+        for (const auto& s : kv) AHA_REQUIRE(s.first % 16 == 0, "packed segments must start on multiples of 16 tokens");
         flash_attn_tc_varlen(c.stream, a, nheads, sg.d_work, sg.n_work, c.split_buf((flash_tc_ws_halfs<128>(a, nheads) + 1) / 2), c.num_sms);
         c.cnt.kernels += 2;
         return;
     }
-    for (const auto& s : sg.segs) {
+    for (size_t j = 0; j < sg.segs.size(); ++j) {
         FlashArgs f = a;
-        f.Sq = f.Skv = s.second; f.q0 = f.kv0 = s.first;
+        f.Sq = sg.segs[j].second; f.q0 = sg.segs[j].first;
+        f.Skv = kv[j].second; f.kv0 = kv[j].first;
         flash_dispatch<128>(c, f, nheads, true);
     }
 }
@@ -430,6 +436,7 @@ struct PagePool {
     void reset() {
         free.clear();
         for (int p = 0; p < num_pages; ++p) free.push_back(p);
+        refs.assign(num_pages, 0);
     }
     // map pages to `t` until it covers n_tokens, and upload the new entries
     void map(PageTable& t, int n_tokens) {
@@ -441,13 +448,28 @@ struct PagePool {
         const int first = t.mapped;
         while (t.mapped < need) {
             t.h[t.mapped++] = free.back();
+            refs[free.back()] = 1;
             free.pop_back();
         }
         AHA_CUDA_CHECK(cudaMemcpyAsync(t.d + first, t.h.data() + first, (size_t)(t.mapped - first) * sizeof(int), cudaMemcpyHostToDevice, stream));
     }
     void release(PageTable& t) {
-        for (int k = 0; k < t.mapped; ++k) free.push_back(t.h[k]);
+        for (int k = 0; k < t.mapped; ++k) unref(t.h[k]);
         t.mapped = 0;
+    }
+    // Shared pages (a batch session's prefix cache): `refs` counts the tables and index entries that hold each page, and a page returns to the
+    // free list when the last one lets go.  map() hands out pages with one reference.
+    std::vector<int> refs;
+    void ref(int p) { ++refs[p]; }
+    void unref(int p) {
+        AHA_REQUIRE(refs[p] > 0, "KV pool: page " + std::to_string(p) + " released more often than it was taken");
+        if (--refs[p] == 0) free.push_back(p);
+    }
+    // t (empty) starts with `pages`, which other holders keep as well; map() then adds the table's own pages behind them
+    void share(PageTable& t, const std::vector<int>& pages) {
+        AHA_REQUIRE(t.mapped == 0, "KV pool: shared pages go first into an empty table");
+        for (int p : pages) { ref(p); t.h[t.mapped++] = p; }
+        if (t.mapped) AHA_CUDA_CHECK(cudaMemcpyAsync(t.d, t.h.data(), (size_t)t.mapped * sizeof(int), cudaMemcpyHostToDevice, stream));
     }
 };
 
@@ -801,6 +823,7 @@ struct TextModel {
             fa.q = qkv; fa.q_tok_stride = qkv_dim; fa.q_head_stride = hd; fa.kv = kv;
             fa.out = attn; fa.o_tok_stride = (size_t)nh_l * hd; fa.o_head_stride = hd;
             fa.Sq = S; fa.Skv = pos0 + S; fa.q0 = 0; fa.kv0 = 0; fa.groups = nh_l / nkv_l; fa.scaling = scaling;
+            if (segs.d_read) { fa.kv.page_table = segs.d_read; fa.Skv = segs.kv_rows; }   // the qk-norm / RoPE kernel above still writes through pt
             if (ps) {
                 ActSplit ao = act_split(c, 1, (size_t)S * std::max(nh_l * hd, I_l));
                 fa.out_hi = ao.hi; fa.out_lo = ao.lo;

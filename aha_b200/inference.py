@@ -309,6 +309,27 @@ class B200Model:
                                                        i32(po), 1 if split_out else 0, f(q), f(k), f(v), f(out)))
         return out
 
+    def debug_prefix_attention(self, q, k, v, impl, segments, page_order=None):
+        """Packed prefill attention over segments with cached prefixes on host data (aha_b200_debug_prefix_attention): segments
+        [(prefix, rows), ...]; q [sum rows][nh][128], k / v [sum (prefix + rows)][nkv][128] laid out segment by segment -> [sum rows][nh][128].
+        impl 0 = wgmma varlen kernel, 1 = SIMT, 2 = mma.sync."""
+        q = np.ascontiguousarray(q, np.float32)
+        k = np.ascontiguousarray(k, np.float32)
+        v = np.ascontiguousarray(v, np.float32)
+        seg = np.ascontiguousarray(np.asarray(segments, np.int32).reshape(-1, 2))
+        Sq, nh, hd = q.shape
+        Skv, nkv = k.shape[:2]
+        if hd != 128 or Sq != int(seg[:, 1].sum()) or Skv != int(seg.sum()) or k.shape != (Skv, nkv, 128) or v.shape != k.shape:
+            raise ValueError("q [sum rows][nh][128], k and v [sum (prefix + rows)][nkv][128]")
+        po = None if page_order is None else np.ascontiguousarray(page_order, np.int32)
+        if po is not None and po.size != -(-Skv // 32):
+            raise ValueError("page_order needs one entry per 32-token page")
+        out = np.empty_like(q)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32)) if a is not None and a.size else None
+        self._check(self._lib.aha_b200_debug_prefix_attention(self._h, int(impl), nh, nkv, i32(seg), len(seg), i32(po), f(q), f(k), f(v), f(out)))
+        return out
+
     def debug_decode_attn(self, qkv, pos, rope_delta, k_cache, v_cache, tables, n_pool_pages, q_norm, k_norm, n_heads, n_kv_heads,
                           eps=1e-6, rope_theta=1e6):
         """The decode attention on host data (aha_b200_debug_decode_attn) for B sequences: qkv [B][(nh + 2 nkv) * 128] raw
@@ -516,6 +537,20 @@ class B200Model:
 
     def batch_close(self):
         self._check(self._lib.aha_b200_batch_close(self._h))
+
+    def batch_prefix_cache(self, max_tokens):
+        """Turn the open session's prefix cache on (aha_b200_batch_prefix_cache): admitted text-only prompts leave their full 32-token
+        pages in an index that keeps up to max_tokens / 32 of them alive, and later requests that start with those pages share them and
+        prefill only what follows.  0 turns it off and releases the pages only the index holds."""
+        self._check(self._lib.aha_b200_batch_prefix_cache(self._h, int(max_tokens)))
+
+    def batch_prefix_stats(self):
+        """-> (stats dict: cached_pages, shared_pages, hit_tokens, lookups, evicted_pages, max_pages, free_pages; {slot: prompt tokens its running
+        request took from the cache} for every slot with a request that hit)."""
+        w = getattr(self, "_batch_width", 8)
+        st, hits = L.PrefixStats(), (C.c_size_t * w)()
+        self._check(self._lib.aha_b200_batch_prefix_stats(self._h, C.byref(st), hits, w))
+        return {name: int(getattr(st, name)) for name, _ in L.PrefixStats._fields_}, {i: int(hits[i]) for i in range(w) if hits[i]}
 
     def generate_stream(self, input_ids, on_token, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None,
                         repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None,

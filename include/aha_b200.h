@@ -318,6 +318,34 @@ int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out /* [cap] */, int32_
  * without such requests launches exactly the kernels it launched before. */
 int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out /* [cap] */, size_t cap);
 
+/* Prefix cache of a batch session (narrow or wide; new design).  With max_tokens > 0 the session keeps an index of the full 32-token KV pages
+ * of admitted text-only prompts (batch_add, batch_add_many, choice 0 of batch_add_n), keyed by their token ids and the page before them,
+ * and keeps up to max_tokens / 32 of those pages alive after their requests finish.  A later request whose prompt starts with cached pages
+ * maps them into its page table (shared, read-only, reference counted) and prefills only what follows.  Its hit is the longest cached chain
+ * of pages that starts its prompt, at most seq_len - 1 tokens and, unless aha_options.gemm_impl is 1, at most seq_len - 32 (at least 32
+ * prompt tokens still run, on the same GEMM as the cold prefill of those rows); only pages cached before the call count, and requests with
+ * multimodal tensors neither hit nor insert.  Admission then needs ceil((seq_len + max_tokens) / 32) minus the hit's pages, from the free
+ * pages plus the pages only the index holds (those this call does not hit); it evicts least-recently-used leaves only as far as it needs,
+ * after every check passed, so a refused call leaves the session and the index unchanged.  Inserting beyond max_tokens evicts LRU pages
+ * only the index holds, and skips the insert when there is none.
+ * Results: a request of at most min(max_prefill, max_ctx) prompt tokens yields exactly the ids and log-probability records it yields
+ * admitted cold through the same entry in the same session kind.  Longer prompts may hit too; their chunks move with the hit.
+ * max_tokens 0 turns the cache off and releases every page only the index holds; batch_close and clear_cache drop the index with the
+ * session.  A session that never calls this runs exactly as before.  usage.prompt_tokens keeps counting the whole prompt. */
+int aha_b200_batch_prefix_cache(aha_model* m, size_t max_tokens);
+typedef struct aha_prefix_stats {
+    uint64_t cached_pages;           /* pages the index holds */
+    uint64_t shared_pages;           /* of those, pages a running request's table holds as well */
+    uint64_t hit_tokens;             /* prompt tokens admitted requests took from the cache in this session */
+    uint64_t lookups;                /* text-only requests admitted while it was on */
+    uint64_t evicted_pages;          /* pages evicted to make room (not those max_tokens 0 released) */
+    uint64_t max_pages;              /* max_tokens / 32 */
+    uint64_t free_pages;             /* pages of the KV pool no table and no index entry holds */
+} aha_prefix_stats;
+/* The prefix cache's counters; hits_out (NULL, or [cap] with cap >= the session width): per slot, the prompt tokens its running request
+ * took from the cache (0 for a free slot) -- what a server reports as usage.prompt_tokens_details.cached_tokens. */
+int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hits_out, size_t cap);
+
 /* WhisperFeatureExtractor::call (src/models/feature_extractor/
  * feature_extraction_whisper.rs:65-115): wave (n) f32 host -> log-mel (n_mels, n_frames) f32 host.
  * Returns frames through *n_frames.  Qwen3-ASR handles only. */
@@ -592,6 +620,13 @@ int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t
 int aha_b200_debug_attention(aha_model* m, int impl, int head_dim, size_t n_heads, size_t n_kv_heads, size_t sq, size_t skv, int causal,
                              const int32_t* segments, size_t n_segments, const int32_t* page_order, int split_out, const float* q,
                              const float* k, const float* v, float* out);
+/* The packed prefill attention over segments with cached prefixes (batch_add_many after prefix-cache hits) on host data: segment j =
+ * segments[2 j .. 2 j + 1] = (prefix p_j, rows q_j) has q_j query rows, laid after the previous segment's, and p_j + q_j keys, laid after
+ * the previous segment's keys (at multiples of 16 rows); query i of segment j sees its keys 0 .. p_j + i.  q [sum q_j][n_heads][128],
+ * k / v [sum (p_j + q_j)][n_kv_heads][128] on a paged pool (logical page p at physical page page_order[p], NULL: identity; every other
+ * slot NaN) -> out [sum q_j][n_heads][128].  impl 0 = the wgmma varlen kernel, 1 = SIMT, 2 = mma.sync (one launch per segment). */
+int aha_b200_debug_prefix_attention(aha_model* m, int impl, size_t n_heads, size_t n_kv_heads, const int32_t* segments, size_t n_segments,
+                                    const int32_t* page_order, const float* q, const float* k, const float* v, float* out);
 /* the decode attention on host data (tests): `batch` sequences, head_dim 128, n_heads / n_kv_heads in {1, 2, 4, 6}.  batch 1 runs
  * decode_attn_kernel, more run decode_attn_batch_kernel, both over kDecodeSplits splits.  Sequence b: qkv row b of
  * [batch][(n_heads + 2 n_kv_heads) * 128] (raw projections), position pos[b] (tokens already cached), rope_delta[b]; its cached K / V are the

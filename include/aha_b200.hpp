@@ -308,6 +308,15 @@ public:
         return out;
     }
     size_t last_prefix_hit() const { return aha_b200_last_prefix_hit(h_); }
+    // The open batch session's prefix cache (aha_b200_batch_prefix_cache / _stats): on with max_tokens > 0, off (its pages released) with 0.
+    // batch_prefix_stats' hits: per slot of the session (width entries), the prompt tokens its running request took from the cache.
+    void batch_prefix_cache(size_t max_tokens) { check(aha_b200_batch_prefix_cache(h_, max_tokens)); }
+    aha_prefix_stats batch_prefix_stats(std::vector<size_t>* hits = nullptr, size_t width = 64) const {
+        aha_prefix_stats st{};
+        if (hits) hits->assign(width, 0);
+        check(aha_b200_batch_prefix_stats(h_, &st, hits ? hits->data() : nullptr, hits ? width : 0));
+        return st;
+    }
     // Prefill continuation (aha_b200_forward_extend): further prompt tokens against the `off` tokens already in the cache.
     std::vector<float> forward_extend(const std::vector<uint32_t>& ids, size_t off) {
         std::vector<float> logits(need_vocab());
