@@ -127,6 +127,7 @@ LOGPROBS_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.P
 
 
 SPEC_PROMPT_LOOKUP = 1
+SPEC_MAX_ROWS = 16
 SPEC_MAX_DRAFT = 15
 SPEC_MAX_NGRAM = 8
 
@@ -211,6 +212,13 @@ SYMBOLS = {
     "aha_b200_generate_speculative": (C.c_int, [_P, _U32P, C.c_size_t, C.POINTER(MM), C.POINTER(GenParams), C.POINTER(SpecParams), _U32P,
                                                 C.POINTER(Logprobs), C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(Usage), C.POINTER(SpecStats)]),
     "aha_b200_debug_verify_attn": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _F32P, _F32P, _F32P]),
+    "aha_b200_debug_verify_attn_batch": (C.c_int, [_P, C.c_size_t, _I32P, _I32P, _I32P, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _F32P, _F32P,
+                                                   _F32P]),
+    "aha_b200_batch_add_speculative": (C.c_int, [_P, C.POINTER(BatchRequest), C.POINTER(SpecParams), C.POINTER(C.c_int32), _U32P,
+                                                 C.POINTER(C.c_int32), C.POINTER(Usage)]),
+    "aha_b200_batch_step_spec": (C.c_int, [_P, _U32P, _U32P, C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "aha_b200_batch_logprobs_spec": (C.c_int, [_P, C.POINTER(Logprobs), C.c_size_t]),
+    "aha_b200_batch_spec_stats": (C.c_int, [_P, C.POINTER(SpecStats), C.c_size_t]),
     "aha_b200_debug_attention": (C.c_int, [_P, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int, _I32P, C.c_size_t,
                                            _I32P, C.c_int, _F32P, _F32P, _F32P, _F32P]),
     "aha_b200_debug_decode_attn": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, _F32P, _I32P, _I32P, _F32P, _F32P, _I32P, C.c_size_t,

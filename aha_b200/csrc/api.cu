@@ -188,9 +188,13 @@ struct aha_model {
         bool lp_valid[kWideSeqs] = {};  // the slot's record row holds the record of the last token its request delivered
         size_t hit[kWideSeqs] = {};     // prompt tokens the slot's request took from the prefix cache
         PrefixIndex prefix;             // aha_b200_batch_prefix_cache; dropped with the session
+        // speculative requests (aha_b200_batch_add_speculative, wide sessions only)
+        bool spec[kWideSeqs] = {};      // the slot runs a speculative request
+        aha_spec_stats spec_stats[kWideSeqs] = {};   // its counters, kept after it finishes until the slot is taken again
+        int last_n[kWideSeqs] = {};     // tokens the slot's last speculative pass delivered (0: its last token came from admission or a plain step)
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
-    SpecDecoder spec;                   // speculative single requests (aha_b200_generate_speculative) on wide_batch's buffers
+    SpecDecoder spec;                   // speculative requests (generate_speculative, batch_add_speculative) on wide_batch's buffers
     // scoring (aha_b200_score / _score_batch): the buffers of one head launch over up to max_prefill rows and the lm_head's tensor map,
     // set up by the first scoring call
     struct ScoreBufs {
@@ -650,6 +654,8 @@ struct RequestReset {
 // ends the batch session, if one is open, and leaves the handle as clear_cache() does
 void session_close(aha_model* m) {
     for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->reset();
+    m->spec.steps.clear();
+    m->spec.built_epoch = ~0ull;
     m->session = aha_model::BatchSession{};
     drop_cache(m);
     m->text.clear_sampler();
@@ -1158,13 +1164,10 @@ void generate_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_
 
 // generate_impl's request in verify passes (speculative.cuh): the same prefill, first token, Reset guard and Usage split; then passes of
 // R = max_draft + 1 rows in bursts, the emitted tokens (and records) read from the request's history after each burst.
-void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params& params,
-                               const aha_spec_params& sp, uint32_t* out_tokens, aha_logprobs* out_lp, size_t cap, size_t* n_out, aha_usage* usage,
-                               aha_spec_stats* stats) {
+// The checks every speculative request passes before any device work (generate_speculative, batch_add_speculative) -> its ngram
+int spec_request_check(aha_model* m, const aha_gen_params& params, const aha_spec_params& sp, const std::string& who) {
     TextModel& T = m->text;
-    const std::string who = "generate_speculative: ";
     AHA_REQUIRE(T.tp_world == 1, who + "speculative decoding is single-GPU");
-    require_no_session(m);
     AHA_REQUIRE(m->kind != aha_model::QWEN3_ASR, who + "Qwen3-ASR handles decode through asr_generate");
     AHA_REQUIRE(BatchDecoder::wide_shapes_ok(T) && T.cfg.hd == 128,
                 who + "every projection's rows and columns must be multiples of 64 and head_dim 128 (hidden " + std::to_string(T.cfg.H) +
@@ -1182,6 +1185,16 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
     AHA_REQUIRE(request_rules(m, params, who).fsm == nullptr,
                 who + "logit rules that name a token automaton are not supported with speculative decoding (a verify row's mask would depend on "
                       "the drafts before it)");
+    return ngram;
+}
+
+void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const aha_mm* mm, const aha_gen_params& params,
+                               const aha_spec_params& sp, uint32_t* out_tokens, aha_logprobs* out_lp, size_t cap, size_t* n_out, aha_usage* usage,
+                               aha_spec_stats* stats) {
+    TextModel& T = m->text;
+    const std::string who = "generate_speculative: ";
+    require_no_session(m);
+    const int ngram = spec_request_check(m, params, sp, who);
     const int lp_n = logprob_request(params, T, who);
     AHA_REQUIRE(lp_n < 0 || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
     const size_t sample_len = token_budget(params);
@@ -1190,7 +1203,7 @@ void generate_speculative_impl(aha_model* m, const uint32_t* ids, size_t seq_len
     AHA_REQUIRE(need <= (size_t)T.max_ctx, who + "prompt + max_tokens + max_draft = " + std::to_string(need) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
     const int R = (int)sp.max_draft + 1;
     SpecDecoder& S = m->spec;
-    S.init(T, m->wide_batch);
+    S.init(T, m->wide_batch, kSpecMaxRows);
     request_logprobs(m, lp_n);
     const auto t0 = clk::now();
     drop_cache(m);
@@ -1304,13 +1317,33 @@ void session_release(aha_model* m, int slot) {
     sl.lp = 0;
     m->session.used[slot] = false;
     m->session.hit[slot] = 0;
+    m->session.spec[slot] = false;
     m->sess().composition_changed();
+}
+// verify rows of the running requests: R for a speculative request, 1 for a plain one
+int session_rows(const aha_model* m) {
+    int rows = 0;
+    for (int i = 0; i < m->session.width; ++i) if (m->session.used[i]) rows += m->session.spec[i] ? m->spec.slots[i].R : 1;
+    return rows;
+}
+bool session_has_spec(const aha_model* m) {
+    for (int i = 0; i < m->session.width; ++i) if (m->session.used[i] && m->session.spec[i]) return true;
+    return false;
+}
+// Beside speculative requests a step's rows must fit the wide kernel's 64-row B tile: `rows` more must fit what runs.  Without speculative
+// requests the rows are the running slots, which the session width already bounds.
+void session_check_rows(const aha_model* m, int rows, const std::string& who) {
+    const int now = session_rows(m);
+    AHA_REQUIRE(now + rows <= kWideSeqs, who + "the step rows of the running requests (" + std::to_string(now) + ", a speculative request counts "
+                                                "max_draft + 1) plus " + std::to_string(rows) + " exceed " + std::to_string(kWideSeqs));
 }
 // the bookkeeping of a request admitted into slot s with its first token: true (and the slot released) when that token is also its last
 bool session_admitted(aha_model* m, int s, size_t sample_len, int lp_n, uint32_t flags, uint32_t tok) {
     m->session.budget[s] = sample_len;
     m->session.produced[s] = 1;
     m->session.lp_valid[s] = lp_n >= 0;
+    m->session.spec_stats[s] = aha_spec_stats{};
+    m->session.last_n[s] = 0;
     bool stop = sample_len == 1;
     if ((flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok) stop = true;
     if (stop) session_release(m, s);
@@ -1376,6 +1409,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) + " of the " + width +
                                       " slots are free (step until requests finish)");
     slot.resize(n);
+    if (session_has_spec(m)) session_check_rows(m, (int)n, who);
     std::vector<size_t> sample_len(n), hit(n);
     std::vector<bool> packed(n), text_only(n);
     std::vector<int> lp_n(n);
@@ -1528,6 +1562,7 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " choices, but only " + std::to_string(slot.size()) + " of the " +
                                       std::to_string(m->session.width) + " slots are free (step until requests finish)");
     slot.resize(n);
+    if (session_has_spec(m)) session_check_rows(m, (int)n, who);
     AHA_REQUIRE(req.ids && req.seq_len >= 1, who + "the request needs input_ids");
     const int lp_n = logprob_request(req.params, T, who);
     for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
@@ -1599,6 +1634,155 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
         slots_out[i] = slot[i]; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
     }
 }
+size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8);
+
+// One speculative request into the lowest free slot of the open wide session (aha_b200_batch_add_speculative): admitted as batch_add admits it
+// (prefilled alone on the slot's table, prefix-cache hit and insert included), with pages for max_draft more positions, and from then on
+// stepped in verify passes of R = max_draft + 1 rows by session_step_spec.  Its control block is the slot's; drafts come from the slot's
+// copy of the prediction and prompt.
+void session_add_spec(aha_model* m, const aha_batch_request& req, const aha_spec_params& sp, int32_t* slot_out, uint32_t* first_token,
+                      int32_t* finished, aha_usage* usage) {
+    TextModel& T = m->text;
+    const std::string who = "batch_add_speculative: ";
+    // ---- every check before any device work: a refused call leaves the session untouched
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    AHA_REQUIRE(m->session.wide, who + "speculative requests need a wide session (aha_b200_batch_open_wide): a narrow session promises the ids of "
+                                       "single-request runs, which verify passes cannot keep");
+    const int ngram = spec_request_check(m, req.params, sp, who);
+    int slot = -1;
+    for (int i = 0; i < m->session.width && slot < 0; ++i) if (!m->session.used[i]) slot = i;
+    AHA_REQUIRE(slot >= 0, who + "all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
+    const int R = (int)sp.max_draft + 1;
+    session_check_rows(m, R, who);
+    AHA_REQUIRE(req.ids && req.seq_len >= 1, who + "the request needs input_ids");
+    const int lp_n = logprob_request(req.params, T, who);
+    for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
+    require_mm_arity(m, req.mm);
+    const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len + sp.max_draft;
+    AHA_REQUIRE(ctx <= (size_t)T.max_ctx, who + "prompt + max_tokens + max_draft = " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
+    bool has_mm = false;
+    for (size_t k = 0; m->kind != aha_model::QWEN3 && k < req.mm->n; ++k) has_mm = has_mm || mm_entry(req.mm, k) != nullptr;
+    const std::vector<int> hit_pages = prefix_hit(m, req.ids, req.seq_len, has_mm);
+    const size_t hit = hit_pages.size() * kPage;
+    const size_t pages = (size_t)ceil_div((int)ctx, kPage) - hit_pages.size();
+    const std::set<int> keep(hit_pages.begin(), hit_pages.end());
+    prefix_check_room(m, pages, keep, who + "the request needs ");
+    const Sampler samp = request_sampler(m, req.params, who);
+    SpecDecoder& S = m->spec;
+    BatchDecoder& B = m->sess();
+    prefix_make_room(m, pages, keep);
+    const auto t0 = clk::now();
+    const std::vector<int> slots{slot};
+    AdmitGuard guard{m, slots};
+    m->session.used[slot] = true;
+    prefix_share(m, slot, hit_pages, req.seq_len);
+    S.init(T, B, kWideSeqs);
+    const uint32_t tok = batch_prefill_slot(m, slot, req, sample_len, lp_n, hit);
+    T.pages.map(B.slots[slot].table, (int)ctx);   // the positions of the last pass's drafts
+    if (sample_len > 1) {
+        const std::vector<uint32_t> pred(sp.prediction, sp.prediction + sp.n_prediction);
+        const bool lookup = (sp.flags & AHA_SPEC_PROMPT_LOOKUP) != 0;
+        const int lp_on = lp_n >= 0 ? lp_n + 1 : 0;
+        S.set_ctl(slot, samp, pred, req.ids, lookup ? req.seq_len : 0, m->stop_ids, (int)sample_len, ngram, lp_on, B.d_states + slot,
+                  B.d_hist + (size_t)slot * T.hist_cap, S.d_slot_lp + (size_t)slot * kSpecMaxRows, 0, lp_on ? B.d_lp_rec + slot : nullptr);
+        S.slots[slot].R = R; S.slots[slot].samp = samp; S.slots[slot].lp = lp_on;
+    }
+    const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
+    guard.ok = true;
+    if (!has_mm) prefix_admitted(m, slot, req.ids, req.seq_len, hit);
+    T.clear_sampler();
+    B.composition_changed();
+    const bool stop = session_admitted(m, slot, sample_len, lp_n, req.params.flags, tok);
+    m->session.spec[slot] = !stop;
+    if (usage) {
+        *usage = aha_usage{};
+        add_usage(usage, req.seq_len, 1, secs, 0.0, vision);
+    }
+    *slot_out = slot; *first_token = tok; *finished = stop ? 1 : 0;
+}
+
+// One step of every running request (aha_b200_batch_step_spec): without a speculative request exactly session_step, else one mixed launch --
+// a decode step of the plain slots and a verify pass of every speculative slot.  tokens_out [cap][kSpecMaxRows], n_tokens / status [cap].
+size_t session_step_spec(aha_model* m, uint32_t* tokens_out, uint32_t* n_tokens, int32_t* status_out, size_t cap) {
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    const int width = m->session.width;
+    AHA_REQUIRE(cap >= (size_t)width, "batch_step_spec: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+    for (size_t i = 0; i < cap * kSpecMaxRows; ++i) tokens_out[i] = 0;
+    for (size_t i = 0; i < cap; ++i) n_tokens[i] = 0;
+    if (!session_has_spec(m)) {
+        std::vector<uint32_t> tok(cap);
+        const size_t n = session_step(m, tok.data(), status_out, cap, false);
+        for (size_t i = 0; i < cap; ++i) if (status_out[i]) { tokens_out[i * kSpecMaxRows] = tok[i]; n_tokens[i] = 1; }
+        return n;
+    }
+    for (size_t i = 0; i < cap; ++i) status_out[i] = 0;
+    std::vector<int> plain, spec;
+    for (int i = 0; i < width; ++i) if (m->session.used[i]) (m->session.spec[i] ? spec : plain).push_back(i);
+    BatchDecoder& B = m->sess();
+    SpecDecoder& S = m->spec;
+    Ctx& c = m->ctx;
+    S.step(plain, spec);
+    std::vector<uint32_t> h_tok((size_t)B.cap);
+    std::vector<DecodeState> h_st((size_t)B.cap);
+    std::vector<SpecCtl> h_ctl((size_t)kWideSeqs);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(h_ctl.data(), S.d_ctl, h_ctl.size() * sizeof(SpecCtl), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    for (int s : spec) {   // the tokens the pass emitted: history [produced, n_hist)
+        const size_t E0 = m->session.produced[s], n = (size_t)h_st[s].n_hist - E0;
+        AHA_REQUIRE(n >= 1 && n <= (size_t)kSpecMaxRows, "batch_step_spec: a verify pass emitted no token");
+        AHA_CUDA_CHECK(cudaMemcpyAsync(tokens_out + (size_t)s * kSpecMaxRows, B.d_hist + (size_t)s * m->text.hist_cap + E0, n * sizeof(uint32_t),
+                                       cudaMemcpyDeviceToHost, c.stream));
+    }
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    for (int s : plain) {
+        const uint32_t t = h_tok[s];
+        tokens_out[(size_t)s * kSpecMaxRows] = t;
+        n_tokens[s] = 1;
+        m->session.produced[s] += 1;
+        m->session.lp_valid[s] = B.slots[s].lp > 0;
+        bool stop = m->session.produced[s] >= m->session.budget[s];
+        for (uint32_t e : m->stop_ids) if (e == t) stop = true;     // an EOS token is delivered, then the request ends (generate.rs:139-141)
+        status_out[s] = stop ? 2 : 1;
+    }
+    for (int s : spec) {
+        const SpecCtl& k = h_ctl[s];
+        const size_t n = (size_t)h_st[s].n_hist - m->session.produced[s];
+        n_tokens[s] = (uint32_t)n;
+        m->session.produced[s] += n;
+        m->session.last_n[s] = (int)n;
+        m->session.lp_valid[s] = S.slots[s].lp > 0;
+        m->session.spec_stats[s] = aha_spec_stats{k.passes, k.drafted, k.accepted, 0};
+        status_out[s] = k.done ? 2 : 1;   // (the accept kernel applies EOS and max_tokens)
+    }
+    for (int s : plain) m->session.last_n[s] = 0;
+    for (int i = 0; i < width; ++i) if (status_out[i] == 2) session_release(m, i);
+    m->text.check_sample_error();
+    return plain.size() + spec.size();
+}
+
+// per slot of the open session, the records of every token its request delivered last (out [width][kSpecMaxRows]; zero records elsewhere)
+std::vector<aha_logprobs> session_records_spec(aha_model* m) {
+    const int width = m->session.width;
+    BatchDecoder& B = m->sess();
+    std::vector<aha_logprobs> last((size_t)width), rows;
+    std::vector<aha_logprobs> out((size_t)width * kSpecMaxRows);
+    if (B.d_lp_rec) AHA_CUDA_CHECK(cudaMemcpyAsync(last.data(), B.d_lp_rec, last.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+    if (m->spec.d_slot_lp) {
+        rows.resize((size_t)width * kSpecMaxRows);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(rows.data(), m->spec.d_slot_lp, rows.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+    }
+    AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+    for (int i = 0; i < width; ++i) {
+        if (!m->session.lp_valid[i]) continue;
+        const int n = m->session.last_n[i];
+        if (n == 0) out[(size_t)i * kSpecMaxRows] = last[i];
+        else for (int k = 0; k < n; ++k) out[(size_t)i * kSpecMaxRows + k] = rows[(size_t)i * kSpecMaxRows + k];
+    }
+    return out;
+}
+
 // tokens_out / status_out: [cap] entries, cap >= the session width (8 for batch_step)
 size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8) {
     AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
@@ -1608,6 +1792,8 @@ size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, siz
     AHA_REQUIRE(cap >= (size_t)width, "batch_step_n: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
     std::vector<int> act;
     for (size_t i = 0; i < cap; ++i) { status_out[i] = 0; tokens_out[i] = 0; }
+    AHA_REQUIRE(!session_has_spec(m), std::string(step8 ? "batch_step" : "batch_step_n") +
+                                          ": a speculative request is running: step the session with aha_b200_batch_step_spec");
     for (int i = 0; i < width; ++i) if (m->session.used[i]) act.push_back(i);
     if (act.empty()) return 0;
     BatchDecoder& B = m->sess();
@@ -1801,6 +1987,43 @@ int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out, size_t cap) {
         AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
         const std::vector<aha_logprobs> h = session_records(m);
         for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? h[i] : aha_logprobs{};
+    });
+}
+
+int aha_b200_batch_add_speculative(aha_model* m, const aha_batch_request* req, const aha_spec_params* spec, int32_t* slot_out,
+                                   uint32_t* first_token_out, int32_t* finished_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(req && spec && slot_out && first_token_out && finished_out, "req, spec, slot_out, first_token_out and finished_out are required");
+        session_add_spec(m, *req, *spec, slot_out, first_token_out, finished_out, usage);
+    });
+}
+
+int aha_b200_batch_step_spec(aha_model* m, uint32_t* tokens_out, uint32_t* n_tokens_out, int32_t* status_out, size_t cap, size_t* n_stepped_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(tokens_out && n_tokens_out && status_out, "tokens_out[cap][16], n_tokens_out[cap] and status_out[cap] are required");
+        const size_t n = session_step_spec(m, tokens_out, n_tokens_out, status_out, cap);
+        if (n_stepped_out) *n_stepped_out = n;
+    });
+}
+
+int aha_b200_batch_logprobs_spec(aha_model* m, aha_logprobs* out, size_t cap) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        AHA_REQUIRE(out, "batch_logprobs_spec: out[cap][16] is required");
+        const int width = m->session.width;
+        AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs_spec: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+        const std::vector<aha_logprobs> h = session_records_spec(m);
+        for (size_t i = 0; i < cap * kSpecMaxRows; ++i) out[i] = i < h.size() ? h[i] : aha_logprobs{};
+    });
+}
+
+int aha_b200_batch_spec_stats(aha_model* m, aha_spec_stats* out, size_t cap) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        AHA_REQUIRE(out, "batch_spec_stats: out[cap] is required");
+        const int width = m->session.width;
+        AHA_REQUIRE(cap >= (size_t)width, "batch_spec_stats: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+        for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? m->session.spec_stats[i] : aha_spec_stats{};
     });
 }
 
@@ -2009,44 +2232,89 @@ void debug_decode_launch(cudaStream_t st, int B, int nkv, const DecodeAttnArgs& 
 }  // namespace
 }  // extern "C++"
 
+extern "C++" {
+namespace {
+// The verify attention over n requests on host data: request j has R[j] rows at positions pos0[j] .. pos0[j] + R[j] - 1 over its own page
+// table `tables[j]` (ceil((pos0[j] + R[j]) / 32) pages of one NaN pool); its K / V are rows [kv_off[j], kv_off[j] + pos0[j] + R[j]) of k / v, its
+// q / out rows start at q_off[j].  ctas: grid.x of the attention (every request's chunks are spread over it).
+void debug_verify_run(aha_model* m, int n, const int* R, const int* pos0, const int* tables, int n_pool_pages, int nh, int nkv, const float* q,
+                      const float* k, const float* v, float* out, int ctas) {
+    constexpr int HD = 128;
+    Ctx& c = m->ctx;
+    AHA_REQUIRE(n >= 1 && n <= kWideSeqs, "debug_verify_attn: 1 to 64 requests");
+    AHA_REQUIRE(nkv >= 1 && nh >= nkv && nh % nkv == 0 && nh <= 64, "debug_verify_attn: bad head counts");
+    HostPool pool(n_pool_pages, nkv, HD);
+    int rows = 0, max_ctx = 0;
+    size_t kv_off = 0, t_off = 0;
+    std::vector<int> tab_off(n), row0(n);
+    for (int j = 0; j < n; ++j) {
+        AHA_REQUIRE(R[j] >= 1 && R[j] <= kSpecMaxRows && pos0[j] >= 0, "debug_verify_attn: every request needs 1 to 16 rows at a position >= 0");
+        const int ctx = pos0[j] + R[j];
+        pool.put(tables + t_off, ctx, k + kv_off * nkv * HD, v + kv_off * nkv * HD);
+        tab_off[j] = (int)t_off; row0[j] = rows;
+        t_off += ceil_div(ctx, kPage); kv_off += ctx; rows += R[j];
+        max_ctx = std::max(max_ctx, ctx);
+    }
+    AHA_REQUIRE(rows <= kWideSeqs, "debug_verify_attn: at most 64 rows in all");
+    std::vector<DecodeState> st(rows);
+    for (int j = 0; j < n; ++j) for (int r = 0; r < R[j]; ++r) st[row0[j] + r] = DecodeState{0, pos0[j] + r, 0, 0, 0, 0, {0, 0}};
+    const int max_chunks = ceil_div(max_ctx, kSpecChunk);
+    Scratch mem;
+    float* d_pool = upload_scratch(mem, c.stream, pool.data.data(), pool.data.size());
+    float* d_q = upload_scratch(mem, c.stream, q, (size_t)rows * nh * HD);
+    float* d_out = mem.alloc<float>((size_t)rows * nh * HD);
+    float* d_part = mem.alloc<float>((size_t)rows * nh * max_chunks * spec_part_stride(HD));
+    const int* d_tables = upload_scratch(mem, c.stream, tables, t_off);
+    std::vector<SpecReq> reqs(n);
+    for (int j = 0; j < n; ++j) reqs[j] = SpecReq{nullptr, d_tables + tab_off[j], row0[j], R[j], pos0[j] + R[j]};
+    const SpecReq* d_reqs = upload_scratch(mem, c.stream, reqs.data(), reqs.size());
+    DecodeState* d_st = upload_scratch(mem, c.stream, st.data(), st.size());
+    SpecAttnArgs a{};
+    a.q = d_q; a.ldq = nh * HD;
+    a.kv = pool.src(d_pool, nullptr);
+    a.reqs = d_reqs; a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
+    a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
+    spec_verify_attn_kernel<HD><<<dim3(std::max(1, std::min(ctas, max_chunks)), nkv, n), kSpecAttnThreads, spec_attn_smem_bytes<HD>(), c.stream>>>(a);
+    spec_verify_merge_kernel<HD><<<dim3(nh, rows), HD, 0, c.stream>>>(a);
+    AHA_CUDA_CHECK(cudaGetLastError());
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)rows * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
+}
+}  // namespace
+}  // extern "C++"
+
 int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
                                const float* v, float* out) {
     return guarded(m, [&] {
         AHA_REQUIRE(q && k && v && out, "q, k, v and out are required");
         AHA_REQUIRE(rows >= 1 && rows <= (size_t)kSpecMaxRows, "debug_verify_attn: rows must be 1 to " + std::to_string(kSpecMaxRows));
         AHA_REQUIRE(n_kv_heads >= 1 && n_heads >= n_kv_heads && n_heads % n_kv_heads == 0 && n_heads <= 64, "debug_verify_attn: bad head counts");
-        constexpr int HD = 128;
-        Ctx& c = m->ctx;
-        const int R = (int)rows, nh = (int)n_heads, nkv = (int)n_kv_heads;
-        const int ctx = (int)pos0 + R;
+        const int R = (int)rows, p0 = (int)pos0;
         // a paged pool with the pages in reverse order and one page no table references
-        const int np = ceil_div(ctx, kPage);
-        HostPool pool(np + 1, nkv, HD);
+        const int np = ceil_div(p0 + R, kPage);
         std::vector<int> table(np);
         for (int p = 0; p < np; ++p) table[p] = np - p;
-        pool.put(table.data(), ctx, k, v);
-        std::vector<DecodeState> st(R);
-        for (int r = 0; r < R; ++r) st[r] = DecodeState{0, (int)pos0 + r, 0, 0, 0, 0, {0, 0}};
-        const int max_chunks = ceil_div(ctx, kSpecChunk);
-        Scratch mem;
-        float* d_pool = upload_scratch(mem, c.stream, pool.data.data(), pool.data.size());
-        float* d_q = upload_scratch(mem, c.stream, q, (size_t)R * nh * HD);
-        float* d_out = mem.alloc<float>((size_t)R * nh * HD);
-        float* d_part = mem.alloc<float>((size_t)R * nh * max_chunks * spec_part_stride(HD));
-        const int* d_table = upload_scratch(mem, c.stream, table.data(), table.size());
-        DecodeState* d_st = upload_scratch(mem, c.stream, st.data(), st.size());
-        SpecAttnArgs a{};
-        a.q = d_q; a.ldq = nh * HD;
-        a.kv = pool.src(d_pool, d_table);
-        a.rows = d_st; a.partial = d_part; a.max_chunks = max_chunks; a.out = d_out; a.ldo = nh * HD;
-        a.R = R; a.nh = nh; a.nkv = nkv; a.scaling = (float)(1.0 / std::sqrt((double)HD));
-        AHA_CUDA_CHECK(cudaFuncSetAttribute(spec_verify_attn_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)spec_attn_smem_bytes<HD>()));
         // few CTAs, so that a CTA walks several chunks
-        spec_verify_attn_kernel<HD><<<dim3(std::min(3, max_chunks), nkv), kSpecAttnThreads, spec_attn_smem_bytes<HD>(), c.stream>>>(a);
-        spec_verify_merge_kernel<HD><<<dim3(nh, R), HD, 0, c.stream>>>(a);
-        AHA_CUDA_CHECK(cudaGetLastError());
-        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-        AHA_CUDA_CHECK(cudaMemcpy(out, d_out, (size_t)R * nh * HD * sizeof(float), cudaMemcpyDeviceToHost));
+        debug_verify_run(m, 1, &R, &p0, table.data(), np + 1, (int)n_heads, (int)n_kv_heads, q, k, v, out, 3);
+    });
+}
+
+int aha_b200_debug_verify_attn_batch(aha_model* m, size_t n, const int32_t* rows, const int32_t* pos0, const int32_t* tables, size_t n_pool_pages,
+                                     size_t n_heads, size_t n_kv_heads, const float* q, const float* k, const float* v, float* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(rows && pos0 && tables && q && k && v && out, "rows, pos0, tables, q, k, v and out are required");
+        AHA_REQUIRE(n >= 1 && n <= (size_t)kWideSeqs, "debug_verify_attn_batch: 1 to 64 requests");
+        size_t t = 0;
+        std::vector<char> seen(n_pool_pages, 0);
+        for (size_t j = 0; j < n; ++j) {
+            AHA_REQUIRE(rows[j] >= 1 && rows[j] <= kSpecMaxRows && pos0[j] >= 0, "debug_verify_attn_batch: every request needs 1 to 16 rows at a position >= 0");
+            for (int p = 0; p < ceil_div(pos0[j] + rows[j], kPage); ++p, ++t) {
+                AHA_REQUIRE(tables[t] >= 0 && (size_t)tables[t] < n_pool_pages && !seen[tables[t]], "debug_verify_attn_batch: the tables' pages must be distinct pages of the pool");
+                seen[tables[t]] = 1;
+            }
+        }
+        debug_verify_run(m, (int)n, rows, pos0, tables, (int)n_pool_pages, (int)n_heads, (int)n_kv_heads, q, k, v, out, 3);
     });
 }
 
@@ -3389,7 +3657,7 @@ int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, s
             src = T.logits; cnt = (size_t)T.cfg.V;
         } else if (w == "batch_graphs") {   // step graphs captured in the open batch session (wide: at most one per running count)
             AHA_REQUIRE(cap >= 1, "out too small");
-            out[0] = (float)m->sess().graphs.size(); *n = 1; return;
+            out[0] = (float)(m->sess().graphs.size() + (m->session.wide ? m->spec.steps.size() : 0)); *n = 1; return;
         } else if (w == "spec_graphs") {    // pass graphs of speculative requests (one per row count R)
             AHA_REQUIRE(cap >= 1, "out too small");
             out[0] = (float)m->spec.graphs.size(); *n = 1; return;

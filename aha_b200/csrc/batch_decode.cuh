@@ -74,7 +74,8 @@ struct BatchDecoder {
     // composition changes
     GraphCache<std::pair<int, bool>> graphs;
     // the set of running requests or a slot's sampler changed: the device copy of the composition is rebuilt before the next step
-    void composition_changed() { table_for.clear(); }
+    void composition_changed() { table_for.clear(); ++epoch; }
+    uint64_t epoch = 0;                  // counts composition changes (a speculative step rebuilds its own device copies on a new one)
     // no sequence holds a slot any more (a session opens or closes)
     void reset() {
         for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; }
@@ -230,6 +231,17 @@ struct BatchDecoder {
         decode_attn_batch_kernel<128, G><<<dim3(kDecodeSplits, T->nkv_l, nb), 256, 0, T->ctx->stream>>>(d_attn + (size_t)l * cap);
     }
 
+    // the attention of rows 0..nb-1 (the active list's first nb slots) in layer l
+    void attn(int l, int nb) {
+        switch (T->nh_l / T->nkv_l) {
+            case 1: launch_attn<1>(l, nb); break;
+            case 2: launch_attn<2>(l, nb); break;
+            case 4: launch_attn<4>(l, nb); break;
+            default: launch_attn<6>(l, nb); break;
+        }
+        T->ctx->cnt.kernels++;
+    }
+
     // rows 0..nb-1: out = epi(W . x), x RMSNorm-ed with norm_w first when given
     void proj(int epi, const LinearW& W, const float* x, int ldx, const float* norm_w, const float* resid, int ldr, float* out, int ldo, int nb) {
         Ctx& c = *T->ctx;
@@ -277,13 +289,7 @@ struct BatchDecoder {
         for (int l = 0; l < cf.L; ++l) {
             TextLayer& Ly = T->layers[l];
             proj(GEPI_STORE, Ly.qkv, xb, H, Ly.ln1, nullptr, 0, qkvb, T->qkv_dim, nb);
-            switch (T->nh_l / T->nkv_l) {
-                case 1: launch_attn<1>(l, nb); break;
-                case 2: launch_attn<2>(l, nb); break;
-                case 4: launch_attn<4>(l, nb); break;
-                default: launch_attn<6>(l, nb); break;
-            }
-            c.cnt.kernels++;
+            attn(l, nb);
             proj(GEPI_RESID, Ly.o, attnb, T->nh_l * cf.hd, nullptr, xb, H, xb, H, nb);
             proj(GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb);
             proj(GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb);
@@ -296,17 +302,33 @@ struct BatchDecoder {
     // (the single-sequence loop does the same).  A request's first token (first = true, packed admission) is drawn the way forward_any draws
     // it: no advance, no overwrite, against the slot's state as the caller set it (empty history, draw index 0); only n_draws moves.
     void head(int nb, bool first) {
+        lm_head(nb);
+        head_rows_at(0, nb, d_act, d_tok, d_states, d_hist, d_samp, d_samp_on, d_lp_on, d_lp_rec, first, lp_any);
+    }
+    // final norm + lm_head and ArgMax stage 1 over rows 0 .. nb-1
+    void lm_head(int nb) {
         Ctx& c = *T->ctx;
-        cudaStream_t st = c.stream;
         const TextCfg& cf = T->cfg;
         LinearW lm; lm.w = T->lm_head; lm.b = nullptr; lm.N = cf.V; lm.K = cf.H;
         proj(GEPI_STORE, lm, xb, cf.H, T->norm, nullptr, 0, logitsb, cf.V, nb);
-        argmax_partial_rows_kernel<<<dim3(n_pcand, nb), 256, 0, st>>>(logitsb, cf.V, cf.V, pmaxb, pidxb);
-        argmax_final_rows_kernel<<<nb, 32, 0, st>>>(pmaxb, pidxb, n_pcand, d_act, d_tok, d_states, d_hist, T->hist_cap, first ? 0 : 1);
-        sample_rows_kernel<<<nb, kSampleThreads, 0, st>>>(d_samp, d_samp_on, d_act, logitsb, cf.V, first ? 0 : 1);
-        c.cnt.kernels += 3;
-        if (lp_any) {
-            logprobs_rows(st, logitsb, cf.V, cf.V, nb, d_act, d_lp_on, lp_part, lp_part_id, d_tok, d_states, first ? 1 : 0, d_lp_rec, 0, cap);
+        argmax_partial_rows_kernel<<<dim3(n_pcand, nb), 256, 0, c.stream>>>(logitsb, cf.V, cf.V, pmaxb, pidxb);
+        c.cnt.kernels++;
+    }
+    // ArgMax stage 2, sampler and (lp) records of rows r0 .. r0 + n - 1, row r0 + j standing for entry act[j] of the per-row arrays given
+    // (tok, st, hist, samp, samp_on, lp_on, rec: a slot's, or a speculative verify row's)
+    void head_rows_at(int r0, int n, const int* act, uint32_t* tok, DecodeState* st, uint32_t* hist, const SampleArgs* samp, const int* samp_on,
+                      const int* lp_on, aha_logprobs* rec, bool first, bool lp) {
+        Ctx& c = *T->ctx;
+        cudaStream_t s = c.stream;
+        const int V = T->cfg.V;
+        const float* logits = logitsb + (size_t)r0 * V;
+        argmax_final_rows_kernel<<<n, 32, 0, s>>>(pmaxb + (size_t)r0 * n_pcand, pidxb + (size_t)r0 * n_pcand, n_pcand, act, tok, st, hist, T->hist_cap, first ? 0 : 1);
+        sample_rows_kernel<<<n, kSampleThreads, 0, s>>>(samp, samp_on, act, logits, V, first ? 0 : 1);
+        c.cnt.kernels += 2;
+        if (lp) {
+            const size_t P = (size_t)lp_parts(V);
+            logprobs_rows(s, logits, V, V, n, act, lp_on, lp_part + (size_t)r0 * P * kLpPartFloats, lp_part_id + (size_t)r0 * P * kLpMaxTop, tok, st,
+                          first ? 1 : 0, rec, 0, cap);
             c.cnt.kernels += 2;
         }
         AHA_CUDA_CHECK(cudaGetLastError());

@@ -286,6 +286,29 @@ class B200Model:
         self._check(self._lib.aha_b200_debug_verify_attn(self._h, R, nh, nkv, int(pos0), f(q), f(k), f(v), f(out)))
         return out
 
+    def debug_verify_attn_batch(self, qs, ks, vs, pos0s, tables, n_pool_pages):
+        """The verify attention over several requests in one launch (aha_b200_debug_verify_attn_batch): request j has q qs[j]
+        [R_j][nh][128] at positions pos0s[j] .. pos0s[j] + R_j - 1 over k / v ks[j], vs[j] [pos0s[j] + R_j][nkv][128] on the page table
+        tables[j] (ceil((pos0s[j] + R_j) / 32) distinct pages of a NaN pool of n_pool_pages) -> [out_j [R_j][nh][128], ...]."""
+        qs = [np.ascontiguousarray(q, np.float32) for q in qs]
+        nh, nkv = qs[0].shape[1], np.shape(ks[0])[1]
+        rows = np.ascontiguousarray([q.shape[0] for q in qs], np.int32)
+        p0 = np.ascontiguousarray(pos0s, np.int32)
+        for j, q in enumerate(qs):
+            want = (int(p0[j]) + q.shape[0], nkv, 128)
+            if q.shape[1:] != (nh, 128) or np.shape(ks[j]) != want or np.shape(vs[j]) != want or np.size(tables[j]) != -(-want[0] // 32):
+                raise ValueError(f"request {j}: q [R][nh][128], k and v [pos0 + R][nkv][128], a table of ceil((pos0 + R) / 32) pages")
+        q = np.ascontiguousarray(np.concatenate(qs), np.float32)
+        k = np.ascontiguousarray(np.concatenate(ks), np.float32)
+        v = np.ascontiguousarray(np.concatenate(vs), np.float32)
+        tb = np.ascontiguousarray(np.concatenate([np.asarray(t, np.int32).reshape(-1) for t in tables]), np.int32)
+        out = np.empty_like(q)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self._check(self._lib.aha_b200_debug_verify_attn_batch(self._h, len(qs), i32(rows), i32(p0), i32(tb), int(n_pool_pages), nh, nkv,
+                                                               f(q), f(k), f(v), f(out)))
+        return np.split(out, np.cumsum(rows)[:-1])
+
     def debug_attention(self, q, k, v, impl, causal, segments=None, page_order=None, split_out=False):
         """The prefill attention on host data (aha_b200_debug_attention): q [Sq][nh][hd], k / v [Skv][nkv][hd] with hd 64 or 128 ->
         [Sq][nh][hd].  impl 0 = wgmma, 1 = SIMT, 2 = mma.sync.  causal: query i sees keys 0 .. Skv - Sq + i, K / V on a paged pool
@@ -534,6 +557,58 @@ class B200Model:
         recs = (L.Logprobs * w)()
         self._check(self._lib.aha_b200_batch_logprobs(self._h, recs, w))
         return {i: L.logprobs_record(recs[i]) for i in range(w) if recs[i].valid}
+
+    def batch_add_speculative(self, input_ids, data=None, prediction=None, prompt_lookup=False, max_draft=7, ngram=3, max_tokens=1024,
+                              temperature=0.0, top_p=None, top_k=None, repeat_penalty=1.0, repeat_last_n=64, seed=299792458, flags=0,
+                              logprobs=False, top_logprobs=0, rules=None, return_usage=False):
+        """Admit a speculative request into the open wide session (aha_b200_batch_add_speculative): admitted as batch_add admits it, then
+        every batch_step_spec runs one verify pass of max_draft + 1 rows for it (drafts as for generate_speculative).  -> (slot, first token,
+        finished), and with return_usage=True also the prompt-side usage dict."""
+        ids = self._ids(input_ids)
+        mm, _keep = self._mm(data)
+        sp, _pred = L.spec_params(prediction, prompt_lookup, max_draft, ngram, self.vocab_size)
+        flags |= L.logprob_flags(logprobs, top_logprobs, self.vocab_size)
+        req = L.BatchRequest()
+        req.ids = ids.ctypes.data_as(C.POINTER(C.c_uint32))
+        req.seq_len = ids.size
+        req.mm = C.pointer(mm) if mm is not None else None
+        req.params = self._gen_params(max_tokens, temperature, top_p, top_k, repeat_penalty, repeat_last_n, seed, flags, rules=rules)
+        slot, fin, tok = C.c_int32(-1), C.c_int32(0), C.c_uint32(0)
+        u = L.Usage()
+        self._check(self._lib.aha_b200_batch_add_speculative(self._h, C.byref(req), C.byref(sp), C.byref(slot), C.byref(tok), C.byref(fin),
+                                                             C.byref(u)))
+        res = (int(slot.value), int(tok.value), bool(fin.value))
+        return (res, self._usage(u)) if return_usage else res
+
+    def batch_step_spec(self):
+        """One step of every running request (aha_b200_batch_step_spec) -> {slot: (tokens, finished)}: one token for a plain request,
+        1 .. max_draft + 1 for a speculative one (empty when nothing is running)."""
+        w = getattr(self, "_batch_width", 8)
+        R = L.SPEC_MAX_ROWS
+        toks, n_tok, status, n = (C.c_uint32 * (w * R))(), (C.c_uint32 * w)(), (C.c_int32 * w)(), C.c_size_t(0)
+        self._check(self._lib.aha_b200_batch_step_spec(self._h, toks, n_tok, status, w, C.byref(n)))
+        return {i: ([int(toks[i * R + k]) for k in range(n_tok[i])], status[i] == 2) for i in range(w) if status[i] != 0}
+
+    def batch_logprobs_spec(self):
+        """-> {slot: [record, ...]} for the slots whose request asked for log-probabilities: the records of every token each delivered in
+        the last batch_step_spec (or at admission)."""
+        w = getattr(self, "_batch_width", 8)
+        R = L.SPEC_MAX_ROWS
+        recs = (L.Logprobs * (w * R))()
+        self._check(self._lib.aha_b200_batch_logprobs_spec(self._h, recs, w))
+        out = {}
+        for i in range(w):
+            got = [L.logprobs_record(recs[i * R + k]) for k in range(R) if recs[i * R + k].valid]
+            if got:
+                out[i] = got
+        return out
+
+    def batch_spec_stats(self):
+        """-> {slot: dict(passes, drafted, accepted)} for the slots whose (running or last) request was speculative."""
+        w = getattr(self, "_batch_width", 8)
+        st = (L.SpecStats * w)()
+        self._check(self._lib.aha_b200_batch_spec_stats(self._h, st, w))
+        return {i: dict(passes=int(st[i].passes), drafted=int(st[i].drafted), accepted=int(st[i].accepted)) for i in range(w) if st[i].passes}
 
     def batch_close(self):
         self._check(self._lib.aha_b200_batch_close(self._h))

@@ -398,6 +398,33 @@ int aha_b200_generate_speculative(aha_model* m, const uint32_t* ids, size_t seq_
                                   const aha_spec_params* spec, uint32_t* out_tokens, aha_logprobs* out_logprobs, size_t cap,
                                   size_t* n_out, aha_usage* usage, aha_spec_stats* stats);
 
+/* Speculative requests inside a wide batch session (new design).  AHA_SPEC_MAX_ROWS: max_draft + 1 at most.
+ * batch_add_speculative admits one request into the lowest free slot of the open WIDE session the way batch_add does (prefilled alone,
+ * prefix-cache hit and insert included) and from then on every step runs one verify pass of R = spec->max_draft + 1 rows for it, drafted by
+ * the rule of generate_speculative.  Its ids, records and aha_spec_stats are bit for bit those generate_speculative yields for it alone with
+ * the same spec params, whatever slot it holds, whatever runs beside it and at whatever step it joins; its plain neighbours yield exactly
+ * what they yield without it.  Refused before any device work, leaving the session, the prefix index and the handle unchanged: what
+ * generate_speculative refuses (Qwen3-ASR, shapes that do not tile by 64 or head_dim != 128, max_draft outside 1..15, ngram outside 0..8,
+ * unknown spec flags, REUSE_PREFIX / CONTINUE_RNG / EOS_ON_FIRST, CONSTRAINED or logit rules naming an automaton, prediction ids >= V), a
+ * narrow session, and a request whose rows do not fit: a plain request counts 1 row, a speculative one R, and the running requests' rows
+ * plus the new ones must fit 64 (batch_add, batch_add_many and batch_add_n check this too while a speculative request runs).  It needs
+ * ceil((seq_len + max_tokens + max_draft) / 32) pages minus its prefix-cache hit.  usage: prompt side, or NULL. */
+#define AHA_SPEC_MAX_ROWS 16
+int aha_b200_batch_add_speculative(aha_model* m, const aha_batch_request* req, const aha_spec_params* spec, int32_t* slot_out,
+                                   uint32_t* first_token_out, int32_t* finished_out, aha_usage* usage);
+/* One step of every running request (narrow or wide session; cap >= the session width): a plain slot delivers 1 token, a speculative slot
+ * 1..R, in tokens_out[slot][0 .. n_tokens_out[slot]).  status_out as for batch_step_n: 0 idle, 1 continues, 2 finished (EOS inside an
+ * accepted run, or max_tokens reached mid-pass; the slot and its pages are free again).  Without a running speculative request it launches
+ * exactly what batch_step_n launches and returns its tokens.  batch_step and batch_step_n refuse while a speculative request runs. */
+int aha_b200_batch_step_spec(aha_model* m, uint32_t* tokens_out /* [cap][AHA_SPEC_MAX_ROWS] */, uint32_t* n_tokens_out /* [cap] */,
+                             int32_t* status_out /* [cap] */, size_t cap, size_t* n_stepped_out /* may be NULL */);
+/* out[slot][k]: the record of the k-th token the slot's request delivered in the last step or at admission (batch_logprobs' validity
+ * rules; zero records beyond them).  batch_logprobs keeps giving the record of the slot's last delivered token, for speculative slots too. */
+int aha_b200_batch_logprobs_spec(aha_model* m, aha_logprobs* out /* [cap][AHA_SPEC_MAX_ROWS] */, size_t cap);
+/* out[slot]: passes / drafted / accepted of the slot's speculative request, as generate_speculative reports them; zeros for a plain or free
+ * slot.  They stay readable after the request finishes, until the slot is taken again. */
+int aha_b200_batch_spec_stats(aha_model* m, aha_spec_stats* out /* [cap] */, size_t cap);
+
 /* Qwen3AsrGenerateModel::generate / generate_stream (qwen3_asr/generate.rs:130-268): per-chunk loop, stop on either EOS id
  * (the handle's stop ids), KV cache cleared per chunk, one sampler for the whole request.  on_token may be NULL. */
 int aha_b200_asr_generate(aha_model* m, const aha_asr_chunk* chunks, size_t n_chunks, const aha_gen_params* params,
@@ -553,7 +580,8 @@ int aha_b200_reset_stats(aha_model* m);
 /* Copy an internal activation to the host: what = "hidden" (text hidden states after layer `index`
  * of the last forward_initial, S*H floats; requires aha_b200_set_trace(m,1)), "vit" (ViT hidden after
  * block `index`), "image_embeds", "audio_embeds", "rope_delta" (1 float), "batch_graphs" (1 float: step graphs
- * captured in the open batch session: at most one per running count, two where requests asking for log-probabilities ran),
+ * captured in the open batch session: at most one per running count, two where requests asking for log-probabilities ran; with
+ * speculative requests one per (plain rows, speculative requests, verify rows, records)),
  * "spec_graphs" (1 float: pass graphs of speculative requests, at most one per row count). */
 int aha_b200_set_trace(aha_model* m, int on);
 int aha_b200_debug_read(aha_model* m, const char* what, int index, float* out, size_t cap, size_t* n);
@@ -608,6 +636,12 @@ int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_
  * In this entry and the two below, every pool slot no page table references, and every slot past a context inside its last page, holds NaN. */
 int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
                                const float* v, float* out);
+/* the same over n requests in one launch (tests): request j has rows[j] (1..16) query rows at positions pos0[j] .. pos0[j] + rows[j] - 1 over
+ * its own page table, the next ceil((pos0[j] + rows[j]) / 32) entries of `tables` (distinct pages of a pool of n_pool_pages).  q, out: the
+ * requests' rows after each other, [sum rows][n_heads][128]; k, v: the requests' positions after each other, [sum (pos0 + rows)][n_kv_heads][128].
+ * At most 64 rows in all. */
+int aha_b200_debug_verify_attn_batch(aha_model* m, size_t n, const int32_t* rows, const int32_t* pos0, const int32_t* tables, size_t n_pool_pages,
+                                     size_t n_heads, size_t n_kv_heads, const float* q, const float* k, const float* v, float* out);
 /* the prefill attention on host data (tests), through the dispatch the models use: impl 0 = wgmma (flash_attn_tc_kernel), 1 = fp32 SIMT,
  * 2 = mma.sync; head_dim 64 or 128.  q, out: [sq][n_heads][head_dim] (q normalised and rotated); k, v: [skv][n_kv_heads][head_dim].
  *   causal, no segments: the LLM prefill; query i attends to keys 0 .. skv - sq + i, K / V on a paged pool whose logical page p is physical

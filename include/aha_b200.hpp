@@ -307,6 +307,37 @@ public:
         if (usage) *usage = Usage{u.prompt_tokens, u.completion_tokens, u.prompt_secs, u.completion_secs, u.vision_secs};
         return out;
     }
+    // A greedy speculative request into the open wide session (aha_b200_batch_add_speculative), stepped by batch_step_spec.
+    struct Admitted { int32_t slot; uint32_t first_token; bool finished; };
+    Admitted batch_add_speculative(const std::vector<uint32_t>& ids, const MultiModalData* data, const GenerationContext& ctx,
+                                   const std::vector<uint32_t>& prediction, bool prompt_lookup = false, uint32_t max_draft = 7, uint32_t ngram = 0) {
+        const aha_mm mm = data ? data->view() : aha_mm{nullptr, 0};
+        aha_batch_request r{};
+        r.ids = ids.data(); r.seq_len = ids.size(); r.mm = data ? &mm : nullptr;
+        r.params.repeat_penalty = ctx.repeat_penalty; r.params.repeat_last_n = (int32_t)ctx.repeat_last_n; r.params.max_tokens = (uint32_t)ctx.sample_len;
+        aha_spec_params s{};
+        s.prediction = prediction.empty() ? nullptr : prediction.data(); s.n_prediction = prediction.size();
+        s.max_draft = max_draft; s.ngram = ngram; s.flags = prompt_lookup ? AHA_SPEC_PROMPT_LOOKUP : 0u;
+        Admitted a{-1, 0, false};
+        int32_t fin = 0;
+        check(aha_b200_batch_add_speculative(h_, &r, &s, &a.slot, &a.first_token, &fin, nullptr));
+        a.finished = fin != 0;
+        return a;
+    }
+    // One step of every running request of the open session (aha_b200_batch_step_spec), `width` = the session width: per slot its status
+    // (0 idle, 1 continues, 2 finished) and the tokens it delivered (1 for a plain request, 1 .. max_draft + 1 for a speculative one).
+    struct SlotStep { int32_t status; std::vector<uint32_t> tokens; };
+    std::vector<SlotStep> batch_step_spec(size_t width) {
+        std::vector<uint32_t> tok(width * AHA_SPEC_MAX_ROWS), n_tok(width);
+        std::vector<int32_t> status(width);
+        check(aha_b200_batch_step_spec(h_, tok.data(), n_tok.data(), status.data(), width, nullptr));
+        std::vector<SlotStep> res(width);
+        for (size_t i = 0; i < width; ++i) {
+            res[i].status = status[i];
+            res[i].tokens.assign(tok.begin() + (std::ptrdiff_t)(i * AHA_SPEC_MAX_ROWS), tok.begin() + (std::ptrdiff_t)(i * AHA_SPEC_MAX_ROWS + n_tok[i]));
+        }
+        return res;
+    }
     size_t last_prefix_hit() const { return aha_b200_last_prefix_hit(h_); }
     // The open batch session's prefix cache (aha_b200_batch_prefix_cache / _stats): on with max_tokens > 0, off (its pages released) with 0.
     // batch_prefix_stats' hits: per slot of the session (width entries), the prompt tokens its running request took from the cache.
