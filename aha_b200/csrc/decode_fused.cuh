@@ -8,9 +8,9 @@
 //     layers -- weight row slabs and paged-KV half pages -- and issues TMA bulk copies
 //     (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes, SASS UBLKCP, L2 evict-first policy) into
 //     a ring of 16 KB shared-memory stages guarded by full/empty mbarriers.  It never waits for activations, so
-//     weights for the next phase keep streaming while the consumers sit in a grid barrier -- but only up to a run-ahead
-//     budget past the end of the consumers' current phase (kFusedAheadBytes), so that the traffic of a phase end
-//     (barrier, activation loads) does not queue behind a full ring of next-phase copies from every SM;
+//     weights for the next phase keep streaming while the consumers sit in a grid barrier -- but with at most
+//     kFusedInflightBytes of copies issued and not yet landed, so that the traffic of a phase end (barrier, activation
+//     loads) does not queue behind a ring's worth of next-phase copies from every SM;
 //   * the other 11 warps are CONSUMERS: per phase they stage the activation vector in shared memory (RMSNorm
 //     fused), and each warp consumes the ring slots it owns: a whole stage of weight rows is reduced by one warp
 //     with fp32 dot products (fp16 weights converted exactly) and the fused epilogue (residual add from the rows
@@ -52,6 +52,7 @@ namespace aha {
 
 constexpr int kFusedStages = 11;                         // ring slots (all in use by default: one per consumer warp)
 constexpr int kFusedStageBytes = 16384;
+constexpr int kFusedSizeWords = (kFusedStages + 3) & ~3;  // the producer's per-slot stage sizes, padded so that xs stays 16-byte aligned
 constexpr int kFusedConsumers = 11;                      // consumer warps (+1 producer = 12 warps: register allocation granularity)
 constexpr int kFusedThreads = (kFusedConsumers + 1) * 32;
 constexpr int kFusedMaxRows = 8;                         // weight rows per stage (<= 16 KB)
@@ -64,17 +65,17 @@ constexpr int kFusedMergeChunk = 20;                     // splits merged per pa
 constexpr int kFusedMaxPages = 1024;                     // page-table entries staged in shared memory as uint16 (32K tokens; physical page ids < 65536)
 constexpr int kFusedMaxH = 4096;                         // residual stream kept per CTA in shared memory (PACKET_RESID)
 constexpr int kFusedMaxTp = 8;                           // tensor-parallel ranks on one NVSwitch domain
-// Run-ahead budget of the producer: stages of a phase the consumers have not entered yet may be issued only while they end at
-// most this many bytes past the end of the consumers' current phase (stages of the current phase are never held back).  Without
-// it every CTA keeps a full ring (176 KB) of the next phases' copies queued in the memory system while it sits in a phase end,
-// and the phase end's own traffic -- the barrier arrival and poll, the activation loads -- waits behind them.  96 KB is the
-// fastest of 0 / 16 / 32 / 48 / 64 / 96 / 128 / 176 KB on an H100 SXM (700 W) at the Qwen3-VL-2B decode shape (DESIGN §4.1):
-// less starves the next phase's first stages, more brings the queueing back.  -DAHA_FUSED_AHEAD_KB=N builds the sweep.
-#ifndef AHA_FUSED_AHEAD_KB
-#define AHA_FUSED_AHEAD_KB 96
+// In-flight cap of the producer: a stage is issued only while the copies issued and not yet landed, that stage included, stay
+// within this many bytes (a stage with nothing else in flight always goes).  Copies QUEUED in the memory system are what a
+// phase end waits behind -- the barrier arrival and poll, the activation loads -- while ring slots holding landed data cost it
+// nothing; and one H100 SM streams at full rate with 32 KB in flight (profiles/stream_bench.cu).  So the producer fills the
+// whole ring through a phase end, 32 KB at a time.  32 KB is the fastest of 32 / 48 / 64 / 96 KB on an H100 SXM (700 W) at the
+// Qwen3-VL-2B decode shape, and faster than any of them combined with a bound on how far the stream runs past the consumers'
+// current phase (DESIGN §4.1).  -DAHA_FUSED_INFLIGHT_KB=N builds the sweep.
+#ifndef AHA_FUSED_INFLIGHT_KB
+#define AHA_FUSED_INFLIGHT_KB 32
 #endif
-constexpr uint32_t kFusedAheadBytes = AHA_FUSED_AHEAD_KB * 1024u;
-constexpr int kFusedGateWord = 28;                       // the gate's word in the `red` scratch ([0, 11) sums / argmax values, [16, 27) argmax indices, [31] last-CTA flag)
+constexpr uint32_t kFusedInflightBytes = AHA_FUSED_INFLIGHT_KB * 1024u;
 
 struct __align__(8) LLPk { float v; uint32_t tag; };     // one tagged packet: 8-byte stores / loads are single-copy atomic
 struct LLPeerTab {                                       // device-resident table of the symmetric blocks of every tensor-parallel rank
@@ -441,16 +442,10 @@ struct Ring {
 };
 
 // ------------------------------------------------------------------------------------------------ producer
-// The run-ahead gate: `gate` holds (schedule bytes up to the end of the consumers' current phase) + kFusedAheadBytes, `issued`
-// counts the schedule bytes this producer has issued including the stage being acquired; the stage waits while it would end
-// past the gate.  No deadlock: consumers enter a phase (and raise the gate) without waiting on any ring slot -- they need only
-// the activations, which come from the other CTAs' consumers under the same rule -- and the stages of the phase they are in
-// always end below the gate.  Wrapping differences: a step's schedule is far below 2 GB per CTA.
-__device__ __forceinline__ uint32_t ld_volatile_shared_u32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
-    return v;
-}
+// No deadlock: besides a free slot (the empty barriers), the producer waits only for copies it has itself issued to land, which
+// the memory system completes without any consumer.  Consumers enter a phase without waiting on any ring slot -- they need only
+// the activations, which come from the other CTAs' consumers under the same rule -- and release every slot of the phase they are
+// in once it has landed, so the producer always gets to the stages of the consumers' current phase.
 struct Producer {
     Ring ring;
     unsigned it = 0;
@@ -458,13 +453,22 @@ struct Producer {
     bool use_hint = false, hint_kv = false;
     uint64_t policy = 0;
     unsigned long long* st_trace = nullptr;
-    const uint32_t* gate = nullptr;
-    uint32_t issued = 0, limit = 0;   // limit: the last value read from the gate (it only grows)
+    // copies in flight: stages [lo, it) have been issued and stage lo has not been seen landed; they hold `flying` bytes, and
+    // sizes[s] holds the bytes of the stage issued last into slot s (shared memory, this thread only)
+    unsigned lo = 0;
+    uint32_t flying = 0;
+    uint32_t* sizes = nullptr;
     __device__ __forceinline__ void acquire(int& slot, uint32_t bytes) {
-        issued += bytes;
-        if ((int)(limit - issued) < 0)
-            while ((int)((limit = ld_volatile_shared_u32(gate)) - issued) < 0) __nanosleep(32);
+        // stage lo must have landed before a stage that would take the bytes in flight past kFusedInflightBytes is issued, and
+        // before its slot is re-armed (so it - lo < ns holds at every look: the full barrier still shows stage lo's phase)
+        while (lo != it && (flying + bytes > kFusedInflightBytes || it - lo >= ns)) {
+            if (!mbar_try_wait(&ring.full[lo % ns], (lo / ns) & 1u)) continue;
+            flying -= sizes[lo % ns];
+            ++lo;
+        }
         slot = it % ns;
+        sizes[slot] = bytes;
+        flying += bytes;
         mbar_wait(&ring.empty[slot], ((it / ns) & 1u) ^ 1u);
         AHA_STAGE_STAMP(st_trace, it, 0);
     }
@@ -531,12 +535,6 @@ struct Consumer {
     bool sync_only = false;    // dbg bit9: no weight stream and no math, only the barriers and activation loads
     unsigned long long* sy_trace = nullptr;   // sync anatomy stamps (AHA_STAGE_TRACE builds, dbg bit10)
     unsigned n_loads = 0;
-    // Called once the phase's activations are staged, before its first wait_full: the producer may now run
-    // kFusedAheadBytes past the end of this phase.  A phase without stages leaves the gate where it is.  Only thread 0
-    // writes the gate word (no register of the hot loops holds it).
-    __device__ __forceinline__ void enter(uint32_t bytes) const {
-        if (threadIdx.x == 0) reinterpret_cast<volatile uint32_t*>(red)[kFusedGateWord] += bytes;
-    }
     __device__ __forceinline__ bool owns(unsigned i) const { return (int)((i % ns) % kFusedConsumers) == warp; }
     __device__ __forceinline__ const uint8_t* wait_full(unsigned i) {
         const int slot = i % ns;
@@ -777,7 +775,6 @@ struct Consumer {
         const Slab s = EPI == FE_QKV ? qkv_slab(a.nh, a.nkv, a.hd, a.nsplit) : cta_slab(N, EPI == FE_SWIGLU ? 2 : 1);
         const int r0 = s.j0;
         const int R = rows_per_stage(K, N, gridDim.x);
-        enter((uint32_t)(s.j1 - s.j0) * K * 2u);
         if (sync_only) { consumer_bar_sync(); return; }
         unsigned i = it;
         for (int j = s.j0, nr; j < s.j1; j += nr, ++i) {
@@ -903,7 +900,6 @@ __device__ void fused_attention(const FusedArgs& a, Consumer& c, AttnSmem<G>& s,
         *reinterpret_cast<float4*>(s.vnew + lane * 4) = v;
     }
     consumer_bar_sync();
-    c.enter((uint32_t)(hp1 - hp0) * 2u * kHalfPage * HD * 4u);   // (a CTA without an item has no stages: its gate stays put)
     const int hp_new = t_new / kHalfPage;
     if (hp_new >= hp0 && hp_new < hp1 && tid < HD) {  // append K,V of the current token to the paged cache
         const int page = spages[t_new >> kPageShift];
@@ -1030,8 +1026,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
     uint8_t* ringbuf = fused_smem_raw;
     uint64_t* full = reinterpret_cast<uint64_t*>(fused_smem_raw + (size_t)kFusedStages * kFusedStageBytes);
     uint64_t* empty = full + kFusedStages;
-    float* red = reinterpret_cast<float*>(empty + kFusedStages);
-    uint32_t* gate = reinterpret_cast<uint32_t*>(red) + kFusedGateWord;   // the producer's run-ahead gate (Consumer::enter)
+    uint32_t* sizes = reinterpret_cast<uint32_t*>(empty + kFusedStages);   // [kFusedStages] the producer's stage sizes (Producer::sizes)
+    float* red = reinterpret_cast<float*>(sizes + kFusedSizeWords);
     float* xown = red + 32;                                     // [kFusedMaxOwnRows] (barrier mode only: PACKET_RESID keeps the whole stream in xres)
     float* cs = xown + (PACKET_RESID ? 0 : kFusedMaxOwnRows);   // [128] cos | sin of the step's rotary angles
     float* xs = cs + 128;                                       // [kFusedMaxK] activations / attention scratch
@@ -1044,7 +1040,6 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
     if (tid == 0) {
         for (int i = 0; i < kFusedStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        *gate = kFusedAheadBytes;   // before the first phase the consumers are in an empty one
     }
     if ((a.dbg & 64) && tid == 0) { unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid)); a.trace[8192 + blockIdx.x * 256 + 255] = smid; }
     const int t_new = a.st->pos;
@@ -1070,7 +1065,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
             p.hint_kv = (a.dbg & 32) == 0;       // bit5: same switch for the KV half-page copies
             p.policy = l2_evict_first_policy();
             p.pages = spages;
-            p.gate = gate;
+            p.sizes = sizes;
 #ifdef AHA_STAGE_TRACE
             if ((a.dbg & 128) && (int)blockIdx.x == ((a.dbg >> 16) & 0xff)) p.st_trace = a.trace + 8192;
 #endif
@@ -1246,7 +1241,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) decode_step_fused_kernel(Fus
 
 template <int G>
 inline size_t fused_smem_bytes(bool packet_resid) {
-    return (packet_resid ? (size_t)kFusedMaxH * sizeof(float) : (size_t)kFusedMaxOwnRows * sizeof(float)) + (size_t)kFusedStages * kFusedStageBytes + 2 * kFusedStages * sizeof(uint64_t) + (32 + 128) * sizeof(float) + (size_t)kFusedMaxK * sizeof(float) +
+    return (packet_resid ? (size_t)kFusedMaxH * sizeof(float) : (size_t)kFusedMaxOwnRows * sizeof(float)) + (size_t)kFusedStages * kFusedStageBytes + 2 * kFusedStages * sizeof(uint64_t) + kFusedSizeWords * sizeof(uint32_t) + (32 + 128) * sizeof(float) + (size_t)kFusedMaxK * sizeof(float) +
            (size_t)kFusedMaxPages * sizeof(uint16_t) + 64;
 }
 

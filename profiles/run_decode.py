@@ -3,17 +3,20 @@
   python profiles/run_decode.py [steps]              one configuration from the environment (AHA_DECODE_IMPL, AHA_FUSED_DBG, ...)
   python profiles/run_decode.py [steps] --sweep SPEC one process, many configurations (weights generated once):
       SPEC = ';'-separated runs, each ','-separated key=value with keys impl, dbg, stages, ctx, tl (1 = print the phase
-      timeline), st (1 = dump the per-stage trace of an AHA_STAGE_TRACE build to profile_out/stage_trace_<tag>.npy)
+      timeline), st (1 = dump the per-stage trace of an AHA_STAGE_TRACE build to profile_out/stage_trace_<tag>.npy and print, per phase
+      boundary, how long the CTA had no copy in flight and how long its producer was held back)
       e.g. --sweep "impl=0;impl=0,dbg=3;impl=3,tl=1"
-      key ahead=N runs the spec on variants/ahead<N>.so, a build of the library with the producer's run-ahead budget set to
+      key inflight=N runs the spec on variants/inflight<N>.so, a build of the library with the producer's in-flight cap set to
       N KB (decode_fused.cuh), loaded side by side with the other builds in this process (same weights, so repeated specs
       alternate builds without process-to-process noise):
-        nvcc <aha_b200/build.py NVCC_FLAGS> -DAHA_FUSED_AHEAD_KB=N -o variants/aheadN.so aha_b200/csrc/api.cu -ldl
-      e.g. --sweep "ahead=0;ahead=64;impl=0;ahead=0;ahead=64;impl=0"
+        nvcc <aha_b200/build.py NVCC_FLAGS> -DAHA_FUSED_INFLIGHT_KB=N -o variants/inflightN.so aha_b200/csrc/api.cu -ldl
+      e.g. --sweep "inflight=48;inflight=64;impl=0;inflight=48;inflight=64;impl=0"
+      key trace=1 does the same with an AHA_STAGE_TRACE build (what st=1 / sy=1 read); the keys combine
+      (variants/inflight48_trace.so), and a variant that is missing is built first
       key lib=PATH runs the spec on the library at PATH the same way, e.g. a build of the parent commit against this tree's:
         --sweep "lib=/tmp/parent.so,tl=1;impl=0,tl=1;lib=/tmp/parent.so;impl=0"
 AHA_SHAPE = vl2 (default) | q0.6; AHA_LIB = path of an alternative libaha_b200.so, loaded instead of the in-tree one."""
-import os, sys, time
+import os, subprocess, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
@@ -61,6 +64,117 @@ def timeline(m, ctx):
     print(f"    producer finished issuing (rel): ", " ".join(f"{n}@{v - t0:.1f}" for n, v in zip(["qkv", "attn", "o", "gate_up", "down"], pb)))
 
 
+VARIANT_KEYS = (("inflight", "-DAHA_FUSED_INFLIGHT_KB="),)
+
+
+def variant_lib(conf):
+    """variants/<name>.so for the build keys of a spec (None: none given), built from this tree when it is missing"""
+    keys = [k for k, _ in VARIANT_KEYS if k in conf]
+    if not keys and not int(conf.get("trace", 0)):
+        return None
+    name = "_".join(f"{k}{conf[k]}" for k in keys) + ("_trace" if int(conf.get("trace", 0)) else "")
+    path = os.path.join(ROOT, "variants", name.strip("_") + ".so")
+    if not os.path.exists(path):
+        from aha_b200 import build
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        defs = [d + conf[k] for k, d in VARIANT_KEYS if k in conf] + (["-DAHA_STAGE_TRACE"] if int(conf.get("trace", 0)) else [])
+        subprocess.run([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + build.NVCC_FLAGS + defs + ["-o", path] + build.SOURCES + ["-ldl"], check=True)
+    return path
+
+
+def rows_per_stage(K, N, grid):   # decode_fused.cuh
+    r = max(1, min(8, 16384 // (2 * K)))
+    if r > 1:
+        r &= ~1
+    while r > 2 and N // grid < r * 5:
+        r >>= 1
+    return r
+
+
+def n_stages(j0, j1, R, ends=()):
+    n, j = 0, j0
+    while j < j1:
+        end = min([e for e in ends if e > j] + [j1])
+        j += min(R, end - j)
+        n += 1
+    return n
+
+
+def layer_phases(cta, grid, ctx):
+    """stages per phase [qkv, attn, o_proj, gate/up, down] of one layer of CTA `cta` (Producer's schedule in decode_fused.cuh)"""
+    H, I, hd, nh, nkv = cfg["hidden_size"], cfg["intermediate_size"], 128, cfg["num_attention_heads"], cfg["num_key_value_heads"]
+    nsplit, G, qkv_dim = max(1, min(32, grid // nkv)), nh // nkv, (nh + 2 * nkv) * hd
+    rows = lambda N, unit: ((N // unit * cta) // grid * unit, (N // unit * (cta + 1)) // grid * unit)
+    out = [0, 0]
+    if cta < nkv * nsplit:
+        n, split = (G + 2) * hd, cta % nsplit
+        out[0] = n_stages(n * split // nsplit, n * (split + 1) // nsplit, rows_per_stage(H, qkv_dim, grid), (G * hd, (G + 1) * hd))
+        nhp = (ctx + 1 + 15) // 16
+        per = (nhp + nsplit - 1) // nsplit
+        out[1] = max(0, min(nhp, split * per + per) - split * per)
+    out.append(n_stages(*rows(H, 1), rows_per_stage(nh * hd, H, grid)))
+    out.append(n_stages(*rows(2 * I, 2), rows_per_stage(H, 2 * I, grid)))
+    out.append(n_stages(*rows(H, 1), rows_per_stage(I, H, grid)))
+    return out
+
+
+def overlap(a0, a1, iv):   # total length of the intervals iv (sorted, disjoint) inside [a0, a1)
+    return sum(max(0.0, min(a1, e) - max(a0, b)) for b, e in iv)
+
+
+def union(iv):
+    out = []
+    for b, e in sorted(iv):
+        if out and b <= out[-1][1]:
+            out[-1][1] = max(out[-1][1], e)
+        else:
+            out.append([b, e])
+    return out
+
+
+def stage_gaps(t, cta, grid, ctx, ns):
+    """Per phase boundary of layers 2 .. L-2: the window from the CTA's last slot release of a phase to its first wait of the
+    next, how much of it the CTA had no copy in flight, and how long the producer was held back in it (able to issue -- the
+    previous stage issued and the slot free -- but not issuing: the in-flight cap, or the run-ahead gate of earlier builds).  A copy is in flight
+    from its issue to its landing; the landing is stamped only when the owner warp was already waiting, so for the other
+    copies it is taken as issue + the median issue-to-landing time of the waited-for ones (an estimate)."""
+    ph = layer_phases(cta, grid, ctx)
+    n = int((t[:, 0] > 0).sum())
+    t = t[:n].astype(np.float64) / 1e3   # us
+    per = sum(ph)
+    waited = t[:, 2] - t[:, 1] > 0.1
+    lat = np.median(t[waited, 2] - t[waited, 0]) if waited.any() else 0.0
+    land = np.where(waited, t[:, 2], np.minimum(t[:, 2], t[:, 0] + lat))
+    busy = union([[a, b] for a, b in zip(t[:, 0], land)])
+    idle = union([[b1, a2] for (_, b1), (a2, _) in zip(busy[:-1], busy[1:]) if a2 > b1])
+    hold = []
+    for i in range(1, n):
+        free = max(t[i - 1, 0], t[i - ns, 3] if i >= ns else 0.0)
+        if t[i, 0] > free:
+            hold.append([free, t[i, 0]])
+    hold = union(hold)
+    names = ["qkv>attn", "attn>o", "o>gate/up", "gate/up>down", "down>qkv"]
+    acc = np.zeros((5, 3))
+    layers = range(2, cfg["num_hidden_layers"] - 1)
+    for l in layers:
+        s0 = l * per
+        b = np.cumsum([0] + ph) + s0
+        for k in range(5):
+            cur, nxt = (b[k], b[k + 1]), (b[k + 1], b[k + 2]) if k < 4 else (b[5], b[5] + ph[0])
+            if cur[1] == cur[0] or nxt[1] == nxt[0]:
+                continue
+            w0, w1 = t[cur[0]:cur[1], 3].max(), t[nxt[0]:nxt[1], 1].min()
+            acc[k] += [max(0.0, w1 - w0), overlap(w0, w1, idle), overlap(w0, w1, hold)]
+    acc /= len(layers)
+    lay = (t[(layers[-1] + 1) * per, 0] - t[layers[0] * per, 0]) / len(layers)
+    tot_idle = overlap(t[layers[0] * per, 0], t[(layers[-1] + 1) * per, 0], idle) / len(layers)
+    tot_hold = overlap(t[layers[0] * per, 0], t[(layers[-1] + 1) * per, 0], hold) / len(layers)
+    print(f"  cta {cta} stages/layer {ph}; per layer {lay:.1f} us, no copy in flight {tot_idle:.1f} us, producer held {tot_hold:.1f} us; "
+          f"median issue-to-landing {lat:.2f} us")
+    for k in range(5):
+        print(f"    boundary {names[k]:13s} window {acc[k, 0]:5.2f} us  no copy in flight {acc[k, 1]:5.2f} us  producer held {acc[k, 2]:5.2f} us")
+
+
 def run(conf, models):
     impl = int(conf.get("impl", os.environ.get("AHA_DECODE_IMPL", "0")))
     ctx = int(conf.get("ctx", os.environ.get("AHA_CTX", "2554")))
@@ -69,7 +183,7 @@ def run(conf, models):
         os.environ["AHA_FUSED_STAGES"] = str(conf["stages"])
     else:
         os.environ.pop("AHA_FUSED_STAGES", None)
-    lib = os.path.join(ROOT, "variants", f"ahead{conf['ahead']}.so") if "ahead" in conf else DEFAULT_LIB
+    lib = variant_lib(conf) or DEFAULT_LIB
     lib = os.path.abspath(conf["lib"]) if "lib" in conf else lib
     lib_tag = os.path.basename(lib)
     if (lib, impl) not in models:
@@ -96,9 +210,11 @@ def run(conf, models):
             m.debug_read("fused_stage_trace", 0, 4 * 8192)   # clears the region
             m.decode_steps(5, ctx, 1)
             t = m.debug_read("fused_stage_trace", 0, 4 * 8192).reshape(8192, 4)
-            tag = f"{shape}_impl{impl}_dbg{dbg}_cta{cta}"
+            tag = f"{shape}_{lib_tag[:-3]}_impl{impl}_dbg{dbg}_cta{cta}"
             np.save(f"profile_out/stage_trace_{tag}.npy", t)
             print(f"  saved profile_out/stage_trace_{tag}.npy ({int((t[:, 0] > 0).sum())} stages)")
+            if cta < torch_sms() and (t[:, 0] > 0).any():
+                stage_gaps(t, cta, torch_sms(), ctx, int(conf.get("stages", conf.get("ns", 11))))
     if int(conf.get("sy", 0)):   # sync anatomy (AHA_STAGE_TRACE build): barrier sub-steps and activation-load sub-steps of 3 CTAs
         os.makedirs("profile_out", exist_ok=True)
         for cta in (0, 77, 147):
@@ -106,7 +222,7 @@ def run(conf, models):
             m.debug_read("fused_sync_trace", 0, 8192)
             m.decode_steps(5, ctx, 1)
             t = m.debug_read("fused_sync_trace", 0, 8192)
-            tag = f"{shape}_impl{impl}_dbg{dbg}_cta{cta}"
+            tag = f"{shape}_{lib_tag[:-3]}_impl{impl}_dbg{dbg}_cta{cta}"
             np.save(f"profile_out/sync_trace_{tag}.npy", t)
             b = t[:4096].reshape(512, 8)[:112]
             l = t[4096:].reshape(1024, 4)[:112]
