@@ -185,6 +185,21 @@ class PrefixStats(C.Structure):
                 ("evicted_pages", C.c_uint64), ("max_pages", C.c_uint64), ("free_pages", C.c_uint64)]
 
 
+class SwapStats(C.Structure):
+    _fields_ = [("host_pages", C.c_uint64), ("free_host_pages", C.c_uint64), ("suspended", C.c_uint64), ("pages_out", C.c_uint64),
+                ("pages_in", C.c_uint64), ("bytes_out", C.c_uint64), ("bytes_in", C.c_uint64), ("suspend_secs", C.c_double),
+                ("resume_secs", C.c_double)]
+
+
+def swap_int(name, v, lo, hi):
+    """v as an int in [lo, hi], refused the way the swap entries' arguments are: TypeError for a non-int (bool included), ValueError out of range"""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+        raise TypeError(f"{name} must be an int, not {type(v).__name__}")
+    if not lo <= int(v) <= hi:
+        raise ValueError(f"{name} must be {lo} to {hi}, got {int(v)}")
+    return int(v)
+
+
 # every symbol include/aha_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 _U32P = C.POINTER(C.c_uint32)
@@ -237,6 +252,14 @@ SYMBOLS = {
     "aha_b200_batch_close": (C.c_int, [_P]),
     "aha_b200_batch_prefix_cache": (C.c_int, [_P, C.c_size_t]),
     "aha_b200_batch_prefix_stats": (C.c_int, [_P, C.POINTER(PrefixStats), C.POINTER(C.c_size_t), C.c_size_t]),
+    "aha_b200_batch_swap_space": (C.c_int, [_P, C.c_size_t]),
+    "aha_b200_batch_cancel": (C.c_int, [_P, C.c_int32]),
+    "aha_b200_batch_suspend": (C.c_int, [_P, C.c_int32, _U32P]),
+    "aha_b200_batch_resume": (C.c_int, [_P, C.c_uint32, _I32P]),
+    "aha_b200_batch_discard": (C.c_int, [_P, C.c_uint32]),
+    "aha_b200_batch_swap_stats": (C.c_int, [_P, C.POINTER(SwapStats)]),
+    "aha_b200_debug_kv_swap": (C.c_int, [_P, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, C.c_size_t, _I32P, _I32P, _I32P, _F32P, _F32P,
+                                         _F32P]),
     "aha_b200_debug_prefix_attention": (C.c_int, [_P, C.c_int, C.c_size_t, C.c_size_t, _I32P, C.c_size_t, _I32P, _F32P, _F32P, _F32P, _F32P]),
     "aha_b200_batch_open_wide": (C.c_int, [_P, C.c_size_t]),
     "aha_b200_batch_step_n": (C.c_int, [_P, _U32P, C.POINTER(C.c_int32), C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -225,6 +225,29 @@ struct aha_model {
     };
     std::map<uint32_t, Rules> rules;
     uint32_t next_rules_id = 1;
+    // Swap preemption (aha_b200_batch_swap_space / _suspend / _resume): a pinned host arena of host pages, each holding one KV page of every
+    // layer ([layer][page_stride] fp32), kept across sessions until it is resized or the handle is destroyed, and its free list -- a pool of
+    // its own, apart from the device PagePool.  The counters run for the handle's lifetime.
+    struct SwapArena {
+        float* host = nullptr;          // cudaHostAlloc-ed
+        size_t pages = 0;
+        std::vector<int> free;          // free host pages
+        uint64_t pages_out = 0, pages_in = 0;
+        double suspend_secs = 0, resume_secs = 0;
+    } swap;
+    // a suspended request of the open session (aha_b200_batch_suspend): everything its slot held, its K/V in the arena
+    struct Suspended {
+        std::vector<int> host_pages;    // logical page p -> host page
+        int mapped = 0;                 // pages its table held
+        DecodeState st{};
+        std::vector<uint32_t> hist;     // history [0, st.n_hist)
+        Sampler sampler;
+        int lp = 0;                     // BatchSlot::lp
+        size_t budget = 0, produced = 0, hit = 0;
+    };
+    std::map<uint32_t, Suspended> suspended;   // by id (>= 1)
+    uint32_t next_suspend_id = 1;
+    size_t swap_page_bytes() const { return (size_t)text.cfg.L * text.page_stride * sizeof(float); }
 };
 
 namespace {
@@ -653,6 +676,8 @@ struct RequestReset {
 };
 // ends the batch session, if one is open, and leaves the handle as clear_cache() does
 void session_close(aha_model* m) {
+    for (auto& e : m->suspended) m->swap.free.insert(m->swap.free.end(), e.second.host_pages.begin(), e.second.host_pages.end());
+    m->suspended.clear();   // suspended requests belong to the session
     for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->reset();
     m->spec.steps.clear();
     m->spec.built_epoch = ~0ull;
@@ -1382,6 +1407,133 @@ void session_open(aha_model* m, int width) {
     m->session.wide = width != 0;
     m->session.width = width == 0 ? kGemvBatchMax : width;
 }
+// ---- ending and swapping requests between steps (aha_b200_batch_cancel / _suspend / _resume / _discard).  Every check runs before anything
+// is copied or written (suspend first reads the slot's DecodeState), so a refused call changes nothing.
+void session_check_slot(const aha_model* m, int32_t slot, const std::string& who) {
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    AHA_REQUIRE(slot >= 0 && slot < m->session.width, who + "slot " + std::to_string(slot) + " is outside the session's " +
+                                                          std::to_string(m->session.width) + " slots");
+    AHA_REQUIRE(m->session.used[slot], who + "slot " + std::to_string(slot) + " runs no request");
+}
+// the request in `slot` ends as if it had finished: its pages go back at once (the prefix index keeps its references) and the slot shows
+// no record; a speculative slot keeps its counters until the slot is taken again
+void session_cancel(aha_model* m, int32_t slot) {
+    session_check_slot(m, slot, "batch_cancel: ");
+    session_release(m, slot);
+    m->session.lp_valid[slot] = false;
+    m->session.last_n[slot] = 0;
+}
+aha_model::Suspended& suspended_of(aha_model* m, uint32_t id, const std::string& who) {
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    const auto it = m->suspended.find(id);
+    AHA_REQUIRE(it != m->suspended.end(), who + "no suspended request of this session has id " + std::to_string(id));
+    return it->second;
+}
+// The request in `slot` to the swap arena: the K/V pages it has written (logical pages 0 .. ceil(pos / 32) - 1, pos from its device
+// DecodeState), its DecodeState, its history and the host-side slot state; then the slot and every page reference it held are released as
+// session_release does.  -> its id.
+uint32_t session_suspend(aha_model* m, int32_t slot) {
+    const std::string who = "batch_suspend: ";
+    session_check_slot(m, slot, who);
+    AHA_REQUIRE(!m->session.spec[slot], who + "slot " + std::to_string(slot) + " runs a speculative request, which cannot be suspended "
+                                                "(aha_b200_batch_cancel ends it)");
+    aha_model::SwapArena& A = m->swap;
+    AHA_REQUIRE(A.pages > 0, who + "the handle has no swap space (aha_b200_batch_swap_space)");
+    AHA_REQUIRE(m->next_suspend_id != 0, who + "the handle has used every suspended-request id");
+    TextModel& T = m->text;
+    BatchDecoder& B = m->sess();
+    BatchSlot& sl = B.slots[slot];
+    Ctx& c = m->ctx;
+    const auto t0 = clk::now();
+    aha_model::Suspended r;
+    AHA_CUDA_CHECK(cudaMemcpyAsync(&r.st, B.d_states + slot, sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    const int pages = ceil_div(r.st.pos, kPage);
+    AHA_REQUIRE(pages >= 1 && pages <= sl.table.mapped && r.st.n_hist >= 1 && r.st.n_hist <= T.hist_cap, who + "slot " + std::to_string(slot) +
+                                                                                                           " holds an inconsistent decode state");
+    AHA_REQUIRE((size_t)pages <= A.free.size(), who + "the request has written " + std::to_string(pages) + " KV pages, but only " +
+                                                    std::to_string(A.free.size()) + " of the " + std::to_string(A.pages) + " host pages are free");
+    r.host_pages.assign(A.free.end() - pages, A.free.end());
+    r.hist.resize((size_t)r.st.n_hist);
+    kv_swap(c, true, T.kv_pool, T.layer_stride, T.page_stride, T.cfg.L, sl.table.h.data(), r.host_pages.data(), A.host, pages);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(r.hist.data(), B.d_hist + (size_t)slot * T.hist_cap, r.hist.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    A.free.resize(A.free.size() - pages);
+    r.mapped = sl.table.mapped;
+    r.sampler = sl.sampler;
+    r.lp = sl.lp;
+    r.budget = m->session.budget[slot]; r.produced = m->session.produced[slot]; r.hit = m->session.hit[slot];
+    const uint32_t id = m->next_suspend_id++;
+    m->suspended.emplace(id, std::move(r));
+    session_release(m, slot);
+    m->session.lp_valid[slot] = false;
+    m->session.last_n[slot] = 0;
+    A.pages_out += (uint64_t)pages;
+    A.suspend_secs += seconds(clk::now() - t0);
+    return id;
+}
+// A suspended request back into the lowest free slot: the same number of pages it held (cached prefix pages may be evicted for them, as at
+// admission; its shared prefix pages come back as its own), its K/V, DecodeState, history and slot state restored, its sampler bound to the
+// new slot.  No token is delivered: its next one comes from the next step.  -> the slot.
+int32_t session_resume(aha_model* m, uint32_t id) {
+    const std::string who = "batch_resume: ";
+    aha_model::Suspended& r = suspended_of(m, id, who);
+    int slot = -1;
+    for (int i = 0; i < m->session.width && slot < 0; ++i) if (!m->session.used[i]) slot = i;
+    AHA_REQUIRE(slot >= 0, who + "all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
+    if (session_has_spec(m)) session_check_rows(m, 1, who);
+    prefix_check_room(m, (size_t)r.mapped, {}, who + "the request needs ");
+    prefix_make_room(m, (size_t)r.mapped, {});
+    TextModel& T = m->text;
+    BatchDecoder& B = m->sess();
+    BatchSlot& sl = B.slots[slot];
+    aha_model::SwapArena& A = m->swap;
+    Ctx& c = m->ctx;
+    const auto t0 = clk::now();
+    const int pages = (int)r.host_pages.size();
+    T.pages.map(sl.table, std::min(r.mapped * kPage, T.max_ctx));
+    m->session.used[slot] = true;
+    kv_swap(c, false, T.kv_pool, T.layer_stride, T.page_stride, T.cfg.L, sl.table.h.data(), r.host_pages.data(), A.host, pages);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + slot, &r.st, sizeof(DecodeState), cudaMemcpyHostToDevice, c.stream));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_hist + (size_t)slot * T.hist_cap, r.hist.data(), r.hist.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
+    if (r.lp > 0) B.ensure_lp();
+    sl.lp = r.lp;
+    B.bind_sampler(slot, r.sampler);
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    m->session.budget[slot] = r.budget; m->session.produced[slot] = r.produced; m->session.hit[slot] = r.hit;
+    m->session.lp_valid[slot] = false;
+    m->session.spec[slot] = false;
+    m->session.spec_stats[slot] = aha_spec_stats{};
+    m->session.last_n[slot] = 0;
+    B.composition_changed();
+    A.free.insert(A.free.end(), r.host_pages.begin(), r.host_pages.end());
+    A.pages_in += (uint64_t)pages;
+    A.resume_secs += seconds(clk::now() - t0);
+    m->suspended.erase(id);
+    return slot;
+}
+void session_discard(aha_model* m, uint32_t id) {
+    aha_model::Suspended& r = suspended_of(m, id, "batch_discard: ");
+    m->swap.free.insert(m->swap.free.end(), r.host_pages.begin(), r.host_pages.end());
+    m->suspended.erase(id);
+}
+// The arena resized to max_tokens / 32 host pages (0 frees it); refused while a request is suspended.  The new arena is allocated before
+// the old one is freed, so a failed allocation leaves the old one in place.
+void swap_space(aha_model* m, size_t max_tokens) {
+    aha_model::SwapArena& A = m->swap;
+    AHA_REQUIRE(m->suspended.empty(), "batch_swap_space: " + std::to_string(m->suspended.size()) + " requests are suspended (resume or "
+                                      "discard them first)");
+    const size_t pages = max_tokens / kPage;
+    if (pages == A.pages) return;
+    float* host = nullptr;
+    if (pages) AHA_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&host), pages * m->swap_page_bytes(), cudaHostAllocPortable));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
+    if (A.host) AHA_CUDA_CHECK(cudaFreeHost(A.host));
+    A.host = host; A.pages = pages;
+    A.free.clear();
+    for (int p = 0; p < (int)pages; ++p) A.free.push_back(p);
+}
+
 // n requests admitted in one call (aha_b200_batch_add_many).  Text-only requests that fit max_prefill are cut, in input order, into packed
 // prefills (TextModel::prefill with PrefillSegments: each request attends only to itself and its positions restart at 0), so one pass over the
 // weights serves them all; their last rows then go through the step's batched lm_head and each request's own ArgMax / sampler.  A request
@@ -2054,6 +2206,43 @@ int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hit
     });
 }
 
+int aha_b200_batch_swap_space(aha_model* m, size_t max_tokens) { return guarded(m, [&] { swap_space(m, max_tokens); }); }
+
+int aha_b200_batch_cancel(aha_model* m, int32_t slot) { return guarded(m, [&] { session_cancel(m, slot); }); }
+
+int aha_b200_batch_suspend(aha_model* m, int32_t slot, uint32_t* id_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(id_out, "batch_suspend: id_out is required");
+        *id_out = session_suspend(m, slot);
+    });
+}
+
+int aha_b200_batch_resume(aha_model* m, uint32_t id, int32_t* slot_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(slot_out, "batch_resume: slot_out is required");
+        *slot_out = session_resume(m, id);
+    });
+}
+
+int aha_b200_batch_discard(aha_model* m, uint32_t id) { return guarded(m, [&] { session_discard(m, id); }); }
+
+int aha_b200_batch_swap_stats(aha_model* m, aha_swap_stats* out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(out, "batch_swap_stats: out is required");
+        const aha_model::SwapArena& A = m->swap;
+        *out = aha_swap_stats{};
+        out->host_pages = A.pages;
+        out->free_host_pages = A.free.size();
+        out->suspended = m->suspended.size();
+        out->pages_out = A.pages_out;
+        out->pages_in = A.pages_in;
+        out->bytes_out = A.pages_out * m->swap_page_bytes();
+        out->bytes_in = A.pages_in * m->swap_page_bytes();
+        out->suspend_secs = A.suspend_secs;
+        out->resume_secs = A.resume_secs;
+    });
+}
+
 int aha_b200_batch_close(aha_model* m) {
     return guarded(m, [&] { AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream)); session_close(m); });
 }
@@ -2121,6 +2310,9 @@ int aha_b200_fsm_destroy(aha_model* m, uint32_t id) {
         for (int i = 0; m->session.open && i < m->session.width; ++i)
             AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].fsm_id == id),
                         "fsm_destroy: token automaton " + std::to_string(id) + " constrains the running request in slot " + std::to_string(i));
+        for (const auto& e : m->suspended)
+            AHA_REQUIRE(e.second.sampler.fsm_id != id,
+                        "fsm_destroy: token automaton " + std::to_string(id) + " constrains suspended request " + std::to_string(e.first));
         for (const auto& r : m->rules)
             AHA_REQUIRE(r.second.fsm != id, "fsm_destroy: token automaton " + std::to_string(id) + " is named by logit-rules object " +
                                                 std::to_string(r.first) + " (destroy that first)");
@@ -2162,6 +2354,9 @@ int aha_b200_rules_destroy(aha_model* m, uint32_t id) {
         for (int i = 0; m->session.open && i < m->session.width; ++i)
             AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].rules_id == id),
                         "rules_destroy: logit-rules object " + std::to_string(id) + " applies to the running request in slot " + std::to_string(i));
+        for (const auto& e : m->suspended)
+            AHA_REQUIRE(e.second.sampler.rules_id != id,
+                        "rules_destroy: logit-rules object " + std::to_string(id) + " applies to suspended request " + std::to_string(e.first));
         AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         if (it->second.mem) AHA_CUDA_CHECK(cudaFree(it->second.mem));
         m->rules.erase(it);
@@ -2283,6 +2478,37 @@ void debug_verify_run(aha_model* m, int n, const int* R, const int* pos0, const 
 }
 }  // namespace
 }  // extern "C++"
+
+int aha_b200_debug_kv_swap(aha_model* m, size_t layers, size_t page_floats, size_t n_pool_pages, size_t n_host_pages, size_t n,
+                           const int32_t* table_out, const int32_t* table_in, const int32_t* host_pages, const float* pool_in, float* host_out,
+                           float* pool_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(table_out && table_in && host_pages && pool_in && host_out && pool_out, "debug_kv_swap: every array is required");
+        AHA_REQUIRE(layers >= 1 && page_floats >= 1, "debug_kv_swap: layers and page_floats must be positive");
+        AHA_REQUIRE(n >= 1 && n <= n_pool_pages && n <= n_host_pages, "debug_kv_swap: 1 <= n <= the pool's and the arena's pages");
+        for (size_t p = 0; p < n; ++p)
+            AHA_REQUIRE(table_out[p] >= 0 && (size_t)table_out[p] < n_pool_pages && table_in[p] >= 0 && (size_t)table_in[p] < n_pool_pages &&
+                        host_pages[p] >= 0 && (size_t)host_pages[p] < n_host_pages, "debug_kv_swap: page index out of range");
+        Ctx& c = m->ctx;
+        Scratch sc;
+        const size_t pool_n = layers * n_pool_pages * page_floats, host_n = n_host_pages * layers * page_floats;
+        float* pool = sc.alloc<float>(pool_n);
+        struct Pinned {
+            float* p = nullptr;
+            ~Pinned() { if (p) cudaFreeHost(p); }
+        } arena;
+        AHA_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&arena.p), host_n * sizeof(float), cudaHostAllocPortable));
+        std::fill(arena.p, arena.p + host_n, std::numeric_limits<float>::quiet_NaN());
+        AHA_CUDA_CHECK(cudaMemcpy(pool, pool_in, pool_n * sizeof(float), cudaMemcpyHostToDevice));
+        const size_t layer_stride = n_pool_pages * page_floats;
+        kv_swap(c, true, pool, layer_stride, page_floats, (int)layers, table_out, host_pages, arena.p, (int)n);
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        std::memcpy(host_out, arena.p, host_n * sizeof(float));
+        kv_swap(c, false, pool, layer_stride, page_floats, (int)layers, table_in, host_pages, arena.p, (int)n);
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+        AHA_CUDA_CHECK(cudaMemcpy(pool_out, pool, pool_n * sizeof(float), cudaMemcpyDeviceToHost));
+    });
+}
 
 int aha_b200_debug_verify_attn(aha_model* m, size_t rows, size_t n_heads, size_t n_kv_heads, size_t pos0, const float* q, const float* k,
                                const float* v, float* out) {
@@ -3557,6 +3783,7 @@ void aha_b200_destroy(aha_model* m) {
     m->ctx.free_all();
     if (m->h_pin) cudaFreeHost(m->h_pin);
     if (m->h_lp_pin) cudaFreeHost(m->h_lp_pin);
+    if (m->swap.host) cudaFreeHost(m->swap.host);
     if (m->ev0) cudaEventDestroy(m->ev0);
     if (m->ev1) cudaEventDestroy(m->ev1);
     for (auto& e : m->ev_tok) if (e) cudaEventDestroy(e);

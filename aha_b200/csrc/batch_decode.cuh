@@ -29,6 +29,7 @@
 #include "gemv_batch.cuh"
 #include "gemv_wide.cuh"
 #include "kv_fork.cuh"
+#include "kv_swap.cuh"
 #include "text_model.cuh"
 
 namespace aha {
@@ -40,6 +41,7 @@ struct BatchSlot {                       // one sequence of the batch
     int lp = 0;                          // 0: the request asked for no log-probabilities, else 1 + its top count
     uint32_t fsm_id = 0;                 // the token automaton the request is constrained by (0: none); it cannot be destroyed while the slot runs
     uint32_t rules_id = 0;               // the request's logit-rules object (0: none); it cannot be destroyed while the slot runs
+    Sampler sampler;                     // the request's sampler as bound (a suspended request takes it along and is bound again at resume)
 };
 
 struct BatchDecoder {
@@ -176,6 +178,7 @@ struct BatchDecoder {
     void bind_sampler(int i, const Sampler& s) {
         BatchSlot& sl = slots[i];
         sl.samp_active = s.active;
+        sl.sampler = s;
         sl.fsm_id = s.fsm_id;
         sl.rules_id = s.rules_id;
         if (s.active) sl.samp = T->bind_sampler(s, d_states + i, d_hist + (size_t)i * T->hist_cap, d_tok + i, workb + (size_t)i * T->cfg.V, counts(s, i));

@@ -627,6 +627,62 @@ class B200Model:
         self._check(self._lib.aha_b200_batch_prefix_stats(self._h, C.byref(st), hits, w))
         return {name: int(getattr(st, name)) for name, _ in L.PrefixStats._fields_}, {i: int(hits[i]) for i in range(w) if hits[i]}
 
+    # ---- cancel, suspend and resume requests of the open session (swap preemption)
+    def batch_swap_space(self, max_tokens):
+        """Size the handle's pinned host arena to max_tokens / 32 host pages (aha_b200_batch_swap_space; 0 frees it).  It outlives sessions;
+        resizing is refused while a request is suspended."""
+        n = L.swap_int("max_tokens", max_tokens, 0, 2 ** 63 - 1)
+        self._check(self._lib.aha_b200_batch_swap_space(self._h, n))
+
+    def batch_cancel(self, slot):
+        """End the request in `slot` now, as if it had finished (a client went away): its pages and the slot are free at once, and
+        batch_logprobs shows no record for it."""
+        slot = L.swap_int("slot", slot, 0, 63)
+        self._check(self._lib.aha_b200_batch_cancel(self._h, slot))
+
+    def batch_suspend(self, slot):
+        """Copy the request in `slot` to the swap arena and free its slot and pages -> its id (>= 1), for batch_resume / batch_discard."""
+        slot, i = L.swap_int("slot", slot, 0, 63), C.c_uint32(0)
+        self._check(self._lib.aha_b200_batch_suspend(self._h, slot, C.byref(i)))
+        return int(i.value)
+
+    def batch_resume(self, id):
+        """Put a suspended request back into the lowest free slot -> that slot.  It delivers its next token at the next step, exactly the
+        token it would have delivered uninterrupted."""
+        id, s = L.swap_int("id", id, 1, 2 ** 32 - 1), C.c_int32(-1)
+        self._check(self._lib.aha_b200_batch_resume(self._h, id, C.byref(s)))
+        return int(s.value)
+
+    def batch_discard(self, id):
+        """Free a suspended request without resuming it."""
+        id = L.swap_int("id", id, 1, 2 ** 32 - 1)
+        self._check(self._lib.aha_b200_batch_discard(self._h, id))
+
+    def batch_swap_stats(self):
+        """-> dict(host_pages, free_host_pages, suspended, pages_out, pages_in, bytes_out, bytes_in, suspend_secs, resume_secs)"""
+        st = L.SwapStats()
+        self._check(self._lib.aha_b200_batch_swap_stats(self._h, C.byref(st)))
+        return {name: (float if name.endswith("secs") else int)(getattr(st, name)) for name, _ in L.SwapStats._fields_}
+
+    def debug_kv_swap(self, pool, table_out, table_in, host_pages, n_host_pages):
+        """The page copies of suspend / resume on host data (aha_b200_debug_kv_swap): pool [layers][n_pool_pages][page_floats]; logical page p goes out from
+        pool page table_out[p] to host page host_pages[p] and back into pool page table_in[p] -> (arena [n_host_pages][layers][page_floats]
+        after the way out, pool after the way back)."""
+        pool = np.ascontiguousarray(pool, np.float32)
+        if pool.ndim != 3:
+            raise ValueError("pool must be [layers][n_pool_pages][page_floats]")
+        layers, n_pool, pf = pool.shape
+        to, ti, hp = (np.ascontiguousarray(np.asarray(a, np.int32).reshape(-1)) for a in (table_out, table_in, host_pages))
+        if not to.size == ti.size == hp.size:
+            raise ValueError("table_out, table_in and host_pages must have one entry per page")
+        host = np.empty((int(n_host_pages), layers, pf), np.float32)
+        out = np.empty_like(pool)
+        f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+        i32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_int32))
+        self._check(self._lib.aha_b200_debug_kv_swap(self._h, layers, pf, n_pool, int(n_host_pages), to.size, i32(to), i32(ti), i32(hp), f(pool),
+                                                     f(host), f(out)))
+        return host, out
+
     def generate_stream(self, input_ids, on_token, data=None, max_tokens=1024, temperature=0.0, top_p=None, top_k=None,
                         repeat_penalty=1.0, repeat_last_n=64, seed=299792458, reuse_prefix=False, logprobs=False, top_logprobs=0, fsm=None,
                         rules=None):

@@ -346,6 +346,41 @@ typedef struct aha_prefix_stats {
  * took from the cache (0 for a free slot) -- what a server reports as usage.prompt_tokens_details.cached_tokens. */
 int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hits_out, size_t cap);
 
+/* Cancel, suspend and resume requests of a batch session (narrow or wide; new design).  All of them run between steps; each checks
+ * everything before it copies or writes anything, so a refused call changes nothing.
+ *   batch_swap_space(max_tokens): the handle's pinned host arena becomes max_tokens / 32 host pages, each holding one KV page of every layer
+ *     (layers x 2 x kv_heads x 32 x head_dim fp32); 0 frees it.  Allocated once (cudaHostAlloc), it stays on the handle across sessions
+ *     until it is resized or the handle is destroyed.  Works with or without an open session; refused while a request is suspended.
+ *   batch_cancel(slot): the running request in `slot` (plain or speculative) ends as if it had finished: its pages go back to the pool at
+ *     once (the prefix index keeps its references), the slot is free, and batch_logprobs shows no record for it.  A speculative slot keeps
+ *     its batch_spec_stats until the slot is taken again.
+ *   batch_suspend(slot, &id): the request's K/V pages written so far (logical pages 0 .. ceil(pos / 32) - 1), its decode state, history,
+ *     sampler, record setting and token budget are copied to free host pages of the arena, then the slot and every page it held are
+ *     released as when it finishes.  *id_out (>= 1) names the suspended request.  Refused for a speculative slot.
+ *   batch_resume(id, &slot): the request goes back into the lowest free slot with as many pages as it held (cached prefix pages are evicted
+ *     for room as at admission; its shared prefix pages come back as its own), its state restored bit for bit and its host pages freed.
+ *     No token is delivered: its next token, and from then on its record, come from the next step.  Refused without a free slot, without
+ *     the pages, or (wide session with speculative requests) when its row would not fit 64; the request then stays suspended.
+ *   batch_discard(id): frees a suspended request without resuming it.
+ * A resumed request yields exactly the ids and records it would have yielded uninterrupted in the same session kind, whatever slot it
+ * resumes into and whatever ran meanwhile.  Suspended requests belong to their session: batch_close and clear_cache discard them.
+ * Refusals: no open session, a slot out of range or not running, an unknown id, no arena or too few free host pages. */
+int aha_b200_batch_swap_space(aha_model* m, size_t max_tokens);
+int aha_b200_batch_cancel(aha_model* m, int32_t slot);
+int aha_b200_batch_suspend(aha_model* m, int32_t slot, uint32_t* id_out);
+int aha_b200_batch_resume(aha_model* m, uint32_t id, int32_t* slot_out);
+int aha_b200_batch_discard(aha_model* m, uint32_t id);
+typedef struct aha_swap_stats {
+    uint64_t host_pages;             /* pages of the arena */
+    uint64_t free_host_pages;        /* of those, pages no suspended request holds */
+    uint64_t suspended;              /* suspended requests */
+    uint64_t pages_out, pages_in;    /* host pages written by suspends / read by resumes, over the handle's lifetime */
+    uint64_t bytes_out, bytes_in;    /* the same in bytes */
+    double suspend_secs;             /* host-clock seconds spent in batch_suspend (each call ends in a stream synchronise) */
+    double resume_secs;              /* the same in batch_resume */
+} aha_swap_stats;
+int aha_b200_batch_swap_stats(aha_model* m, aha_swap_stats* out);
+
 /* WhisperFeatureExtractor::call (src/models/feature_extractor/
  * feature_extraction_whisper.rs:65-115): wave (n) f32 host -> log-mel (n_mels, n_frames) f32 host.
  * Returns frames through *n_frames.  Qwen3-ASR handles only. */
@@ -538,7 +573,7 @@ int aha_b200_nccl_unique_id(uint8_t out[128]);
 /* Token automata (AHA_GEN_CONSTRAINED).  aha_b200_fsm_check (host only, no handle): 0 when `fsm` is well formed over a vocabulary of
  * `vocab` tokens, else 1 with the reason in aha_b200_last_error(NULL).  aha_b200_fsm_create checks it against the handle's vocabulary and
  * copies it to device memory: *id_out (>= 1) names it in params.reserved until aha_b200_fsm_destroy or aha_b200_destroy frees it.
- * aha_b200_fsm_destroy refuses an id that a running batch slot uses. */
+ * aha_b200_fsm_destroy refuses an id that a running batch slot or a suspended request uses. */
 int aha_b200_fsm_check(const aha_token_fsm* fsm, size_t vocab);
 int aha_b200_fsm_create(aha_model* m, const aha_token_fsm* fsm, uint32_t* id_out);
 int aha_b200_fsm_destroy(aha_model* m, uint32_t id);
@@ -546,7 +581,7 @@ int aha_b200_fsm_destroy(aha_model* m, uint32_t id);
 /* Logit-rules objects (AHA_GEN_LOGIT_RULES).  aha_b200_rules_check (host only, no handle): 0 when `r` is well formed over a vocabulary of
  * `vocab` tokens, else 1 with the reason in aha_b200_last_error(NULL) (r->fsm is not looked up).  aha_b200_rules_create also checks that
  * r->fsm names an automaton on the handle, and copies the bias list to device memory: *id_out (>= 1) names it in params.reserved until
- * aha_b200_rules_destroy or aha_b200_destroy frees it.  aha_b200_rules_destroy refuses an id that a running batch slot uses, and
+ * aha_b200_rules_destroy or aha_b200_destroy frees it.  aha_b200_rules_destroy refuses an id that a running batch slot or a suspended request uses, and
  * aha_b200_fsm_destroy refuses an automaton that a live rules object names.  A server creates the rules of a request and destroys them
  * after it. */
 int aha_b200_rules_check(const aha_logit_rules* r, size_t vocab);
@@ -630,6 +665,13 @@ int aha_b200_bench_kernel(aha_model* m, const char* which, int iters, double* av
  * impl 0 = score_head_kernel, 1 = the gemm_tc + row-kernel twin (a [M][V] logits block, then the generation path's stage-1 kernel) */
 int aha_b200_debug_score_head(aha_model* m, int impl, const float* hidden, size_t M, const uint32_t* targets, uint32_t n_top,
                               aha_logprobs* out);
+/* the page copies of batch_suspend / batch_resume on host data (tests): a pool of n_pool_pages pages per layer, pool_in / pool_out
+ * [layers][n_pool_pages][page_floats], and a pinned arena of n_host_pages host pages, each [layers][page_floats], filled with NaN.  Logical
+ * page p (0 .. n-1) goes out, every layer, from pool page table_out[p] to host page host_pages[p] (host_out: the arena afterwards,
+ * [n_host_pages][layers][page_floats]), then comes back from that host page into pool page table_in[p] (pool_out: the pool afterwards). */
+int aha_b200_debug_kv_swap(aha_model* m, size_t layers, size_t page_floats, size_t n_pool_pages, size_t n_host_pages, size_t n,
+                           const int32_t* table_out, const int32_t* table_in, const int32_t* host_pages, const float* pool_in, float* host_out,
+                           float* pool_out);
 /* the verify attention of speculative decoding on host data (tests): `rows` query rows at positions pos0 .. pos0 + rows - 1 over K / V of
  * pos0 + rows positions (laid out on a paged pool with the pages in reverse order), head_dim 128.  q, out: [rows][n_heads][128] (q
  * normalised and rotated); k, v: [pos0 + rows][n_kv_heads][128].  Row r attends to positions 0 .. pos0 + r.

@@ -348,6 +348,26 @@ public:
         check(aha_b200_batch_prefix_stats(h_, &st, hits ? hits->data() : nullptr, hits ? width : 0));
         return st;
     }
+    // Cancel, suspend and resume requests of the open session (aha_b200_batch_swap_space / _cancel / _suspend / _resume / _discard):
+    // batch_suspend returns the suspended request's id, batch_resume the slot it went back into.
+    void batch_swap_space(size_t max_tokens) { check(aha_b200_batch_swap_space(h_, max_tokens)); }
+    void batch_cancel(int32_t slot) { check(aha_b200_batch_cancel(h_, slot)); }
+    uint32_t batch_suspend(int32_t slot) {
+        uint32_t id = 0;
+        check(aha_b200_batch_suspend(h_, slot, &id));
+        return id;
+    }
+    int32_t batch_resume(uint32_t id) {
+        int32_t slot = -1;
+        check(aha_b200_batch_resume(h_, id, &slot));
+        return slot;
+    }
+    void batch_discard(uint32_t id) { check(aha_b200_batch_discard(h_, id)); }
+    aha_swap_stats batch_swap_stats() const {
+        aha_swap_stats st{};
+        check(aha_b200_batch_swap_stats(h_, &st));
+        return st;
+    }
     // Prefill continuation (aha_b200_forward_extend): further prompt tokens against the `off` tokens already in the cache.
     std::vector<float> forward_extend(const std::vector<uint32_t>& ids, size_t off) {
         std::vector<float> logits(need_vocab());
