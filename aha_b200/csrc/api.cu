@@ -3336,7 +3336,7 @@ int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, 
                         const float* resid, float* out, int iters, double* device_ms) {
     return guarded(m, [&] {
         AHA_REQUIRE(x && w && out && M > 0 && N > 0 && K > 0, "x, w, out and positive sizes are required");
-        AHA_REQUIRE((impl >= 1 && impl <= 3) || (impl >= 5 && impl <= 7), "impl must be 1 (SIMT), 2 / 3 (wgmma 128 x 128 / 128 x 256), 5 / 6 (batched GEMV) or 7 (wide batched GEMV)");
+        AHA_REQUIRE(impl >= 1 && impl <= 7, "impl must be 1 (SIMT), 2 / 3 (wgmma 128 x 128 / 128 x 256), 4 (batch-1 GEMV), 5 / 6 (batched GEMV) or 7 (wide batched GEMV)");
         Ctx& c = m->ctx;
         const int Nout = epi == EPI_SWIGLU ? N / 2 : N;
         Scratch mem;
@@ -3381,6 +3381,21 @@ int aha_b200_debug_gemm(aha_model* m, int impl, int epi, int act, int M, int N, 
                 if (ones) rmsnorm_split_kernel<<<M, 256, 0, c.stream>>>(dx, ones, 1e-6f, hi, lo, K);
                 else split_f32_to_f16x2_kernel<<<(unsigned)(((size_t)M * K / 4 + 255) / 256), 256, 0, c.stream>>>(dx, K, hi, lo, M, K);
                 gemv_wide(c.stream, gepi, tm, hi, lo, a, c.num_sms);
+            };
+            run();
+            ms = timed_ms(m, n, [&](size_t) { run(); });
+        } else if (impl == 4) {   // the batch-1 decode GEMV (gemv.cuh), once per activation row; epilogues and SwiGLU prologue as impl 5
+            AHA_REQUIRE(epi == EPI_STORE || epi == EPI_RESID || epi == EPI_SWIGLU, "batch-1 GEMV: epilogue store / residual / SwiGLU");
+            const int gepi = epi == EPI_STORE ? GEPI_STORE : (epi == EPI_RESID ? GEPI_RESID : GEPI_SWIGLU);
+            const int pro = epi == EPI_SWIGLU ? PRO_RMSNORM : PRO_NONE;
+            const float* ones = pro == PRO_RMSNORM ? unit_gain() : nullptr;
+            auto run = [&] {
+                for (int r = 0; r < M; ++r) {
+                    GemvArgs a{};
+                    a.W = dw; a.x = dx + (size_t)r * K; a.norm_w = ones; a.eps = ones ? 1e-6f : 0.f; a.bias = db;
+                    a.resid = dr ? dr + (size_t)r * N : nullptr; a.out = dy + (size_t)r * Nout; a.N = N; a.K = K;
+                    gemv(c.stream, pro, gepi, a);
+                }
             };
             run();
             ms = timed_ms(m, n, [&](size_t) { run(); });

@@ -785,24 +785,14 @@ struct Consumer {
 #pragma unroll
             for (int q = 0; q < kFusedMaxRows; ++q) v[q] = 0.f;
             if (!(a.dbg & 2)) {
-                if (nr == R) {
-                    switch (R) {
-                        case 8: stage_dots<8, 1>(st, K, v); break;
-                        case 4: stage_dots<4, 2>(st, K, v); break;
-                        case 2: stage_dots<2, 2>(st, K, v); break;
-                        default: stage_dots<1, 4>(st, K, v); break;
-                    }
-                } else {   // tail stage of the slab: row by row
-                    for (int q = 0; q < nr; ++q) {
-                        float t[kFusedMaxRows];
-                        // a qkv row takes the accumulators of a full stage (NA 1 at R 8, else 2): its sum must not depend on where
-                        // the shares of its kv group end
-                        if (EPI == FE_QKV && R == 8) stage_dots<1, 1>(st + (size_t)q * K * 2, K, t);
-                        else if (EPI == FE_QKV) stage_dots<1, 2>(st + (size_t)q * K * 2, K, t);
-                        else stage_dots<1, 4>(st + (size_t)q * K * 2, K, t);
-#pragma unroll
-                        for (int z = 0; z < kFusedMaxRows; ++z) if (z == q) v[z] = t[0];
-                    }
+                // the tail stage of a slab (nr < R rows) runs as a full one, its rows past nr read from the slot and never stored: a
+                // row's sum must not depend on where its slab ends -- for a qkv row, where the shares of its kv group end; for equal
+                // lm_head rows, whether their logits tie exactly, as the first-maximal-index argmax needs
+                switch (R) {
+                    case 8: stage_dots<8, 1>(st, K, v); break;
+                    case 4: stage_dots<4, 2>(st, K, v); break;
+                    case 2: stage_dots<2, 2>(st, K, v); break;
+                    default: stage_dots<1, 4>(st, K, v); break;
                 }
             }
             release(i);   // every shared-memory read of the stage fed v[] above; __syncwarp orders the lanes

@@ -971,7 +971,9 @@ class B200Model:
         return ms.value, int(nb.value)
 
     def debug_gemm(self, x, w16, bias=None, resid=None, impl=2, epi=0, act=0, iters=0):
-        """y = epilogue(x @ w16.T + bias) through the library's GEMM (impl 1 = SIMT, 2 / 3 = wgmma 128x128 / 128x256 tiles). -> (y, ms)"""
+        """y = epilogue(x @ w16.T + bias) through the library's GEMM (impl 1 = SIMT, 2 / 3 = wgmma 128x128 / 128x256 tiles) or a decode
+        projection kernel (4 = the batch-1 GEMV once per row, 5 / 6 = the batched GEMV, registers / cp.async ring, M <= 8, 7 = the wide
+        batched GEMV, M <= 64; their SwiGLU epilogue runs behind a unit-gain RMSNorm prologue). -> (y, ms)"""
         x = np.ascontiguousarray(x, np.float32)
         w16 = np.ascontiguousarray(w16, np.float16)
         M, K = x.shape

@@ -716,7 +716,8 @@ int aha_b200_debug_decode_attn(aha_model* m, size_t batch, size_t n_heads, size_
                                const float* q_norm, const float* k_norm, float eps, float rope_theta, float* out, float* out_repeat,
                                float* pool_out);
 /* Run ONE Linear layer y = epilogue(x W^T + b) through the library's GEMM dispatch on host data (unit tests of the
- * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 5 = the batched decode GEMV (M <= 8; its SwiGLU
+ * wgmma and SIMT kernels against numpy): impl 1 = SIMT fp32, 2 / 3 = wgmma split-fp16 (128x128 / 128x256 tiles), 4 = the batch-1 decode GEMV
+ * (gemv.cuh) once per row, with the epilogues and SwiGLU prologue of impl 5, 5 = the batched decode GEMV (M <= 8; its SwiGLU
  * instantiation runs with a unit-gain RMSNorm prologue), 6 = the same with the cp.async weight ring, 7 = the wide batched decode GEMV
  * (wgmma, M <= 64, N and K multiples of 64; epilogues and SwiGLU prologue as impl 5); epi 0 = store, 1 = residual
  * add (resid [M,N]), 2 = activation (act: 1 silu, 2 gelu-erf, 3 gelu-tanh), 3 = SwiGLU on interleaved columns

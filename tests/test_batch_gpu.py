@@ -30,11 +30,16 @@ def q3():
     m.close()
 
 
+# N 4728 / 4736 and 9464 / 9472 sit on either side of gemv_pick_rpw's thresholds (N / 16 >= 296 -> 2 rows per warp, N / 32 >= 296 -> 4);
+# the last four are the Qwen3-VL-8B text projections: qkv, o_proj, gate/up, down (K = 12288 stages 48 KB in gemv_kernel, six 2048 passes here)
 @pytest.mark.parametrize("M", [1, 3, 4, 5, 8])
-@pytest.mark.parametrize("N,K", [(64, 256), (2048, 2048), (4096, 1024), (12288, 2048), (2048, 6144), (1000, 4112)])
+@pytest.mark.parametrize("N,K", [(64, 256), (2048, 2048), (4096, 1024), (12288, 2048), (2048, 6144), (1000, 4112),
+                                 (4728, 1024), (4736, 1024), (9464, 1024), (9472, 1024),
+                                 (6144, 4096), (4096, 4096), (24576, 4096), (4096, 12288)])
 def test_batched_gemv_matches_numpy_and_the_simt_gemm(q3, M, N, K):
     """gemv_batch_kernel (impl 5) on M <= 8 activation rows: store / residual / SwiGLU epilogues, K spanning one and several 2048-element
-    passes (and a ragged last pass), every rows-per-warp variant (N picks 1 / 2 / 4)."""
+    passes (and a ragged last pass), every rows-per-warp variant (N picks 1 / 2 / 4).  Every row of impl 5 and of its cp.async-ring twin
+    (impl 6) is bit-identical to the batch-1 gemv_kernel (impl 4) on that row alone: a batched step reproduces the per-op step."""
     cfg, w, m, o = q3
     rng = np.random.default_rng(N + K + M)
     x = rng.standard_normal((M, K)).astype(np.float32)
@@ -48,9 +53,12 @@ def test_batched_gemv_matches_numpy_and_the_simt_gemm(q3, M, N, K):
     assert np.abs(got - simt).max() <= 1e-4 * max(1.0, np.abs(ref).max())
     ring, _ = m.debug_gemm(x, W, bias=bias, impl=6, epi=0)        # weights through the cp.async ring: the same fmas in the same order
     assert np.array_equal(ring, got)
+    one, _ = m.debug_gemm(x, W, bias=bias, impl=4, epi=0)
+    assert np.array_equal(one, got)
     got, _ = m.debug_gemm(x, W, resid=resid, impl=5, epi=1)
     assert np.abs(got - (ref + resid)).max() <= 2e-4 * max(1.0, np.abs(ref).max())
     assert np.array_equal(m.debug_gemm(x, W, resid=resid, impl=6, epi=1)[0], got)
+    assert np.array_equal(m.debug_gemm(x, W, resid=resid, impl=4, epi=1)[0], got)
     if N % 2 == 0:   # SwiGLU on interleaved (gate, up) rows, behind a unit-gain RMSNorm prologue
         xn = x / np.sqrt((x.astype(np.float64) ** 2).mean(-1, keepdims=True) + 1e-6)
         r2 = xn @ W.astype(np.float64).T
@@ -60,6 +68,7 @@ def test_batched_gemv_matches_numpy_and_the_simt_gemm(q3, M, N, K):
         assert got.shape == (M, N // 2)
         assert np.abs(got - want).max() <= 2e-4 * max(1.0, np.abs(want).max())
         assert np.array_equal(m.debug_gemm(x, W, impl=6, epi=3)[0], got)
+        assert np.array_equal(m.debug_gemm(x, W, impl=4, epi=3)[0], got)
 
 
 def _requests(V, spec):

@@ -12,7 +12,9 @@ from conftest import TOL, make_model, make_oracle
 
 pytestmark = pytest.mark.gpu
 
-SHAPES = [(64, 256), (1024, 256), (2048, 2048), (4096, 1024), (2048, 6144), (12288, 2048)]
+# the last four are the Qwen3-VL-8B text projections (qkv, o_proj, gate/up, down: wide_plan splits K = 12288 nine ways)
+SHAPES = [(64, 256), (1024, 256), (2048, 2048), (4096, 1024), (2048, 6144), (12288, 2048), (6144, 4096), (4096, 4096), (24576, 4096),
+          (4096, 12288)]
 ROWS = [1, 2, 8, 9, 33, 64]
 
 
