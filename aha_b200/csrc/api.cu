@@ -178,20 +178,13 @@ struct aha_model {
     size_t last_prefix_hit = 0;         // tokens the last generate call did not have to prefill
     BatchDecoder batch;                 // several sequences decoded in lockstep (aha_b200_generate_batch); buffers allocated on first use
     BatchDecoder wide_batch;            // the tensor-core decoder of wide sessions (aha_b200_batch_open_wide); buffers allocated on first use
-    // Continuous batching (aha_b200_batch_open / _add / _step / _close): requests join and leave a running batch between steps
+    // Continuous batching (aha_b200_batch_open / _add / _step / _close): requests join and leave a running batch between steps.  Each slot's
+    // request state is the decoder's BatchSlot, its host bookkeeping BatchSlot::req.
     struct BatchSession {
         bool open = false;
         bool wide = false;              // opened by batch_open_wide: wide_batch runs it
         int width = kGemvBatchMax;      // slots of the session
-        bool used[kWideSeqs] = {};
-        size_t budget[kWideSeqs] = {}, produced[kWideSeqs] = {};
-        bool lp_valid[kWideSeqs] = {};  // the slot's record row holds the record of the last token its request delivered
-        size_t hit[kWideSeqs] = {};     // prompt tokens the slot's request took from the prefix cache
         PrefixIndex prefix;             // aha_b200_batch_prefix_cache; dropped with the session
-        // speculative requests (aha_b200_batch_add_speculative, wide sessions only)
-        bool spec[kWideSeqs] = {};      // the slot runs a speculative request
-        aha_spec_stats spec_stats[kWideSeqs] = {};   // its counters, kept after it finishes until the slot is taken again
-        int last_n[kWideSeqs] = {};     // tokens the slot's last speculative pass delivered (0: its last token came from admission or a plain step)
     } session;
     BatchDecoder& sess() { return session.wide ? wide_batch : batch; }   // the decoder of the open session (batch when none is open)
     SpecDecoder spec;                   // speculative requests (generate_speculative, batch_add_speculative) on wide_batch's buffers
@@ -241,9 +234,9 @@ struct aha_model {
         int mapped = 0;                 // pages its table held
         DecodeState st{};
         std::vector<uint32_t> hist;     // history [0, st.n_hist)
-        Sampler sampler;
-        int lp = 0;                     // BatchSlot::lp
-        size_t budget = 0, produced = 0, hit = 0;
+        Sampler sampler;                // BatchSlot::sampler, ::lp and ::req
+        int lp = 0;
+        SlotRequest req;
     };
     std::map<uint32_t, Suspended> suspended;   // by id (>= 1)
     uint32_t next_suspend_id = 1;
@@ -1325,7 +1318,6 @@ void prefix_share(aha_model* m, int slot, const std::vector<int>& pages, size_t 
 // after a successful admission: the request's full prompt pages enter the index, and the statistics count its lookup
 void prefix_admitted(aha_model* m, int slot, const uint32_t* ids, size_t seq_len, size_t hit) {
     PrefixIndex& X = m->session.prefix;
-    m->session.hit[slot] = hit;
     if (!X.on()) return;
     X.lookups += 1;
     X.hit_tokens += hit;
@@ -1335,54 +1327,148 @@ void prefix_admitted(aha_model* m, int slot, const uint32_t* ids, size_t seq_len
 // ---- continuous batching: the same slots and the same step, with requests joining and leaving between steps -------------------------
 // (new design; the reference's server holds ONE request behind a write lock, server/api.rs:117.)  A finished request's pages go back to the
 // free list at once, so a waiting request can take its place while the others keep decoding.
+aha_model::BatchSession& open_session(aha_model* m) {
+    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    return m->session;
+}
+SlotRequest& slot_req(aha_model* m, int slot) { return m->sess().slots[slot].req; }
+// a finished request leaves its slot (SlotRequest::release)
 void session_release(aha_model* m, int slot) {
     BatchSlot& sl = m->sess().slots[slot];
     m->text.pages.release(sl.table);
     sl.samp_active = false;
     sl.lp = 0;
-    m->session.used[slot] = false;
-    m->session.hit[slot] = 0;
-    m->session.spec[slot] = false;
+    sl.req.release();
     m->sess().composition_changed();
 }
+// a cancelled or suspended request, or one whose admission failed, leaves its slot (SlotRequest::clear)
+void session_clear(aha_model* m, int slot) {
+    session_release(m, slot);
+    slot_req(m, slot).clear();
+}
 // verify rows of the running requests: R for a speculative request, 1 for a plain one
-int session_rows(const aha_model* m) {
+int session_rows(aha_model* m) {
     int rows = 0;
-    for (int i = 0; i < m->session.width; ++i) if (m->session.used[i]) rows += m->session.spec[i] ? m->spec.slots[i].R : 1;
+    for (int i = 0; i < m->session.width; ++i) {
+        const SlotRequest& r = slot_req(m, i);
+        if (r.used) rows += r.spec ? r.R : 1;
+    }
     return rows;
 }
-bool session_has_spec(const aha_model* m) {
-    for (int i = 0; i < m->session.width; ++i) if (m->session.used[i] && m->session.spec[i]) return true;
+bool session_has_spec(aha_model* m) {
+    for (int i = 0; i < m->session.width; ++i) if (slot_req(m, i).used && slot_req(m, i).spec) return true;
     return false;
 }
-// Beside speculative requests a step's rows must fit the wide kernel's 64-row B tile: `rows` more must fit what runs.  Without speculative
-// requests the rows are the running slots, which the session width already bounds.
-void session_check_rows(const aha_model* m, int rows, const std::string& who) {
+// The n lowest free slots for an admission or a resume, after the slot checks: enough free slots (batch_add_n counts choices), and room for
+// `rows` more step rows.  Beside speculative requests a step's rows must fit the wide kernel's 64-row B tile; without them the rows are the
+// running slots, which the session width already bounds.
+std::vector<int> free_slots(aha_model* m, size_t n, int rows, const std::string& who, bool choices = false) {
+    const std::string width = std::to_string(m->session.width);
+    std::vector<int> slot;
+    for (int i = 0; i < m->session.width; ++i) if (!slot_req(m, i).used) slot.push_back(i);
+    AHA_REQUIRE(choices || !slot.empty(), who + "all " + width + " slots are decoding (step until one finishes)");
+    AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + (choices ? " choices" : " requests") + ", but only " + std::to_string(slot.size()) +
+                                      " of the " + width + " slots are free (step until requests finish)");
+    slot.resize(n);
     const int now = session_rows(m);
     AHA_REQUIRE(now + rows <= kWideSeqs, who + "the step rows of the running requests (" + std::to_string(now) + ", a speculative request counts "
-                                                "max_draft + 1) plus " + std::to_string(rows) + " exceed " + std::to_string(kWideSeqs));
+                                              "max_draft + 1) plus " + std::to_string(rows) + " exceed " + std::to_string(kWideSeqs));
+    return slot;
 }
-// the bookkeeping of a request admitted into slot s with its first token: true (and the slot released) when that token is also its last
-bool session_admitted(aha_model* m, int s, size_t sample_len, int lp_n, uint32_t flags, uint32_t tok) {
-    m->session.budget[s] = sample_len;
-    m->session.produced[s] = 1;
-    m->session.lp_valid[s] = lp_n >= 0;
-    m->session.spec_stats[s] = aha_spec_stats{};
-    m->session.last_n[s] = 0;
-    bool stop = sample_len == 1;
-    if ((flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok) stop = true;
-    if (stop) session_release(m, s);
-    return stop;
+void require_ctx(const aha_model* m, size_t ctx, const std::string& what) {
+    AHA_REQUIRE(ctx <= (size_t)m->text.max_ctx, what + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(m->text.max_ctx));
 }
-struct AdmitGuard {   // a failed admission leaves the session as it was: every slot the call took is released with its pages
-    aha_model* m; const std::vector<int>& slots;
-    bool ok = false;
-    ~AdmitGuard() {
-        if (ok) return;
-        for (int s : slots) { session_release(m, s); m->session.lp_valid[s] = false; }
+// What admission needs of one request, from the checks every admission path runs on it before any device work
+struct AdmitReq {
+    const aha_batch_request* r;
+    int lp_n;                       // logprob_request
+    size_t budget;                  // token_budget
+    size_t ctx;                     // the positions its pages hold: prompt + budget (+ max_draft)
+    bool has_mm;                    // (a qwen3 handle ignores the tensors)
+    std::vector<int> hit_pages;     // prefix_hit: the cached pages its table starts with
+    size_t hit() const { return hit_pages.size() * kPage; }
+    // fresh pages for n copies of it (the first one shares the hit pages)
+    size_t pages(size_t n = 1) const { return n * ((ctx + kPage - 1) / kPage) - hit_pages.size(); }
+};
+// i: the request's index in a batch_add_many call, -1 for the call's only request; extra: positions beyond prompt + budget
+AdmitReq admit_check(aha_model* m, const aha_batch_request& r, const std::string& who, int i, size_t extra = 0) {
+    const TextModel& T = m->text;
+    const std::string at = i < 0 ? who : who + "request " + std::to_string(i) + ": ";
+    AHA_REQUIRE(r.ids && r.seq_len >= 1, who + (i < 0 ? "the request" : "request " + std::to_string(i)) + " needs input_ids");
+    AdmitReq a{&r};
+    a.lp_n = logprob_request(r.params, T, at);
+    for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
+    AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
+    request_rules(m, r.params, at);
+    require_mm_arity(m, r.mm);
+    a.budget = token_budget(r.params);
+    a.ctx = r.seq_len + a.budget + extra;
+    for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) a.has_mm = a.has_mm || mm_entry(r.mm, k) != nullptr;
+    a.hit_pages = prefix_hit(m, r.ids, r.seq_len, a.has_mm);
+    return a;
+}
+// One admission call: its slots (request k into slots[k]; every choice of batch_add_n is a[0]'s) and its checked requests.  Once it has
+// taken the slots and until it commits, its destructor leaves the session as it was: every slot it took is cleared with its pages.
+struct Admission {
+    aha_model* m;
+    std::vector<int> slots;
+    std::vector<AdmitReq> a;
+    bool taken = false, ok = false;
+    ~Admission() {
+        if (!taken || ok) return;
+        for (int s : slots) session_clear(m, s);
         m->have_rope_delta = false; m->rope_delta = 0; m->text.clear_sampler();
     }
+    std::set<int> keep() const {   // pages the requests hit: never evicted by this call
+        std::set<int> k;
+        for (const AdmitReq& q : a) k.insert(q.hit_pages.begin(), q.hit_pages.end());
+        return k;
+    }
+    void check_room(size_t pages, const std::string& what) const { prefix_check_room(m, pages, keep(), what); }
+    // after every check: evicts cached prefixes as far as `pages` fresh pages need, takes the slots and starts each request's table with
+    // its hit pages
+    void take(size_t pages) {
+        prefix_make_room(m, pages, keep());
+        taken = true;
+        for (int s : slots) slot_req(m, s).used = true;
+        for (size_t k = 0; k < a.size(); ++k) prefix_share(m, slots[k], a[k].hit_pages, a[k].r->seq_len);
+    }
+    // Slot k has its first token tok[k]: the requests' prompt pages enter the prefix index, each slot's record starts (a slot whose first
+    // token is also its last is released), and the outputs of slot k are filled.
+    void commit(const std::vector<uint32_t>& tok, const std::vector<double>& secs, const std::vector<double>& vision, int32_t* slots_out,
+                uint32_t* first_tokens, int32_t* finished, aha_usage* usage) {
+        ok = true;
+        for (size_t k = 0; k < a.size(); ++k) if (!a[k].has_mm) prefix_admitted(m, slots[k], a[k].r->ids, a[k].r->seq_len, a[k].hit());
+        m->text.clear_sampler();
+        m->sess().composition_changed();
+        for (size_t k = 0; k < slots.size(); ++k) {
+            const AdmitReq& q = a[std::min(k, a.size() - 1)];
+            SlotRequest& r = slot_req(m, slots[k]);
+            r = SlotRequest{};
+            r.used = true; r.budget = q.budget; r.produced = 1; r.hit = k < a.size() ? q.hit() : 0; r.lp_valid = q.lp_n >= 0;
+            bool stop = q.budget == 1;
+            if ((q.r->params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[k]) stop = true;
+            if (stop) session_release(m, slots[k]);
+            if (usage) {
+                usage[k] = aha_usage{};
+                add_usage(&usage[k], q.r->seq_len, 1, secs[k], 0.0, vision[k]);
+            }
+            slots_out[k] = slots[k]; first_tokens[k] = tok[k]; finished[k] = stop ? 1 : 0;
+        }
+    }
 };
+// the first tokens just drawn into the session decoder's d_tok and their decode states (draw counts, automaton states), read back once,
+// then the sampler check
+void read_first_tokens(aha_model* m, std::vector<uint32_t>& tok, std::vector<DecodeState>& st) {
+    BatchDecoder& B = m->sess();
+    Ctx& c = m->ctx;
+    tok.resize((size_t)B.cap);
+    st.resize((size_t)B.cap);
+    AHA_CUDA_CHECK(cudaMemcpyAsync(tok.data(), B.d_tok, tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaMemcpyAsync(st.data(), B.d_states, st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
+    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    m->text.check_sample_error();
+}
 // width 0: the narrow session (8 slots, batched CUDA-core GEMV); 1..64: a wide session (gemv_wide.cuh)
 void session_open(aha_model* m, int width) {
     TextModel& T = m->text;
@@ -1409,22 +1495,20 @@ void session_open(aha_model* m, int width) {
 }
 // ---- ending and swapping requests between steps (aha_b200_batch_cancel / _suspend / _resume / _discard).  Every check runs before anything
 // is copied or written (suspend first reads the slot's DecodeState), so a refused call changes nothing.
-void session_check_slot(const aha_model* m, int32_t slot, const std::string& who) {
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+void session_check_slot(aha_model* m, int32_t slot, const std::string& who) {
+    open_session(m);
     AHA_REQUIRE(slot >= 0 && slot < m->session.width, who + "slot " + std::to_string(slot) + " is outside the session's " +
                                                           std::to_string(m->session.width) + " slots");
-    AHA_REQUIRE(m->session.used[slot], who + "slot " + std::to_string(slot) + " runs no request");
+    AHA_REQUIRE(slot_req(m, slot).used, who + "slot " + std::to_string(slot) + " runs no request");
 }
 // the request in `slot` ends as if it had finished: its pages go back at once (the prefix index keeps its references) and the slot shows
 // no record; a speculative slot keeps its counters until the slot is taken again
 void session_cancel(aha_model* m, int32_t slot) {
     session_check_slot(m, slot, "batch_cancel: ");
-    session_release(m, slot);
-    m->session.lp_valid[slot] = false;
-    m->session.last_n[slot] = 0;
+    session_clear(m, slot);
 }
 aha_model::Suspended& suspended_of(aha_model* m, uint32_t id, const std::string& who) {
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    open_session(m);
     const auto it = m->suspended.find(id);
     AHA_REQUIRE(it != m->suspended.end(), who + "no suspended request of this session has id " + std::to_string(id));
     return it->second;
@@ -1435,8 +1519,8 @@ aha_model::Suspended& suspended_of(aha_model* m, uint32_t id, const std::string&
 uint32_t session_suspend(aha_model* m, int32_t slot) {
     const std::string who = "batch_suspend: ";
     session_check_slot(m, slot, who);
-    AHA_REQUIRE(!m->session.spec[slot], who + "slot " + std::to_string(slot) + " runs a speculative request, which cannot be suspended "
-                                                "(aha_b200_batch_cancel ends it)");
+    AHA_REQUIRE(!slot_req(m, slot).spec, who + "slot " + std::to_string(slot) + " runs a speculative request, which cannot be suspended "
+                                               "(aha_b200_batch_cancel ends it)");
     aha_model::SwapArena& A = m->swap;
     AHA_REQUIRE(A.pages > 0, who + "the handle has no swap space (aha_b200_batch_swap_space)");
     AHA_REQUIRE(m->next_suspend_id != 0, who + "the handle has used every suspended-request id");
@@ -1462,12 +1546,10 @@ uint32_t session_suspend(aha_model* m, int32_t slot) {
     r.mapped = sl.table.mapped;
     r.sampler = sl.sampler;
     r.lp = sl.lp;
-    r.budget = m->session.budget[slot]; r.produced = m->session.produced[slot]; r.hit = m->session.hit[slot];
+    r.req = sl.req;
     const uint32_t id = m->next_suspend_id++;
     m->suspended.emplace(id, std::move(r));
-    session_release(m, slot);
-    m->session.lp_valid[slot] = false;
-    m->session.last_n[slot] = 0;
+    session_clear(m, slot);
     A.pages_out += (uint64_t)pages;
     A.suspend_secs += seconds(clk::now() - t0);
     return id;
@@ -1478,10 +1560,7 @@ uint32_t session_suspend(aha_model* m, int32_t slot) {
 int32_t session_resume(aha_model* m, uint32_t id) {
     const std::string who = "batch_resume: ";
     aha_model::Suspended& r = suspended_of(m, id, who);
-    int slot = -1;
-    for (int i = 0; i < m->session.width && slot < 0; ++i) if (!m->session.used[i]) slot = i;
-    AHA_REQUIRE(slot >= 0, who + "all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
-    if (session_has_spec(m)) session_check_rows(m, 1, who);
+    const int slot = free_slots(m, 1, 1, who)[0];
     prefix_check_room(m, (size_t)r.mapped, {}, who + "the request needs ");
     prefix_make_room(m, (size_t)r.mapped, {});
     TextModel& T = m->text;
@@ -1492,7 +1571,8 @@ int32_t session_resume(aha_model* m, uint32_t id) {
     const auto t0 = clk::now();
     const int pages = (int)r.host_pages.size();
     T.pages.map(sl.table, std::min(r.mapped * kPage, T.max_ctx));
-    m->session.used[slot] = true;
+    sl.req = r.req;              // budget, produced and hit; a suspended request ran plain steps only, so its spec state is clear
+    sl.req.lp_valid = false;     // the record of its last token was read before it was suspended
     kv_swap(c, false, T.kv_pool, T.layer_stride, T.page_stride, T.cfg.L, sl.table.h.data(), r.host_pages.data(), A.host, pages);
     AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + slot, &r.st, sizeof(DecodeState), cudaMemcpyHostToDevice, c.stream));
     AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_hist + (size_t)slot * T.hist_cap, r.hist.data(), r.hist.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c.stream));
@@ -1500,11 +1580,6 @@ int32_t session_resume(aha_model* m, uint32_t id) {
     sl.lp = r.lp;
     B.bind_sampler(slot, r.sampler);
     AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    m->session.budget[slot] = r.budget; m->session.produced[slot] = r.produced; m->session.hit[slot] = r.hit;
-    m->session.lp_valid[slot] = false;
-    m->session.spec[slot] = false;
-    m->session.spec_stats[slot] = aha_spec_stats{};
-    m->session.last_n[slot] = 0;
     B.composition_changed();
     A.free.insert(A.free.end(), r.host_pages.begin(), r.host_pages.end());
     A.pages_in += (uint64_t)pages;
@@ -1552,52 +1627,22 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     Ctx& c = m->ctx;
     const std::string who = pack ? "batch_add_many: " : "batch_add: ";
     // ---- every check before any device work: a refused call leaves the session untouched
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    open_session(m);
     AHA_REQUIRE(n >= 1, who + "no requests");
-    std::vector<int> slot;   // request i takes the i-th lowest free slot
-    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) slot.push_back(i);
-    const std::string width = std::to_string(m->session.width);
-    AHA_REQUIRE(!slot.empty(), who + "all " + width + " slots are decoding (step until one finishes)");
-    AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " requests, but only " + std::to_string(slot.size()) + " of the " + width +
-                                      " slots are free (step until requests finish)");
-    slot.resize(n);
-    if (session_has_spec(m)) session_check_rows(m, (int)n, who);
-    std::vector<size_t> sample_len(n), hit(n);
-    std::vector<bool> packed(n), text_only(n);
-    std::vector<int> lp_n(n);
-    std::vector<std::vector<int>> hit_pages(n);
-    std::set<int> keep;   // pages this call hits: never evicted by it
+    Admission ad{m, free_slots(m, n, (int)n, who)};   // request i takes the i-th lowest free slot
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
-        const aha_batch_request& r = reqs[i];
-        AHA_REQUIRE(r.ids && r.seq_len >= 1, who + "request " + std::to_string(i) + " needs input_ids");
-        lp_n[i] = logprob_request(r.params, T, who + "request " + std::to_string(i) + ": ");
-        for (size_t k = 0; k < r.seq_len; ++k) AHA_REQUIRE(r.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
-        AHA_REQUIRE((r.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-        request_rules(m, r.params, who + "request " + std::to_string(i) + ": ");
-        require_mm_arity(m, r.mm);
-        sample_len[i] = token_budget(r.params);
-        bool has_mm = false;   // (a qwen3 handle ignores the tensors)
-        for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) has_mm = has_mm || mm_entry(r.mm, k) != nullptr;
-        text_only[i] = !has_mm;
-        hit_pages[i] = prefix_hit(m, r.ids, r.seq_len, has_mm);
-        hit[i] = hit_pages[i].size() * kPage;
-        keep.insert(hit_pages[i].begin(), hit_pages[i].end());
-        pages += (r.seq_len + sample_len[i] + kPage - 1) / kPage - hit_pages[i].size();
-        packed[i] = pack && !has_mm && r.seq_len <= (size_t)T.max_prefill;
+        ad.a.push_back(admit_check(m, reqs[i], who, (int)i));
+        pages += ad.a[i].pages();
     }
-    prefix_check_room(m, pages, keep, who + "the requests need ");
-    for (size_t i = 0; i < n; ++i) {   // (only reachable when max_ctx is not a multiple of the page)
-        const size_t ctx = reqs[i].seq_len + sample_len[i];
-        AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
-    }
-    prefix_make_room(m, pages, keep);
+    ad.check_room(pages, who + "the requests need ");
+    for (const AdmitReq& q : ad.a) require_ctx(m, q.ctx, "context of ");   // (only reachable when max_ctx is not a multiple of the page)
+    ad.take(pages);
     const auto t0 = clk::now();
-    AdmitGuard guard{m, slot};
-    for (int s : slot) m->session.used[s] = true;
-    for (size_t i = 0; i < n; ++i) prefix_share(m, slot[i], hit_pages[i], reqs[i].seq_len);
+    const std::vector<int>& slot = ad.slots;
     std::vector<uint32_t> tok(n);
     std::vector<double> secs(n), vision(n, 0.0);
+    std::vector<bool> packed(n);
     // ---- packed requests: map every page each can touch (as batch_prefill_slot does after its prefill), then prefill them pack by pack
     // With prefix hits a request's pack segment is the part of its prompt the cache does not hold: ids[hit, seq_len) at positions hit ..
     std::vector<size_t> pk, pk_pre;
@@ -1605,10 +1650,12 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     std::vector<size_t> pk_lens;
     bool any_hit = false;
     for (size_t i = 0; i < n; ++i) {
+        const size_t hit = ad.a[i].hit();
+        packed[i] = pack && !ad.a[i].has_mm && reqs[i].seq_len <= (size_t)T.max_prefill;
         if (!packed[i]) continue;
-        pk.push_back(i); pk_ids.push_back(reqs[i].ids + hit[i]); pk_lens.push_back(reqs[i].seq_len - hit[i]); pk_pre.push_back(hit[i]);
-        any_hit = any_hit || hit[i] > 0;
-        T.pages.map(B.slots[slot[i]].table, (int)(reqs[i].seq_len + sample_len[i]));
+        pk.push_back(i); pk_ids.push_back(reqs[i].ids + hit); pk_lens.push_back(reqs[i].seq_len - hit); pk_pre.push_back(hit);
+        any_hit = any_hit || hit > 0;
+        T.pages.map(B.slots[slot[i]].table, (int)ad.a[i].ctx);
     }
     if (!any_hit) pk_pre.clear();
     if (!pk.empty()) {
@@ -1653,18 +1700,15 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
             const Sampler samp = request_sampler(m, reqs[i].params, who);
             B.bind_sampler(slot[i], samp);
             empty[slot[i]].fsm_state = samp.fsm_start;
-            B.slots[slot[i]].lp = lp_n[i] + 1;
-            if (lp_n[i] >= 0) B.ensure_lp();
+            B.slots[slot[i]].lp = ad.a[i].lp_n + 1;
+            if (ad.a[i].lp_n >= 0) B.ensure_lp();
             act.push_back(slot[i]);
         }
         for (int s : act) AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, &empty[s], sizeof(DecodeState), cudaMemcpyHostToDevice, c.stream));
         B.head_rows(act, true);
-        std::vector<uint32_t> h_tok((size_t)B.cap);
-        std::vector<DecodeState> h_st((size_t)B.cap);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-        T.check_sample_error();
+        std::vector<uint32_t> h_tok;
+        std::vector<DecodeState> h_st;
+        read_first_tokens(m, h_tok, h_st);
         const double t_first = seconds(clk::now() - t0);
         for (size_t i : pk) {   // (their pages were mapped before the prefill)
             B.adopt(slot[i], h_tok[slot[i]], (int)reqs[i].seq_len, 0, h_st[slot[i]].n_draws, h_st[slot[i]].fsm_state);
@@ -1675,22 +1719,11 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     // ---- the others: one prefill each, on the slot's own table
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
-        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], sample_len[i], lp_n[i], hit[i]);
+        tok[i] = batch_prefill_slot(m, slot[i], reqs[i], ad.a[i].budget, ad.a[i].lp_n, ad.a[i].hit());
         secs[i] = seconds(clk::now() - t0);
         vision[i] = m->last_vision_secs;
     }
-    guard.ok = true;
-    for (size_t i = 0; i < n; ++i) if (text_only[i]) prefix_admitted(m, slot[i], reqs[i].ids, reqs[i].seq_len, hit[i]);
-    T.clear_sampler();
-    B.composition_changed();
-    for (size_t i = 0; i < n; ++i) {
-        const bool stop = session_admitted(m, slot[i], sample_len[i], lp_n[i], reqs[i].params.flags, tok[i]);
-        if (usage) {
-            usage[i] = aha_usage{};
-            add_usage(&usage[i], reqs[i].seq_len, 1, secs[i], 0.0, vision[i]);
-        }
-        slots_out[i] = slot[i]; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
-    }
+    ad.commit(tok, secs, vision, slots_out, first_tokens, finished, usage);
 }
 
 // OpenAI `n` (aha_b200_batch_add_n): n choices of one request in the n lowest free slots.  The prompt is prefilled once, into choice 0's
@@ -1707,45 +1740,28 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
     Ctx& c = m->ctx;
     const std::string who = "batch_add_n: ";
     // ---- every check before any device work: a refused call leaves the session untouched
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    open_session(m);
     AHA_REQUIRE(n >= 1, who + "n must be at least 1");
-    std::vector<int> slot;
-    for (int i = 0; i < m->session.width; ++i) if (!m->session.used[i]) slot.push_back(i);
-    AHA_REQUIRE(n <= slot.size(), who + std::to_string(n) + " choices, but only " + std::to_string(slot.size()) + " of the " +
-                                      std::to_string(m->session.width) + " slots are free (step until requests finish)");
-    slot.resize(n);
-    if (session_has_spec(m)) session_check_rows(m, (int)n, who);
-    AHA_REQUIRE(req.ids && req.seq_len >= 1, who + "the request needs input_ids");
-    const int lp_n = logprob_request(req.params, T, who);
-    for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
-    AHA_REQUIRE((req.params.flags & (AHA_GEN_CONTINUE_RNG | AHA_GEN_REUSE_PREFIX)) == 0, who + "CONTINUE_RNG / REUSE_PREFIX are per-handle states of the single-request calls");
-    request_rules(m, req.params, who);
-    require_mm_arity(m, req.mm);
-    const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len;
-    AHA_REQUIRE(ctx <= (size_t)T.max_ctx, "context of " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
-    bool has_mm = false;
-    for (size_t k = 0; m->kind != aha_model::QWEN3 && k < req.mm->n; ++k) has_mm = has_mm || mm_entry(req.mm, k) != nullptr;
-    const std::vector<int> hit_pages = prefix_hit(m, req.ids, req.seq_len, has_mm);   // choice 0's table starts with them
-    const size_t hit = hit_pages.size() * kPage;
-    const size_t pages = n * (size_t)ceil_div((int)ctx, kPage) - hit_pages.size();
-    const std::set<int> keep(hit_pages.begin(), hit_pages.end());
-    prefix_check_room(m, pages, keep, who + std::to_string(n) + " choices need ");
+    Admission ad{m, free_slots(m, n, (int)n, who, true)};
+    ad.a.push_back(admit_check(m, req, who, -1));
+    const AdmitReq& q = ad.a[0];   // choice 0's table starts with its hit pages
+    require_ctx(m, q.ctx, "context of ");
+    const size_t pages = q.pages(n);
+    ad.check_room(pages, who + std::to_string(n) + " choices need ");
     std::vector<aha_batch_request> r(n, req);
     std::vector<Sampler> samp(n);
     for (size_t i = 0; i < n; ++i) {
         r[i].params.seed = seeds ? seeds[i] : req.params.seed + i;
         samp[i] = request_sampler(m, r[i].params, who);
     }
-    prefix_make_room(m, pages, keep);
+    ad.take(pages);
     const auto t0 = clk::now();
-    AdmitGuard guard{m, slot};
-    for (int s : slot) m->session.used[s] = true;
+    const std::vector<int>& slot = ad.slots;
     std::vector<uint32_t> tok(n);
-    prefix_share(m, slot[0], hit_pages, req.seq_len);
-    tok[0] = batch_prefill_slot(m, slot[0], r[0], sample_len, lp_n, hit);
+    tok[0] = batch_prefill_slot(m, slot[0], r[0], q.budget, q.lp_n, q.hit());
     if (n > 1) {
         const std::vector<int> dst(slot.begin() + 1, slot.end());
-        for (int s : dst) T.pages.map(B.slots[s].table, (int)ctx);
+        for (int s : dst) T.pages.map(B.slots[s].table, (int)q.ctx);
         B.fork(slot[0], dst, (int)req.seq_len);
         const DecodeState empty{0, 0, 0, 0, 0, samp[0].fsm_start, {0, 0}};   // first_token's state: empty history, draw index 0, start state
         for (size_t i = 1; i < n; ++i) {
@@ -1754,219 +1770,206 @@ void session_add_n(aha_model* m, const aha_batch_request& req, size_t n, const u
             AHA_CUDA_CHECK(cudaMemcpyAsync(T.d_state, &empty, sizeof(empty), cudaMemcpyHostToDevice, c.stream));
             T.finish_argmax(0);
             T.sample(0);
-            if (lp_n >= 0) T.logprobs(true, B.d_lp_rec + s, false);
+            if (q.lp_n >= 0) T.logprobs(true, B.d_lp_rec + s, false);
             // the draw's token and draw count, collected in the slot's own rows and read back once below
             AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_tok + s, T.d_argmax, sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
             AHA_CUDA_CHECK(cudaMemcpyAsync(B.d_states + s, T.d_state, sizeof(DecodeState), cudaMemcpyDeviceToDevice, c.stream));
-            B.slots[s].lp = lp_n + 1;
+            B.slots[s].lp = q.lp_n + 1;
             B.bind_sampler(s, samp[i]);
         }
-        std::vector<uint32_t> h_tok((size_t)B.cap);
-        std::vector<DecodeState> h_st((size_t)B.cap);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-        T.check_sample_error();
+        std::vector<uint32_t> h_tok;
+        std::vector<DecodeState> h_st;
+        read_first_tokens(m, h_tok, h_st);
         for (size_t i = 1; i < n; ++i) {
             tok[i] = h_tok[slot[i]];
             B.adopt(slot[i], tok[i], (int)req.seq_len, decode_rope_delta(m), h_st[slot[i]].n_draws, h_st[slot[i]].fsm_state);
         }
     }
     const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
-    guard.ok = true;
-    if (!has_mm) prefix_admitted(m, slot[0], req.ids, req.seq_len, hit);
-    T.clear_sampler();
-    B.composition_changed();
-    for (size_t i = 0; i < n; ++i) {
-        const bool stop = session_admitted(m, slot[i], sample_len, lp_n, req.params.flags, tok[i]);
-        if (usage) {
-            usage[i] = aha_usage{};
-            add_usage(&usage[i], req.seq_len, 1, secs, 0.0, vision);
-        }
-        slots_out[i] = slot[i]; first_tokens[i] = tok[i]; finished[i] = stop ? 1 : 0;
-    }
+    ad.commit(tok, std::vector<double>(n, secs), std::vector<double>(n, vision), slots_out, first_tokens, finished, usage);
 }
-size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8);
 
 // One speculative request into the lowest free slot of the open wide session (aha_b200_batch_add_speculative): admitted as batch_add admits it
 // (prefilled alone on the slot's table, prefix-cache hit and insert included), with pages for max_draft more positions, and from then on
-// stepped in verify passes of R = max_draft + 1 rows by session_step_spec.  Its control block is the slot's; drafts come from the slot's
+// stepped in verify passes of R = max_draft + 1 rows by session_step_core.  Its control block is the slot's; drafts come from the slot's
 // copy of the prediction and prompt.
 void session_add_spec(aha_model* m, const aha_batch_request& req, const aha_spec_params& sp, int32_t* slot_out, uint32_t* first_token,
                       int32_t* finished, aha_usage* usage) {
     TextModel& T = m->text;
     const std::string who = "batch_add_speculative: ";
     // ---- every check before any device work: a refused call leaves the session untouched
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+    open_session(m);
     AHA_REQUIRE(m->session.wide, who + "speculative requests need a wide session (aha_b200_batch_open_wide): a narrow session promises the ids of "
                                        "single-request runs, which verify passes cannot keep");
     const int ngram = spec_request_check(m, req.params, sp, who);
-    int slot = -1;
-    for (int i = 0; i < m->session.width && slot < 0; ++i) if (!m->session.used[i]) slot = i;
-    AHA_REQUIRE(slot >= 0, who + "all " + std::to_string(m->session.width) + " slots are decoding (step until one finishes)");
     const int R = (int)sp.max_draft + 1;
-    session_check_rows(m, R, who);
-    AHA_REQUIRE(req.ids && req.seq_len >= 1, who + "the request needs input_ids");
-    const int lp_n = logprob_request(req.params, T, who);
-    for (size_t k = 0; k < req.seq_len; ++k) AHA_REQUIRE(req.ids[k] < (uint32_t)T.cfg.V, "token id out of range");
-    require_mm_arity(m, req.mm);
-    const size_t sample_len = token_budget(req.params), ctx = req.seq_len + sample_len + sp.max_draft;
-    AHA_REQUIRE(ctx <= (size_t)T.max_ctx, who + "prompt + max_tokens + max_draft = " + std::to_string(ctx) + " tokens exceeds max_ctx " + std::to_string(T.max_ctx));
-    bool has_mm = false;
-    for (size_t k = 0; m->kind != aha_model::QWEN3 && k < req.mm->n; ++k) has_mm = has_mm || mm_entry(req.mm, k) != nullptr;
-    const std::vector<int> hit_pages = prefix_hit(m, req.ids, req.seq_len, has_mm);
-    const size_t hit = hit_pages.size() * kPage;
-    const size_t pages = (size_t)ceil_div((int)ctx, kPage) - hit_pages.size();
-    const std::set<int> keep(hit_pages.begin(), hit_pages.end());
-    prefix_check_room(m, pages, keep, who + "the request needs ");
+    Admission ad{m, free_slots(m, 1, R, who)};
+    ad.a.push_back(admit_check(m, req, who, -1, sp.max_draft));   // (spec_request_check refused its flags and rules already)
+    const AdmitReq& q = ad.a[0];
+    require_ctx(m, q.ctx, who + "prompt + max_tokens + max_draft = ");
+    ad.check_room(q.pages(), who + "the request needs ");
     const Sampler samp = request_sampler(m, req.params, who);
     SpecDecoder& S = m->spec;
     BatchDecoder& B = m->sess();
-    prefix_make_room(m, pages, keep);
+    ad.take(q.pages());
     const auto t0 = clk::now();
-    const std::vector<int> slots{slot};
-    AdmitGuard guard{m, slots};
-    m->session.used[slot] = true;
-    prefix_share(m, slot, hit_pages, req.seq_len);
+    const int slot = ad.slots[0];
     S.init(T, B, kWideSeqs);
-    const uint32_t tok = batch_prefill_slot(m, slot, req, sample_len, lp_n, hit);
-    T.pages.map(B.slots[slot].table, (int)ctx);   // the positions of the last pass's drafts
-    if (sample_len > 1) {
+    const uint32_t tok = batch_prefill_slot(m, slot, req, q.budget, q.lp_n, q.hit());
+    T.pages.map(B.slots[slot].table, (int)q.ctx);   // the positions of the last pass's drafts
+    if (q.budget > 1) {
         const std::vector<uint32_t> pred(sp.prediction, sp.prediction + sp.n_prediction);
         const bool lookup = (sp.flags & AHA_SPEC_PROMPT_LOOKUP) != 0;
-        const int lp_on = lp_n >= 0 ? lp_n + 1 : 0;
-        S.set_ctl(slot, samp, pred, req.ids, lookup ? req.seq_len : 0, m->stop_ids, (int)sample_len, ngram, lp_on, B.d_states + slot,
+        const int lp_on = q.lp_n >= 0 ? q.lp_n + 1 : 0;
+        S.set_ctl(slot, samp, pred, req.ids, lookup ? req.seq_len : 0, m->stop_ids, (int)q.budget, ngram, lp_on, B.d_states + slot,
                   B.d_hist + (size_t)slot * T.hist_cap, S.d_slot_lp + (size_t)slot * kSpecMaxRows, 0, lp_on ? B.d_lp_rec + slot : nullptr);
-        S.slots[slot].R = R; S.slots[slot].samp = samp; S.slots[slot].lp = lp_on;
     }
     const double secs = seconds(clk::now() - t0), vision = m->last_vision_secs;
-    guard.ok = true;
-    if (!has_mm) prefix_admitted(m, slot, req.ids, req.seq_len, hit);
-    T.clear_sampler();
-    B.composition_changed();
-    const bool stop = session_admitted(m, slot, sample_len, lp_n, req.params.flags, tok);
-    m->session.spec[slot] = !stop;
-    if (usage) {
-        *usage = aha_usage{};
-        add_usage(usage, req.seq_len, 1, secs, 0.0, vision);
-    }
-    *slot_out = slot; *first_token = tok; *finished = stop ? 1 : 0;
+    ad.commit({tok}, {secs}, {vision}, slot_out, first_token, finished, usage);
+    if (!*finished) { slot_req(m, slot).spec = true; slot_req(m, slot).R = R; }
 }
 
-// One step of every running request (aha_b200_batch_step_spec): without a speculative request exactly session_step, else one mixed launch --
-// a decode step of the plain slots and a verify pass of every speculative slot.  tokens_out [cap][kSpecMaxRows], n_tokens / status [cap].
-size_t session_step_spec(aha_model* m, uint32_t* tokens_out, uint32_t* n_tokens, int32_t* status_out, size_t cap) {
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
-    const int width = m->session.width;
-    AHA_REQUIRE(cap >= (size_t)width, "batch_step_spec: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-    for (size_t i = 0; i < cap * kSpecMaxRows; ++i) tokens_out[i] = 0;
-    for (size_t i = 0; i < cap; ++i) n_tokens[i] = 0;
-    if (!session_has_spec(m)) {
-        std::vector<uint32_t> tok(cap);
-        const size_t n = session_step(m, tok.data(), status_out, cap, false);
-        for (size_t i = 0; i < cap; ++i) if (status_out[i]) { tokens_out[i * kSpecMaxRows] = tok[i]; n_tokens[i] = 1; }
-        return n;
-    }
-    for (size_t i = 0; i < cap; ++i) status_out[i] = 0;
-    std::vector<int> plain, spec;
-    for (int i = 0; i < width; ++i) if (m->session.used[i]) (m->session.spec[i] ? spec : plain).push_back(i);
+// One step of every running request, the core of batch_step, batch_step_n and batch_step_spec: a decode step of the plain slots
+// (BatchDecoder::step) or, beside a speculative request, one mixed launch (SpecDecoder::step) -- a decode step of the plain slots and a
+// verify pass of every speculative slot.  Slot s delivers its tokens into tokens[s * stride ..] (stride kSpecMaxRows once a speculative
+// request runs) and their count into n_tokens[s] when given; status[s] = 1 running, 2 finished.  The caller zeroes the outputs.  Finished
+// slots are released.  -> the requests stepped
+size_t session_step_core(aha_model* m, uint32_t* tokens, size_t stride, uint32_t* n_tokens, int32_t* status) {
     BatchDecoder& B = m->sess();
-    SpecDecoder& S = m->spec;
     Ctx& c = m->ctx;
-    S.step(plain, spec);
+    std::vector<int> plain, spec;
+    for (int i = 0; i < m->session.width; ++i) if (slot_req(m, i).used) (slot_req(m, i).spec ? spec : plain).push_back(i);
+    if (plain.empty() && spec.empty()) return 0;
+    if (spec.empty()) B.step(plain);
+    else m->spec.step(plain, spec);
     std::vector<uint32_t> h_tok((size_t)B.cap);
-    std::vector<DecodeState> h_st((size_t)B.cap);
-    std::vector<SpecCtl> h_ctl((size_t)kWideSeqs);
+    std::vector<DecodeState> h_st(spec.empty() ? 0 : (size_t)B.cap);
+    std::vector<SpecCtl> h_ctl(spec.empty() ? 0 : (size_t)kWideSeqs);
     AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, c.stream));
-    AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
-    AHA_CUDA_CHECK(cudaMemcpyAsync(h_ctl.data(), S.d_ctl, h_ctl.size() * sizeof(SpecCtl), cudaMemcpyDeviceToHost, c.stream));
-    AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
-    for (int s : spec) {   // the tokens the pass emitted: history [produced, n_hist)
-        const size_t E0 = m->session.produced[s], n = (size_t)h_st[s].n_hist - E0;
-        AHA_REQUIRE(n >= 1 && n <= (size_t)kSpecMaxRows, "batch_step_spec: a verify pass emitted no token");
-        AHA_CUDA_CHECK(cudaMemcpyAsync(tokens_out + (size_t)s * kSpecMaxRows, B.d_hist + (size_t)s * m->text.hist_cap + E0, n * sizeof(uint32_t),
-                                       cudaMemcpyDeviceToHost, c.stream));
+    if (!spec.empty()) {
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_st.data(), B.d_states, h_st.size() * sizeof(DecodeState), cudaMemcpyDeviceToHost, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(h_ctl.data(), m->spec.d_ctl, h_ctl.size() * sizeof(SpecCtl), cudaMemcpyDeviceToHost, c.stream));
     }
     AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    if (!spec.empty()) {
+        for (int s : spec) {   // the tokens the pass emitted: history [produced, n_hist)
+            const size_t E0 = slot_req(m, s).produced, n = (size_t)h_st[s].n_hist - E0;
+            AHA_REQUIRE(n >= 1 && n <= (size_t)kSpecMaxRows, "batch_step_spec: a verify pass emitted no token");
+            AHA_CUDA_CHECK(cudaMemcpyAsync(tokens + (size_t)s * stride, B.d_hist + (size_t)s * m->text.hist_cap + E0, n * sizeof(uint32_t),
+                                           cudaMemcpyDeviceToHost, c.stream));
+        }
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));
+    }
+    // a request whose sampler failed (all-zero weights) poisons only the check below; the session is closed by the caller's error path
     for (int s : plain) {
+        SlotRequest& r = slot_req(m, s);
         const uint32_t t = h_tok[s];
-        tokens_out[(size_t)s * kSpecMaxRows] = t;
-        n_tokens[s] = 1;
-        m->session.produced[s] += 1;
-        m->session.lp_valid[s] = B.slots[s].lp > 0;
-        bool stop = m->session.produced[s] >= m->session.budget[s];
+        tokens[(size_t)s * stride] = t;
+        if (n_tokens) n_tokens[s] = 1;
+        r.produced += 1;
+        r.lp_valid = B.slots[s].lp > 0;
+        r.last_n = 0;
+        bool stop = r.produced >= r.budget;
         for (uint32_t e : m->stop_ids) if (e == t) stop = true;     // an EOS token is delivered, then the request ends (generate.rs:139-141)
-        status_out[s] = stop ? 2 : 1;
+        status[s] = stop ? 2 : 1;
     }
     for (int s : spec) {
+        SlotRequest& r = slot_req(m, s);
         const SpecCtl& k = h_ctl[s];
-        const size_t n = (size_t)h_st[s].n_hist - m->session.produced[s];
+        const size_t n = (size_t)h_st[s].n_hist - r.produced;
         n_tokens[s] = (uint32_t)n;
-        m->session.produced[s] += n;
-        m->session.last_n[s] = (int)n;
-        m->session.lp_valid[s] = S.slots[s].lp > 0;
-        m->session.spec_stats[s] = aha_spec_stats{k.passes, k.drafted, k.accepted, 0};
-        status_out[s] = k.done ? 2 : 1;   // (the accept kernel applies EOS and max_tokens)
+        r.produced += n;
+        r.last_n = (int)n;
+        r.lp_valid = B.slots[s].lp > 0;
+        r.spec_stats = aha_spec_stats{k.passes, k.drafted, k.accepted, 0};
+        status[s] = k.done ? 2 : 1;   // (the accept kernel applies EOS and max_tokens)
     }
-    for (int s : plain) m->session.last_n[s] = 0;
-    for (int i = 0; i < width; ++i) if (status_out[i] == 2) session_release(m, i);
+    for (int i = 0; i < m->session.width; ++i) if (status[i] == 2) session_release(m, i);
+    // sampler errors surface after the bookkeeping so that the slots stay consistent
     m->text.check_sample_error();
     return plain.size() + spec.size();
 }
+// batch_step / batch_step_n: tokens_out / status_out: [cap] entries, cap >= the session width (8 for batch_step)
+size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8) {
+    const int width = open_session(m).width;
+    if (step8)
+        AHA_REQUIRE(width <= kGemvBatchMax, "batch_step: tokens_out[8] cannot hold a session of " + std::to_string(width) + " slots: use aha_b200_batch_step_n");
+    AHA_REQUIRE(cap >= (size_t)width, "batch_step_n: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+    for (size_t i = 0; i < cap; ++i) { status_out[i] = 0; tokens_out[i] = 0; }
+    AHA_REQUIRE(!session_has_spec(m), std::string(step8 ? "batch_step" : "batch_step_n") +
+                                          ": a speculative request is running: step the session with aha_b200_batch_step_spec");
+    return session_step_core(m, tokens_out, 1, nullptr, status_out);
+}
+// batch_step_spec: tokens_out [cap][kSpecMaxRows], n_tokens / status [cap]
+size_t session_step_spec(aha_model* m, uint32_t* tokens_out, uint32_t* n_tokens, int32_t* status_out, size_t cap) {
+    const int width = open_session(m).width;
+    AHA_REQUIRE(cap >= (size_t)width, "batch_step_spec: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
+    for (size_t i = 0; i < cap * kSpecMaxRows; ++i) tokens_out[i] = 0;
+    for (size_t i = 0; i < cap; ++i) { n_tokens[i] = 0; status_out[i] = 0; }
+    return session_step_core(m, tokens_out, kSpecMaxRows, n_tokens, status_out);
+}
 
-// per slot of the open session, the records of every token its request delivered last (out [width][kSpecMaxRows]; zero records elsewhere)
-std::vector<aha_logprobs> session_records_spec(aha_model* m) {
+// Per slot of the open session, `rows` records of the tokens its request delivered last (zero records elsewhere): rows 1 (batch_logprobs)
+// the record of its last token, rows kSpecMaxRows (batch_logprobs_spec) one per token its last speculative pass delivered.
+std::vector<aha_logprobs> session_records(aha_model* m, int rows) {
     const int width = m->session.width;
     BatchDecoder& B = m->sess();
-    std::vector<aha_logprobs> last((size_t)width), rows;
-    std::vector<aha_logprobs> out((size_t)width * kSpecMaxRows);
+    std::vector<aha_logprobs> last((size_t)width), pass, out((size_t)width * rows);
     if (B.d_lp_rec) AHA_CUDA_CHECK(cudaMemcpyAsync(last.data(), B.d_lp_rec, last.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
-    if (m->spec.d_slot_lp) {
-        rows.resize((size_t)width * kSpecMaxRows);
-        AHA_CUDA_CHECK(cudaMemcpyAsync(rows.data(), m->spec.d_slot_lp, rows.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
+    if (rows > 1 && m->spec.d_slot_lp) {
+        pass.resize((size_t)width * kSpecMaxRows);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(pass.data(), m->spec.d_slot_lp, pass.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
     }
     AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
     for (int i = 0; i < width; ++i) {
-        if (!m->session.lp_valid[i]) continue;
-        const int n = m->session.last_n[i];
-        if (n == 0) out[(size_t)i * kSpecMaxRows] = last[i];
-        else for (int k = 0; k < n; ++k) out[(size_t)i * kSpecMaxRows + k] = rows[(size_t)i * kSpecMaxRows + k];
+        const SlotRequest& r = slot_req(m, i);
+        if (!r.lp_valid) continue;
+        const int n = rows > 1 ? r.last_n : 0;
+        if (n == 0) out[(size_t)i * rows] = last[i];
+        else for (int k = 0; k < n; ++k) out[(size_t)i * rows + k] = pass[(size_t)i * kSpecMaxRows + k];
     }
     return out;
 }
 
-// tokens_out / status_out: [cap] entries, cap >= the session width (8 for batch_step)
-size_t session_step(aha_model* m, uint32_t* tokens_out, int32_t* status_out, size_t cap, bool step8) {
-    AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
-    const int width = m->session.width;
-    if (step8)
-        AHA_REQUIRE(width <= kGemvBatchMax, "batch_step: tokens_out[8] cannot hold a session of " + std::to_string(width) + " slots: use aha_b200_batch_step_n");
-    AHA_REQUIRE(cap >= (size_t)width, "batch_step_n: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-    std::vector<int> act;
-    for (size_t i = 0; i < cap; ++i) { status_out[i] = 0; tokens_out[i] = 0; }
-    AHA_REQUIRE(!session_has_spec(m), std::string(step8 ? "batch_step" : "batch_step_n") +
-                                          ": a speculative request is running: step the session with aha_b200_batch_step_spec");
-    for (int i = 0; i < width; ++i) if (m->session.used[i]) act.push_back(i);
-    if (act.empty()) return 0;
-    BatchDecoder& B = m->sess();
-    B.step(act);
-    std::vector<uint32_t> h_tok((size_t)B.cap);
-    AHA_CUDA_CHECK(cudaMemcpyAsync(h_tok.data(), B.d_tok, h_tok.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, m->ctx.stream));
-    AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-    // a request whose sampler failed (all-zero weights) poisons only the check below; the session is closed by the caller's error path
-    for (int slot : act) {
-        const uint32_t t = h_tok[slot];
-        tokens_out[slot] = t;
-        m->session.produced[slot] += 1;
-        m->session.lp_valid[slot] = B.slots[slot].lp > 0;
-        bool stop = m->session.produced[slot] >= m->session.budget[slot];
-        for (uint32_t e : m->stop_ids) if (e == t) stop = true;     // an EOS token is delivered, then the request ends (generate.rs:139-141)
-        status_out[slot] = stop ? 2 : 1;
+// A narrow session run to completion, the driver of generate_batch and generate_n: admit(slot, first, finished) admits the n requests (or
+// choices) into a fresh session, then it steps until every one has finished.  Request i's tokens go to out_tokens[i * cap ..] and, when
+// out_lp is given, their records to out_lp[i * cap ..]; its usage gets its completion time and token count.  Whatever happens, the handle
+// is left as after clear_cache().
+void narrow_session_run(aha_model* m, size_t n, uint32_t* out_tokens, aha_logprobs* out_lp, size_t cap, size_t* n_out, aha_usage* usage,
+                        const std::function<void(int32_t* slot, uint32_t* first, int32_t* finished)>& admit) {
+    session_open(m, 0);
+    struct Close {
+        aha_model* m;
+        ~Close() { session_close(m); }
+    } close{m};
+    std::vector<int32_t> slot(n), fin(n);
+    std::vector<uint32_t> first(n);
+    admit(slot.data(), first.data(), fin.data());
+    std::vector<aha_logprobs> rec;
+    auto take = [&](size_t i, int s, uint32_t t) {
+        out_tokens[i * cap + n_out[i]] = t;
+        if (out_lp) out_lp[i * cap + n_out[i]] = rec[s];
+        ++n_out[i];
+    };
+    if (out_lp) rec = session_records(m, 1);
+    std::vector<int> req_of(kGemvBatchMax, -1);   // slot -> request
+    for (size_t i = 0; i < n; ++i) {
+        take(i, slot[i], first[i]);
+        if (!fin[i]) req_of[slot[i]] = (int)i;
     }
-    for (int slot : act) if (status_out[slot] == 2) session_release(m, slot);
-    // sampler errors surface after the bookkeeping so that the slots stay consistent
-    m->text.check_sample_error();
-    return act.size();
+    const auto t_dec = clk::now();
+    uint32_t tok[kGemvBatchMax];
+    int32_t status[kGemvBatchMax];
+    while (session_step(m, tok, status, kGemvBatchMax, true) > 0) {
+        if (out_lp) rec = session_records(m, 1);
+        for (int s = 0; s < kGemvBatchMax; ++s) {
+            if (!status[s]) continue;
+            const int i = req_of[s];
+            take((size_t)i, s, tok[s]);
+            if (status[s] == 2 && usage) usage[i].completion_secs = seconds(clk::now() - t_dec);
+        }
+    }
+    if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
 }
 
 // Static batching: a narrow session that admits the n requests one by one (each prefilled alone on its own page table) and steps until all
@@ -1987,43 +1990,9 @@ void generate_batch_impl(aha_model* m, const aha_batch_request* reqs, size_t n, 
         n_out[i] = 0;
     }
     AHA_REQUIRE(pages <= (size_t)T.num_pages, "the requests of the batch need " + std::to_string(pages * kPage) + " tokens of KV capacity, max_ctx is " + std::to_string(T.max_ctx));
-    session_open(m, 0);
-    struct Close {   // whatever happens, the handle is left as after clear_cache()
-        aha_model* m;
-        ~Close() { session_close(m); }
-    } close{m};
-    std::vector<int> req_of(kGemvBatchMax, -1);   // slot -> request
-    for (size_t i = 0; i < n; ++i) {
-        int32_t slot = 0, fin = 0;
-        session_add_many(m, reqs + i, 1, &slot, out_tokens + i * cap, &fin, usage ? usage + i : nullptr, false);
-        n_out[i] = 1;
-        if (!fin) req_of[slot] = (int)i;
-    }
-    const auto t_dec = clk::now();
-    uint32_t tok[kGemvBatchMax];
-    int32_t status[kGemvBatchMax];
-    while (session_step(m, tok, status, kGemvBatchMax, true) > 0) {
-        for (int slot = 0; slot < kGemvBatchMax; ++slot) {
-            if (!status[slot]) continue;
-            const int i = req_of[slot];
-            out_tokens[(size_t)i * cap + n_out[i]++] = tok[slot];
-            if (status[slot] == 2 && usage) usage[i].completion_secs = seconds(clk::now() - t_dec);
-        }
-    }
-    if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
-}
-
-// per slot of the open session, the record of the last token its request delivered (a zero record where there is none)
-std::vector<aha_logprobs> session_records(aha_model* m) {
-    const int width = m->session.width;
-    BatchDecoder& B = m->sess();
-    std::vector<aha_logprobs> h((size_t)width);
-    if (B.d_lp_rec) {
-        AHA_CUDA_CHECK(cudaMemcpyAsync(h.data(), B.d_lp_rec, h.size() * sizeof(aha_logprobs), cudaMemcpyDeviceToHost, m->ctx.stream));
-        AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
-    }
-    for (int i = 0; i < width; ++i) if (!m->session.lp_valid[i]) h[i] = aha_logprobs{};
-    return h;
+    narrow_session_run(m, n, out_tokens, nullptr, cap, n_out, usage, [&](int32_t* slot, uint32_t* first, int32_t* fin) {
+        for (size_t i = 0; i < n; ++i) session_add_many(m, reqs + i, 1, slot + i, first + i, fin + i, usage ? usage + i : nullptr, false);
+    });
 }
 
 // n choices of one request (OpenAI `n`, 1..8): a narrow session, one batch_add_n, steps until every choice has finished.  Choice i yields
@@ -2038,40 +2007,10 @@ void generate_n_impl(aha_model* m, const uint32_t* ids, size_t seq_len, const ah
     const bool lp = logprob_request(params, T, who) >= 0;
     AHA_REQUIRE(!lp || out_lp, who + "AHA_GEN_LOGPROBS needs out_logprobs");
     for (size_t i = 0; i < n; ++i) n_out[i] = 0;
-    session_open(m, 0);
-    struct Close {   // whatever happens, the handle is left as after clear_cache()
-        aha_model* m;
-        ~Close() { session_close(m); }
-    } close{m};
     const aha_batch_request req{ids, seq_len, mm, params};
-    std::vector<int32_t> slot(n), fin(n);
-    std::vector<uint32_t> first(n);
-    session_add_n(m, req, n, seeds, slot.data(), first.data(), fin.data(), usage);
-    std::vector<int> choice_of(kGemvBatchMax, -1);   // slot -> choice
-    auto take = [&](int s, size_t i, uint32_t t, const std::vector<aha_logprobs>& rec) {
-        out_tokens[i * cap + n_out[i]] = t;
-        if (lp) out_lp[i * cap + n_out[i]] = rec[s];
-        ++n_out[i];
-    };
-    const std::vector<aha_logprobs> none;
-    std::vector<aha_logprobs> rec = lp ? session_records(m) : none;
-    for (size_t i = 0; i < n; ++i) {
-        take(slot[i], i, first[i], rec);
-        if (!fin[i]) choice_of[slot[i]] = (int)i;
-    }
-    const auto t_dec = clk::now();
-    uint32_t tok[kGemvBatchMax];
-    int32_t status[kGemvBatchMax];
-    while (session_step(m, tok, status, kGemvBatchMax, true) > 0) {
-        if (lp) rec = session_records(m);
-        for (int s = 0; s < kGemvBatchMax; ++s) {
-            if (!status[s]) continue;
-            const int i = choice_of[s];
-            take(s, (size_t)i, tok[s], rec);
-            if (status[s] == 2 && usage) usage[i].completion_secs = seconds(clk::now() - t_dec);
-        }
-    }
-    if (usage) for (size_t i = 0; i < n; ++i) usage[i].completion_tokens = (uint32_t)n_out[i];
+    narrow_session_run(m, n, out_tokens, lp ? out_lp : nullptr, cap, n_out, usage, [&](int32_t* slot, uint32_t* first, int32_t* fin) {
+        session_add_n(m, req, n, seeds, slot, first, fin, usage);
+    });
 }
 }  // namespace
 
@@ -2133,11 +2072,10 @@ int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out, int32_t* status_ou
 
 int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out, size_t cap) {
     return guarded(m, [&] {
-        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        const int width = open_session(m).width;
         AHA_REQUIRE(out, "batch_logprobs: out[cap] is required");
-        const int width = m->session.width;
         AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-        const std::vector<aha_logprobs> h = session_records(m);
+        const std::vector<aha_logprobs> h = session_records(m, 1);
         for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? h[i] : aha_logprobs{};
     });
 }
@@ -2160,29 +2098,26 @@ int aha_b200_batch_step_spec(aha_model* m, uint32_t* tokens_out, uint32_t* n_tok
 
 int aha_b200_batch_logprobs_spec(aha_model* m, aha_logprobs* out, size_t cap) {
     return guarded(m, [&] {
-        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        const int width = open_session(m).width;
         AHA_REQUIRE(out, "batch_logprobs_spec: out[cap][16] is required");
-        const int width = m->session.width;
         AHA_REQUIRE(cap >= (size_t)width, "batch_logprobs_spec: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-        const std::vector<aha_logprobs> h = session_records_spec(m);
+        const std::vector<aha_logprobs> h = session_records(m, kSpecMaxRows);
         for (size_t i = 0; i < cap * kSpecMaxRows; ++i) out[i] = i < h.size() ? h[i] : aha_logprobs{};
     });
 }
 
 int aha_b200_batch_spec_stats(aha_model* m, aha_spec_stats* out, size_t cap) {
     return guarded(m, [&] {
-        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        const int width = open_session(m).width;
         AHA_REQUIRE(out, "batch_spec_stats: out[cap] is required");
-        const int width = m->session.width;
         AHA_REQUIRE(cap >= (size_t)width, "batch_spec_stats: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
-        for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? m->session.spec_stats[i] : aha_spec_stats{};
+        for (size_t i = 0; i < cap; ++i) out[i] = i < (size_t)width ? slot_req(m, (int)i).spec_stats : aha_spec_stats{};
     });
 }
 
 int aha_b200_batch_prefix_cache(aha_model* m, size_t max_tokens) {
     return guarded(m, [&] {
-        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
-        PrefixIndex& X = m->session.prefix;
+        PrefixIndex& X = open_session(m).prefix;
         TextModel& T = m->text;
         X.max_pages = max_tokens / kPage;
         if (!X.on()) { X.clear(T.pages); return; }
@@ -2192,9 +2127,8 @@ int aha_b200_batch_prefix_cache(aha_model* m, size_t max_tokens) {
 
 int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hits_out, size_t cap) {
     return guarded(m, [&] {
-        AHA_REQUIRE(m->session.open, "no batch session is open (aha_b200_batch_open)");
+        const int width = open_session(m).width;
         AHA_REQUIRE(out, "batch_prefix_stats: out is required");
-        const int width = m->session.width;
         AHA_REQUIRE(!hits_out || cap >= (size_t)width, "batch_prefix_stats: cap " + std::to_string(cap) + " is smaller than the session width " + std::to_string(width));
         const PrefixIndex& X = m->session.prefix;
         *out = aha_prefix_stats{};
@@ -2202,7 +2136,7 @@ int aha_b200_batch_prefix_stats(aha_model* m, aha_prefix_stats* out, size_t* hit
         for (const auto& e : X.blocks) out->shared_pages += m->text.pages.refs[e.first] > 1;
         out->hit_tokens = X.hit_tokens; out->lookups = X.lookups; out->evicted_pages = X.evicted; out->max_pages = X.max_pages;
         out->free_pages = m->text.pages.free_count();
-        if (hits_out) for (size_t i = 0; i < cap; ++i) hits_out[i] = i < (size_t)width ? m->session.hit[i] : 0;
+        if (hits_out) for (size_t i = 0; i < cap; ++i) hits_out[i] = i < (size_t)width ? slot_req(m, (int)i).hit : 0;
     });
 }
 
@@ -2308,7 +2242,7 @@ int aha_b200_fsm_destroy(aha_model* m, uint32_t id) {
         const auto it = m->fsms.find(id);
         AHA_REQUIRE(it != m->fsms.end(), "fsm_destroy: no token automaton has id " + std::to_string(id) + " on this handle");
         for (int i = 0; m->session.open && i < m->session.width; ++i)
-            AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].fsm_id == id),
+            AHA_REQUIRE(!(slot_req(m, i).used && m->sess().slots[i].fsm_id == id),
                         "fsm_destroy: token automaton " + std::to_string(id) + " constrains the running request in slot " + std::to_string(i));
         for (const auto& e : m->suspended)
             AHA_REQUIRE(e.second.sampler.fsm_id != id,
@@ -2352,7 +2286,7 @@ int aha_b200_rules_destroy(aha_model* m, uint32_t id) {
         const auto it = m->rules.find(id);
         AHA_REQUIRE(it != m->rules.end(), "rules_destroy: no logit-rules object has id " + std::to_string(id) + " on this handle");
         for (int i = 0; m->session.open && i < m->session.width; ++i)
-            AHA_REQUIRE(!(m->session.used[i] && m->sess().slots[i].rules_id == id),
+            AHA_REQUIRE(!(slot_req(m, i).used && m->sess().slots[i].rules_id == id),
                         "rules_destroy: logit-rules object " + std::to_string(id) + " applies to the running request in slot " + std::to_string(i));
         for (const auto& e : m->suspended)
             AHA_REQUIRE(e.second.sampler.rules_id != id,

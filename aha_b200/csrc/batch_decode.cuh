@@ -34,6 +34,22 @@
 
 namespace aha {
 
+// The host state of the request a batch-session slot runs (api.cu's session layer keeps it; a speculative step reads R)
+struct SlotRequest {
+    bool used = false;                   // the slot runs a request
+    size_t budget = 0, produced = 0;     // its max_tokens and the tokens it has delivered
+    size_t hit = 0;                      // prompt tokens it took from the prefix cache
+    bool spec = false;                   // a speculative request, stepped in verify passes of R rows
+    int R = 1;
+    aha_spec_stats spec_stats{};         // its counters
+    bool lp_valid = false;               // the slot's record row holds the record of the last token its request delivered
+    int last_n = 0;                      // tokens its last speculative pass delivered (0: its last token came from admission or a plain step)
+    // a finished request: the slot is free, and its record, last_n and spec counters stay readable until the slot is taken again
+    void release() { used = false; hit = 0; spec = false; }
+    // a cancelled or suspended request, or a failed admission: as release, but the slot shows no record
+    void clear() { release(); lp_valid = false; last_n = 0; }
+};
+
 struct BatchSlot {                       // one sequence of the batch
     PageTable table;                     // its pages, which it holds from its prefill until it is released; device copy: row of BatchDecoder::d_tables
     bool samp_active = false;
@@ -42,6 +58,7 @@ struct BatchSlot {                       // one sequence of the batch
     uint32_t fsm_id = 0;                 // the token automaton the request is constrained by (0: none); it cannot be destroyed while the slot runs
     uint32_t rules_id = 0;               // the request's logit-rules object (0: none); it cannot be destroyed while the slot runs
     Sampler sampler;                     // the request's sampler as bound (a suspended request takes it along and is bound again at resume)
+    SlotRequest req;
 };
 
 struct BatchDecoder {
@@ -80,7 +97,7 @@ struct BatchDecoder {
     uint64_t epoch = 0;                  // counts composition changes (a speculative step rebuilds its own device copies on a new one)
     // no sequence holds a slot any more (a session opens or closes)
     void reset() {
-        for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; }
+        for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; sl.req = SlotRequest{}; }
         table_for.clear();
         lp_any = false;
         graphs.clear();

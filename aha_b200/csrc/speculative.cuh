@@ -397,9 +397,6 @@ struct SpecDecoder {
     int* d_vcnt = nullptr;                             // [kWideSeqs][V] count rows, allocated when a request first asks
     float* partial = nullptr; int max_chunks = 0, partial_rows = 0;
     uint32_t* d_buf[kWideSeqs] = {}; size_t buf_cap[kWideSeqs] = {};   // per control block: prediction | prompt | stop ids
-    // per session slot, what its verify rows are bound to when a composition is built
-    struct Slot { int R = 0; Sampler samp; int lp = 0; };
-    Slot slots[kWideSeqs];
     GraphCache<int> graphs;                            // single requests: keyed by R
     GraphCache<std::array<int, 4>> steps;              // session steps: keyed by (plain rows, requests, verify rows, records)
     std::vector<int> built_plain, built_spec;          // the composition the device copies were built for
@@ -481,8 +478,9 @@ struct SpecDecoder {
         AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // host temporaries
     }
     // the device copy of a composition: requests (slot = control block, page table, R) in order, their rows after each other, every
-    // verify row bound to its request's sampler (the request's history, the row's own state / token / scratch / count row) and record flag
-    void build(const std::vector<int>& ctl_of, const std::vector<const int*>& table_of, const std::vector<const Slot*>& of,
+    // verify row bound to its request's sampler (the request's history, the row's own state / token / scratch / count row) and record flag,
+    // which of[q] holds (R in of[q]->req)
+    void build(const std::vector<int>& ctl_of, const std::vector<const int*>& table_of, const std::vector<const BatchSlot*>& of,
                const std::vector<uint32_t*>& hist_of) {
         Ctx& c = *T->ctx;
         std::vector<SpecReq> reqs;
@@ -491,15 +489,15 @@ struct SpecDecoder {
         std::vector<SampleArgs> samp(kWideSeqs);
         int row = 0;
         for (size_t q = 0; q < ctl_of.size(); ++q) {
-            const Slot& s = *of[q];
-            reqs.push_back(SpecReq{d_ctl + ctl_of[q], table_of[q], row, s.R, 0});
-            for (int r = 0; r < s.R; ++r, ++row) {
+            const BatchSlot& s = *of[q];
+            reqs.push_back(SpecReq{d_ctl + ctl_of[q], table_of[q], row, s.req.R, 0});
+            for (int r = 0; r < s.req.R; ++r, ++row) {
                 row_table.push_back(table_of[q]);
-                on[row] = s.samp.active ? 1 : 0;
+                on[row] = s.sampler.active ? 1 : 0;
                 lp[row] = s.lp;
                 // the request's history holds the emitted tokens followed by the drafts, so row r's counts (frequency / presence, each row
                 // its own count row) cover the context a sequential decode would see at that draw
-                if (s.samp.active) samp[row] = T->bind_sampler(s.samp, d_vst + row, hist_of[q], d_vtok + row, d_vwork + (size_t)row * T->cfg.V, counts(s.samp, row));
+                if (s.sampler.active) samp[row] = T->bind_sampler(s.sampler, d_vst + row, hist_of[q], d_vtok + row, d_vwork + (size_t)row * T->cfg.V, counts(s.sampler, row));
             }
         }
         AHA_REQUIRE(row <= kWideSeqs, "speculative step: more than 64 verify rows");
@@ -515,7 +513,7 @@ struct SpecDecoder {
     void prepare(int R, const Sampler& samp, const std::vector<uint32_t>& pred, const uint32_t* prompt, size_t n_prompt,
                  const std::vector<uint32_t>& stop, int max_tokens, int ngram, int lp_on) {
         set_ctl(0, samp, pred, prompt, n_prompt, stop, max_tokens, ngram, lp_on, T->d_state, T->d_history, T->d_lp, 1, nullptr);
-        Slot s; s.R = R; s.samp = samp; s.lp = lp_on;
+        BatchSlot s; s.req.R = R; s.sampler = samp; s.lp = lp_on;
         build({0}, {T->table.d}, {&s}, {T->d_history});
         built_epoch = ~0ull;                  // a later session builds its own composition
         B->zero_rows_from(R);
@@ -530,9 +528,9 @@ struct SpecDecoder {
         if (B->epoch != built_epoch || plain != built_plain || spec != built_spec) {
             B->build_attn_table(plain);
             std::vector<const int*> tab;
-            std::vector<const Slot*> of;
+            std::vector<const BatchSlot*> of;
             std::vector<uint32_t*> hist;
-            for (int s : spec) { tab.push_back(B->slots[s].table.d); of.push_back(&slots[s]); hist.push_back(B->d_hist + (size_t)s * T->hist_cap); }
+            for (int s : spec) { tab.push_back(B->slots[s].table.d); of.push_back(&B->slots[s]); hist.push_back(B->d_hist + (size_t)s * T->hist_cap); }
             build(spec, tab, of, hist);
             built_plain = plain; built_spec = spec; built_epoch = B->epoch;
         }
@@ -540,7 +538,7 @@ struct SpecDecoder {
         int ns = 0;
         bool lp = false;
         for (int s : plain) lp = lp || B->slots[s].lp > 0;
-        for (int s : spec) { ns += slots[s].R; lp = lp || slots[s].lp > 0; }
+        for (int s : spec) { ns += B->slots[s].req.R; lp = lp || B->slots[s].lp > 0; }
         B->zero_rows_from(np + ns);
         if (!B->use_graph) { launches(np, nq, ns, lp); return; }
         steps.run(*T->ctx, {np, nq, ns, lp ? 1 : 0}, [&] { launches(np, nq, ns, lp); });
