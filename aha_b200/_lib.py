@@ -280,6 +280,10 @@ SYMBOLS = {
     "aha_b200_fsm_check": (C.c_int, [C.POINTER(TokenFsm), C.c_size_t]),
     "aha_b200_fsm_create": (C.c_int, [_P, C.POINTER(TokenFsm), _U32P]),
     "aha_b200_fsm_destroy": (C.c_int, [_P, C.c_uint32]),
+    "aha_b200_lora_create": (C.c_int, [_P, C.POINTER(TensorDesc), C.c_size_t, C.c_float, _U32P]),
+    "aha_b200_lora_destroy": (C.c_int, [_P, C.c_uint32]),
+    "aha_b200_batch_add_lora": (C.c_int, [_P, C.POINTER(BatchRequest), _U32P, C.c_size_t, C.POINTER(C.c_int32), _U32P, C.POINTER(C.c_int32),
+                                          C.POINTER(Usage)]),
     "aha_b200_mel_spectrogram": (C.c_int, [_P, _F32P, C.c_size_t, _F32P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "aha_b200_image_patchify": (C.c_int, [_P, C.POINTER(C.c_uint8), C.c_size_t, C.c_size_t, _F32P, C.c_size_t, _U32P]),
     "aha_b200_img_smart_resize": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, _U32P, _U32P]),

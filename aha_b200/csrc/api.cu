@@ -44,11 +44,13 @@ int guarded_host(F&& f) {   // host-only entries (no handle)
 // A batch session's prefix cache (aha_b200_batch_prefix_cache): full 32-token pages of admitted prompts, keyed by their token ids and their
 // parent page, so that a later request whose prompt starts with the same pages maps them into its table instead of prefilling them.  Every
 // block holds one reference on its page (PagePool::refs); the blocks form a tree from the prompts' first pages.  A key's hash only narrows
-// the search: a match is confirmed on the 32 ids.
+// the search: a match is confirmed on the 32 ids.  A prompt's first page hangs below the root of the LoRA adapter its request ran
+// (root(0) = -1 for the base model), so a request only finds pages written under its own adapter.
 struct PrefixIndex {
+    static int root(uint32_t lora) { return -1 - (int)lora; }
     struct Block {
         uint32_t ids[kPage];
-        int parent = -1;     // page of the block before it in the prompt (-1: the prompt's first page)
+        int parent = -1;     // page of the block before it in the prompt (< 0: the prompt's first page, below root(its adapter))
         int children = 0;    // cached blocks whose parent this is
         uint64_t used = 0;   // LRU clock of the last admission that hit or inserted it
     };
@@ -71,10 +73,10 @@ struct PrefixIndex {
         }
         return -1;
     }
-    // the pages of the longest cached chain of full pages that starts ids[0, n)
-    std::vector<int> chain(const uint32_t* ids, size_t n) const {
+    // the pages of the longest cached chain of full pages that starts ids[0, n) under adapter `lora`
+    std::vector<int> chain(const uint32_t* ids, size_t n, uint32_t lora) const {
         std::vector<int> pages;
-        int parent = -1;
+        int parent = root(lora);
         for (size_t t = 0; t + kPage <= n; t += kPage) {
             const int p = find(parent, ids + t);
             if (p < 0) break;
@@ -111,11 +113,28 @@ struct PrefixIndex {
         blocks.erase(page);
         pool.unref(page);
     }
+    // every block cached under adapter `lora` (aha_b200_lora_destroy): one pass finds each block's root and depth (memoised along the
+    // chain), then the adapter's blocks are erased deepest first, so every block is a leaf when it goes
+    void drop(PagePool& pool, uint32_t lora) {
+        std::unordered_map<int, std::pair<int, int>> at;   // page -> (root, depth)
+        std::vector<int> chain;
+        for (const auto& e : blocks) {
+            int q = e.first;
+            chain.clear();
+            while (q >= 0 && !at.count(q)) { chain.push_back(q); q = blocks.at(q).parent; }
+            std::pair<int, int> rd = q >= 0 ? at.at(q) : std::make_pair(q, -1);
+            for (auto it = chain.rbegin(); it != chain.rend(); ++it) { rd.second += 1; at[*it] = rd; }
+        }
+        std::vector<std::pair<int, int>> mine;   // (depth, page)
+        for (const auto& e : at) if (e.second.first == root(lora)) mine.emplace_back(e.second.second, e.first);
+        std::sort(mine.rbegin(), mine.rend());
+        for (const auto& d : mine) erase(pool, d.second);
+    }
     // The full pages of an admitted prompt that the table `t` holds (its first hit / kPage of them are the cached chain it hit), in prompt
     // order.  Inserting beyond max_pages evicts LRU leaves first; the chain stops at the first page that cannot be inserted.
-    void insert(PagePool& pool, const uint32_t* ids, size_t n, const PageTable& t) {
+    void insert(PagePool& pool, const uint32_t* ids, size_t n, const PageTable& t, uint32_t lora) {
         ++clock;
-        int parent = -1;
+        int parent = root(lora);
         for (size_t b = 0; (b + 1) * kPage <= n; ++b) {
             const int page = t.h[b];
             const int have = find(parent, ids + b * kPage);
@@ -218,6 +237,7 @@ struct aha_model {
     };
     std::map<uint32_t, Rules> rules;
     uint32_t next_rules_id = 1;
+    uint32_t next_lora_id = 1;          // LoRA adapters (aha_b200_lora_create) live in text.lora
     // Swap preemption (aha_b200_batch_swap_space / _suspend / _resume): a pinned host arena of host pages, each holding one KV page of every
     // layer ([layer][page_stride] fp32), kept across sessions until it is resized or the handle is destroyed, and its free list -- a pool of
     // its own, apart from the device PagePool.  The counters run for the handle's lifetime.
@@ -1290,11 +1310,11 @@ uint32_t batch_prefill_slot(aha_model* m, int slot, const aha_batch_request& r, 
 // The hit rule of every admission path: the longest cached chain of full pages that starts the prompt, capped at seq_len - 1 tokens and,
 // unless every GEMM runs on the SIMT kernel, at seq_len - kPage, so that the rows still prefilled run on the wgmma GEMM as the cold prefill of
 // the same rows does (gemm_on_tc: M < 32 takes SIMT).  The pages it returns hold ids[0, kPage * size()).  Multimodal requests never hit.
-std::vector<int> prefix_hit(const aha_model* m, const uint32_t* ids, size_t seq_len, bool has_mm) {
+std::vector<int> prefix_hit(const aha_model* m, const uint32_t* ids, size_t seq_len, bool has_mm, uint32_t lora) {
     const PrefixIndex& X = m->session.prefix;
     if (!X.on() || has_mm) return {};
     const size_t cap = m->ctx.gemm_impl == 1 ? seq_len - 1 : (seq_len >= (size_t)kPage ? seq_len - kPage : 0);
-    return X.chain(ids, cap / kPage * kPage);
+    return X.chain(ids, cap / kPage * kPage, lora);
 }
 // Admission's page check: `pages` fresh pages must fit the free list plus the pages only the prefix cache holds, less those this call hits
 // (`keep`).  Once the call has passed every check, prefix_make_room evicts LRU leaves only as far as the call needs.
@@ -1316,12 +1336,12 @@ void prefix_share(aha_model* m, int slot, const std::vector<int>& pages, size_t 
     (void)seq_len;
 }
 // after a successful admission: the request's full prompt pages enter the index, and the statistics count its lookup
-void prefix_admitted(aha_model* m, int slot, const uint32_t* ids, size_t seq_len, size_t hit) {
+void prefix_admitted(aha_model* m, int slot, const uint32_t* ids, size_t seq_len, size_t hit, uint32_t lora) {
     PrefixIndex& X = m->session.prefix;
     if (!X.on()) return;
     X.lookups += 1;
     X.hit_tokens += hit;
-    X.insert(m->text.pages, ids, seq_len, m->sess().slots[slot].table);
+    X.insert(m->text.pages, ids, seq_len, m->sess().slots[slot].table, lora);
 }
 
 // ---- continuous batching: the same slots and the same step, with requests joining and leaving between steps -------------------------
@@ -1386,12 +1406,13 @@ struct AdmitReq {
     size_t ctx;                     // the positions its pages hold: prompt + budget (+ max_draft)
     bool has_mm;                    // (a qwen3 handle ignores the tensors)
     std::vector<int> hit_pages;     // prefix_hit: the cached pages its table starts with
+    uint32_t lora = 0;              // its LoRA adapter (0: the base model)
     size_t hit() const { return hit_pages.size() * kPage; }
     // fresh pages for n copies of it (the first one shares the hit pages)
     size_t pages(size_t n = 1) const { return n * ((ctx + kPage - 1) / kPage) - hit_pages.size(); }
 };
 // i: the request's index in a batch_add_many call, -1 for the call's only request; extra: positions beyond prompt + budget
-AdmitReq admit_check(aha_model* m, const aha_batch_request& r, const std::string& who, int i, size_t extra = 0) {
+AdmitReq admit_check(aha_model* m, const aha_batch_request& r, const std::string& who, int i, size_t extra = 0, uint32_t lora = 0) {
     const TextModel& T = m->text;
     const std::string at = i < 0 ? who : who + "request " + std::to_string(i) + ": ";
     AHA_REQUIRE(r.ids && r.seq_len >= 1, who + (i < 0 ? "the request" : "request " + std::to_string(i)) + " needs input_ids");
@@ -1404,7 +1425,8 @@ AdmitReq admit_check(aha_model* m, const aha_batch_request& r, const std::string
     a.budget = token_budget(r.params);
     a.ctx = r.seq_len + a.budget + extra;
     for (size_t k = 0; m->kind != aha_model::QWEN3 && k < r.mm->n; ++k) a.has_mm = a.has_mm || mm_entry(r.mm, k) != nullptr;
-    a.hit_pages = prefix_hit(m, r.ids, r.seq_len, a.has_mm);
+    a.lora = lora;
+    a.hit_pages = prefix_hit(m, r.ids, r.seq_len, a.has_mm, lora);
     return a;
 }
 // One admission call: its slots (request k into slots[k]; every choice of batch_add_n is a[0]'s) and its checked requests.  Once it has
@@ -1438,14 +1460,14 @@ struct Admission {
     void commit(const std::vector<uint32_t>& tok, const std::vector<double>& secs, const std::vector<double>& vision, int32_t* slots_out,
                 uint32_t* first_tokens, int32_t* finished, aha_usage* usage) {
         ok = true;
-        for (size_t k = 0; k < a.size(); ++k) if (!a[k].has_mm) prefix_admitted(m, slots[k], a[k].r->ids, a[k].r->seq_len, a[k].hit());
+        for (size_t k = 0; k < a.size(); ++k) if (!a[k].has_mm) prefix_admitted(m, slots[k], a[k].r->ids, a[k].r->seq_len, a[k].hit(), a[k].lora);
         m->text.clear_sampler();
         m->sess().composition_changed();
         for (size_t k = 0; k < slots.size(); ++k) {
             const AdmitReq& q = a[std::min(k, a.size() - 1)];
             SlotRequest& r = slot_req(m, slots[k]);
             r = SlotRequest{};
-            r.used = true; r.budget = q.budget; r.produced = 1; r.hit = k < a.size() ? q.hit() : 0; r.lp_valid = q.lp_n >= 0;
+            r.used = true; r.budget = q.budget; r.produced = 1; r.hit = k < a.size() ? q.hit() : 0; r.lp_valid = q.lp_n >= 0; r.lora = q.lora;
             bool stop = q.budget == 1;
             if ((q.r->params.flags & AHA_GEN_EOS_ON_FIRST) != 0) for (uint32_t e : m->stop_ids) if (e == tok[k]) stop = true;
             if (stop) session_release(m, slots[k]);
@@ -1560,6 +1582,9 @@ uint32_t session_suspend(aha_model* m, int32_t slot) {
 int32_t session_resume(aha_model* m, uint32_t id) {
     const std::string who = "batch_resume: ";
     aha_model::Suspended& r = suspended_of(m, id, who);
+    AHA_REQUIRE(!(r.req.lora && session_has_spec(m)), who + "suspended request " + std::to_string(id) + " runs LoRA adapter " +
+                                                          std::to_string(r.req.lora) + " and a speculative request is running: speculative "
+                                                          "requests and adapters do not share a session");
     const int slot = free_slots(m, 1, 1, who)[0];
     prefix_check_room(m, (size_t)r.mapped, {}, who + "the request needs ");
     prefix_make_room(m, (size_t)r.mapped, {});
@@ -1609,6 +1634,20 @@ void swap_space(aha_model* m, size_t max_tokens) {
     for (int p = 0; p < (int)pages; ++p) A.free.push_back(p);
 }
 
+// The LoRA adapters of the rows of the prefills run while it lives: ad[row] an adapter index (< 0: the base model).  Rows of the base model
+// alone set nothing, so such prefills run exactly as without adapters.
+struct LoraPrefill {
+    LoraSet& L;
+    LoraPrefill(aha_model* m, const std::vector<int>& ad) : L(m->text.lora) {
+        if (std::any_of(ad.begin(), ad.end(), [](int a) { return a >= 0; })) L.prefill_begin(m->ctx.stream, ad);
+    }
+    ~LoraPrefill() { L.prefill_end(); }
+};
+bool session_has_lora(aha_model* m) {
+    for (int i = 0; i < m->session.width; ++i) if (slot_req(m, i).used && slot_req(m, i).lora) return true;
+    return false;
+}
+
 // n requests admitted in one call (aha_b200_batch_add_many).  Text-only requests that fit max_prefill are cut, in input order, into packed
 // prefills (TextModel::prefill with PrefillSegments: each request attends only to itself and its positions restart at 0), so one pass over the
 // weights serves them all; their last rows then go through the step's batched lm_head and each request's own ArgMax / sampler.  A request
@@ -1621,18 +1660,19 @@ void swap_space(aha_model* m, size_t max_tokens) {
 // page at positions >= seq_len, which its decode steps overwrite before any step reads them.  A 32-token round-up never reaches a 64-token KV
 // tile or a 128-token query tile that the request's own rows do not already touch, so each request runs the attention tiles it runs alone.
 void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int32_t* slots_out, uint32_t* first_tokens, int32_t* finished,
-                      aha_usage* usage, bool pack) {
+                      aha_usage* usage, bool pack, const uint32_t* adapters = nullptr) {
     TextModel& T = m->text;
     BatchDecoder& B = m->sess();
     Ctx& c = m->ctx;
-    const std::string who = pack ? "batch_add_many: " : "batch_add: ";
+    const std::string who = adapters ? "batch_add_lora: " : (pack ? "batch_add_many: " : "batch_add: ");
+    auto lora_of = [&](size_t i) { return adapters ? adapters[i] : 0u; };
     // ---- every check before any device work: a refused call leaves the session untouched
     open_session(m);
     AHA_REQUIRE(n >= 1, who + "no requests");
     Admission ad{m, free_slots(m, n, (int)n, who)};   // request i takes the i-th lowest free slot
     size_t pages = 0;
     for (size_t i = 0; i < n; ++i) {
-        ad.a.push_back(admit_check(m, reqs[i], who, (int)i));
+        ad.a.push_back(admit_check(m, reqs[i], who, (int)i, 0, lora_of(i)));
         pages += ad.a[i].pages();
     }
     ad.check_room(pages, who + "the requests need ");
@@ -1688,7 +1728,15 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
                 p.sg.kv_rows = (int)p.KV;
             }
             upload_pack(m, p);
-            T.prefill(pt, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
+            std::vector<int> row_lora(p.S, -1);   // every row of a segment, its filler included, runs its request's adapter
+            for (size_t j = p.first; j < p.last; ++j) {
+                const auto& sg = p.sg.segs[j - p.first];
+                std::fill(row_lora.begin() + sg.first, row_lora.begin() + sg.first + sg.second, T.lora.index_of(lora_of(pk[j])));
+            }
+            {
+                LoraPrefill lp(m, row_lora);
+                T.prefill(pt, (int)p.S, 0, false, nullptr, 0, {}, p.sg);
+            }
             gather_rows_kernel<<<(unsigned)(p.last - p.first), 256, 0, c.stream>>>(m->d_pack_rows, T.x, B.xb + p.first * H, H);
             c.cnt.kernels++;
             first = p.last;
@@ -1719,6 +1767,7 @@ void session_add_many(aha_model* m, const aha_batch_request* reqs, size_t n, int
     // ---- the others: one prefill each, on the slot's own table
     for (size_t i = 0; i < n; ++i) {
         if (packed[i]) continue;
+        LoraPrefill lp(m, std::vector<int>(std::min((size_t)T.max_prefill, reqs[i].seq_len - ad.a[i].hit()), T.lora.index_of(lora_of(i))));
         tok[i] = batch_prefill_slot(m, slot[i], reqs[i], ad.a[i].budget, ad.a[i].lp_n, ad.a[i].hit());
         secs[i] = seconds(clk::now() - t0);
         vision[i] = m->last_vision_secs;
@@ -1802,6 +1851,7 @@ void session_add_spec(aha_model* m, const aha_batch_request& req, const aha_spec
     AHA_REQUIRE(m->session.wide, who + "speculative requests need a wide session (aha_b200_batch_open_wide): a narrow session promises the ids of "
                                        "single-request runs, which verify passes cannot keep");
     const int ngram = spec_request_check(m, req.params, sp, who);
+    AHA_REQUIRE(!session_has_lora(m), who + "a LoRA request is running: speculative requests and adapters do not share a session");
     const int R = (int)sp.max_draft + 1;
     Admission ad{m, free_slots(m, 1, R, who)};
     ad.a.push_back(admit_check(m, req, who, -1, sp.max_draft));   // (spec_request_check refused its flags and rules already)
@@ -2294,6 +2344,171 @@ int aha_b200_rules_destroy(aha_model* m, uint32_t id) {
         AHA_CUDA_CHECK(cudaStreamSynchronize(m->ctx.stream));
         if (it->second.mem) AHA_CUDA_CHECK(cudaFree(it->second.mem));
         m->rules.erase(it);
+    });
+}
+
+}  // extern "C"
+
+namespace {
+// One PEFT tensor name of the text stack: [base_model.model.]<prefix>layers.<l>.<self_attn.{q,k,v,o}_proj | mlp.{gate,up,down}_proj>.lora_{A,B}.weight
+struct LoraName { int layer = 0, group = 0, sub = 0; bool b = false; };
+bool parse_lora_name(const std::string& prefix, std::string n, LoraName& t) {
+    const std::string bm = "base_model.model.", lp = prefix + "layers.";
+    if (n.compare(0, bm.size(), bm) == 0) n = n.substr(bm.size());
+    if (n.compare(0, lp.size(), lp) != 0) return false;
+    size_t j = lp.size();
+    while (j < n.size() && j - lp.size() < 6 && n[j] >= '0' && n[j] <= '9') ++j;
+    if (j == lp.size() || j >= n.size() || n[j] != '.') return false;
+    t.layer = std::stoi(n.substr(lp.size(), j - lp.size()));
+    const std::string rest = n.substr(j + 1);
+    static const struct { const char* name; int g, sub; } kTargets[] = {
+        {"self_attn.q_proj", LORA_QKV, 0}, {"self_attn.k_proj", LORA_QKV, 1}, {"self_attn.v_proj", LORA_QKV, 2}, {"self_attn.o_proj", LORA_O, 0},
+        {"mlp.gate_proj", LORA_GU, 0}, {"mlp.up_proj", LORA_GU, 1}, {"mlp.down_proj", LORA_DOWN, 0}};
+    for (const auto& x : kTargets)
+        for (int b = 0; b < 2; ++b)
+            if (rest == std::string(x.name) + (b ? ".lora_B.weight" : ".lora_A.weight")) { t.group = x.g; t.sub = x.sub; t.b = b != 0; return true; }
+    return false;
+}
+
+// Checks every tensor of an adapter (names, pairs, ranks, shapes, dtypes, fp16 range) and stages it as fp16 blocks in the pool layout of
+// lora.cuh; nothing touches the device.
+LoraAdapter lora_stage(const aha_model* m, const aha_tensor_desc* tensors, size_t n, float scale) {
+    const TextModel& T = m->text;
+    const TextCfg& cf = T.cfg;
+    const std::string who = "lora_create: ";
+    AHA_REQUIRE(T.tp_world == 1, who + "LoRA adapters are single-GPU (tp_world > 1 is not supported)");
+    AHA_REQUIRE(std::isfinite(scale), who + "scale must be finite");
+    AHA_REQUIRE(tensors && n >= 2, who + "an adapter needs at least one lora_A / lora_B pair");
+    // (layer, group, sub) -> A, B
+    std::map<std::array<int, 3>, std::array<const aha_tensor_desc*, 2>> pairs;
+    int r = 0;
+    for (size_t i = 0; i < n; ++i) {
+        const aha_tensor_desc& d = tensors[i];
+        const std::string name = d.name ? d.name : "";
+        LoraName t;
+        AHA_REQUIRE(parse_lora_name(T.wprefix, name, t), who + "tensor '" + name + "' is not a lora_A / lora_B weight of a q/k/v/o/gate/up/down "
+                                                                  "projection of the text stack (DoRA and other PEFT methods are not supported)");
+        AHA_REQUIRE(t.layer < cf.L, who + "tensor '" + name + "': the model has " + std::to_string(cf.L) + " layers");
+        AHA_REQUIRE(d.dtype == AHA_F16 || d.dtype == AHA_BF16 || d.dtype == AHA_F32, who + "tensor '" + name + "' must be f16, bf16 or f32");
+        AHA_REQUIRE(d.data && d.rank == 2, who + "tensor '" + name + "' must be a 2-D matrix");
+        auto& slot = pairs[{t.layer, t.group, t.sub}][t.b ? 1 : 0];
+        AHA_REQUIRE(!slot, who + "tensor '" + name + "' appears twice");
+        slot = &d;
+        const int rank = (int)(t.b ? d.shape[1] : d.shape[0]);
+        AHA_REQUIRE(r == 0 || rank == r, who + "tensor '" + name + "' has rank " + std::to_string(rank) + ", the adapter's other tensors " + std::to_string(r));
+        r = rank;
+    }
+    AHA_REQUIRE(r >= 1 && r <= kLoraMaxRank, who + "rank " + std::to_string(r) + " is outside 1 .. " + std::to_string(kLoraMaxRank));
+    const int H = cf.H, q = T.nh_l * cf.hd, kv = T.nkv_l * cf.hd;
+    auto dims = [&](int g, int sub, int& N, int& K) {   // the base projection of a target: out N, in K
+        switch (g) {
+            case LORA_QKV: N = sub == 0 ? q : kv; K = H; break;
+            case LORA_O: N = H; K = q; break;
+            case LORA_GU: N = T.I_l; K = H; break;
+            default: N = H; K = T.I_l; break;
+        }
+    };
+    std::set<int> subs[kLoraGroups];
+    for (const auto& e : pairs) {
+        const int g = e.first[1], sub = e.first[2];
+        const aha_tensor_desc* A = e.second[0];
+        const aha_tensor_desc* B = e.second[1];
+        AHA_REQUIRE(A && B, who + "layer " + std::to_string(e.first[0]) + ": a lora_" + (A ? "A" : "B") + " weight without its lora_" + (A ? "B" : "A"));
+        int N = 0, K = 0;
+        dims(g, sub, N, K);
+        AHA_REQUIRE(A->shape[0] == r && A->shape[1] == K, who + "tensor '" + std::string(A->name) + "' must be [" + std::to_string(r) + ", " +
+                                                               std::to_string(K) + "] (rank x the projection's input)");
+        AHA_REQUIRE(B->shape[0] == N && B->shape[1] == r, who + "tensor '" + std::string(B->name) + "' must be [" + std::to_string(N) + ", " +
+                                                               std::to_string(r) + "] (the projection's output x rank)");
+        subs[g].insert(sub);
+    }
+    LoraAdapter ad;
+    ad.r = r;
+    ad.scale = scale;
+    const WeightTable wt(tensors, n);
+    for (int g = 0; g < kLoraGroups; ++g) {
+        ad.w[g] = ceil_div((int)subs[g].size() * r, kLoraAlign) * kLoraAlign;
+        ad.A[g].assign(cf.L, {});
+        ad.B[g].assign(cf.L, {});
+    }
+    for (const auto& e : pairs) {
+        const int l = e.first[0], g = e.first[1], sub = e.first[2], w = ad.w[g];
+        const int col = (int)std::distance(subs[g].begin(), subs[g].find(sub)) * r;   // the target's sub-block
+        int N = 0, K = 0;
+        dims(g, sub, N, K);
+        const int Kg = T.lora.K[g], Ng = T.lora.N[g];
+        std::vector<__half>& a = ad.A[g][l];
+        std::vector<__half>& b = ad.B[g][l];
+        if (a.empty()) { a.assign((size_t)w * Kg, __float2half_rn(0.f)); b.assign((size_t)Ng * w, __float2half_rn(0.f)); }
+        wt.rows_to_half(e.second[0]->name, r, K, 0, r, 0, K, a.data() + (size_t)col * Kg, Kg);
+        std::vector<__half> bs((size_t)N * r);
+        wt.rows_to_half(e.second[1]->name, N, r, 0, N, 0, r, bs.data(), r);
+        for (int i = 0; i < N; ++i) {   // the base row layout: q | k | v stacked, gate / up interleaved
+            int row = i;
+            if (g == LORA_QKV) row = sub == 0 ? i : (sub == 1 ? q + i : q + kv + i);
+            if (g == LORA_GU) row = 2 * i + sub;
+            std::copy(bs.begin() + (size_t)i * r, bs.begin() + (size_t)(i + 1) * r, b.begin() + (size_t)row * w + col);
+        }
+    }
+    return ad;
+}
+}  // namespace
+
+extern "C" {
+
+int aha_b200_lora_create(aha_model* m, const aha_tensor_desc* tensors, size_t n, float scale, uint32_t* id_out) {
+    return guarded(m, [&] {
+        AHA_REQUIRE(id_out, "lora_create: id_out is required");
+        AHA_REQUIRE(m->next_lora_id < (uint32_t)std::numeric_limits<int>::max(), "lora_create: the handle has used every adapter id");
+        LoraAdapter ad = lora_stage(m, tensors, n, scale);
+        ad.id = m->next_lora_id;
+        LoraSet& L = m->text.lora;
+        L.ads.push_back(std::move(ad));
+        try {
+            L.rebuild(m->ctx.stream);
+        } catch (...) {
+            L.ads.pop_back();
+            L.rebuild(m->ctx.stream);
+            throw;
+        }
+        for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->composition_changed();
+        *id_out = m->next_lora_id++;
+    });
+}
+
+int aha_b200_lora_destroy(aha_model* m, uint32_t id) {
+    return guarded(m, [&] {
+        LoraSet& L = m->text.lora;
+        const int idx = L.index_of(id);
+        AHA_REQUIRE(id != 0 && idx >= 0, "lora_destroy: no LoRA adapter has id " + std::to_string(id) + " on this handle");
+        for (int i = 0; m->session.open && i < m->session.width; ++i)
+            AHA_REQUIRE(!(slot_req(m, i).used && slot_req(m, i).lora == id),
+                        "lora_destroy: adapter " + std::to_string(id) + " runs the request in slot " + std::to_string(i));
+        for (const auto& e : m->suspended)
+            AHA_REQUIRE(e.second.req.lora != id, "lora_destroy: adapter " + std::to_string(id) + " runs suspended request " + std::to_string(e.first));
+        if (m->session.open && m->session.prefix.on()) m->session.prefix.drop(m->text.pages, id);
+        L.ads.erase(L.ads.begin() + idx);
+        L.rebuild(m->ctx.stream);
+        for (BatchDecoder* B : {&m->batch, &m->wide_batch}) B->composition_changed();
+    });
+}
+
+int aha_b200_batch_add_lora(aha_model* m, const aha_batch_request* reqs, const uint32_t* adapters, size_t n, int32_t* slots_out,
+                            uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage) {
+    return guarded(m, [&] {
+        const std::string who = "batch_add_lora: ";
+        AHA_REQUIRE(reqs && adapters && slots_out && first_tokens_out && finished_out, "reqs, adapters, slots_out, first_tokens_out and finished_out are required");
+        open_session(m);
+        AHA_REQUIRE(m->session.wide, who + "LoRA requests need a wide session (aha_b200_batch_open_wide): a narrow session promises the ids of "
+                                           "single-request runs, and its CUDA-core GEMV has no adapter tail");
+        bool any = false;
+        for (size_t i = 0; i < n; ++i) {
+            AHA_REQUIRE(adapters[i] == 0 || m->text.lora.index_of(adapters[i]) >= 0,
+                        who + "request " + std::to_string(i) + ": no LoRA adapter has id " + std::to_string(adapters[i]) + " on this handle");
+            any = any || adapters[i] != 0;
+        }
+        AHA_REQUIRE(!any || !session_has_spec(m), who + "a speculative request is running: speculative requests and adapters do not share a session");
+        session_add_many(m, reqs, n, slots_out, first_tokens_out, finished_out, usage, true, adapters);
     });
 }
 

@@ -44,8 +44,9 @@ struct SlotRequest {
     aha_spec_stats spec_stats{};         // its counters
     bool lp_valid = false;               // the slot's record row holds the record of the last token its request delivered
     int last_n = 0;                      // tokens its last speculative pass delivered (0: its last token came from admission or a plain step)
+    uint32_t lora = 0;                   // the LoRA adapter it runs (aha_b200_batch_add_lora; 0: the base model)
     // a finished request: the slot is free, and its record, last_n and spec counters stay readable until the slot is taken again
-    void release() { used = false; hit = 0; spec = false; }
+    void release() { used = false; hit = 0; spec = false; lora = 0; }
     // a cancelled or suspended request, or a failed admission: as release, but the slot shows no record
     void clear() { release(); lp_valid = false; last_n = 0; }
 };
@@ -89,9 +90,16 @@ struct BatchDecoder {
     // registers, 1 = exact SIMT GEMM (validation twin), 2 = batched GEMV with the cp.async weight ring -- and eager launches instead of graphs
     int gemv = 2;
     bool use_graph = true;
-    // one CUDA graph per (running count, any request asks for log-probabilities) (~170 launches per step become one); they outlive
-    // composition changes
-    GraphCache<std::pair<int, bool>> graphs;
+    // one CUDA graph per (running count, any request asks for log-probabilities, any runs a LoRA adapter) (~170 launches per step become
+    // one); they outlive composition changes
+    GraphCache<std::pair<int, int>> graphs;
+    // LoRA (lora.cuh), wide sessions only: per slot the index of its request's adapter (-1: none), the tail lists of the adapters the
+    // composition runs and the t rows of the step; allocated from T->lora's memory, so they are re-made whenever its pools are rebuilt
+    bool lora_any = false;               // a request of the current composition runs an adapter
+    uint64_t lora_version = 0;           // the pools (LoraSet::version) the buffers and the adapter graphs were made for
+    int* d_slot_lora = nullptr;          // [cap]
+    int* d_lora_list = nullptr;          // [4][LoraSet::list_stride()]
+    __half *lt_hi = nullptr, *lt_lo = nullptr;   // [64][LoraSet::Rmax]
     // the set of running requests or a slot's sampler changed: the device copy of the composition is rebuilt before the next step
     void composition_changed() { table_for.clear(); ++epoch; }
     uint64_t epoch = 0;                  // counts composition changes (a speculative step rebuilds its own device copies on a new one)
@@ -100,6 +108,7 @@ struct BatchDecoder {
         for (auto& sl : slots) { sl.table.mapped = 0; sl.lp = 0; sl.req = SlotRequest{}; }
         table_for.clear();
         lp_any = false;
+        lora_any = false;
         graphs.clear();
     }
 
@@ -237,6 +246,7 @@ struct BatchDecoder {
         for (int i = 0; i < cap; ++i) lp_on[i] = slots[i].lp;
         for (int s : act) lp_any = lp_any || slots[s].lp > 0;
         Ctx& c = *T->ctx;
+        lora_table(act);
         if (d_lp_on) AHA_CUDA_CHECK(cudaMemcpyAsync(d_lp_on, lp_on.data(), lp_on.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_attn, h.data(), h.size() * sizeof(DecodeAttnArgs), cudaMemcpyHostToDevice, c.stream));
         AHA_CUDA_CHECK(cudaMemcpyAsync(d_act, act.data(), act.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
@@ -262,13 +272,23 @@ struct BatchDecoder {
         T->ctx->cnt.kernels++;
     }
 
-    // rows 0..nb-1: out = epi(W . x), x RMSNorm-ed with norm_w first when given
-    void proj(int epi, const LinearW& W, const float* x, int ldx, const float* norm_w, const float* resid, int ldr, float* out, int ldo, int nb) {
+    // rows 0..nb-1: out = epi(W . x), x RMSNorm-ed with norm_w first when given; (l, g): the layer and LoRA group of a projection adapters
+    // may target (g < 0: none)
+    void proj(int epi, const LinearW& W, const float* x, int ldx, const float* norm_w, const float* resid, int ldr, float* out, int ldo, int nb,
+              int l = -1, int g = -1) {
         Ctx& c = *T->ctx;
         if (wide) {
             const WideAct& in = W.K == act_h.K ? act_h : (W.K == act_i.K ? act_i : act_q);   // (any [64][K] operand of the right K will do)
             wide_prep(x, ldx, norm_w, in, nb);
-            wide_proj(epi, W, in, resid, ldr, out, ldo, nb);
+            LoraTail tail;
+            if (lora_any && g >= 0 && T->lora.Rp[g] > 0) {   // the rows' shrink outputs from the operand the projection reads, then the tail
+                const LoraSet& Lr = T->lora;
+                lora_shrink(c.stream, nb, in.hi, in.lo, nullptr, in.K, in.K, Lr.A[g][l], Lr.Rp[g], Lr.d_tab, g, d_slot_lora, d_act, lt_hi, lt_lo, nullptr);
+                c.cnt.kernels++;
+                tail.t_hi = lt_hi; tail.t_lo = lt_lo; tail.B = Lr.B[g][l]; tail.Rp = Lr.Rp[g];
+                tail.list = d_lora_list + (size_t)g * Lr.list_stride();
+            }
+            wide_proj(epi, W, in, resid, ldr, out, ldo, nb, &tail);
             return;
         }
         if (gemv == 1) {   // validation twin: the exact fp32 SIMT GEMM over the nb rows (normalised beforehand when a prologue is asked for)
@@ -290,15 +310,56 @@ struct BatchDecoder {
         c.cnt.kernels++;
     }
 
+    // The adapters of the composition `act` (wide sessions): the slots' adapter indices and the tail lists to the device.  New pools
+    // (an adapter was created or destroyed) drop the buffers and the step graphs that read the old ones.
+    void lora_table(const std::vector<int>& act) {
+        LoraSet& Lr = T->lora;
+        if (lora_version != Lr.version) {
+            lora_version = Lr.version;
+            d_slot_lora = d_lora_list = nullptr; lt_hi = lt_lo = nullptr;
+            std::vector<GraphCache<std::pair<int, int>>::Entry> keep;
+            for (auto& e : graphs.entries) {
+                if (e.key.second & 2) { if (e.exec) cudaGraphExecDestroy(e.exec); }
+                else keep.push_back(e);
+            }
+            graphs.entries.swap(keep);
+        }
+        std::vector<int> ad((size_t)cap, -1), used;
+        lora_any = false;
+        for (int s : act) {
+            if (!slots[s].req.lora) continue;
+            ad[s] = Lr.index_of(slots[s].req.lora);
+            AHA_REQUIRE(ad[s] >= 0, "batch step: slot " + std::to_string(s) + " runs an adapter that is not loaded");
+            used.push_back(ad[s]);
+            lora_any = true;
+        }
+        if (!lora_any) return;
+        AHA_REQUIRE(wide, "LoRA adapters run in wide sessions only");
+        Ctx& c = *T->ctx;
+        if (!d_slot_lora) {
+            d_slot_lora = Lr.dalloc<int>((size_t)cap);
+            d_lora_list = Lr.dalloc<int>((size_t)kLoraGroups * Lr.list_stride());
+            lt_hi = Lr.dalloc<__half>((size_t)kWideSeqs * Lr.Rmax);
+            lt_lo = Lr.dalloc<__half>((size_t)kWideSeqs * Lr.Rmax);
+            AHA_CUDA_CHECK(cudaMemsetAsync(lt_hi, 0, (size_t)kWideSeqs * Lr.Rmax * sizeof(__half), c.stream));
+            AHA_CUDA_CHECK(cudaMemsetAsync(lt_lo, 0, (size_t)kWideSeqs * Lr.Rmax * sizeof(__half), c.stream));
+        }
+        const std::vector<int> lists = Lr.lists(used);
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_slot_lora, ad.data(), ad.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaMemcpyAsync(d_lora_list, lists.data(), lists.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
+        AHA_CUDA_CHECK(cudaStreamSynchronize(c.stream));   // host vectors
+    }
+
     // one decode step of the sequences in `act` (slot indices, at most cap); leaves every slot's next token in d_tok[slot] and its DecodeState advanced
     void step(const std::vector<int>& act) {
         Ctx& c = *T->ctx;
         AHA_REQUIRE(!act.empty() && (int)act.size() <= cap, "batch step: bad active list");
+        if (T->lora.version != lora_version) table_for.clear();
         if (act != table_for) build_attn_table(act);
         const int nb = (int)act.size();
         if (wide) zero_rows_from(nb);
         if (!use_graph) { launches(nb); return; }
-        graphs.run(c, {nb, lp_any}, [&] { launches(nb); });
+        graphs.run(c, {nb, (lp_any ? 1 : 0) | (lora_any ? 2 : 0)}, [&] { launches(nb); });
     }
     void launches(int nb) {
         Ctx& c = *T->ctx;
@@ -308,11 +369,11 @@ struct BatchDecoder {
         c.cnt.kernels++;
         for (int l = 0; l < cf.L; ++l) {
             TextLayer& Ly = T->layers[l];
-            proj(GEPI_STORE, Ly.qkv, xb, H, Ly.ln1, nullptr, 0, qkvb, T->qkv_dim, nb);
+            proj(GEPI_STORE, Ly.qkv, xb, H, Ly.ln1, nullptr, 0, qkvb, T->qkv_dim, nb, l, LORA_QKV);
             attn(l, nb);
-            proj(GEPI_RESID, Ly.o, attnb, T->nh_l * cf.hd, nullptr, xb, H, xb, H, nb);
-            proj(GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb);
-            proj(GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb);
+            proj(GEPI_RESID, Ly.o, attnb, T->nh_l * cf.hd, nullptr, xb, H, xb, H, nb, l, LORA_O);
+            proj(GEPI_SWIGLU, Ly.gu, xb, H, Ly.ln2, nullptr, 0, hb, T->I_l, nb, l, LORA_GU);
+            proj(GEPI_RESID, Ly.down, hb, T->I_l, nullptr, xb, H, xb, H, nb, l, LORA_DOWN);
         }
         head(nb, false);
     }
@@ -386,14 +447,14 @@ struct BatchDecoder {
         }
         c.cnt.kernels++;
     }
-    void wide_proj(int epi, const LinearW& W, const WideAct& in, const float* resid, int ldr, float* out, int ldo, int nb) {
+    void wide_proj(int epi, const LinearW& W, const WideAct& in, const float* resid, int ldr, float* out, int ldo, int nb, const LoraTail* tail = nullptr) {
         Ctx& c = *T->ctx;
         WideArgs a{};
         a.bias = W.b; a.resid = resid; a.ldr = ldr; a.out = out; a.ldo = ldo; a.N = W.N; a.K = W.K; a.nb = nb;
         a.ws = wide_ws; a.counters = wide_cnt;
         AHA_REQUIRE(W.K == in.K, "wide projection: operand width mismatch");
         const CUtensorMap tm = W.has_tmap ? W.tmap : make_tmap_f16(W.w, (uint64_t)W.N, (uint64_t)W.K);
-        gemv_wide(c.stream, epi, tm, in.hi, in.lo, a, c.num_sms);
+        gemv_wide(c.stream, epi, tm, in.hi, in.lo, a, c.num_sms, tail);
         c.cnt.kernels++;
     }
 };

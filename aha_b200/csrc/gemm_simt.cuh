@@ -23,6 +23,9 @@ struct GemmArgs {
     float* C; int ldc;
     int M, N, K;
     int act;
+    // LoRA tail (lora.cuh): K2 more columns of the sum, A2 [M][K2] (fp32, ld lda2) times W2 [N][K2], after the K base columns
+    const float* A2 = nullptr; int lda2 = 0;
+    const __half* W2 = nullptr; int K2 = 0;
 };
 
 template <int EPI>
@@ -43,14 +46,18 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
     uint4 rb;
 
     auto load_tiles = [&](int k0) {
+        const bool tail = k0 >= g.K;
+        const float* A = tail ? g.A2 : g.A;
+        const __half* W = tail ? g.W2 : g.W;
+        const int lda = tail ? g.lda2 : g.lda, ldw = tail ? g.K2 : g.K, k = tail ? k0 - g.K : k0;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             int m = m0 + a_row + i * 64;
-            ra[i] = (m < g.M) ? *reinterpret_cast<const float4*>(g.A + (size_t)m * g.lda + k0 + a_k)
+            ra[i] = (m < g.M) ? *reinterpret_cast<const float4*>(A + (size_t)m * lda + k + a_k)
                               : make_float4(0.f, 0.f, 0.f, 0.f);
         }
         int n = n0 + b_row;
-        rb = (n < g.N) ? *reinterpret_cast<const uint4*>(g.W + (size_t)n * g.K + k0 + b_k) : make_uint4(0, 0, 0, 0);
+        rb = (n < g.N) ? *reinterpret_cast<const uint4*>(W + (size_t)n * ldw + k + b_k) : make_uint4(0, 0, 0, 0);
     };
     auto store_tiles = [&](int buf) {
 #pragma unroll
@@ -72,7 +79,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
 
-    const int nk = g.K / BK;
+    const int nk = (g.K + g.K2) / BK;
     load_tiles(0);
     store_tiles(0);
     __syncthreads();
@@ -131,7 +138,8 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
 }
 
 inline void gemm_simt(cudaStream_t st, int epi, const GemmArgs& g) {
-    AHA_REQUIRE(g.K % 16 == 0, "gemm_simt: K must be a multiple of 16");
+    AHA_REQUIRE(g.K % 16 == 0 && g.K2 % 16 == 0, "gemm_simt: K must be a multiple of 16");
+    AHA_REQUIRE(g.K2 == 0 || (g.A2 && g.W2 && g.lda2 % 4 == 0), "gemm_simt: the tail needs A2 / W2");
     AHA_REQUIRE(g.N % 4 == 0 && g.lda % 4 == 0 && g.ldc % 2 == 0, "gemm_simt: N/lda alignment");
     if (g.M == 0) return;
     dim3 grid(ceil_div(g.N, 128), ceil_div(g.M, 128));

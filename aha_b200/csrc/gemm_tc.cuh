@@ -13,6 +13,8 @@
 //   warpgroups 0, 1: consumers -- 64 rows each: per k-block 8 wgmma.m64nBNk16 (4 k-steps x {hi, lo}) into the fp32 accumulator
 //                in registers; a slot is released on its `empty` mbarrier once the wgmmas that read it have retired, then
 //                the fused bias / residual / activation / SwiGLU epilogue stores straight from the accumulator fragment.
+// LoRA tail (TAIL = true, lora.cuh): after the base k-blocks the producer streams the k-blocks of the device list g.tail -- t hi / lo
+// (128 rows x 64 columns) and B_pool (BN rows x 64 columns) in place of A and W -- into the same ring and accumulator.
 // Replaces candle Linear::forward at the reference call sites src/models/common/modules.rs:81-87,
 // 538-577 and qwen3vl/model.rs:96-103,168-184,232-278 (prefill shapes); validated against gemm_simt.cuh.
 #pragma once
@@ -21,6 +23,7 @@
 #include "common.cuh"
 #include "decode_fused.cuh"  // mbarrier helpers
 #include "gemm_simt.cuh"
+#include "lora.cuh"
 #include "wgmma.cuh"
 
 namespace aha {
@@ -95,6 +98,7 @@ struct GemmTcArgs {
     __half* out_hi = nullptr;   // when set, the result (after bias / activation / SwiGLU) is written as fp16 hi + lo halves [M, ldo] for the
     __half* out_lo = nullptr;   // next GEMM instead of fp32 C (EPI_STORE / EPI_ACT / EPI_SWIGLU)
     int ldo = 0;
+    const int* tail = nullptr;  // TAIL: device [count, k-block indices] of the LoRA pool
 };
 
 // one thread's two adjacent accumulator columns (n, n + 1) of output row `row` (n even): bias / residual / activation / SwiGLU, then
@@ -183,9 +187,11 @@ __device__ __forceinline__ void tc_mainloop(float (&acc)[BN / 2], uint8_t* tiles
 }
 
 // ------------------------------------------------------------------------------------------------ the GEMM kernel
-template <int EPI, int BN>
+template <int EPI, int BN, bool TAIL>
 __global__ void __launch_bounds__(kTcThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
-                                                               const __grid_constant__ CUtensorMap tm_w, GemmTcArgs g) {
+                                                               const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_thi,
+                                                               const __grid_constant__ CUtensorMap tm_tlo, const __grid_constant__ CUtensorMap tm_b,
+                                                               GemmTcArgs g) {
     constexpr int S = tc_stages<BN>(), SB = tc_stage_bytes<BN>();
     extern __shared__ __align__(1024) uint8_t tc_smem_raw[];
     // SWIZZLE_128B tiles need 1024-byte alignment in the shared window: align by hand (1 KB of slack is allocated)
@@ -195,7 +201,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) gemm_tc_kernel(const __grid_con
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int m0 = blockIdx.y * kTcBM, n0 = blockIdx.x * BN;
-    const int nkb = g.K / kTcBK;
+    const int nkb = g.K / kTcBK, nt = TAIL ? g.tail[0] : 0;
 
     if (tid == 0) {
         for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }   // 8 consumer warps release a slot
@@ -205,14 +211,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) gemm_tc_kernel(const __grid_con
 
     if (warp == 8) {
         // ======================= TMA producer
-        if (lane == 0)
+        if (lane == 0) {
             for (int kb = 0; kb < nkb; ++kb) tc_produce<BN>(tiles, full, empty, &tm_hi, &tm_lo, &tm_w, kb, kb, m0, n0);
+            for (int i = 0; i < nt; ++i) tc_produce<BN>(tiles, full, empty, &tm_thi, &tm_tlo, &tm_b, nkb + i, g.tail[1 + i], m0, n0);
+        }
         return;
     }
     // ======================= consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the tile
     const int wg = warp >> 2;
     float acc[BN / 2];
-    tc_mainloop<BN>(acc, tiles, full, empty, 0, nkb, wg, lane);
+    tc_mainloop<BN>(acc, tiles, full, empty, 0, nkb + nt, wg, lane);
     const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), col = n0 + 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
@@ -227,17 +235,19 @@ inline bool gemm_tc_supported(int M, int N, int K) { return K % kTcBK == 0 && N 
 
 // The > 48 KB dynamic shared memory opt-in is a per-device function attribute: aha_b200_create calls this after
 // cudaSetDevice for every handle (a process-wide once-flag would leave a second device without it).
-template <int BN>
+template <int BN, bool TAIL>
 inline void gemm_tc_init_bn() {
     const int smem = (int)gemm_tc_smem_bytes<BN>();
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_STORE, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_RESID, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_ACT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_SWIGLU, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_STORE, BN, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_RESID, BN, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_ACT, BN, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<EPI_SWIGLU, BN, TAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
 }
 inline void gemm_tc_init() {
-    gemm_tc_init_bn<128>();
-    gemm_tc_init_bn<256>();
+    gemm_tc_init_bn<128, false>();
+    gemm_tc_init_bn<256, false>();
+    gemm_tc_init_bn<128, true>();
+    gemm_tc_init_bn<256, true>();
 }
 
 // W map with `box_rows`-row boxes (the 128 x 256 tile loads 256 W rows per k-block)
@@ -255,15 +265,36 @@ inline CUtensorMap make_tmap_f16_rows(const void* ptr, uint64_t rows, uint64_t K
 }
 
 // A already split: hi/lo fp16 [M, K] row-major.  tm_w describes W [N, K] with BN-row boxes (make_tmap_f16 for 128,
-// make_tmap_f16_rows(w, N, K, 256) for 256).
+// make_tmap_f16_rows(w, N, K, 256) for 256).  tail (optional, Rp > 0): t hi / lo [M][Rp], B_pool [N][Rp] and the device list of k-blocks.
 template <int BN>
-inline void gemm_tc_launch(cudaStream_t st, int epi, const __half* a_hi, const __half* a_lo, const CUtensorMap& tm_w, const GemmTcArgs& g) {
+inline void gemm_tc_launch(cudaStream_t st, int epi, const __half* a_hi, const __half* a_lo, const CUtensorMap& tm_w, const GemmTcArgs& g0,
+                           const LoraTail* tail = nullptr) {
+    GemmTcArgs g = g0;
     const CUtensorMap tm_hi = make_tmap_f16(a_hi, (uint64_t)g.M, (uint64_t)g.K);
     const CUtensorMap tm_lo = make_tmap_f16(a_lo, (uint64_t)g.M, (uint64_t)g.K);
     const size_t smem = gemm_tc_smem_bytes<BN>();
     dim3 grid(ceil_div(g.N, BN), ceil_div(g.M, kTcBM));
+    if (tail && tail->Rp > 0) {
+        AHA_REQUIRE(tail->Rp % kTcBK == 0 && tail->list, "gemm_tc: the LoRA tail needs a pool of whole k-blocks and a k-block list");
+        const CUtensorMap tm_thi = make_tmap_f16(tail->t_hi, (uint64_t)g.M, (uint64_t)tail->Rp);
+        const CUtensorMap tm_tlo = make_tmap_f16(tail->t_lo, (uint64_t)g.M, (uint64_t)tail->Rp);
+        const CUtensorMap tm_b = make_tmap_f16_rows(tail->B, (uint64_t)g.N, (uint64_t)tail->Rp, BN);
+        g.tail = tail->list;
+        switch (epi) {
+#define AHA_TC_TAIL_CASE(E)                                                                                                        \
+    case E: gemm_tc_kernel<E, BN, true><<<grid, kTcThreads, smem, st>>>(tm_hi, tm_lo, tm_w, tm_thi, tm_tlo, tm_b, g); break;
+            AHA_TC_TAIL_CASE(EPI_STORE)
+            AHA_TC_TAIL_CASE(EPI_RESID)
+            AHA_TC_TAIL_CASE(EPI_ACT)
+            AHA_TC_TAIL_CASE(EPI_SWIGLU)
+            default: AHA_REQUIRE(false, "gemm_tc: bad epilogue");
+        }
+#undef AHA_TC_TAIL_CASE
+        AHA_CUDA_CHECK(cudaGetLastError());
+        return;
+    }
 #define AHA_TC_CASE(E)                                                                                                             \
-    case E: gemm_tc_kernel<E, BN><<<grid, kTcThreads, smem, st>>>(tm_hi, tm_lo, tm_w, g); break;
+    case E: gemm_tc_kernel<E, BN, false><<<grid, kTcThreads, smem, st>>>(tm_hi, tm_lo, tm_w, tm_hi, tm_lo, tm_w, g); break;
     switch (epi) {
         AHA_TC_CASE(EPI_STORE)
         AHA_TC_CASE(EPI_RESID)

@@ -17,9 +17,14 @@
 // `splits` parts that depend only on (N, K) and the SM count (wide_plan), never on nb.  Every CTA writes its fp32 partial tile to a
 // workspace; the last CTA of a row tile (an atomic counter, reset by that CTA) adds the partials in split order 0, 1, ... and runs the
 // epilogue.  No float atomics: the sums are the same whichever CTA finishes last.
+//
+// LoRA tail (TAIL = true, lora.cuh): after its base k-blocks the last split streams the k-blocks of the device list a.tail -- a B_pool tile
+// (128 rows x 64 columns) and the t hi / lo tiles of the same 64 columns in place of W and X -- into the same ring and accumulator.  The
+// tail rides in that one split whatever the list holds, so a row's partial sums keep their split order.
 #pragma once
 #include "gemm_tc.cuh"
 #include "gemv.cuh"   // GemvEpi
+#include "lora.cuh"   // LoraTail
 
 namespace aha {
 
@@ -57,11 +62,14 @@ struct WideArgs {
     int splits, kper;               // wide_plan
     float* ws;                      // [tiles * splits][kWidePartFloats] when splits > 1
     int* counters;                  // [tiles], zero between launches
+    const int* tail = nullptr;      // TAIL: device [count, k-block indices] of the LoRA pool (lora.cuh)
 };
 
-template <int EPI>
+template <int EPI, bool TAIL>
 __global__ void __launch_bounds__(kWideThreads, 2) gemv_wide_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_hi,
-                                                                    const __grid_constant__ CUtensorMap tm_lo, WideArgs a) {
+                                                                    const __grid_constant__ CUtensorMap tm_lo, const __grid_constant__ CUtensorMap tm_b,
+                                                                    const __grid_constant__ CUtensorMap tm_thi, const __grid_constant__ CUtensorMap tm_tlo,
+                                                                    WideArgs a) {
     extern __shared__ __align__(1024) uint8_t wide_smem_raw[];
     uint8_t* tiles = wide_smem_raw + ((1024u - (smem_u32(wide_smem_raw) & 1023u)) & 1023u);   // [stages][W | X hi | X lo]
     uint64_t* full = reinterpret_cast<uint64_t*>(tiles + (size_t)kWideStages * kWideStageBytes);
@@ -71,6 +79,7 @@ __global__ void __launch_bounds__(kWideThreads, 2) gemv_wide_kernel(const __grid
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile = blockIdx.x, split = blockIdx.y, n0 = tile * kWideBM;
     const int kb0 = split * a.kper, nk = min(a.K / kTcBK, kb0 + a.kper) - kb0;
+    const int nt = TAIL && split == a.splits - 1 ? a.tail[0] : 0;
 
     if (tid == 0) {
         for (int i = 0; i < kWideStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
@@ -80,14 +89,22 @@ __global__ void __launch_bounds__(kWideThreads, 2) gemv_wide_kernel(const __grid
 
     if (warp == 8) {
         if (lane == 0) {
-            for (int i = 0; i < nk; ++i) {
-                const int s = i % kWideStages, k = (kb0 + i) * kTcBK;
+            for (int i = 0; i < nk + nt; ++i) {
+                const int s = i % kWideStages;
                 mbar_wait(&empty[s], ((i / kWideStages) & 1) ^ 1);
                 uint8_t* st = tiles + (size_t)s * kWideStageBytes;
                 mbar_expect_tx(&full[s], kWideStageBytes);
-                tma_load_2d(st, &tm_w, k, n0, &full[s]);
-                tma_load_2d(st + kWideWBytes, &tm_hi, k, 0, &full[s]);
-                tma_load_2d(st + kWideWBytes + kWideXBytes, &tm_lo, k, 0, &full[s]);
+                if (!TAIL || i < nk) {
+                    const int k = (kb0 + i) * kTcBK;
+                    tma_load_2d(st, &tm_w, k, n0, &full[s]);
+                    tma_load_2d(st + kWideWBytes, &tm_hi, k, 0, &full[s]);
+                    tma_load_2d(st + kWideWBytes + kWideXBytes, &tm_lo, k, 0, &full[s]);
+                } else {
+                    const int k = a.tail[1 + i - nk] * kTcBK;
+                    tma_load_2d(st, &tm_b, k, n0, &full[s]);
+                    tma_load_2d(st + kWideWBytes, &tm_thi, k, 0, &full[s]);
+                    tma_load_2d(st + kWideWBytes + kWideXBytes, &tm_tlo, k, 0, &full[s]);
+                }
             }
         }
         return;
@@ -96,7 +113,7 @@ __global__ void __launch_bounds__(kWideThreads, 2) gemv_wide_kernel(const __grid
     float acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-    for (int i = 0; i < nk; ++i) {
+    for (int i = 0; i < nk + nt; ++i) {
         const int s = i % kWideStages;
         mbar_wait(&full[s], (i / kWideStages) & 1);
         const uint32_t st = smem_u32(tiles + (size_t)s * kWideStageBytes);
@@ -171,14 +188,19 @@ __global__ void __launch_bounds__(kWideThreads, 2) gemv_wide_kernel(const __grid
 
 inline void gemv_wide_init() {
     const int smem = (int)gemv_wide_smem_bytes();
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_SWIGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_STORE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_RESID, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_SWIGLU, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_STORE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_RESID, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    AHA_CUDA_CHECK(cudaFuncSetAttribute(gemv_wide_kernel<GEPI_SWIGLU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
 }
 
 // X hi / lo: [64][K] fp16 (rows >= nb zero or stale), tm_w: W [N, K] with 128-row boxes (make_tmap_f16 / LinearW::tmap).
 // ws / counters: sized by wide_ws_floats / the tile count of the widest projection.
-inline void gemv_wide(cudaStream_t st, int epi, const CUtensorMap& tm_w, const __half* x_hi, const __half* x_lo, WideArgs a, int num_sms) {
+// tail (optional, Rp > 0): t hi / lo [64][Rp], B_pool [N][Rp] and the device list of k-blocks to stream (lora.cuh).
+inline void gemv_wide(cudaStream_t st, int epi, const CUtensorMap& tm_w, const __half* x_hi, const __half* x_lo, WideArgs a, int num_sms,
+                      const LoraTail* tail = nullptr) {
     AHA_REQUIRE(a.nb >= 1 && a.nb <= kWideSeqs, "gemv_wide: 1..64 sequences");
     AHA_REQUIRE(gemv_wide_supported(a.N, a.K), "gemv_wide: N and K must be multiples of 64");
     const WidePlan p = wide_plan(a.N, a.K, num_sms);
@@ -188,10 +210,25 @@ inline void gemv_wide(cudaStream_t st, int epi, const CUtensorMap& tm_w, const _
     const CUtensorMap tm_lo = make_tmap_f16_rows(x_lo, kWideSeqs, (uint64_t)a.K, kWideSeqs);
     const dim3 grid(p.tiles, p.splits);
     const size_t smem = gemv_wide_smem_bytes();
-    switch (epi) {
-        case GEPI_STORE: gemv_wide_kernel<GEPI_STORE><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, a); break;
-        case GEPI_RESID: gemv_wide_kernel<GEPI_RESID><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, a); break;
-        case GEPI_SWIGLU: gemv_wide_kernel<GEPI_SWIGLU><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, a); break;
+    if (tail && tail->Rp > 0) {
+        AHA_REQUIRE(tail->Rp % kTcBK == 0 && tail->list, "gemv_wide: the LoRA tail needs a pool of whole k-blocks and a k-block list");
+        const CUtensorMap tm_b = make_tmap_f16(tail->B, (uint64_t)a.N, (uint64_t)tail->Rp);
+        const CUtensorMap tm_thi = make_tmap_f16_rows(tail->t_hi, kWideSeqs, (uint64_t)tail->Rp, kWideSeqs);
+        const CUtensorMap tm_tlo = make_tmap_f16_rows(tail->t_lo, kWideSeqs, (uint64_t)tail->Rp, kWideSeqs);
+        a.tail = tail->list;
+        switch (epi) {
+            case GEPI_STORE: gemv_wide_kernel<GEPI_STORE, true><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_b, tm_thi, tm_tlo, a); break;
+            case GEPI_RESID: gemv_wide_kernel<GEPI_RESID, true><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_b, tm_thi, tm_tlo, a); break;
+            case GEPI_SWIGLU: gemv_wide_kernel<GEPI_SWIGLU, true><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_b, tm_thi, tm_tlo, a); break;
+            default: AHA_REQUIRE(false, "gemv_wide: bad epilogue");
+        }
+        AHA_CUDA_CHECK(cudaGetLastError());
+        return;
+    }
+    switch (epi) {   // (the tail maps are not read: the base W / X maps fill their places)
+        case GEPI_STORE: gemv_wide_kernel<GEPI_STORE, false><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_w, tm_hi, tm_lo, a); break;
+        case GEPI_RESID: gemv_wide_kernel<GEPI_RESID, false><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_w, tm_hi, tm_lo, a); break;
+        case GEPI_SWIGLU: gemv_wide_kernel<GEPI_SWIGLU, false><<<grid, kWideThreads, smem, st>>>(tm_w, tm_hi, tm_lo, tm_w, tm_hi, tm_lo, a); break;
         default: AHA_REQUIRE(false, "gemv_wide: bad epilogue");
     }
     AHA_CUDA_CHECK(cudaGetLastError());

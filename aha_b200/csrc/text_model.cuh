@@ -21,6 +21,7 @@
 #include "json.hpp"
 #include "kernels_common.cuh"
 #include "logprobs.cuh"
+#include "lora.cuh"
 #include "nccl_shim.h"
 #include "sampling.cuh"
 
@@ -270,9 +271,10 @@ inline ActSplit act_split(Ctx& c, int which, size_t halfs) {
 inline bool gemm_on_tc(const Ctx& c, int M, const LinearW& W) {
     return c.gemm_impl != 1 && gemm_tc_supported(M, W.N, W.K) && !(c.gemm_impl == 0 && M < 32);
 }
-// the tensor-core GEMM on activations that are already split ([M, K] contiguous halves); `out`: write the result split as well
+// the tensor-core GEMM on activations that are already split ([M, K] contiguous halves); `out`: write the result split as well; `tail`: the
+// LoRA update as extra k-blocks (lora.cuh)
 inline void linear_gemm_split(Ctx& c, int epi, const __half* hi, const __half* lo, LinearW& W, const float* resid, int ldr, float* C, int ldc, int M,
-                              int act = ACT_NONE, ActSplit out = ActSplit(), int ldo = 0) {
+                              int act = ACT_NONE, ActSplit out = ActSplit(), int ldo = 0, const LoraTail* tail = nullptr) {
     if (M == 0) return;
     AHA_REQUIRE(gemm_on_tc(c, M, W), "linear_gemm_split: shape does not run on the tensor-core kernels");
     AHA_REQUIRE(!out || epi != EPI_RESID, "linear_gemm_split: the residual epilogue writes fp32");
@@ -282,19 +284,21 @@ inline void linear_gemm_split(Ctx& c, int epi, const __half* hi, const __half* l
     g.out_hi = out.hi; g.out_lo = out.lo; g.ldo = ldo;
     if (c.gemm_impl == 3 || (c.gemm_impl == 0 && c.gemm_wide && W.N >= 256)) {
         if (!W.has_tmap256) { W.tmap256 = make_tmap_f16_rows(W.w, (uint64_t)W.N, (uint64_t)W.K, 256); W.has_tmap256 = true; }
-        gemm_tc_launch<256>(c.stream, epi, hi, lo, W.tmap256, g);
+        gemm_tc_launch<256>(c.stream, epi, hi, lo, W.tmap256, g, tail);
     } else {
-        gemm_tc_launch<128>(c.stream, epi, hi, lo, W.tmap, g);
+        gemm_tc_launch<128>(c.stream, epi, hi, lo, W.tmap, g, tail);
     }
     c.cnt.kernels++;
 }
-inline void linear_gemm(Ctx& c, int epi, const float* A, int lda, LinearW& W, const float* resid, int ldr, float* C, int ldc, int M, int act = ACT_NONE) {
+inline void linear_gemm(Ctx& c, int epi, const float* A, int lda, LinearW& W, const float* resid, int ldr, float* C, int ldc, int M, int act = ACT_NONE,
+                        const LoraTail* tail = nullptr) {
     if (M == 0) return;
     const bool tc_ok = gemm_tc_supported(M, W.N, W.K) && lda % 4 == 0;
     AHA_REQUIRE(c.gemm_impl < 2 || tc_ok, "gemm_impl=2/3 (wgmma) requested but the shape does not tile (K % 64, N % 32)");
     if (c.gemm_impl == 1 || !tc_ok || (c.gemm_impl == 0 && M < 32)) {
         GemmArgs g;
         g.A = A; g.lda = lda; g.W = W.w; g.bias = W.b; g.resid = resid; g.ldr = ldr; g.C = C; g.ldc = ldc; g.M = M; g.N = W.N; g.K = W.K; g.act = act;
+        if (tail && tail->Rp > 0) { g.A2 = tail->t_f32; g.lda2 = tail->Rp; g.W2 = tail->B; g.K2 = tail->Rp; }
         gemm_simt(c.stream, epi, g);
         c.cnt.kernels++;
         return;
@@ -305,7 +309,7 @@ inline void linear_gemm(Ctx& c, int epi, const float* A, int lda, LinearW& W, co
     const size_t n4 = halfs / 4;
     split_f32_to_f16x2_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, c.stream>>>(A, lda, hi, lo, M, W.K);
     c.cnt.kernels++;
-    linear_gemm_split(c, epi, hi, lo, W, resid, ldr, C, ldc, M, act);
+    linear_gemm_split(c, epi, hi, lo, W, resid, ldr, C, ldc, M, act, ActSplit(), 0, tail);
 }
 
 // Upload `names` stacked along the output dimension ([sum N_i, K]); optional row interleave of two
@@ -487,6 +491,8 @@ struct TextModel {
     float* inv_freq = nullptr;
     uint8_t* mrope_sel = nullptr;
     uint64_t weight_bytes = 0, decode_weight_bytes = 0;
+    std::string wprefix;                 // the weight names' prefix of the text stack ("model.", "model.language_model.", ...)
+    LoraSet lora;                        // LoRA adapters (aha_b200_lora_create): wide batch sessions add them to the four projections
 
     // paged KV
     int max_ctx = 0, num_pages = 0;
@@ -553,7 +559,7 @@ struct TextModel {
     // ---------------------------------------------------------------------------------------------
     void load(Ctx& c, const TextCfg& cf, const WeightTable& wt, const std::string& prefix, const std::string& lm_head_name,
               int rank, int world) {
-        ctx = &c; cfg = cf; tp_rank = rank; tp_world = world;
+        ctx = &c; cfg = cf; tp_rank = rank; tp_world = world; wprefix = prefix;
         AHA_REQUIRE(cfg.hd == 128, "head_dim must be 128 (Qwen3 family)");
         AHA_REQUIRE(cfg.nh % cfg.nkv == 0, "num_attention_heads must be a multiple of num_key_value_heads");
         AHA_REQUIRE(cfg.nkv % world == 0 && cfg.I % world == 0, "tensor-parallel world must divide num_key_value_heads and intermediate_size");
@@ -596,6 +602,11 @@ struct TextModel {
             T.qn = upload_vec(c, wt, p + "self_attn.q_norm.weight", hd);
             T.kn = upload_vec(c, wt, p + "self_attn.k_norm.weight", hd);
         }
+        lora.L = cfg.L;
+        lora.N[LORA_QKV] = qkv_dim; lora.K[LORA_QKV] = H;
+        lora.N[LORA_O] = H; lora.K[LORA_O] = nh_l * hd;
+        lora.N[LORA_GU] = 2 * I_l; lora.K[LORA_GU] = H;
+        lora.N[LORA_DOWN] = H; lora.K[LORA_DOWN] = I_l;
         weight_bytes = c.alloc_bytes - before;
         decode_weight_bytes = 0;
         for (auto& T : layers)
@@ -739,8 +750,9 @@ struct TextModel {
     }
 
     // ---- GEMM dispatch (SIMT exact path; the wgmma path plugs in here)
-    void gemm(int epi, const float* A, int lda, LinearW& W, const float* resid, int ldr, float* C, int ldc, int M, int act = ACT_NONE) {
-        linear_gemm(*ctx, epi, A, lda, W, resid, ldr, C, ldc, M, act);
+    void gemm(int epi, const float* A, int lda, LinearW& W, const float* resid, int ldr, float* C, int ldc, int M, int act = ACT_NONE,
+              const LoraTail* tail = nullptr) {
+        linear_gemm(*ctx, epi, A, lda, W, resid, ldr, C, ldc, M, act, tail);
     }
 
     void init_tp(const void* unique_id) {
@@ -803,6 +815,8 @@ struct TextModel {
         if (!embeds_ready) { embed_gather_kernel<<<S, 256, 0, st>>>(d_ids, embed, x, S, H, cfg.V); c.cnt.kernels++; }
         RopeArgs rp{inv_freq, mrope_sel, d_pos3, S};
         const float scaling = (float)(1.0 / std::sqrt((double)hd));
+        LoraTail lt;
+        AHA_REQUIRE(!lora.pf_on || (tp_world == 1 && S <= (int)lora.pf_rows), "LoRA prefill: rows beyond the adapters' row array");
         for (int l = 0; l < cfg.L; ++l) {
             TextLayer& T = layers[l];
             // pre-split data flow (Ctx::presplit): norm -> [hi|lo] -> qkv GEMM; attention -> [hi|lo] -> o_proj; norm -> [hi|lo] -> gate/up
@@ -811,10 +825,11 @@ struct TextModel {
             if (ps) {
                 ActSplit n1 = act_split(c, 0, (size_t)S * H);
                 rmsnorm_split_kernel<<<S, 256, 0, st>>>(x, T.ln1, cfg.eps, n1.hi, n1.lo, H); c.cnt.kernels++;
-                linear_gemm_split(c, EPI_STORE, n1.hi, n1.lo, T.qkv, nullptr, 0, qkv, qkv_dim, S);
+                linear_gemm_split(c, EPI_STORE, n1.hi, n1.lo, T.qkv, nullptr, 0, qkv, qkv_dim, S, ACT_NONE, ActSplit(), 0,
+                                  pf_tail(lt, l, LORA_QKV, S, n1.hi, n1.lo, nullptr, H));
             } else {
                 rmsnorm_kernel<<<S, 256, 0, st>>>(x, T.ln1, cfg.eps, xn, H); c.cnt.kernels++;
-                gemm(EPI_STORE, xn, H, T.qkv, nullptr, 0, qkv, qkv_dim, S);
+                gemm(EPI_STORE, xn, H, T.qkv, nullptr, 0, qkv, qkv_dim, S, ACT_NONE, pf_tail(lt, l, LORA_QKV, S, nullptr, nullptr, xn, H));
             }
             KVSrc kv = kv_src(l, pt);
             qk_norm_rope_kv_kernel<128><<<dim3(S, nh_l + 2 * nkv_l), 128, 0, st>>>(qkv, T.qn, T.kn, cfg.eps, rp, const_cast<float*>(kv.k), const_cast<float*>(kv.v), kv, nh_l, nkv_l, pos0);
@@ -830,21 +845,24 @@ struct TextModel {
                 if (segs.empty()) flash_dispatch<128>(c, fa, nh_l, true);
                 else flash_dispatch_segments(c, fa, nh_l, segs);
                 if (tp_world > 1) { linear_gemm_split(c, EPI_STORE, ao.hi, ao.lo, T.o, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
-                else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.o, x, H, x, H, S);
+                else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.o, x, H, x, H, S, ACT_NONE, ActSplit(), 0,
+                                       pf_tail(lt, l, LORA_O, S, ao.hi, ao.lo, nullptr, nh_l * hd));
                 ActSplit n2 = act_split(c, 0, (size_t)S * H);
                 rmsnorm_split_kernel<<<S, 256, 0, st>>>(x, T.ln2, cfg.eps, n2.hi, n2.lo, H); c.cnt.kernels++;
-                linear_gemm_split(c, EPI_SWIGLU, n2.hi, n2.lo, T.gu, nullptr, 0, nullptr, 0, S, ACT_NONE, ao, I_l);
+                linear_gemm_split(c, EPI_SWIGLU, n2.hi, n2.lo, T.gu, nullptr, 0, nullptr, 0, S, ACT_NONE, ao, I_l,
+                                  pf_tail(lt, l, LORA_GU, S, n2.hi, n2.lo, nullptr, H));
                 if (tp_world > 1) { linear_gemm_split(c, EPI_STORE, ao.hi, ao.lo, T.down, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
-                else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.down, x, H, x, H, S);
+                else linear_gemm_split(c, EPI_RESID, ao.hi, ao.lo, T.down, x, H, x, H, S, ACT_NONE, ActSplit(), 0,
+                                       pf_tail(lt, l, LORA_DOWN, S, ao.hi, ao.lo, nullptr, I_l));
             } else {
                 if (segs.empty()) flash_dispatch<128>(c, fa, nh_l, true);
                 else flash_dispatch_segments(c, fa, nh_l, segs);
                 if (tp_world > 1) { gemm(EPI_STORE, attn, nh_l * hd, T.o, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
-                else gemm(EPI_RESID, attn, nh_l * hd, T.o, x, H, x, H, S);
+                else gemm(EPI_RESID, attn, nh_l * hd, T.o, x, H, x, H, S, ACT_NONE, pf_tail(lt, l, LORA_O, S, nullptr, nullptr, attn, nh_l * hd));
                 rmsnorm_kernel<<<S, 256, 0, st>>>(x, T.ln2, cfg.eps, xn, H); c.cnt.kernels++;
-                gemm(EPI_SWIGLU, xn, H, T.gu, nullptr, 0, hbuf, I_l, S);
+                gemm(EPI_SWIGLU, xn, H, T.gu, nullptr, 0, hbuf, I_l, S, ACT_NONE, pf_tail(lt, l, LORA_GU, S, nullptr, nullptr, xn, H));
                 if (tp_world > 1) { gemm(EPI_STORE, hbuf, I_l, T.down, nullptr, 0, tp_tmp, H, S); tp_reduce_add(tp_tmp, x, (size_t)S * H); }
-                else gemm(EPI_RESID, hbuf, I_l, T.down, x, H, x, H, S);
+                else gemm(EPI_RESID, hbuf, I_l, T.down, x, H, x, H, S, ACT_NONE, pf_tail(lt, l, LORA_DOWN, S, nullptr, nullptr, hbuf, I_l));
             }
             if (l < (int)deepstack.size() && n_visual > 0) {
                 scatter_rows_kernel<<<n_visual, 256, 0, st>>>(d_visual_idx, deepstack[l], x, H, 1); c.cnt.kernels++;
@@ -855,6 +873,19 @@ struct TextModel {
         AHA_CUDA_CHECK(cudaGetLastError());
         // last-token logits: final RMSNorm fused into the lm_head GEMV (qwen3/model.rs:186-187,142)
         if (segs.empty()) head(x + (size_t)(S - 1) * H);
+    }
+
+    // The LoRA tail of group g in layer l over the S rows of the running prefill, or null when it adds none (LoraSet::pf_on): the shrink
+    // runs here, from the operand the projection reads -- its hi / lo halves ([S][K] contiguous), or fp32 rows ldx floats apart.
+    const LoraTail* pf_tail(LoraTail& t, int l, int g, int S, const __half* hi, const __half* lo, const float* xf, int ldx) {
+        if (!lora.pf_on || lora.Rp[g] == 0) return nullptr;
+        t.t_hi = lora.pf_hi; t.t_lo = lora.pf_lo; t.t_f32 = lora.pf_f32;
+        t.B = lora.B[g][l]; t.Rp = lora.Rp[g];
+        t.list = lora.pf_list + (size_t)g * lora.list_stride();
+        lora_shrink(ctx->stream, S, hi, lo, xf, hi ? lora.K[g] : ldx, lora.K[g], lora.A[g][l], lora.Rp[g], lora.d_tab, g, lora.pf_ad, nullptr, lora.pf_hi,
+                    lora.pf_lo, lora.pf_f32);
+        ctx->cnt.kernels++;
+        return &t;
     }
 
     void head(const float* xrow) {
@@ -1075,6 +1106,7 @@ struct TextModel {
         for (int w = 0; w < kFusedMaxTp; ++w)
             if (ll_peer_sym[w] && w != tp_rank) { cudaIpcCloseMemHandle(ll_peer_sym[w]); ll_peer_sym[w] = nullptr; }
         step_graph.clear();
+        lora.free_all();
         if (comm) { NcclApi::get().CommDestroy(comm); comm = nullptr; }
     }
 };

@@ -427,6 +427,36 @@ class B200Model:
         """Free a token automaton (refused while a running batch slot uses it or a logit-rules object names it)."""
         self._check(self._lib.aha_b200_fsm_destroy(self._h, int(fsm)))
 
+    # ---- LoRA adapters: many fine-tunes of the base model in one wide session
+    def lora_create(self, tensors, scale):
+        """Load one adapter (aha_b200_lora_create) -> its id, the adapter of batch_add_lora.  tensors: {PEFT name: array [r, K] (lora_A) or
+        [N, r] (lora_B)}, f16 / bf16 / f32, as in adapter_model.safetensors; scale: lora_alpha / r (lora_alpha / sqrt(r) for rsLoRA)."""
+        names = list(tensors.keys())
+        arrs = [tensors[n] if (isinstance(tensors[n], np.ndarray) and tensors[n].flags["C_CONTIGUOUS"]) else np.ascontiguousarray(tensors[n])
+                for n in names]
+        descs = (L.TensorDesc * max(len(names), 1))(*[L.make_desc(a, n) for a, n in zip(arrs, names)])
+        i = C.c_uint32(0)
+        self._check(self._lib.aha_b200_lora_create(self._h, descs, len(names), float(scale), C.byref(i)))
+        return int(i.value)
+
+    def lora_destroy(self, adapter):
+        """Free an adapter (refused while a running or suspended request uses it); its prefix-cache pages are dropped."""
+        self._check(self._lib.aha_b200_lora_destroy(self._h, int(adapter)))
+
+    def batch_add_lora(self, requests, adapters, return_usage=False):
+        """batch_add_many with request i running adapter adapters[i] (0: the base model); wide sessions only.  All or nothing.
+        -> [(slot, first token, finished), ...] in input order, and with return_usage=True also the prompt-side usage dicts."""
+        n = len(requests)
+        ad = np.ascontiguousarray(np.asarray(adapters, dtype=np.uint32).reshape(-1))
+        if ad.size != n:
+            raise ValueError(f"adapters must hold one id per request ({n}), got {ad.size}")
+        arr, _keep = self._batch_requests(requests)
+        slots, toks, fins = (C.c_int32 * max(n, 1))(), (C.c_uint32 * max(n, 1))(), (C.c_int32 * max(n, 1))()
+        us = (L.Usage * max(n, 1))()
+        self._check(self._lib.aha_b200_batch_add_lora(self._h, arr, ad.ctypes.data_as(C.POINTER(C.c_uint32)), n, slots, toks, fins, us))
+        res = [(int(slots[i]), int(toks[i]), bool(fins[i])) for i in range(n)]
+        return (res, [self._usage(us[i]) for i in range(n)]) if return_usage else res
+
     # ---- OpenAI presence_penalty / frequency_penalty / logit_bias: logit-rules objects on the handle
     def rules_create(self, presence_penalty=0.0, frequency_penalty=0.0, logit_bias=None, fsm=None):
         """A logit-rules object (aha_b200_rules_create) -> its id, the `rules` argument of the generation entries.  Penalties in [-2, 2];

@@ -318,6 +318,31 @@ int aha_b200_batch_step_n(aha_model* m, uint32_t* tokens_out /* [cap] */, int32_
  * without such requests launches exactly the kernels it launched before. */
 int aha_b200_batch_logprobs(aha_model* m, aha_logprobs* out /* [cap] */, size_t cap);
 
+/* LoRA adapters (new design): many fine-tunes of the handle's base model served by one wide session, each request naming its adapter.
+ * aha_b200_lora_create loads one adapter: tensors use PEFT's names -- the base text-layer weight name with `.weight` replaced by
+ * `.lora_A.weight` / `.lora_B.weight`, optionally behind `base_model.model.` (e.g. model.layers.3.self_attn.q_proj.lora_A.weight for
+ * "qwen3", model.language_model.layers... for "qwen3vl", thinker.model.layers... for the ASR thinker) -- for any subset of the
+ * q/k/v/o/gate/up/down projections of any layer.  A is [r, K] and B [N, r] of the projection y = W x they target, 1 <= r <= 64, one r per
+ * adapter; f16, bf16 or f32, narrowed to fp16 with the base loader's range check.  scale is the caller's lora_alpha / r (lora_alpha /
+ * sqrt(r) for rsLoRA, from adapter_config.json): the projection becomes y = W x + scale * B (A x).  Unknown names (DoRA's
+ * lora_magnitude_vector included), an A without its B, a shape that disagrees with the base projection, a non-finite scale and a handle
+ * with tp_world > 1 are refused before anything is uploaded.  *id_out (>= 1) names the adapter until lora_destroy or aha_b200_destroy.
+ * aha_b200_lora_destroy refuses an adapter that a running or suspended request uses, and drops the prefix-cache pages written under it.
+ *
+ * aha_b200_batch_add_lora admits requests exactly like batch_add_many (packed prefills, prefix cache, all or nothing), request i running
+ * adapter adapters[i] (0: the base model), in a wide session only: a narrow session's CUDA-core step has no adapter path and is refused.
+ * It is refused while a speculative request runs (and batch_add_speculative while an adapter request runs).  Adapters apply to the text
+ * stack's projections; towers, embeddings and lm_head are the base model's.  The update runs as extra k-blocks of the same tensor-core
+ * kernels (the B columns of the adapters in use after the base weights; DESIGN.md section 4.14), so a request's ids do not depend on its
+ * slot, its neighbours or their adapters, the step it joins, or whether it was packed (prompts of 32 tokens or more); base requests yield
+ * the ids they yield in a session without adapters, and a session that never admits an adapter request launches the same kernels and
+ * graphs.  A request's prefix-cache hits come only from pages written under its own adapter.  batch_suspend / batch_resume carry the
+ * adapter; batch_cancel and the request's end release it. */
+int aha_b200_lora_create(aha_model* m, const aha_tensor_desc* tensors, size_t n, float scale, uint32_t* id_out);
+int aha_b200_lora_destroy(aha_model* m, uint32_t id);
+int aha_b200_batch_add_lora(aha_model* m, const aha_batch_request* reqs, const uint32_t* adapters, size_t n, int32_t* slots_out,
+                            uint32_t* first_tokens_out, int32_t* finished_out, aha_usage* usage);
+
 /* Prefix cache of a batch session (narrow or wide; new design).  With max_tokens > 0 the session keeps an index of the full 32-token KV pages
  * of admitted text-only prompts (batch_add, batch_add_many, choice 0 of batch_add_n), keyed by their token ids and the page before them,
  * and keeps up to max_tokens / 32 of those pages alive after their requests finish.  A later request whose prompt starts with cached pages

@@ -218,6 +218,13 @@ public:
         return id;
     }
     void rules_destroy(uint32_t id) { check(aha_b200_rules_destroy(h_, id)); }
+    // LoRA adapters (aha_b200_lora_create): PEFT-named lora_A / lora_B tensors and lora_alpha / r; the id goes into batch_add_lora.
+    uint32_t lora_create(const std::vector<aha_tensor_desc>& tensors, float scale) {
+        uint32_t id = 0;
+        check(aha_b200_lora_create(h_, tensors.data(), tensors.size(), scale, &id));
+        return id;
+    }
+    void lora_destroy(uint32_t id) { check(aha_b200_lora_destroy(h_, id)); }
     // The whole request with the decode loop on the device (generate_generic semantics, aha_b200_generate).
     // reuse_prefix (new design; the reference clears the cache after every request, generate.rs:147): keep the K/V of this request and
     // prefill only what follows the prefix the prompt shares with the cache -- same tokens, shorter time to the first one.
@@ -323,6 +330,17 @@ public:
         check(aha_b200_batch_add_speculative(h_, &r, &s, &a.slot, &a.first_token, &fin, nullptr));
         a.finished = fin != 0;
         return a;
+    }
+    // Requests into the open wide session, request i running adapter adapters[i] (0: the base model); all or nothing.
+    std::vector<Admitted> batch_add_lora(const std::vector<aha_batch_request>& reqs, const std::vector<uint32_t>& adapters) {
+        if (adapters.size() != reqs.size()) throw std::runtime_error("batch_add_lora: one adapter id per request");
+        const size_t n = reqs.size();
+        std::vector<int32_t> slots(n), fin(n);
+        std::vector<uint32_t> first(n);
+        check(aha_b200_batch_add_lora(h_, reqs.data(), adapters.data(), n, slots.data(), first.data(), fin.data(), nullptr));
+        std::vector<Admitted> out(n);
+        for (size_t i = 0; i < n; ++i) out[i] = Admitted{slots[i], first[i], fin[i] != 0};
+        return out;
     }
     // One step of every running request of the open session (aha_b200_batch_step_spec), `width` = the session width: per slot its status
     // (0 idle, 1 continues, 2 finished) and the tokens it delivered (1 for a plain request, 1 .. max_draft + 1 for a speculative one).
